@@ -1,14 +1,14 @@
 #!/usr/bin/env python
-"""bench.py -- reads/sec through coordinate sort + mark duplicates + BQSR gather/finalize/apply on B200.
+"""bench.py -- reads/sec through coordinate sort + mark duplicates + BQSR gather/finalize/apply on H100.
 
 One "step" = one pass of the whole hot path over one batch of synthetic 150-bp paired reads:
   value : whole-job reads/s with the reads already resident in HBM when the timed region starts
           (elp_sort_markdup + elp_bqsr_gather + [allreduce of the tables at N>1] + elp_bqsr_finalize + elp_bqsr_apply)
   e2e   : the same metric through the C ABI with HOST buffers: elp_append_batch (H2D from pinned memory) ... elp_fetch (D2H)
 Timing: CUDA events on the library's own stream (elp_timer_start/stop), barrier + synchronize on both sides, max over ranks.
-Each step re-ingests ~270 B/read (>> the 126 MB L2), so no kernel ever sees a warm L2 from the previous step.
+Each step re-ingests ~270 B/read (>> the 50 MB L2), so no kernel ever sees a warm L2 from the previous step.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--reads R] [--impl reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--reads R] [--impl reference] [--dump-outputs DIR]
 N>1 is launched by torchrun (one rank per GPU): ONE hg38-shaped genome is partitioned over the ranks by contig group (sfm-style,
 cmd/sfm.go); 1 % of the pairs span two groups.  All cross-GPU traffic of the hot path is NCCL inside the library (C ABI): the spread-pair
 exchange of elp_sort_markdup (grouped ncclSend/ncclRecv of 128-byte mate records) and one ncclAllReduce of the integer BQSR tables.  --impl reference times the CPU restatement of the reference algorithm (oracle/, the Go
@@ -33,6 +33,9 @@ sys.path.insert(0, ROOT)
 METRIC = "reads/sec through sort+markdup+BQSR"
 DEFAULT_READS = 30_000_000          # configs[1] scale (WES-scale 30M reads), with the full sort+markdup+BQSR path of configs[2]
 GENOME_SCALE = 20.0                 # hg38 / 20 = 155 Mbp  ->  30 M x 150 bp = 29x coverage, WGS-30x-like group statistics
+HBM_PEAK_GBS = 3350.0               # H100 SXM data sheet; the denominator of every "frac" below
+DUMP_BYTES = 64 << 20               # --dump-outputs writes at most this many bytes
+DUMP_READS = 1 << 16                # output records in the seeded sample of --dump-outputs
 
 
 def log(*a):
@@ -40,7 +43,7 @@ def log(*a):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
     def __init__(self, index=0):
@@ -147,6 +150,29 @@ def verify_against_oracle(ctx, w, out_np, n_reads, threads):
             "against": "oracle/ (C restatement of the reference) on the same reads", "seconds": round(time.time() - t0, 1)}
 
 
+def timed_outputs(ctx, out_np, n_reads):
+    """what a caller of the timed path receives after its last step, as float arrays: the BQSR tables and EmpiricalQuality in full, and
+    for a fixed, seeded sample of output records their record index, FLAG and recalibrated QUAL bytes"""
+    idx, flag, qoff, qual = out_np
+    tables, emp = ctx.tables_get(), ctx.empirical_get()
+    pick = np.sort(np.random.default_rng(0).choice(n_reads, size=min(DUMP_READS, n_reads), replace=False)).astype(np.int64)
+    lo, hi = qoff[pick].astype(np.int64), qoff[pick + 1].astype(np.int64)
+    budget = (DUMP_BYTES - 8 * tables.size - 4 * emp.size - 28 * pick.size - 8) // 4     # float32 QUAL bytes that still fit
+    keep = int(np.searchsorted(np.cumsum(hi - lo), budget, side="right"))
+    q_sel = np.concatenate([np.arange(a, b) for a, b in zip(lo[:keep], hi[:keep])]) if keep else np.zeros(0, np.int64)
+    q_off = np.zeros(keep + 1, np.int64)
+    q_off[1:] = np.cumsum(hi[:keep] - lo[:keep])
+    return {"bqsr_tables": tables.astype(np.float64), "empirical_quality": emp.astype(np.float32),
+            "sample_output_position": pick.astype(np.float64), "sample_record_index": idx[pick].astype(np.float64),
+            "sample_flag": flag[pick].astype(np.float32), "sample_qual_offset": q_off.astype(np.float64), "sample_qual": qual[q_sel].astype(np.float32)}
+
+
+def write_outputs(out_dir, arrays):
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -159,6 +185,7 @@ def main():
     ap.add_argument("--e2e-contexts", type=int, default=3, choices=(1, 3), help="contexts in the e2e pipeline ring (1: sequential, for runs where one context fills the HBM)")
     ap.add_argument("--verify", dest="verify", action="store_true", default=None, help="check the last step's output against the oracle (default: on at --gpus 1)")
     ap.add_argument("--no-verify", dest="verify", action="store_false")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step computed on rank 0 to DIR/<name>.npy (float32/float64; a seeded sample of the records)")
     args = ap.parse_args()
     rank, world, local = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("LOCAL_RANK", 0))
     from elprep_b200 import synth
@@ -286,6 +313,8 @@ def main():
         dev_ms.append(a); in_ms.append(b); out_ms.append(c_); coll_ms.append(d_)
     launches = ctx.launch_count()
     stats = ctx.kernel_stats()
+    # rank 0's outputs only (one 64 MB budget); taken before the e2e run reuses ctx and out_np
+    dumped = timed_outputs(ctx, out_np, n_reads) if args.dump_outputs and rank == 0 else None
     # ---- e2e: the same K steps through the public API with host buffers, software-pipelined over a ring of three contexts: while the
     # batch of step s uploads into one context, the context of step s-1 runs its device phases and starts its download, and the download of
     # step s-2 drains into the other of two page-locked output buffers.  The host->device copy engine -- the longest stage -- never waits.
@@ -355,33 +384,20 @@ def main():
     value = total_reads * args.steps / (dev_total_ms / 1e3)
     e2e = total_reads * args.steps / (e2e_total_ms / 1e3)
     # roofline of the dominant kernel (largest summed device time over the timed steps)
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
-    peak, peak_src = (peaks.get("hbm_gbs"), "measured (MEASURED_PEAKS.json hbm_gbs)") if peaks.get("hbm_gbs") else (6650.0, "fallback (B200_PROFILING.md)")
-    def roof_of(names, label, traffic_key=None):
+    peak, peak_src = HBM_PEAK_GBS, "NVIDIA H100 SXM data sheet (HBM3, 700 W card)"
+    def roof_of(names, label):
         ks = [stats[nm] for nm in names if nm in stats]
         if not ks:
             return None
         ms, by, ln = sum(k["ms"] for k in ks), sum(k["alg_bytes"] for k in ks), sum(k["launches"] for k in ks)
         ach = by / (ms / 1e3) / 1e9 if ms > 0 else None
-        traffic = None
-        try:   # DRAM bytes per launch from an `ncu --set full` capture of this same workload and build (profiles/r02_traffic.json names the capture)
-            tr = json.load(open(os.path.join(ROOT, "profiles", "r02_traffic.json")))
-            ent = tr["kernels"].get(traffic_key or names[0])
-            if ent and abs(tr["reads"] - n_reads) <= 0.01 * n_reads and world == 1:
-                traffic = ent["dram_bytes_per_launch"]
-        except Exception:
-            pass
-        return {"bound": "hbm", "kernel": label, "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak if ach else None, "traffic": traffic, "peak_source": peak_src,
+        return {"bound": "hbm", "kernel": label, "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak if ach else None, "peak_source": peak_src,
                 "launches": ln, "avg_launch_ms": ms / max(1, ln), "alg_bytes_per_launch": by / max(1, ln), "ms_per_step": ms / args.steps}
     dom = max(stats.items(), key=lambda kv: kv[1]["ms"]) if stats else (None, None)
     roof = roof_of([dom[0]], dom[0]) if dom[0] else None
     gather_names = [k for k in stats if k.startswith("bqsr_g_")]
     graded = {"radix_sort": roof_of(["radix_onesweep_u64"], "radix_onesweep_u64 (one digit pass: N*2*(8+4) B)"),
-              "covariate_histogram": roof_of(gather_names, "elp_bqsr_gather: " + "+".join(sorted(gather_names)) + " (N_eligible*(19+4+4c+L/2+L) + genome once)", "bqsr_g_count")}
+              "covariate_histogram": roof_of(gather_names, "elp_bqsr_gather: " + "+".join(sorted(gather_names)) + " (N_eligible*(19+4+4c+L/2+L) + genome once)")}
     kern = {n: {"ms_per_step": v["ms"] / args.steps, "launches_per_step": v["launches"] / args.steps,
                 "GBps": (v["alg_bytes"] / (v["ms"] / 1e3) / 1e9) if v["ms"] > 0 and v["alg_bytes"] > 0 else None} for n, v in sorted(stats.items(), key=lambda kv: -kv[1]["ms"])}
     cpu = None
@@ -406,6 +422,8 @@ def main():
             "phases_per_rank": phases_per_rank, "roofline_graded": graded,
             "gpu_launches": launches, "verified": (verified or {}).get("ok"), "verify": verified, "roofline": roof, "cpu_baseline": cpu, "clocks": clocks, "kernels": kern}
     print(json.dumps(line))
+    if dumped is not None:
+        write_outputs(args.dump_outputs, dumped)
     if dist:
         dist.barrier(); dist.destroy_process_group()
 

@@ -102,7 +102,7 @@ int upload_small(elp_ctx* c, void* dst, const void* src, size_t bytes) {
 
 int qual_presence_update(elp_ctx* c, uint64_t first_byte, uint64_t n_bytes) {
     if (!n_bytes) return E_OK;
-    const unsigned grid = (unsigned)std::min<uint64_t>((n_bytes / 16 + 255) / 256 + 1, 148 * 16);
+    const unsigned grid = (unsigned)std::min<uint64_t>((n_bytes / 16 + 255) / 256 + 1, 132 * 16);
     c->launches++;
     qual_presence_kernel<<<grid, 256, 0, c->stream>>>(c->qual.p + first_byte, n_bytes, c->d_qpresent);
     LAUNCH_CHECK(c);
@@ -304,8 +304,8 @@ static uint64_t sum_lengths(const int32_t* l, uint64_t n, uint64_t* seq_bytes) {
 }
 
 // Large host<->device copies go out whole by default.  (A copy engine serves its queue in order, so cutting a copy into pieces that are all
-// enqueued at once does not let another context's small copies overtake it -- measured with tools/e2e_probe.py: 32 MB pieces cost 5 % of the
-// duplex upload rate and the small copies waited just the same.  The phases therefore avoid the copy engines for their small uploads
+// enqueued at once does not let another context's small copies overtake it; the pieces only cost upload rate (tools/e2e_probe.py
+// compares the two).  The phases therefore avoid the copy engines for their small uploads
 // (upload_small), and a pipelined caller orders its downloads so that none is in flight while another context's phases read back.)
 // ELPREP_B200_COPY_CHUNK_MB > 0 restores the pieces for experiments.
 static cudaError_t copy_chunked(void* dst, const void* src, size_t bytes, cudaMemcpyKind kind, cudaStream_t s) {

@@ -420,7 +420,7 @@ int run_apply_kernel(elp_ctx* c, bool with_lut) {
             B.lpr = std::min(32, std::max(1, (c->h_ranges.lseq_max + 31) / 32)); B.rpw = 32 / B.lpr; B.err = c->d_err;
             if (!c->d_rowtab) { CUDA_TRY(c, cudaMalloc(&c->d_rowtab, 512)); CUDA_TRY(c, cudaMemsetAsync(c->d_rowtab, 0, 512, c->stream)); }
             B.rowtab = c->d_rowtab;
-            int sms = 148; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device);
+            int sms = 132; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device);
             const size_t smem = ((size_t)B.clut_bytes + 15) / 16 * 16 + (size_t)AP2_WARPS * (B.rpw * B.lpr * 32 + 32) + 16;
             CUDA_TRY(c, cudaFuncSetAttribute(bqsr_apply2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
             const uint64_t n_pass = (n + B.rpw - 1) / B.rpw;

@@ -815,7 +815,7 @@ int gather_general(elp_ctx* c, GatherArgs A, const uint32_t* in_list, uint32_t n
         for (int s = 0; s < A.n_slots; s++) { A.qslot[qs[s]] = (int8_t)s; A.slot_q[s] = (uint8_t)qs[s]; }
     }
     const size_t smem = (size_t)c->geom.n_cov * (A.n_slots + 1) * A.ncols_s * 4 * 2;
-    int sms = 148; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device);
+    int sms = 132; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device);
     // descriptors (48 B/read, indexed by read) and the overflow skip bitmasks live in scratch buffers that are free in this phase
     CUDA_TRY(c, c->keys_a.reserve(n * 6 + 8, c->stream));
     CUDA_TRY(c, c->vals_b.reserve(2 * n + 16, c->stream));
@@ -945,7 +945,7 @@ int phase_bqsr_gather(elp_ctx* c) {
         } else {
             const int n_cls = 2 * c->geom.n_cov;
             const int lpr = std::min(32, std::max(1, (c->h_ranges.lseq_max + 31) / 32)), rpw = 32 / lpr;
-            int sms = 148; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device);
+            int sms = 132; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device);
             // small device words: [0,64) class histogram | [64,129) region bases | [136,265) list counters | [272,274) segment counts | [276,278) queue heads
             uint32_t* sm = c->d_bq_small;
             uint32_t *d_hist = sm, *d_region = sm + 64, *d_keycnt = sm + 136, *d_nseg = sm + 272, *d_next = sm + 276;

@@ -1,4 +1,4 @@
-// common.cuh -- shared device/host helpers for the elprep_b200 CUDA library (sm_100a only).
+// common.cuh -- shared device/host helpers for the elprep_b200 CUDA library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>

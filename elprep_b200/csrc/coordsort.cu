@@ -114,9 +114,20 @@ __global__ void __launch_bounds__(256) chunk_keys_kernel(uint64_t m, const uint3
     else if (chunk == 2) key = ((uint64_t)mod_flag(c.flag[a]) << 8) | c.mapq[a];
     else if (chunk < 3 + nq) {
         const int qc = nq - 1 - (chunk - 3);
-        const uint64_t q0 = c.qname_off[a], q1 = c.qname_off[a + 1];
+        const uint64_t q0 = c.qname_off[a], q1 = c.qname_off[a + 1], lo = q0 + (uint64_t)qc * 8;
         key = 0;
-        for (int b = 0; b < 8; b++) { const uint64_t o = q0 + (uint64_t)qc * 8 + b; key = (key << 8) | (o < q1 ? c.qname[o] : 0); }
+        if (lo < q1) {
+            // every load is unconditional and inside the name (index clamped to its last byte); bytes past the end are masked to
+            // zero afterwards.  Keep this form: on the H100 the equivalent per-byte form `o < q1 ? qname[o] : 0` gave nonzero key
+            // bytes past the end of names shorter than the chunk, in whole warps, and long tie runs came out misordered
+            // (tests/test_gpu_parity_large.py).  The two are the same function in C++ and no fault is visible in the SASS of the
+            // old form, so what went wrong in its execution is not known.
+            const uint64_t avail = q1 - lo;
+            for (int b = 0; b < 8; b++) {
+                const uint32_t byte = c.qname[min(lo + (uint64_t)b, q1 - 1)];
+                key = (key << 8) | ((uint64_t)b < avail ? byte : 0u);
+            }
+        }
     } else {
         const int32_t r = refid[a];
         const uint64_t rr = (r < 0 || r >= L.n_contigs) ? (uint64_t)L.n_contigs : (uint64_t)r;

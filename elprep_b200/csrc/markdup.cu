@@ -424,7 +424,7 @@ int phase_adapt(elp_ctx* c) {
     DeviceRanges init{}; init.pos_max = 0; init.upos_min = INT_MAX; init.upos_max = INT_MIN; init.score_max = 0; init.lseq_max = 0;
     { int rcu = upload_small(c, c->d_ranges, &init, sizeof init); if (rcu) return rcu; }
     if (n) {
-        int sms = 148; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device);
+        int sms = 132; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device);
         AdaptArgs A{};
         A.n = n; A.flag = c->flag.p; A.pos = c->pos.p; A.rg = c->rg.p; A.rg_lib = c->d_rg_lib; A.n_rg = c->n_rg; A.cigar_off = c->cigar_off.p; A.cigar = c->cigar.p;
         A.qual_off = c->qual_off.p; A.qual = c->qual.p; A.qname_off = c->qname_off.p; A.qname = c->qname.p; A.upos = c->upos.p; A.score = c->score.p; A.qhash = c->qhash.p;

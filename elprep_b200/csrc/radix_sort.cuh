@@ -1,4 +1,4 @@
-// radix_sort.cuh -- hand-written onesweep LSD radix sort for sm_100a (keys u64 or u128, u32 payload).
+// radix_sort.cuh -- hand-written onesweep LSD radix sort for sm_90a (keys u64 or u128, u32 payload).
 //
 // Replaces pargo sort.StableSort as used by By(CoordinateLess).ParallelStableSort (sam/sam-types.go:599-641)
 // and the sharded-map grouping of filters/mark-duplicates.go:210-396 (sort-by-key + segmented scan instead of

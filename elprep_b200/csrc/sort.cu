@@ -28,7 +28,7 @@ int radix_sort_impl(elp_ctx* c, K* ka, K* kb, uint32_t* va, uint32_t* vb, uint64
     CUDA_TRY(c, cudaMemsetAsync(ws.counters, 0, MAX_PASSES * 4, c->stream));
     CUDA_TRY(c, cudaMemsetAsync(ws.status, 0, need, c->stream));
 
-    int dev_sms = 148;
+    int dev_sms = 132;
     cudaDeviceGetAttribute(&dev_sms, cudaDevAttrMultiProcessorCount, c->device);
     std::string nm = std::string("radix_hist_") + tag;
     {

@@ -1,5 +1,5 @@
 /*
- * elprep_b200.h -- C ABI of the B200-native hot path of elPrep 5.1.3:
+ * elprep_b200.h -- C ABI of the H100-native hot path of elPrep 5.1.3:
  * coordinate sort -> mark duplicates -> BQSR gather -> finalize -> apply.
  *
  * Plain C: pointers and sizes only, no CUDA/torch types.  Every entry point names the reference

@@ -18,11 +18,13 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 class FakeContext:
     SO_COORDINATE = 4
     live = 0
+    made = []
 
     def __init__(self, header, device=0, profile=False, **kw):
         self.header, self.batch, self.ref, self.sites = header, None, {}, {}
         self.n, self._launches, self._t0, self.res = 0, 0, None, None
         FakeContext.live += 1
+        FakeContext.made.append(self)
 
     # side inputs / lifecycle
     def set_reference(self, ci, bases): self.ref[ci] = bases
@@ -93,8 +95,8 @@ class FakeEvent:
     def elapsed_time(self, other): return 1e3 * (other.t - self.t)
 
 
-@pytest.mark.parametrize("extra", [[], ["--e2e-contexts", "1", "--steps", "1"]])
-def test_bench_main_runs_and_prints_one_contract_line(monkeypatch, extra):
+@pytest.mark.parametrize("extra", [[], ["--e2e-contexts", "1", "--steps", "1"], ["--dump-outputs", "{tmp}"]])
+def test_bench_main_runs_and_prints_one_contract_line(monkeypatch, tmp_path, extra):
     import torch
     sys.path.insert(0, ROOT)
     import bench
@@ -107,12 +109,14 @@ def test_bench_main_runs_and_prints_one_contract_line(monkeypatch, extra):
     monkeypatch.setattr(torch.cuda, "Event", FakeEvent)
     monkeypatch.setattr(torch.cuda, "mem_get_info", lambda *a: (100 * 10**9, 180 * 10**9))
     monkeypatch.setattr(device, "Context", FakeContext)
+    monkeypatch.setattr(FakeContext, "made", [])
     monkeypatch.setattr(device, "SO_COORDINATE", 4, raising=False)
     monkeypatch.setattr(bench.ClockSampler, "start", lambda self: None)
     monkeypatch.setattr(bench.ClockSampler, "stop", lambda self: {"sm_mhz": 1965.0, "sm_max_mhz": 1965.0, "reasons": [], "samples": 3})
     monkeypatch.setattr(bench, "GENOME_SCALE", 3000.0)              # a ~1 Mbp genome for 12 k reads
     for k in ("RANK", "WORLD_SIZE", "LOCAL_RANK"):
         monkeypatch.delenv(k, raising=False)
+    extra = [a.replace("{tmp}", str(tmp_path / "out")) for a in extra]
     argv = ["bench.py", "--reads", "12000", "--steps", "4", "--warmup", "1", "--cpu-sample", "6000"] + extra
     monkeypatch.setattr(sys, "argv", argv)
     buf = io.StringIO()
@@ -127,10 +131,25 @@ def test_bench_main_runs_and_prints_one_contract_line(monkeypatch, extra):
     assert d["n_gpus"] == 1 and d["unit"] == "reads/s" and d["higher_is_better"] is True and d["config"]["workload"]
     assert d["verified"] is True and all(d["verify"]["checks"].values())
     e = d["e2e"]
-    assert e["h2d_bytes_per_step"] > 0 and e["d2h_bytes_per_step"] > 0 and e["value"] > 0 and e["contexts"] == (1 if extra else 3)
-    assert (e["steady_ms_per_step"] is None) == bool(extra)         # needs >= 3 pipelined steps
+    assert e["h2d_bytes_per_step"] > 0 and e["d2h_bytes_per_step"] > 0 and e["value"] > 0 and e["contexts"] == (1 if "--e2e-contexts" in extra else 3)
+    assert (e["steady_ms_per_step"] is None) == ("--steps" in extra)     # needs >= 3 pipelined steps
     assert d["roofline"]["kernel"] == "bqsr_apply" and 0 < d["roofline"]["frac"] and set(d["roofline_graded"]) == {"radix_sort", "covariate_histogram"}
     assert d["cpu_baseline"]["kind"] == "port" and d["cpu_baseline"]["value"] > 0 and d["gpu_launches"] > 0
+    if "--dump-outputs" in extra:
+        out = tmp_path / "out"
+        got = {f.stem: np.load(f) for f in out.glob("*.npy")}
+        assert set(got) == {"bqsr_tables", "empirical_quality", "sample_output_position", "sample_record_index", "sample_flag", "sample_qual_offset", "sample_qual"}
+        assert all(a.dtype in (np.float32, np.float64) for a in got.values()) and sum(f.stat().st_size for f in out.glob("*.npy")) <= 64 << 20
+        assert got["bqsr_tables"].sum() > 0 and got["sample_record_index"].size == d["config"]["reads_per_gpu"] and got["sample_qual"].size == got["sample_qual_offset"][-1] > 0
+        # the values are the timed context's results (every step computes the same from the same input)
+        timed = FakeContext.made[0]
+        pos = got["sample_output_position"].astype(np.int64)
+        assert np.array_equal(got["sample_record_index"], timed.perm[pos].astype(np.float64))
+        assert np.array_equal(got["sample_flag"], timed.srt.flag[pos].astype(np.float32))
+        q = np.concatenate([timed.srt.qual[int(timed.srt.qual_off[i]):int(timed.srt.qual_off[i + 1])] for i in pos])
+        assert np.array_equal(got["sample_qual"], q[:got["sample_qual"].size].astype(np.float32))
+        assert np.array_equal(got["bqsr_tables"], timed.tables_get().astype(np.float64))
+        assert np.array_equal(got["empirical_quality"], timed.empirical_get().astype(np.float32))
 
 
 def _rank_main(rank, world, port, out_dir):

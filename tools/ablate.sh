@@ -5,7 +5,7 @@ cd "$(dirname "$0")/../elprep_b200/csrc"
 mkdir -p ../lib/exp
 rm -f ../lib/exp/*.so
 SRCS="api.cu bgzf.cpp bam_ingest.cu sort.cu markdup.cu optical.cu coordsort.cu bqsr_gather.cu bqsr_apply.cu bqsr_finalize.cu"
-FL="-O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -lineinfo -Xcompiler -fPIC,-ffp-contract=off -shared"
+FL="-O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -lineinfo -Xcompiler -fPIC,-ffp-contract=off -shared"
 for spec in "$@"; do
   name="${spec%%:*}"; defs="${spec#*:}"; [ "$defs" = "$spec" ] && defs=""
   nvcc $FL $defs -o ../lib/exp/lib_$name.so $SRCS -lcudart -lz &

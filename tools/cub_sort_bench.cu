@@ -1,7 +1,7 @@
 // cub_sort_bench.cu -- YARD-STICK ONLY (SURVEY.md section 7 step 6): cub::DeviceRadixSort::SortPairs on the same problem the
 // library's own onesweep sort is timed on (30 M 64-bit keys, 34 / 40 / 64 significant bits, 32-bit payload), on the same box.
 // A stand-alone binary: nothing of CUB is linked into libelprep_b200.so or used on the product path.
-//   nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -o tools/_build/cub_sort_bench tools/cub_sort_bench.cu
+//   nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -o tools/_build/cub_sort_bench tools/cub_sort_bench.cu
 #include <cub/cub.cuh>
 #include <cstdint>
 #include <cstdio>
@@ -38,8 +38,8 @@ int main(int argc, char** argv) {
                 cudaMemcpy(hk.data(), k2.Current(), n * 8, cudaMemcpyDeviceToHost);
                 bool ok = true; for (size_t i = 1; i < n; i++) if (hk[i - 1] > hk[i]) { ok = false; break; }
                 const int passes = (bits + 7) / 8;
-                printf("%s{\"key_bits\": %d, \"ms\": %.4f, \"sorted\": %s, \"passes_8bit\": %d, \"GBps_alg\": %.1f, \"frac_of_6561\": %.3f}", bi ? ", " : "", bits, best, ok ? "true" : "false",
-                       passes, (double)n * (8.0 + 2.0 * passes * 12.0) / (best * 1e-3) / 1e9, (double)n * (8.0 + 2.0 * passes * 12.0) / (best * 1e-3) / 1e9 / 6561.3);
+                printf("%s{\"key_bits\": %d, \"ms\": %.4f, \"sorted\": %s, \"passes_8bit\": %d, \"GBps_alg\": %.1f, \"frac_of_3350\": %.3f}", bi ? ", " : "", bits, best, ok ? "true" : "false",
+                       passes, (double)n * (8.0 + 2.0 * passes * 12.0) / (best * 1e-3) / 1e9, (double)n * (8.0 + 2.0 * passes * 12.0) / (best * 1e-3) / 1e9 / 3350.0);
             }
         }
         cudaFree(tmp);
