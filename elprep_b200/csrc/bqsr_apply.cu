@@ -440,9 +440,15 @@ int run_apply_kernel(elp_ctx* c, bool with_lut) {
             c->qual_out_valid = true;
             return E_OK;
         }
+        // bqsr_apply_kernel's output image holds WARPS reads of at most CHUNK * 32 bases: longer reads are refused here, before
+        // the launch (inside the kernel the block's slice of the output stream would overrun the image)
+        if (c->h_ranges.lseq_max > CHUNK * 32)
+            return c->fail(E_LIMIT, "BQSR: read longer than the device kernel supports (%d bases; without the shared-memory apply table the limit is %d)",
+                           c->h_ranges.lseq_max, CHUNK * 32);
         A.lanes_per_read = std::min(32, std::max(1, (c->h_ranges.lseq_max + CHUNK - 1) / CHUNK));
         const uint64_t reads_per_block = (uint64_t)WARPS * (32 / A.lanes_per_read);
-        c->begin(with_lut ? "bqsr_apply" : "qual_materialize", bytes);
+        // its own stats name, so that a caller can tell which apply kernel ran ("bqsr_apply" is bqsr_apply2_kernel)
+        c->begin(with_lut ? "bqsr_apply_gmem" : "qual_materialize", bytes);
         bqsr_apply_kernel<<<(unsigned)((n + reads_per_block - 1) / reads_per_block), WARPS * 32, 0, c->stream>>>(A);
         c->end(); LAUNCH_CHECK(c);
     }

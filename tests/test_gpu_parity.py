@@ -97,10 +97,12 @@ def test_read_lengths(L):
 
 
 def test_mixed_read_lengths():
-    """reads of different lengths in one context (lanes per read follow the longest)"""
+    """reads of 20 to 300 bases in one context (lanes per read follow the longest)"""
     a = synth.make_workload(2_000, SMALL, seed=201, L=150)
-    b = synth.make_workload(2_000, SMALL, seed=202, L=49)
-    w = synth.Workload(a.header, sam.AlignmentBatch.concat([a.batch, b.batch]), a.contig_bases, a.sites, a.params)
+    parts = [a.batch] + [synth.make_workload(600, SMALL, seed=202 + k, L=L, genome_seed=201, pair_id_base=(k + 1) << 24, want_reference=False).batch
+                         for k, L in enumerate((20, 32, 33, 49, 100, 151, 250, 300))]
+    w = synth.Workload(a.header, sam.AlignmentBatch.concat(parts), a.contig_bases, a.sites, a.params)
+    assert int(w.batch.lseq.min()) == 20 and int(w.batch.lseq.max()) == 300
     g = gpu_pipeline(w, n_batches=3)
     o = oracle_pipeline(w)
     _compare(w, g, o)
@@ -149,8 +151,8 @@ def test_empty_and_single():
     _compare(w, gpu_pipeline(w), oracle_pipeline(w))
 
 
-def _adversarial_records():
-    """hand-built reads covering clip/indel/adaptor/N/low-qual-tail corner cases (SURVEY.md Appendix C)"""
+def _adversarial_records(quals=(2, 2, 5, 6, 12, 23, 37, 40)):
+    """hand-built reads covering clip/indel/adaptor/N/low-qual-tail corner cases (SURVEY.md Appendix C); QUAL drawn from ``quals``"""
     rng = np.random.default_rng(77)
     recs, L = [], 60
     cigars = ["60M", "5S55M", "55M5S", "3H5S50M5S", "20M3I37M", "20M4D40M", "10S20M2I10M3D18M", "5S20M5D30M5S", "1M1I58M", "58M1I1M",
@@ -168,7 +170,7 @@ def _adversarial_records():
         ins = int(rng.integers(20, 160))
         pnext = pos - ins + 50 if rev else pos + ins - 50
         tlen = (-ins if rev else ins) if paired else 0
-        q = rng.choice([2, 2, 5, 6, 12, 23, 37, 40], size=L).astype(int)
+        q = rng.choice(list(quals), size=L).astype(int)
         if t % 7 == 0:
             q[:8] = 2
         if t % 11 == 0:
@@ -180,13 +182,34 @@ def _adversarial_records():
     return recs
 
 
-def test_adversarial_clipping_cases():
+def _adversarial_run(quals):
     contigs = [("chr20", 4_000)]
     base = synth.make_workload(10, contigs, seed=5)       # header + reference + sites
-    b = sam.AlignmentBatch.from_records(base.header, _adversarial_records())
+    b = sam.AlignmentBatch.from_records(base.header, _adversarial_records(quals))
+    assert set(np.unique(b.qual).tolist()) == set(quals) | {1}
     sites = [np.array([[1005, 1005], [1100, 1109], [1200, 1200], [1250, 1300]], dtype=np.int32)]
     w = synth.Workload(base.header, b, base.contig_bases, sites, {})
-    _compare(w, gpu_pipeline(w), oracle_pipeline(w))
+    g = gpu_pipeline(w, profile=True)
+    _compare(w, g, oracle_pipeline(w))
+    return g
+
+
+def test_adversarial_clipping_cases():
+    """five QUAL values >= 6: the general kernels gather every read"""
+    from util import bqsr_paths
+    g = _adversarial_run((2, 2, 5, 6, 12, 23, 37, 40))
+    assert bqsr_paths(g["stats"])[0] == "general", sorted(g["stats"])
+
+
+def test_adversarial_clipping_cases_fast_path():
+    """the same reads with an alphabet the count kernel accepts ({1,2,3,12,23,37}: S = 3, six values): checks closed_form_clip on the
+    device, <= 2 known-site ranges, the indel records and the hand-off of the remaining reads to the general kernels (cx_list), both
+    adding into one table"""
+    from util import bqsr_paths
+    g = _adversarial_run((2, 3, 12, 23, 37))
+    assert bqsr_paths(g["stats"])[0] == "fast", sorted(g["stats"])
+    assert g["stats"]["bqsr_g_count"]["launches"] and g["stats"]["bqsr_g_count_indel"]["launches"]
+    assert "bqsr_g_prep" in g["stats"], "no read was handed to the general kernels"
 
 
 def test_invalid_qual_is_an_error():

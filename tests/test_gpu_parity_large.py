@@ -9,15 +9,15 @@ import numpy as np
 import pytest
 
 from elprep_b200 import synth
-from util import oracle_tables_dense
+from util import bqsr_paths, fast_plan, oracle_tables_dense, with_qual_alphabet
 
 pytestmark = pytest.mark.gpu
 THREADS = min(os.cpu_count() or 1, 64)
 
 
-def _run_gpu(w, sort, markdup, bqsr, n_batches):
+def _run_gpu(w, sort, markdup, bqsr, n_batches, profile=False):
     from elprep_b200 import device
-    ctx = device.Context(w.header)
+    ctx = device.Context(w.header, profile=profile)
     try:
         if bqsr:
             for ci in range(len(w.header.SQ)):
@@ -37,6 +37,8 @@ def _run_gpu(w, sort, markdup, bqsr, n_batches):
             ctx.bqsr_apply()
         idx, flag, qoff, qual = ctx.fetch()
         res.update(perm=idx, flag=flag, qual=qual[:int(qoff[-1])], qual_off=qoff)
+        if profile:
+            res["stats"] = ctx.kernel_stats()
         return res
     finally:
         ctx.close()
@@ -78,12 +80,28 @@ def test_c1_2m_sort_only():
     _compare(g, o, False)
 
 
-def test_c1_2m_full_path():
+def _c1_full_path(quals=None):
     w = synth.make_workload(1_000_000, [("chr20", 64_444_167)], seed=20260925, threads=THREADS)
-    g = _run_gpu(w, True, True, True, 3)
+    if quals:
+        w = with_qual_alphabet(w, quals, seed=25)
+    g = _run_gpu(w, True, True, True, 3, profile=True)
     o = _run_oracle(w, True, True, True)
     _compare(g, o, True)
     assert int(((g["flag"] & 0x400) != 0).sum()) > 100_000
+    assert bqsr_paths(g["stats"])[0] == "fast"
+
+
+def test_c1_2m_full_path():
+    """the generator's four QUAL levels: count kernel S = 3"""
+    _c1_full_path()
+
+
+def test_c1_2m_full_path_s4_alphabet():
+    """a five-value alphabet (count kernel S = 4, classifier shift 3): every read-group class runs many 255-pass segments through a
+    contended work queue"""
+    quals = (2, 10, 18, 26, 34)
+    assert fast_plan(quals, 4, 150) == (4, 3)
+    _c1_full_path(quals)
 
 
 def test_c2_30m_full_path():

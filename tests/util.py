@@ -41,14 +41,82 @@ def oracle_tables_dense(t, max_cycle=500):
     return d, e
 
 
+SYNTH_QUALS = (2, 12, 23, 37)      # the four QUAL levels of the synthetic generator (Q4 in synth.cpp)
+
+
+def with_qual_alphabet(w, values, seed=0):
+    """A copy of workload ``w`` whose QUAL arena uses exactly ``values``: the generator's four levels map monotonically onto the sorted
+    targets; with more targets than levels, each level is split between neighbouring targets by a seeded RNG.  Duplicate scores and
+    BQSR both follow from QUAL, so the oracle simply runs on the remapped batch."""
+    from elprep_b200 import synth
+    vals = sorted(set(int(v) for v in values))
+    k = len(vals)
+    assert k >= 1 and 0 <= vals[0] and vals[-1] <= 93
+    q = w.batch.qual
+    assert set(np.nonzero(np.bincount(q, minlength=256))[0].tolist()) <= set(SYNTH_QUALS), "with_qual_alphabet starts from the generator's four levels"
+    groups = []
+    for i in range(4):
+        lo = i * k // 4
+        groups.append(np.array(vals[lo:max(lo + 1, (i + 1) * k // 4)], dtype=np.uint8))
+    rng = np.random.default_rng(seed)
+    out = np.empty_like(q)
+    step = 1 << 24                                    # chunks keep the temporaries small on C1-sized arenas
+    for s in range(0, q.size, step):
+        qs, os_ = q[s:s + step], out[s:s + step]
+        r = rng.integers(0, 1 << 16, size=qs.size, dtype=np.uint16)
+        for lv, g in zip(SYNTH_QUALS, groups):
+            m = qs == lv
+            os_[m] = g[r[m] % g.size]
+    b = w.batch.copy()
+    b.qual = out
+    assert np.nonzero(np.bincount(out, minlength=256))[0].tolist() == vals, "the remapped workload does not use exactly the requested QUAL alphabet"
+    return synth.Workload(w.header, b, w.contig_bases, w.sites, dict(w.params, quals=tuple(vals)))
+
+
+def fast_plan(values, n_cov, lseq_max):
+    """Restatement of plan_fast (csrc/bqsr_gather.cu): (S, sh) of the bqsr_count_kernel instance the library picks for a QUAL alphabet,
+    or None when the general kernels gather."""
+    vals = sorted(set(int(v) for v in values))
+    slots = [q for q in vals if q >= 6]
+    if max(vals) > 93 or not slots or len(slots) > 4 or len(vals) > 8:
+        return None
+    if n_cov < 1 or 2 * n_cov > 64 or not 1 <= lseq_max <= 1024:
+        return None
+    for sh in range(5):
+        if len({(q >> sh) & 7 for q in vals}) == len(vals):
+            return len(slots), sh
+    return None
+
+
+def apply_plan(values, n_cov, lseq_max, max_cycle=500):
+    """Which apply kernel elp_bqsr_apply picks (run_apply_kernel / build_compact_lut): "v2" (bqsr_apply2_kernel, compact table in
+    shared memory) when the table of the QUAL values >= 6 present fits 80 KB, else "gmem" (bqsr_apply_kernel, global table)"""
+    S = sum(1 for q in set(values) if q >= 6)
+    Lc = max(1, min(max_cycle, lseq_max))
+    blk = n_cov * S * 17
+    blk += 1 - (blk & 1)
+    nbytes = ((2 * Lc + 1 + 64) * blk + 15) // 16 * 16
+    return "v2" if S and n_cov and nbytes <= 80 * 1024 and lseq_max <= min(Lc, 1024) else "gmem"
+
+
+def bqsr_paths(stats):
+    """(gather, apply) kernels a profiled context ran, from kernel_stats(): gather "fast" (bqsr_count_kernel, with bqsr_g_prep only for the
+    reads it hands to the general kernels) or "general" (bqsr_prep + bqsr_chunk over every read); apply "v2" or "gmem"."""
+    fast, general = "bqsr_g_count" in stats, "bqsr_g_chunk" in stats
+    assert not (fast and general), sorted(stats)
+    if fast:
+        assert "bqsr_g_count_indel" in stats and "bqsr_g_prep2" in stats, sorted(stats)
+    v2, gmem = "bqsr_apply" in stats, "bqsr_apply_gmem" in stats
+    assert not (v2 and gmem), sorted(stats)
+    return ("fast" if fast else "general" if general else None), ("v2" if v2 else "gmem" if gmem else None)
+
+
 def gpu_pipeline(w, bqsr=True, n_batches=1, max_cycle=500, quantize_levels=0, sqq=None, sort=True, markdup=True, profile=False, keep_ctx=False):
     from elprep_b200 import device
     ctx = device.Context(w.header, max_cycle=max_cycle, quantize_levels=quantize_levels, sqq=sqq, profile=profile)
     try:
         if bqsr:
-            for ci in range(len(w.header.SQ)):
-                ctx.set_reference(ci, w.contig_bases[ci])
-                ctx.set_known_sites(ci, w.sites[ci], already_flat=True)
+            set_side_inputs(ctx, w)
         n = w.batch.n
         if n_batches <= 1 or n < n_batches:
             ctx.append(w.batch)
@@ -56,28 +124,41 @@ def gpu_pipeline(w, bqsr=True, n_batches=1, max_cycle=500, quantize_levels=0, sq
             bounds = [n * i // n_batches for i in range(n_batches + 1)]
             for a, b in zip(bounds[:-1], bounds[1:]):
                 ctx.append(w.batch.take(np.arange(a, b)))
-        ctx.sort_markdup(device.SO_COORDINATE if sort else device.SO_KEEP, markdup)
-        res = {}
-        if bqsr:
-            ctx.bqsr_gather()
-            res["tables"] = ctx.tables_get()
-            with tempfile.TemporaryDirectory() as d:
-                p = os.path.join(d, "g.recal")
-                ctx.bqsr_finalize(p)
-                res["report"] = open(p).read()
-            res["emp"] = ctx.empirical_get()
-            ctx.bqsr_apply()
-        idx, flag, qoff, qual = ctx.fetch()
-        res.update(perm=idx, flag=flag, qual=qual[:int(qoff[-1])] if n else qual[:0], qual_off=qoff)
-        if profile:
-            res["stats"] = ctx.kernel_stats()
-        res["launches"] = ctx.launch_count()
+        res = gpu_phases(ctx, bqsr=bqsr, sort=sort, markdup=markdup, profile=profile)
         if keep_ctx:
             res["ctx"] = ctx
         return res
     finally:
         if not keep_ctx:
             ctx.close()
+
+
+def set_side_inputs(ctx, w):
+    for ci in range(len(w.header.SQ)):
+        ctx.set_reference(ci, w.contig_bases[ci])
+        ctx.set_known_sites(ci, w.sites[ci], already_flat=True)
+
+
+def gpu_phases(ctx, bqsr=True, sort=True, markdup=True, profile=False):
+    """sort + duplicate marking (+ BQSR gather, finalize, apply) over the reads already appended to ``ctx``, then fetch"""
+    from elprep_b200 import device
+    ctx.sort_markdup(device.SO_COORDINATE if sort else device.SO_KEEP, markdup)
+    res = {}
+    if bqsr:
+        ctx.bqsr_gather()
+        res["tables"] = ctx.tables_get()
+        with tempfile.TemporaryDirectory() as d:
+            p = os.path.join(d, "g.recal")
+            ctx.bqsr_finalize(p)
+            res["report"] = open(p).read()
+        res["emp"] = ctx.empirical_get()
+        ctx.bqsr_apply()
+    idx, flag, qoff, qual = ctx.fetch()
+    res.update(perm=idx, flag=flag, qual=qual[:int(qoff[-1])] if ctx.n else qual[:0], qual_off=qoff)
+    if profile:
+        res["stats"] = ctx.kernel_stats()
+    res["launches"] = ctx.launch_count()
+    return res
 
 
 # ---- BAM alignment records (sam/bam-files.go:300-400) for the device ingest tests ----

@@ -16,7 +16,7 @@ for ci in range(len(contigs)):
 for rep in range(3):
     ctx.reset(); ctx.append(hb); ctx.reset_stats(); ctx.sort_markdup(); ctx.bqsr_gather(); ctx.bqsr_finalize(None); ctx.bqsr_apply(); ctx.synchronize()
 st = ctx.kernel_stats()
-print(os.environ.get("ELPREP_B200_LIB","default").split("/")[-1], "  ".join("%%s %%.2f" %% (k, st[k]["ms"]) for k in ("bqsr_gather", "bqsr_gather_indel", "bqsr_gather_general", "bqsr_gen_list", "bqsr_prep", "bqsr_apply", "adapt") if k in st), flush=True)
+print(os.environ.get("ELPREP_B200_LIB","default").split("/")[-1], "  ".join("%%s %%.2f" %% (k, st[k]["ms"]) for k in ("bqsr_gather", "bqsr_gather_indel", "bqsr_gather_general", "bqsr_gen_list", "bqsr_prep", "bqsr_apply", "bqsr_apply_gmem", "adapt") if k in st), flush=True)
 ''' % ROOT
 for name in sys.argv[1:]:
     env = dict(os.environ)
