@@ -147,6 +147,7 @@ int elp_create(const elp_config* cfg, elp_ctx** out) {
     auto bail = [&](int code) { g_create_error = c->err; elp_destroy(c); return code; };
     if (cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess) { c->err = "cudaStreamCreate failed"; return bail(ELP_ECUDA); }
     c->n_contigs = cfg->n_contigs;
+    c->has_contig_names = cfg->contig_names != nullptr;
     for (int i = 0; i < cfg->n_contigs; i++) { c->contig_len.push_back(cfg->contig_lengths[i]); c->contig_names.push_back(cfg->contig_names && cfg->contig_names[i] ? cfg->contig_names[i] : ""); }
     // library ids: equal LB strings share an id (lbTable, mark-duplicates.go:413-423); covariates: PU if present else ID (bqsr.go:35-51)
     c->n_rg = cfg->n_read_groups;
@@ -194,6 +195,7 @@ void elp_destroy(elp_ctx* c) {
     if (!c) return;
     cudaSetDevice(c->device);
     if (c->stream) cudaStreamSynchronize(c->stream);
+    sam_state_release(c);
     for (auto p : c->d_ref) if (p) cudaFree(p);
     for (auto p : c->d_refnib_raw) if (p) cudaFree(p);
     for (auto p : c->d_refhot_raw) if (p) cudaFree(p);

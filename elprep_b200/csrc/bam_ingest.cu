@@ -308,17 +308,25 @@ extern "C" int elp_append_bam(elp_ctx* c, const uint8_t* records, uint64_t n_byt
         n_records = walked.size() - 1;
         record_off = walked.data();
     }
-    uint64_t bn = n_records;
-    if (bn == 0) return ELP_OK;
-    if (record_off[bn] != n_bytes) return c->fail(E_INVAL, "elp_append_bam: record_off[n_records] must equal n_bytes");
-    for (uint64_t i = 0; i < bn; i++) if (record_off[i + 1] < record_off[i] || record_off[i + 1] > n_bytes) return c->fail(E_INVAL, "elp_append_bam: record_off must be non-decreasing and within n_bytes");
+    const uint64_t nrec = n_records;
+    if (nrec == 0) return ELP_OK;
+    if (record_off[nrec] != n_bytes) return c->fail(E_INVAL, "elp_append_bam: record_off[n_records] must equal n_bytes");
+    for (uint64_t i = 0; i < nrec; i++) if (record_off[i + 1] < record_off[i] || record_off[i + 1] > n_bytes) return c->fail(E_INVAL, "elp_append_bam: record_off must be non-decreasing and within n_bytes");
+    if (c->n + nrec >= (1ull << 32)) return c->fail(E_LIMIT, "more than 2^32-1 reads in one context");
+    TRY(grow(c, c->bam_raw, n_bytes + 64, 0)); TRY(grow(c, c->bam_off, nrec + 2, 0));
+    CUDA_TRY(c, cudaMemcpyAsync(c->bam_raw.p, records, n_bytes, cudaMemcpyHostToDevice, c->stream));
+    CUDA_TRY(c, cudaMemcpyAsync(c->bam_off.p, record_off, (nrec + 1) * 8, cudaMemcpyHostToDevice, c->stream));
+    return bam_ingest_core(c, n_bytes, nrec);
+}
+
+// The device-resident part of elp_append_bam, shared with elp_append_sam: nrec records (n_bytes in all) already sit in bam_raw, and
+// bam_off[0..nrec] holds their chained offsets (bam_off[nrec] == n_bytes).  The caller holds append_mu and has checked the phase
+// and the 2^32 read limit.  From here on: ingest filters, fixed fields and RG:Z, segmented copies, QUAL presence, the bam_all arena.
+int bam_ingest_core(elp_ctx* c, uint64_t n_bytes, uint64_t nrec) {
+    uint64_t bn = nrec;                                       // becomes the number of records that pass the filters
     const uint64_t n0 = c->n;
-    if (n0 + bn >= (1ull << 32)) return c->fail(E_LIMIT, "more than 2^32-1 reads in one context");
     cudaStream_t s = c->stream;
-    const uint64_t nrec = bn;                                 // records handed over; bn becomes the number that pass the filters
-    TRY(grow(c, c->bam_raw, n_bytes + 64, 0)); TRY(grow(c, c->bam_off, nrec + 2, 0)); TRY(grow(c, c->bam_start, nrec + 2, 0));
-    CUDA_TRY(c, cudaMemcpyAsync(c->bam_raw.p, records, n_bytes, cudaMemcpyHostToDevice, s));
-    CUDA_TRY(c, cudaMemcpyAsync(c->bam_off.p, record_off, (nrec + 1) * 8, cudaMemcpyHostToDevice, s));
+    TRY(grow(c, c->bam_start, nrec + 2, 0));
     const uint64_t* d_start = c->bam_off.p;                   // without filters: record i is read n0 + i
     if (c->filter_mask || c->filter_min_mapq > 0) {
         TRY(grow(c, c->scan_tmp, nrec + 8, 0)); TRY(grow(c, c->off_stage, nrec + 2, 0));

@@ -22,6 +22,7 @@
 #define E_LIMIT (-15)
 #define E_TILE (-17)
 #define E_BAM (-18)
+#define E_SAM (-20)
 #define E_STATE (-16)
 
 // device-side error word bits (one u32 in global memory, OR-ed by kernels, read by the host after the phase)

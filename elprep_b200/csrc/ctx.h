@@ -108,6 +108,8 @@ struct elp_ctx {
     uint32_t filter_mask = 0; int32_t filter_min_mapq = 0; uint64_t n_filtered = 0;   // elp_set_ingest_filter
     std::vector<int32_t*> d_regions; std::vector<uint64_t> n_regions; const int32_t** d_region_ptrs = nullptr; uint64_t* d_n_regions = nullptr; bool regions_dirty = true;   // target regions (BED) of RemoveNonOverlappingReads
     uint64_t n_cleaned = 0;                  // reads whose CIGAR elp_clean_sam rewrote
+    bool has_contig_names = false;           // elp_config.contig_names was given (elp_append_sam resolves RNAME / RNEXT against it)
+    struct SamState* sam = nullptr;          // device tables and staging of elp_append_sam (sam_ingest.cu)
     uint8_t* d_rg_names = nullptr; uint32_t* d_rg_name_off = nullptr; std::vector<std::string> rg_ids;   // @RG IDs for the RG:Z match
     DBuf<int32_t> lseq_stage;       // staging for l_seq of the batch being appended
     DBuf<uint64_t> off_stage;       // staging for batch-relative offsets
@@ -245,3 +247,5 @@ int spread_exchange_begin(elp_ctx* c);
 int spread_exchange_end(elp_ctx* c);
 int exclusive_scan_u64_from_u32(elp_ctx* c, const uint32_t* in, uint64_t* out, uint64_t n, uint64_t base);   // out[n+1], out[0] = base
 int qual_presence_update(elp_ctx* c, uint64_t first_byte, uint64_t n_bytes);   // api.cu: called by both ingest paths
+int bam_ingest_core(elp_ctx* c, uint64_t n_bytes, uint64_t nrec);   // bam_ingest.cu: records staged in bam_raw / bam_off -> reads (elp_append_bam, elp_append_sam)
+void sam_state_release(elp_ctx* c);   // sam_ingest.cu

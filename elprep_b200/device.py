@@ -147,6 +147,15 @@ class Context:
         off = np.ascontiguousarray(record_off, dtype=np.uint64) if record_off is not None else None
         self._ck(self.L.elp_append_bam(self.h, _vp(rec), rec.size, _vp(off), (off.size - 1) if off is not None else 0))
 
+    def append_sam(self, text):
+        """text: bytes or a uint8 array of SAM alignment lines (no header; the last line may lack its newline)"""
+        if isinstance(text, (bytes, bytearray, memoryview)):
+            buf = bytes(text)
+            self._ck(self.L.elp_append_sam(self.h, buf, len(buf)))
+        else:
+            t = np.ascontiguousarray(text, dtype=np.uint8)
+            self._ck(self.L.elp_append_sam(self.h, C.cast(_vp(t), C.c_char_p), t.size))
+
     @property
     def n(self):
         return int(self.L.elp_n_reads(self.h))

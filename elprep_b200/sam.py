@@ -256,3 +256,64 @@ class AlignmentBatch:
                               qname=np.frombuffer(bytes(qn), dtype=np.uint8), cigar_off=np.array(coff, dtype=np.uint64),
                               cigar=np.array(cg, dtype=np.uint32), seq=np.frombuffer(bytes(sq), dtype=np.uint8),
                               qual=np.frombuffer(bytes(ql), dtype=np.uint8).copy(), **cols)
+
+
+def _is_user_tag(code):
+    """IsHeaderUserTag (sam/sam-types.go:49-56): a record type code with a lower-case letter"""
+    return any("a" <= ch <= "z" for ch in code)
+
+
+def _header_line(line):
+    """parseSamHeaderLine (sam/sam-files.go:38-63): TG:value fields separated by tabs, no repeated TG"""
+    rec, i = {}, 0
+    while i < len(line):
+        j = line.find(":", i)
+        if j < 0 or j - i != 2:
+            raise ValueError(f"invalid field tag {line[i:j if j >= 0 else len(line)]!r}")
+        k = line.find("\t", j + 1)
+        k = len(line) if k < 0 else k
+        tag, value = line[i:j], line[j + 1:k]
+        if tag in rec:
+            raise ValueError(f"duplicate field tag {tag} in a SAM header line")
+        rec[tag] = value
+        i = k + 1
+    return rec
+
+
+def parse_sam_header(buf):
+    """``ParseSamHeader`` (sam/sam-files.go:70-120) over the start of a SAM file -> (Header, n_header_bytes): the alignment lines
+    (for ``Context.append_sam``) start at n_header_bytes.  @HD, @SQ and @RG are kept with all their fields; @PG, @CO and user
+    records are checked and skipped.  ValueError where the reference panics: @HD not on the first line, an unknown record type
+    code, a malformed field."""
+    data = bytes(buf)
+    h = Header()
+    h.HD = {}
+    pos, first = 0, True
+    while pos < len(data) and data[pos:pos + 1] == b"@":
+        nl = data.find(b"\n", pos)
+        end = len(data) if nl < 0 else nl
+        raw = data[pos:end].decode("latin-1")
+        nxt = len(data) if nl < 0 else nl + 1
+        if len(raw) < 4:                                  # (bytes[4:length] panics in the reference)
+            raise ValueError(f"SAM header line too short: {raw!r}")
+        code, line = raw[:4], raw[4:]
+        if code == "@HD\t":
+            if not first:
+                raise ValueError("@HD line not in first line when parsing a SAM header")
+            h.HD = _header_line(line)
+        elif code == "@SQ\t":
+            h.SQ.append(_header_line(line))
+        elif code == "@RG\t":
+            h.RG.append(_header_line(line))
+        elif code == "@PG\t":
+            _header_line(line)
+        elif raw[:3] == "@CO":
+            pass
+        elif _is_user_tag(raw[:3]):
+            if raw[3] != "\t":
+                raise ValueError(f"header code {raw[:3]} not followed by a tab when parsing a SAM header")
+            _header_line(line)
+        else:
+            raise ValueError(f"unknown SAM record type code {raw[:3]}")
+        pos, first = nxt, False
+    return h, pos

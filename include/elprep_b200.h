@@ -37,6 +37,7 @@ extern "C" {
 #define ELP_ETILE (-17)      /* a QNAME tile/x/y field that strconv.ParseInt rejects (filters/mark-optical-duplicates.go:57-64) */
 #define ELP_EBAM (-18)       /* malformed BAM alignment record, or an RG:Z value that is not an @RG ID */
 #define ELP_EBGZF (-19)      /* malformed BGZF block (header, BC subfield, CRC32 or ISIZE), utils/bgzf/bgzf-files.go:95-127 */
+#define ELP_ESAM (-20)       /* malformed SAM alignment line; elp_last_error names the line (0-based, within the call) and the field */
 
 /* sam.SortingOrder (sam/sam-types.go:40-58) */
 #define ELP_SO_KEEP 0
@@ -125,6 +126,17 @@ int elp_append_wait(elp_ctx *ctx);
  * 1-based; the RG:Z tag is matched against elp_config.rg_id (an unknown value is ELP_EBAM, no RG tag is rg = -1).
  * Not supported: the CG:B long-CIGAR convention (ELP_ELIMIT).  Thread-safe like elp_append_batch. */
 int elp_append_bam(elp_ctx *ctx, const uint8_t *records, uint64_t n_bytes, const uint64_t *record_off, uint64_t n_records);
+/* SAM text alignment lines (no header), whole lines only; the last line may lack its '\n'; a '\r' before '\n' is dropped.
+ * Parsed on the device as parseSamAlignment (sam/sam-files.go:386-410) and stored as the record formatBamAlignment
+ * (sam/bam-files.go:635-737) writes for it, then ingested as by elp_append_bam (filters, RG:Z, sr, elp_fetch_bam).
+ * RNAME/RNEXT are resolved against elp_config.contig_names as AddREFID does (filters/simple-filters.go:208-231), so a context
+ * with @SQ lines must have been created with contig_names (else ELP_EINVAL).  Thread-safe like elp_append_bam.
+ * On any error nothing of the call is appended: ELP_ESAM for a line the reference rejects (log.Panic) and for three lines it would
+ * write as a malformed BAM record -- a QNAME longer than 254 bytes, a merged CIGAR operation of 2^28 or more, QUAL and SEQ of
+ * different lengths; ELP_ESAM as well for a hexadecimal float, a tab as the value of an A field and a tag name that contains a tab
+ * (the reference accepts these three); ELP_ELIMIT for a CIGAR of more than 65535 operations (the CG:B convention); ELP_EBAM for an
+ * RG:Z value that is not an @RG ID. */
+int elp_append_sam(elp_ctx *ctx, const char *text, uint64_t n_bytes);
 /* Per-record filters fused into elp_append_bam (SURVEY.md 8f row 4): a record that fails a requested predicate never becomes a read
  * of the context (later calls; elp_n_filtered counts them).  filters/simple-filters.go: RemoveUnmappedReads (:73-75),
  * RemoveUnmappedReadsStrict (:79-83: FLAG 0x4, POS 0 or RNAME *), RemoveNonExactMappingReads (:90-99: only M and S operations),
@@ -249,7 +261,7 @@ uint64_t elp_fetch_qual_bytes(elp_ctx *ctx, uint64_t first, uint64_t n);
 int elp_fetch_async(elp_ctx *ctx, uint64_t first, uint64_t n, uint32_t *record_index32, uint16_t *flag, uint64_t *qual_off, uint8_t *qual, uint64_t qual_capacity);
 int elp_fetch_wait(elp_ctx *ctx);
 /* per-read temps of adaptAlignment (filters/mark-duplicates.go:153-156), arrival order; for parity tests */
-/* The same as BAM alignment records (only if every read came in through elp_append_bam): output records [first, first+n) are
+/* The same as BAM alignment records (only if every read came in through elp_append_bam or elp_append_sam): output records [first, first+n) are
  * the stored records with FLAG and -- once elp_bqsr_apply has run -- QUAL replaced; names, CIGAR and optional fields are the
  * input bytes.  This stands in for formatting every *sam.Alignment again (sam/bam-files.go:635-735); the caller BGZF-
  * compresses the result.  record_off[n+1] may be NULL. */
