@@ -209,7 +209,7 @@ void elp_destroy(elp_ctx* c) {
     c->refid.release(); c->pos.release(); c->nref.release(); c->pnext.release(); c->tlen.release(); c->rg.release(); c->flag.release(); c->mapq.release(); c->optf.release(); c->s_optf.release();
     c->qname_off.release(); c->cigar_off.release(); c->qual_off.release(); c->seq_off.release(); c->qname.release(); c->seq.release(); c->qual.release(); c->cigar.release();
     c->bam_raw.release(); c->bam_off.release(); c->bam_all.release(); c->bam_all_off.release(); c->bam_start.release(); c->lseq_stage.release(); c->off_stage.release(); c->upos.release(); c->score.release(); c->qhash.release(); c->keys_a.release(); c->keys_b.release();
-    c->bq_recs.release(); c->bq_segs.release(); c->vals_a.release(); c->vals_b.release(); c->mate.release(); c->pair_a.release(); c->pair_b.release(); c->scan_tmp.release(); c->scan_blk.release(); c->bytes_tmp.release();
+    c->bq_recs.release(); c->bq_segs.release(); c->vals_a.release(); c->vals_b.release(); c->mate.release(); c->pair_a.release(); c->pair_b.release(); c->pair_score.release(); c->tie_bits.release(); c->scan_tmp.release(); c->scan_blk.release(); c->bytes_tmp.release();
     c->perm.release(); c->s_refid.release(); c->s_pos.release(); c->s_nref.release(); c->s_pnext.release(); c->s_tlen.release(); c->s_rg.release(); c->s_lseq.release();
     c->s_flag.release(); c->s_mapq.release(); c->s_qual_off.release(); c->s_seq_off.release(); c->s_cigar_off.release(); c->s_out_off.release(); c->s_ncigar.release(); c->qual_out.release();
     for (auto& pe : c->pending) { cudaEventDestroy(pe.a); cudaEventDestroy(pe.b); }

@@ -78,36 +78,11 @@ __global__ void __launch_bounds__(128) tie_short_kernel(uint64_t n, const uint64
     }
 }
 
-// flag[j] = 1 if j belongs to a run longer than SHORT_RUN (checked against the element SHORT_RUN places away on either side)
-__global__ void __launch_bounds__(256) tie_long_flag_kernel(uint64_t n, const uint64_t* __restrict__ keys, uint32_t* __restrict__ long_flag) {
-    const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= n) return;
-    const uint64_t k0 = keys[j];
-    // run length > SHORT_RUN  <=>  some window of SHORT_RUN+1 consecutive equal keys covers j
-    uint64_t lo = j, hi = j;
-    while (lo > 0 && j - lo < (uint64_t)SHORT_RUN && keys[lo - 1] == k0) lo--;
-    while (hi + 1 < n && hi - lo < (uint64_t)SHORT_RUN && keys[hi + 1] == k0) hi++;
-    long_flag[j] = (hi - lo >= (uint64_t)SHORT_RUN) ? 1u : 0u;
-}
-
-__global__ void __launch_bounds__(256) compact_long_kernel(uint64_t n, const uint32_t* __restrict__ long_flag, const uint64_t* __restrict__ slot,
-                                                            const uint32_t* __restrict__ vals, uint32_t* __restrict__ pos_list, uint32_t* __restrict__ elem) {
-    const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= n || !long_flag[j]) return;
-    const uint64_t s = slot[j];
-    pos_list[s] = (uint32_t)j; elem[s] = vals[j];
-}
-
 // chunk key of the composite secondary key; chunk ids (least significant first):
 //   0: TLEN   1: NextREFID|PNEXT (0 unless paired)   2: modFlag|MAPQ   3+k: QNAME bytes [8*(nq-1-k), +8) big-endian, zero padded
 //   last: the primary coordinate key itself (keeps the runs apart and in place)
-__global__ void __launch_bounds__(256) chunk_keys_kernel(uint64_t m, const uint32_t* __restrict__ elem, int chunk, int nq, TieCols c,
-                                                          const uint64_t* __restrict__ prim_keys, const uint32_t* __restrict__ pos_list_unused,
-                                                          const int32_t* __restrict__ refid, const int32_t* __restrict__ pos, CoordLayout L,
-                                                          uint64_t* __restrict__ keys, uint32_t* __restrict__ vals) {
-    const uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (k >= m) return;
-    const uint32_t a = elem[k];
+__device__ __forceinline__ uint64_t chunk_key(uint32_t a, int chunk, int nq, const TieCols& c, const int32_t* __restrict__ refid, const int32_t* __restrict__ pos,
+                                              const CoordLayout& L) {
     uint64_t key;
     if (chunk == 0) key = (uint64_t)((uint32_t)c.tlen[a] ^ 0x80000000u);
     else if (chunk == 1) key = (c.flag[a] & F_MULTIPLE) ? (((uint64_t)((uint32_t)c.nref[a] ^ 0x80000000u) << 32) | (uint64_t)((uint32_t)c.pnext[a] ^ 0x80000000u)) : 0ull;
@@ -133,7 +108,58 @@ __global__ void __launch_bounds__(256) chunk_keys_kernel(uint64_t m, const uint3
         const uint64_t rr = (r < 0 || r >= L.n_contigs) ? (uint64_t)L.n_contigs : (uint64_t)r;
         key = ((c.flag[a] & F_REVERSED) ? 1ull : 0ull) | ((uint64_t)(uint32_t)pos[a] << 1) | (rr << (1 + L.bP));
     }
-    keys[k] = key; vals[k] = a;
+    return key;
+}
+
+__global__ void __launch_bounds__(256) chunk_keys_kernel(uint64_t m, const uint32_t* __restrict__ elem, int chunk, int nq, TieCols c,
+                                                          const int32_t* __restrict__ refid, const int32_t* __restrict__ pos, CoordLayout L,
+                                                          uint64_t* __restrict__ keys, uint32_t* __restrict__ vals) {
+    const uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= m) return;
+    const uint32_t a = elem[k];
+    keys[k] = chunk_key(a, chunk, nq, c, refid, pos, L); vals[k] = a;
+}
+
+// flag[j] = 1 if j belongs to a run longer than SHORT_RUN (checked against the element SHORT_RUN places away on either side).
+// Over the elements of all long runs, bits[ch] accumulates the OR and bits[n_chunks + ch] the AND of chunk key ch: a bit
+// where the two differ is the only kind that can reorder anything in the tie rounds.
+__global__ void __launch_bounds__(256) tie_long_flag_kernel(uint64_t n, const uint64_t* __restrict__ keys, const uint32_t* __restrict__ vals, uint32_t* __restrict__ long_flag,
+                                                             int n_chunks, int nq, TieCols c, const int32_t* __restrict__ refid, const int32_t* __restrict__ pos,
+                                                             CoordLayout L, unsigned long long* __restrict__ bits) {
+    extern __shared__ unsigned long long s_bits[];   // [n_chunks] OR, [n_chunks] AND
+    unsigned long long *s_or = s_bits, *s_and = s_bits + n_chunks;
+    const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    bool lng = false;
+    if (j < n) {
+        const uint64_t k0 = keys[j];
+        // run length > SHORT_RUN  <=>  some window of SHORT_RUN+1 consecutive equal keys covers j
+        uint64_t lo = j, hi = j;
+        while (lo > 0 && j - lo < (uint64_t)SHORT_RUN && keys[lo - 1] == k0) lo--;
+        while (hi + 1 < n && hi - lo < (uint64_t)SHORT_RUN && keys[hi + 1] == k0) hi++;
+        lng = hi - lo >= (uint64_t)SHORT_RUN;
+        long_flag[j] = lng ? 1u : 0u;
+    }
+    if (!__syncthreads_or(lng)) return;
+    for (int ch = threadIdx.x; ch < n_chunks; ch += blockDim.x) { s_or[ch] = 0; s_and[ch] = ~0ull; }
+    __syncthreads();
+    const uint32_t a = lng ? vals[j] : 0u;
+    const unsigned lane = threadIdx.x & 31;
+    for (int ch = 0; ch < n_chunks; ch++) {
+        const uint64_t k = lng ? chunk_key(a, ch, nq, c, refid, pos, L) : 0ull;
+        uint64_t o = k, an = lng ? k : ~0ull;
+        for (int d = 16; d; d >>= 1) { o |= __shfl_xor_sync(FULL_MASK, o, d); an &= __shfl_xor_sync(FULL_MASK, an, d); }
+        if (lane == 0) { atomicOr(&s_or[ch], (unsigned long long)o); atomicAnd(&s_and[ch], (unsigned long long)an); }
+    }
+    __syncthreads();
+    for (int ch = threadIdx.x; ch < n_chunks; ch += blockDim.x) { atomicOr(bits + ch, s_or[ch]); atomicAnd(bits + n_chunks + ch, s_and[ch]); }
+}
+
+__global__ void __launch_bounds__(256) compact_long_kernel(uint64_t n, const uint32_t* __restrict__ long_flag, const uint64_t* __restrict__ slot,
+                                                            const uint32_t* __restrict__ vals, uint32_t* __restrict__ pos_list, uint32_t* __restrict__ elem) {
+    const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= n || !long_flag[j]) return;
+    const uint64_t s = slot[j];
+    pos_list[s] = (uint32_t)j; elem[s] = vals[j];
 }
 
 __global__ void __launch_bounds__(256) scatter_long_kernel(uint64_t m, const uint32_t* __restrict__ pos_list, const uint32_t* __restrict__ sorted_elem, uint32_t* __restrict__ vals) {
@@ -210,16 +236,24 @@ int phase_coordinate_sort(elp_ctx* c, int order) {   // 0 keep, 1 coordinate, 2 
         uint64_t* keys_free = in_b ? c->keys_a.p : c->keys_b.p;
 
         TieCols tc{c->flag.p, c->mapq.p, c->nref.p, c->pnext.p, c->tlen.p, c->qname_off.p, c->qname.p};
+        const int nq = std::max(1, (int)((c->h_ranges.qname_max + 7) / 8));   // longest QNAME, from the adapt kernel's range reduction
+        const int n_chunks = 3 + nq + 1;
         // long runs first (flags computed from the keys only), then short runs in place
         CUDA_TRY(c, c->scan_tmp.reserve(n + 4, c->stream));
+        CUDA_TRY(c, c->tie_bits.reserve(2 * n_chunks, c->stream));
+        CUDA_TRY(c, cudaMemsetAsync(c->tie_bits.p, 0, n_chunks * 8, c->stream));
+        CUDA_TRY(c, cudaMemsetAsync(c->tie_bits.p + n_chunks, 0xff, n_chunks * 8, c->stream));
         c->begin("tie_long_flag", (double)n * 12);
-        tie_long_flag_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(n, keys, c->scan_tmp.p);
+        tie_long_flag_kernel<<<nblk(n, 256), 256, 2 * n_chunks * 8, c->stream>>>(n, keys, vals, c->scan_tmp.p, n_chunks, nq, tc, c->refid.p, c->pos.p, L,
+                                                                  reinterpret_cast<unsigned long long*>(c->tie_bits.p));
         c->end(); LAUNCH_CHECK(c);
         uint64_t* slot = keys_free;   // n+1 u64
         rc = exclusive_scan_u32_to_u64(c, c->scan_tmp.p, slot, n);
         if (rc) return rc;
         uint64_t m = 0;
+        std::vector<uint64_t> tie_bits(2 * n_chunks);
         CUDA_TRY(c, cudaMemcpyAsync(&m, slot + n, 8, cudaMemcpyDeviceToHost, c->stream));
+        CUDA_TRY(c, cudaMemcpyAsync(tie_bits.data(), c->tie_bits.p, tie_bits.size() * 8, cudaMemcpyDeviceToHost, c->stream));
         CUDA_TRY(c, cudaStreamSynchronize(c->stream));
         c->begin("tie_short", (double)n * 12);
         tie_short_kernel<<<nblk(n, 128), 128, 0, c->stream>>>(n, keys, vals, tc, nullptr, nullptr);
@@ -231,22 +265,22 @@ int phase_coordinate_sort(elp_ctx* c, int order) {   // 0 keep, 1 coordinate, 2 
             c->begin("tie_compact", (double)n * 16);
             compact_long_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(n, c->scan_tmp.p, slot, vals, pos_list, elem);
             c->end(); LAUNCH_CHECK(c);
-            int nq;
-            nq = (int)((c->h_ranges.qname_max + 7) / 8);   // longest QNAME, from the adapt kernel's range reduction
-            if (nq < 1) nq = 1;
             CUDA_TRY(c, c->bytes_tmp.reserve((size_t)m * 16 + 64, c->stream));
             uint64_t* ka = reinterpret_cast<uint64_t*>(c->bytes_tmp.p);
             uint64_t* kb = ka + m;
             CUDA_TRY(c, c->mate.reserve(2 * m + 16, c->stream));
             uint32_t* va = c->mate.p; uint32_t* vb = c->mate.p + ((m + 3) & ~(uint64_t)3);   // 16-byte aligned: the sort stages payloads with 16-byte async copies
-            const int n_chunks = 3 + nq + 1;
             for (int ch = 0; ch < n_chunks; ch++) {
+                // a chunk whose bits are equal on every long-run element cannot reorder anything: skip it; sort the others only over
+                // the range from their lowest to their highest differing bit
+                const uint64_t diff = tie_bits[ch] ^ tie_bits[n_chunks + ch];
+                if (diff == 0) continue;
+                const int lo_bit = __builtin_ctzll(diff), hi_bit = 63 - __builtin_clzll(diff);
                 c->begin("tie_chunk_keys", (double)m * 32);
-                chunk_keys_kernel<<<nblk(m, 256), 256, 0, c->stream>>>(m, elem, ch, nq, tc, keys, pos_list, c->refid.p, c->pos.p, L, ka, va);
+                chunk_keys_kernel<<<nblk(m, 256), 256, 0, c->stream>>>(m, elem, ch, nq, tc, c->refid.p, c->pos.p, L, ka, va);
                 c->end(); LAUNCH_CHECK(c);
                 bool b2 = false;
-                int kb_bits = (ch == 0) ? 32 : (ch == 2 ? 24 : (ch == n_chunks - 1 ? L.key_bits : 64));
-                rc = radix_sort_u64(c, ka, kb, va, vb, m, kb_bits, &b2, "u64");
+                rc = radix_sort_u64(c, ka, kb, va, vb, m, hi_bit - lo_bit + 1, &b2, "u64", lo_bit);
                 if (rc) return rc;
                 CUDA_TRY(c, cudaMemcpyAsync(elem, b2 ? vb : va, m * 4, cudaMemcpyDeviceToDevice, c->stream));
             }
@@ -268,7 +302,7 @@ int phase_coordinate_sort(elp_ctx* c, int order) {   // 0 keep, 1 coordinate, 2 
         const uint32_t* elem = c->vals_a.p;
         for (int ch = 0; ch < nq; ch++) {
             c->begin("qname_chunk_keys", (double)n * 32);
-            chunk_keys_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(n, elem, 3 + ch, nq, tc, nullptr, nullptr, c->refid.p, c->pos.p, L, c->keys_a.p, c->vals_a.p);
+            chunk_keys_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(n, elem, 3 + ch, nq, tc, c->refid.p, c->pos.p, L, c->keys_a.p, c->vals_a.p);
             c->end(); LAUNCH_CHECK(c);
             bool b2 = false;
             rc = radix_sort_u64(c, c->keys_a.p, c->keys_b.p, c->vals_a.p, c->vals_b.p, n, 64, &b2, "u64");

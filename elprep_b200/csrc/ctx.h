@@ -128,6 +128,8 @@ struct elp_ctx {
     rs::Workspace ws;
     DBuf<uint32_t> mate;                      // [n] mate index or 0xffffffff
     DBuf<uint32_t> pair_a, pair_b, scan_tmp, scan_blk;
+    DBuf<int32_t> pair_score;                 // [npairs] summed phred score of both mates of a pair (duplicate marking)
+    DBuf<uint64_t> tie_bits;                  // [2][chunks] OR and AND of each chunk key over the long tie runs (coordinate sort)
     DBuf<uint8_t> bytes_tmp;
     DBuf<uint4> bq_recs, bq_segs;             // BQSR count kernel: work records of the eligible reads, segment table
     uint32_t* d_bq_small = nullptr;           // class histogram, region bases, list counters, segment counts, work-queue heads
@@ -225,13 +227,14 @@ struct elp_ctx {
 #define LAUNCH_CHECK(ctx) CUDA_TRY(ctx, cudaGetLastError())
 
 // ---- internal phase entry points (implemented in the .cu files) ----
-int radix_sort_u64(elp_ctx* c, uint64_t* keys_a, uint64_t* keys_b, uint32_t* vals_a, uint32_t* vals_b, uint64_t n, int key_bits, bool* result_in_b, const char* tag);
-int radix_sort_u128(elp_ctx* c, uint64_t* keys_a, uint64_t* keys_b, uint32_t* vals_a, uint32_t* vals_b, uint64_t n, int key_bits, bool* result_in_b, const char* tag);
+// stable sort by key bits [lo_bit, lo_bit + key_bits); the bits below lo_bit do not take part in the order
+int radix_sort_u64(elp_ctx* c, uint64_t* keys_a, uint64_t* keys_b, uint32_t* vals_a, uint32_t* vals_b, uint64_t n, int key_bits, bool* result_in_b, const char* tag, int lo_bit = 0);
+int radix_sort_u128(elp_ctx* c, uint64_t* keys_a, uint64_t* keys_b, uint32_t* vals_a, uint32_t* vals_b, uint64_t n, int key_bits, bool* result_in_b, const char* tag, int lo_bit = 0);
 int exclusive_scan_u32_to_u64(elp_ctx* c, const uint32_t* in, uint64_t* out, uint64_t n);   // out[n+1]
 int exclusive_scan_u64(elp_ctx* c, const uint64_t* in, uint64_t* out, uint64_t n, uint64_t base);          // out[n+1], out[0]=base
 int phase_adapt(elp_ctx* c);
 int phase_markdup(elp_ctx* c, bool optical);
-int phase_optical(elp_ctx* c, uint64_t npairs, const uint64_t* sorted_keys, const uint32_t* sorted_vals, int bS);
+int phase_optical(elp_ctx* c, uint64_t npairs, const uint64_t* sorted_keys, const uint32_t* sorted_vals, int key_words);   // key_words: 1 (u64 keys) or 2 (u128 as lo,hi)
 int phase_coordinate_sort(elp_ctx* c, int order);   // 0 keep, 1 coordinate, 2 queryname
 int phase_bqsr_gather(elp_ctx* c);
 int phase_bqsr_finalize(elp_ctx* c, const char* report_path);

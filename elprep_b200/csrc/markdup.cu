@@ -4,11 +4,11 @@
 // same equivalence classes are formed by sorting exact packed keys (no hashing of group keys, so no collisions):
 //   adapt_kernel        adaptAlignment (:153-156): unclipped 5' position (:79-110) + clamped phred sum (:36-68),
 //                       plus a 39-bit (library, QNAME) hash for the mate join and the value ranges that size the keys
-//   fragment groups     key (lib, refid, unclipped pos, strand | pair-read-first, score desc) -> radix sort ->
+//   fragment groups     key (lib, refid, unclipped pos, strand | is_frag, score desc) -> radix sort of the group bits only ->
 //                       frag_mark_kernel: one thread per group head walks its run (classifyFragment :210-254)
 //   mate join           sort by the (lib,QNAME) hash, verify on bytes, pair up in arrival order
 //                       (DeleteOrStore on pairFragment :336)
-//   pair groups         128-bit key (lib, refid1, refid2, upos1, upos2, rev1, rev2 | score desc) -> radix sort ->
+//   pair groups         key (lib, refid1, refid2, rev1, rev2, upos1, upos2), 64 bits when it fits, else 128 -> radix sort ->
 //                       pair_mark_kernel (classifyPair :329-396): both mates of every loser get 0x400
 // Results are deterministic; where the reference depends on goroutine scheduling (equal score AND equal QNAME) the
 // outcome equals a single goroutine processing reads in arrival order (the later read/pair survives, :231-238,380-386).
@@ -250,29 +250,34 @@ __global__ void __launch_bounds__(256) frag_keys_kernel(uint64_t n, const uint16
     keys[i] = key; vals[i] = (uint32_t)i;
 }
 
+// keys sorted by the group bits (>= bS + 1) only, so a group is in arrival order; score and is_frag are read from the low key bits
 __global__ void __launch_bounds__(256) frag_mark_kernel(uint64_t m, const uint64_t* __restrict__ keys, const uint32_t* __restrict__ vals, int bS,
                                                          const uint64_t* __restrict__ qname_off, const uint8_t* __restrict__ qname, uint16_t* __restrict__ flag) {
     const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= m) return;
     const uint64_t k0 = keys[j], g = k0 >> (bS + 1);
     if (j > 0 && (keys[j - 1] >> (bS + 1)) == g) return;   // not a group head
-    const bool head_is_pair = ((k0 >> bS) & 1) == 0;
-    if (head_is_pair) {
-        // a true-pair read in the group: every true fragment is a duplicate, pair reads are untouched (:225-227,245-252)
-        for (uint64_t t = j + 1; t < m; t++) { const uint64_t k = keys[t]; if ((k >> (bS + 1)) != g) break; if ((k >> bS) & 1) atomic_or_u16(flag, vals[t], F_DUPLICATE); }
-        return;
+    if (j + 1 == m || (keys[j + 1] >> (bS + 1)) != g) return;   // a read alone in its group is never a duplicate
+    const uint64_t smask = (1ull << bS) - 1;
+    // winner among fragments = max score (smallest score_max - score), then smallest QNAME (:228-243); full ties: the later arrival survives
+    bool has_pair = false;
+    uint64_t e = j, win = j;
+    uint64_t best = ~0ull;
+    for (; e < m; e++) {
+        const uint64_t k = keys[e];
+        if ((k >> (bS + 1)) != g) break;
+        if (((k >> bS) & 1) == 0) { has_pair = true; continue; }
+        if (has_pair) continue;
+        const uint64_t sc = k & smask;
+        if (sc < best) { best = sc; win = e; }
+        else if (sc == best) {
+            const uint32_t a = vals[e], b = vals[win];
+            if (qname_compare(qname, qname_off[a], qname_off[a + 1], qname_off[b], qname_off[b + 1]) <= 0) win = e;
+        }
     }
-    // only fragments: best score first. Winner = max score, then smallest QNAME (:228-243); full ties: the later arrival survives
-    uint64_t t1 = j + 1;
-    uint64_t win = j;
-    while (t1 < m && keys[t1] == k0) {
-        const uint32_t a = vals[t1], b = vals[win];
-        if (qname_compare(qname, qname_off[a], qname_off[a + 1], qname_off[b], qname_off[b + 1]) <= 0) win = t1;
-        t1++;
-    }
-    for (uint64_t t = j; t < m; t++) {
-        if (t >= t1 && (keys[t] >> (bS + 1)) != g) break;
-        if (t != win) atomic_or_u16(flag, vals[t], F_DUPLICATE);
+    // a true-pair read in the group: every true fragment is a duplicate, pair reads are untouched (:225-227,245-252)
+    for (uint64_t t = j; t < e; t++) {
+        if (has_pair ? ((keys[t] >> bS) & 1) != 0 : t != win) atomic_or_u16(flag, vals[t], F_DUPLICATE);
     }
 }
 
@@ -288,6 +293,8 @@ __global__ void __launch_bounds__(256) join_keys_kernel(uint64_t n, const uint16
     mate[i] = NONE;
 }
 
+__device__ __forceinline__ int32_t lib_of(const int32_t* rg, const int32_t* rg_lib, int n_rg, uint32_t i) { const int32_t g = rg[i]; return (g >= 0 && g < n_rg) ? rg_lib[g] : -1; }
+
 __global__ void __launch_bounds__(256) join_kernel(uint64_t m, const uint64_t* __restrict__ keys, const uint32_t* __restrict__ vals,
                                                     const int32_t* __restrict__ rg, const int32_t* __restrict__ rg_lib, int n_rg,
                                                     const uint64_t* __restrict__ qname_off, const uint8_t* __restrict__ qname, uint32_t* __restrict__ mate) {
@@ -297,16 +304,23 @@ __global__ void __launch_bounds__(256) join_kernel(uint64_t m, const uint64_t* _
     if (j > 0 && keys[j - 1] == k0) return;
     uint64_t e = j + 1;
     while (e < m && keys[e] == k0) e++;
+    if (e - j == 2) {   // the common case: both reads still unpaired (join_keys_kernel), all loads issued before any compare
+        const uint32_t va = vals[j], vb = vals[j + 1];
+        const int32_t ga = rg[va], gb = rg[vb];
+        const uint64_t a0 = qname_off[va], a1 = qname_off[va + 1], b0 = qname_off[vb], b1 = qname_off[vb + 1];
+        const int32_t la = (ga >= 0 && ga < n_rg) ? rg_lib[ga] : -1, lb = (gb >= 0 && gb < n_rg) ? rg_lib[gb] : -1;
+        if (la == lb && qname_compare(qname, a0, a1, b0, b1) == 0) { mate[va] = vb; mate[vb] = va; }
+        return;
+    }
     // arrival order inside the run (stable sort): first unmatched same-(lib,QNAME) read stores, the next one deletes and pairs (:336)
     for (uint64_t a = j; a < e; a++) {
         const uint32_t va = vals[a];
-        if (mate[va] != NONE) continue;
-        const int32_t ga = rg[va]; const int32_t la = (ga >= 0 && ga < n_rg) ? rg_lib[ga] : -1;
+        if (a > j && mate[va] != NONE) continue;   // the run's first read is still unpaired
+        const int32_t la = lib_of(rg, rg_lib, n_rg, va);
         for (uint64_t b = a + 1; b < e; b++) {
             const uint32_t vb = vals[b];
             if (mate[vb] != NONE) continue;
-            const int32_t gb = rg[vb]; const int32_t lb = (gb >= 0 && gb < n_rg) ? rg_lib[gb] : -1;
-            if (la != lb) continue;
+            if (la != lib_of(rg, rg_lib, n_rg, vb)) continue;
             if (qname_compare(qname, qname_off[va], qname_off[va + 1], qname_off[vb], qname_off[vb + 1]) != 0) continue;
             mate[va] = vb; mate[vb] = va;
             break;
@@ -321,7 +335,7 @@ __global__ void __launch_bounds__(256) pair_flag_kernel(uint64_t n, const uint32
     flags[i] = (m != NONE && m < i) ? 1u : 0u;   // the later mate triggers classifyPair
 }
 
-struct PairLayout { int bS, bU, bR, bL; int32_t upos_min, score_max; int key_bits; };
+struct PairLayout { int bU, bR, bL; int32_t upos_min; int key_bits; };
 
 __device__ __forceinline__ void put128(uint64_t& lo, uint64_t& hi, int& sh, uint64_t v, int bits) {
     if (bits == 0) return;
@@ -333,8 +347,8 @@ __device__ __forceinline__ void put128(uint64_t& lo, uint64_t& hi, int& sh, uint
 __global__ void __launch_bounds__(256) pair_keys_kernel(uint64_t n, const uint32_t* __restrict__ mate, const uint64_t* __restrict__ slot,
                                                          const uint16_t* __restrict__ flag, const int32_t* __restrict__ refid, const int32_t* __restrict__ rg,
                                                          const int32_t* __restrict__ rg_lib, int n_rg, const int32_t* __restrict__ upos, const int32_t* __restrict__ score,
-                                                         PairLayout L, uint64_t* __restrict__ keys /*lo,hi interleaved*/, uint32_t* __restrict__ vals,
-                                                         uint32_t* __restrict__ pair_a, uint32_t* __restrict__ pair_b) {
+                                                         PairLayout L, uint64_t* __restrict__ keys /*u64, or u128 as lo,hi*/, uint32_t* __restrict__ vals,
+                                                         uint32_t* __restrict__ pair_a, uint32_t* __restrict__ pair_b, int32_t* __restrict__ pair_score) {
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const uint32_t m = mate[i];
@@ -350,41 +364,42 @@ __global__ void __launch_bounds__(256) pair_keys_kernel(uint64_t n, const uint32
     const int32_t g = rg[a1];
     const uint64_t lib = (uint64_t)(((g >= 0 && g < n_rg) ? rg_lib[g] : -1) + 1);
     uint64_t lo = 0, hi = 0; int sh = 0;
-    put128(lo, hi, sh, (uint64_t)(uint32_t)(L.score_max - (score[a1] + score[a2])), L.bS);
     put128(lo, hi, sh, (uint64_t)(uint32_t)(p2 - L.upos_min), L.bU);
     put128(lo, hi, sh, (uint64_t)(uint32_t)(p1 - L.upos_min), L.bU);
     put128(lo, hi, sh, v2, 1); put128(lo, hi, sh, v1, 1);
     put128(lo, hi, sh, (uint64_t)(uint32_t)(r2 + 1), L.bR); put128(lo, hi, sh, (uint64_t)(uint32_t)(r1 + 1), L.bR);
     put128(lo, hi, sh, lib, L.bL);
-    keys[2 * p] = lo; keys[2 * p + 1] = hi; vals[p] = (uint32_t)p;
-    pair_a[p] = a1; pair_b[p] = a2;
+    if (L.key_bits <= 64) keys[p] = lo;
+    else { keys[2 * p] = lo; keys[2 * p + 1] = hi; }
+    vals[p] = (uint32_t)p;
+    pair_a[p] = a1; pair_b[p] = a2; pair_score[p] = score[a1] + score[a2];
 }
 
-__device__ __forceinline__ void shr128(uint64_t lo, uint64_t hi, int s, uint64_t& olo, uint64_t& ohi) {
-    if (s == 0) { olo = lo; ohi = hi; }
-    else if (s < 64) { olo = (lo >> s) | (hi << (64 - s)); ohi = hi >> s; }
-    else { olo = hi >> (s - 64); ohi = 0; }
+__device__ __forceinline__ bool same_key(const uint64_t* keys, uint64_t a, uint64_t b, int words) {
+    return words == 1 ? keys[a] == keys[b] : (keys[2 * a] == keys[2 * b] && keys[2 * a + 1] == keys[2 * b + 1]);
 }
 
-__global__ void __launch_bounds__(256) pair_mark_kernel(uint64_t m, const uint64_t* __restrict__ keys, const uint32_t* __restrict__ vals, int bS,
-                                                         const uint32_t* __restrict__ pair_a, const uint32_t* __restrict__ pair_b,
+// keys sorted by the signature only, so a group is in pair arrival order
+__global__ void __launch_bounds__(256) pair_mark_kernel(uint64_t m, const uint64_t* __restrict__ keys, const uint32_t* __restrict__ vals, int words,
+                                                         const uint32_t* __restrict__ pair_a, const uint32_t* __restrict__ pair_b, const int32_t* __restrict__ pair_score,
                                                          const uint64_t* __restrict__ qname_off, const uint8_t* __restrict__ qname, uint16_t* __restrict__ flag) {
     const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= m) return;
-    const uint64_t klo = keys[2 * j], khi = keys[2 * j + 1];
-    uint64_t glo, ghi; shr128(klo, khi, bS, glo, ghi);
-    if (j > 0) { uint64_t a, b; shr128(keys[2 * j - 2], keys[2 * j - 1], bS, a, b); if (a == glo && b == ghi) return; }
-    // group head = best score. Winner = max score, then smallest aln1.QNAME (:375-395); full ties: the later pair survives
-    uint64_t t1 = j + 1, win = j;
-    while (t1 < m && keys[2 * t1] == klo && keys[2 * t1 + 1] == khi) {
-        const uint32_t a = pair_a[vals[t1]], b = pair_a[vals[win]];
-        if (qname_compare(qname, qname_off[a], qname_off[a + 1], qname_off[b], qname_off[b + 1]) <= 0) win = t1;
-        t1++;
+    if (j > 0 && same_key(keys, j - 1, j, words)) return;   // not a group head
+    if (j + 1 == m || !same_key(keys, j, j + 1, words)) return;   // a single pair (most groups): no score needed
+    // winner = max score, then smallest aln1.QNAME (:375-395); full ties: the later pair survives
+    uint64_t e = j + 1, win = j;
+    int32_t best = pair_score[vals[j]];
+    for (; e < m && same_key(keys, j, e, words); e++) {
+        const int32_t sc = pair_score[vals[e]];
+        if (sc > best) { best = sc; win = e; }
+        else if (sc == best) {
+            const uint32_t a = pair_a[vals[e]], b = pair_a[vals[win]];
+            if (qname_compare(qname, qname_off[a], qname_off[a + 1], qname_off[b], qname_off[b + 1]) <= 0) win = e;
+        }
     }
-    for (uint64_t t = j; t < m; t++) {
-        if (t >= t1) { uint64_t a, b; shr128(keys[2 * t], keys[2 * t + 1], bS, a, b); if (a != glo || b != ghi) break; }
+    for (uint64_t t = j; t < e; t++)
         if (t != win) { const uint32_t p = vals[t]; atomic_or_u16(flag, pair_a[p], F_DUPLICATE); atomic_or_u16(flag, pair_b[p], F_DUPLICATE); }
-    }
 }
 
 inline unsigned nblk(uint64_t n, int t) { return (unsigned)((n + t - 1) / t); }
@@ -478,24 +493,29 @@ static int mark_pairs(elp_ctx* c, bool optical, uint64_t nt, uint64_t n_true_pai
     CUDA_TRY(c, cudaMemcpyAsync(&npairs, slot + nt, 8, cudaMemcpyDeviceToHost, c->stream));
     CUDA_TRY(c, cudaStreamSynchronize(c->stream));
     if (npairs >= (optical ? 1u : 2u)) {
-        CUDA_TRY(c, c->pair_a.reserve(npairs + 4, c->stream)); CUDA_TRY(c, c->pair_b.reserve(npairs + 4, c->stream));
-        PairLayout L{}; L.bS = bits_for((uint64_t)R.score_max * 2); L.bU = bU; L.bR = bR; L.bL = bL; L.upos_min = R.upos_min; L.score_max = R.score_max * 2;
-        L.key_bits = L.bS + 2 * L.bU + 2 + 2 * L.bR + L.bL;
+        CUDA_TRY(c, c->pair_a.reserve(npairs + 4, c->stream)); CUDA_TRY(c, c->pair_b.reserve(npairs + 4, c->stream)); CUDA_TRY(c, c->pair_score.reserve(npairs + 4, c->stream));
+        // the signature without the score; bU comes from the allreduced ranges, so every rank picks the same key width
+        PairLayout L{}; L.bU = bU; L.bR = bR; L.bL = bL; L.upos_min = R.upos_min;
+        L.key_bits = 2 * L.bU + 2 + 2 * L.bR + L.bL;
         if (L.key_bits > 128) return c->fail(E_LIMIT, "pair signature needs %d bits (>128)", L.key_bits);
-        // 128-bit keys live in keys_a as (lo,hi) pairs; slot[] occupies keys_b, so sort into a separate buffer
-        CUDA_TRY(c, c->bytes_tmp.reserve((size_t)npairs * 16 + 64, c->stream));
+        const int words = L.key_bits <= 64 ? 1 : 2;
+        // keys live in keys_a (u128 as (lo,hi) pairs); slot[] occupies keys_b, so sort into a separate buffer
+        CUDA_TRY(c, c->bytes_tmp.reserve((size_t)npairs * 8 * words + 64, c->stream));
         uint64_t* kb2 = reinterpret_cast<uint64_t*>(c->bytes_tmp.p);
-        c->begin("pair_keys", (double)nt * 12 + (double)npairs * (2 * 18 + 16 + 12));
+        c->begin("pair_keys", (double)nt * 12 + (double)npairs * (2 * 18 + 8 * words + 16));
         pair_keys_kernel<<<nblk(nt, 256), 256, 0, c->stream>>>(nt, c->mate.p, slot, c->flag.p, c->refid.p, c->rg.p, c->d_rg_lib, c->n_rg, c->upos.p, c->score.p, L,
-                                                              c->keys_a.p, c->vals_a.p, c->pair_a.p, c->pair_b.p);
+                                                              c->keys_a.p, c->vals_a.p, c->pair_a.p, c->pair_b.p, c->pair_score.p);
         c->end(); LAUNCH_CHECK(c);
-        rc = radix_sort_u128(c, c->keys_a.p, kb2, c->vals_a.p, c->vals_b.p, npairs, L.key_bits, &in_b, "u128");
+        rc = words == 1 ? radix_sort_u64(c, c->keys_a.p, kb2, c->vals_a.p, c->vals_b.p, npairs, L.key_bits, &in_b, "u64")
+                        : radix_sort_u128(c, c->keys_a.p, kb2, c->vals_a.p, c->vals_b.p, npairs, L.key_bits, &in_b, "u128");
         if (rc) return rc;
-        c->begin("pair_mark", (double)npairs * 20);
-        pair_mark_kernel<<<nblk(npairs, 256), 256, 0, c->stream>>>(npairs, in_b ? kb2 : c->keys_a.p, in_b ? c->vals_b.p : c->vals_a.p, L.bS, c->pair_a.p, c->pair_b.p,
+        const uint64_t* skeys = in_b ? kb2 : c->keys_a.p;
+        const uint32_t* svals = in_b ? c->vals_b.p : c->vals_a.p;
+        c->begin("pair_mark", (double)npairs * (8 * words + 8));
+        pair_mark_kernel<<<nblk(npairs, 256), 256, 0, c->stream>>>(npairs, skeys, svals, words, c->pair_a.p, c->pair_b.p, c->pair_score.p,
                                                                   c->qname_off.p, c->qname.p, c->flag.p);
         c->end(); LAUNCH_CHECK(c);
-        if (optical) return phase_optical(c, npairs, in_b ? kb2 : c->keys_a.p, in_b ? c->vals_b.p : c->vals_a.p, L.bS);
+        if (optical) return phase_optical(c, npairs, skeys, svals, words);
     }
     return optical ? phase_optical(c, 0, nullptr, nullptr, 0) : E_OK;
 }
@@ -521,7 +541,7 @@ int phase_markdup(elp_ctx* c, bool optical) {
             const int bU = bits_for((uint64_t)((int64_t)R.upos_max - (int64_t)R.upos_min));
             // both packed key layouts are checked before any marking kernel runs, so that a refusal leaves the FLAG column untouched
             {
-                const int frag_bits = bits_for((uint64_t)R.score_max) + 2 + bU + bR + bL, pair_bits = bits_for((uint64_t)R.score_max * 2) + 2 * bU + 2 + 2 * bR + bL;
+                const int frag_bits = bits_for((uint64_t)R.score_max) + 2 + bU + bR + bL, pair_bits = 2 * bU + 2 + 2 * bR + bL;
                 if (n && R.n_entering && frag_bits > 64) return c->fail(E_LIMIT, "fragment signature needs %d bits (>64): too many contigs/libraries for the packed key", frag_bits);
                 if (pair_bits > 128) return c->fail(E_LIMIT, "pair signature needs %d bits (>128)", pair_bits);
             }
@@ -533,8 +553,9 @@ int phase_markdup(elp_ctx* c, bool optical) {
                 c->begin("frag_keys", (double)n * (2 + 4 + 4 + 4 + 4 + 8 + 4));
                 frag_keys_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(n, c->flag.p, c->refid.p, c->rg.p, c->d_rg_lib, c->n_rg, c->upos.p, c->score.p, L, c->keys_a.p, c->vals_a.p);
                 c->end(); LAUNCH_CHECK(c);
+                // only the group (bits from bS + 1 up) needs to be contiguous: frag_mark_kernel finds the winner from the low bits
                 bool in_b = false;
-                int r2 = radix_sort_u64(c, c->keys_a.p, c->keys_b.p, c->vals_a.p, c->vals_b.p, n, L.key_bits, &in_b, "u64");
+                int r2 = radix_sort_u64(c, c->keys_a.p, c->keys_b.p, c->vals_a.p, c->vals_b.p, n, L.key_bits - (L.bS + 1), &in_b, "u64", L.bS + 1);
                 if (r2) return r2;
                 const uint64_t m = R.n_entering;
                 c->begin("frag_mark", (double)m * 12);

@@ -9,7 +9,8 @@
 // the pair signature, so an origin's list is simply a run of equal signatures:
 //   * every pair of a run other than the winner has both mates flagged 0x400 (classifyPair :375-395), i.e. is attached;
 //     the winner is the origin and contributes its own first-of-pair read (:276-286) -- so the list is the whole run and
-//     the winner's identity does not matter;
+//     neither the winner's identity nor the order of the pairs inside the run (arrival order) matters: every count below,
+//     including the LIST_CAP test, is taken over the whole run;
 //   * singletons (the vast majority) only bump duplicatesCountHistogram[1] / nonOptical[1] and need no QNAME parse;
 //   * runs of <= 32 pairs are clustered by one thread (sequential union-find), longer ones by one block
 //     (lock-free union-find with atomicCAS hooking).  Σ(cluster size − 1) = members − clusters.
@@ -94,12 +95,9 @@ __device__ int parse_i64(const uint8_t* s, int n, long long* out) {
     return 0;
 }
 
-__device__ __forceinline__ void group_of(const uint64_t* keys, uint64_t j, int bS, uint64_t& glo, uint64_t& ghi) {
-    const uint64_t lo = keys[2 * j], hi = keys[2 * j + 1];
-    if (bS == 0) { glo = lo; ghi = hi; } else if (bS < 64) { glo = (lo >> bS) | (hi << (64 - bS)); ghi = hi >> bS; } else { glo = hi >> (bS - 64); ghi = 0; }
-}
-__device__ __forceinline__ bool same_group(const uint64_t* keys, uint64_t a, uint64_t b, int bS) {
-    uint64_t al, ah, bl, bh; group_of(keys, a, bS, al, ah); group_of(keys, b, bS, bl, bh); return al == bl && ah == bh;
+// the pair keys are the signature alone: one word (u64) or two (u128 as lo,hi)
+__device__ __forceinline__ bool same_group(const uint64_t* keys, uint64_t a, uint64_t b, int words) {
+    return words == 1 ? keys[a] == keys[b] : (keys[2 * a] == keys[2 * b] && keys[2 * a + 1] == keys[2 * b + 1]);
 }
 
 // member info bits (m_info): bit0 strand of the list read, bit1 parse error, bit2 value outside int32, bits 8.. = rg + 1
@@ -108,7 +106,7 @@ __device__ __forceinline__ bool same_group(const uint64_t* keys, uint64_t a, uin
 #define MI_PLIM 4u
 
 struct MemberArgs {
-    uint64_t npairs; const uint64_t* keys; const uint32_t* vals; int bS;
+    uint64_t npairs; const uint64_t* keys; const uint32_t* vals; int key_words;
     const uint32_t* pair_a; const uint32_t* pair_b; const uint16_t* flag; const int32_t* rg; const int32_t* rg_lib; int n_rg;
     const uint64_t* qname_off; const uint8_t* qname;
     int32_t* m_t; int32_t* m_x; int32_t* m_y; uint32_t* m_info;
@@ -124,8 +122,8 @@ __global__ void __launch_bounds__(256) opt_members_kernel(MemberArgs M, OptAcc A
         const int32_t g = M.rg[a1];
         slot = ((g >= 0 && g < M.n_rg) ? M.rg_lib[g] : -1) + 1;
         both_dup = (f1 & F_DUPLICATE) && (f2 & F_DUPLICATE);
-        const bool head = j == 0 || !same_group(M.keys, j - 1, j, M.bS);
-        const bool last = j + 1 == M.npairs || !same_group(M.keys, j, j + 1, M.bS);
+        const bool head = j == 0 || !same_group(M.keys, j - 1, j, M.key_words);
+        const bool last = j + 1 == M.npairs || !same_group(M.keys, j, j + 1, M.key_words);
         single = head && last;
         if (!single) {
             const uint32_t e = (f1 & F_FIRST) ? a1 : a2;                       // :216-221, :276-281
@@ -175,9 +173,9 @@ __device__ __forceinline__ bool optical_edge(const MemberArgs& M, uint64_t a, ui
 __global__ void __launch_bounds__(256) opt_small_groups_kernel(MemberArgs M, OptAcc A, int dist, uint32_t* __restrict__ err) {
     const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= M.npairs) return;
-    if (j > 0 && same_group(M.keys, j - 1, j, M.bS)) return;
+    if (j > 0 && same_group(M.keys, j - 1, j, M.key_words)) return;
     uint64_t e = j + 1;
-    while (e < M.npairs && e - j <= SMALL_MAX && same_group(M.keys, j, e, M.bS)) e++;
+    while (e < M.npairs && e - j <= SMALL_MAX && same_group(M.keys, j, e, M.key_words)) e++;
     const int n = (int)(e - j);
     if (n == 1) return;
     if (n > SMALL_MAX) { const uint32_t k = atomicAdd(A.big_n, 1u); if (k < A.big_cap) A.big[k] = (uint32_t)j; return; }
@@ -229,7 +227,7 @@ __global__ void __launch_bounds__(256) opt_big_groups_kernel(MemberArgs M, OptAc
     __syncthreads();
     for (uint64_t base = j + 1; base < M.npairs; base += blockDim.x) {     // cooperative search for the end of the run
         const uint64_t t = base + threadIdx.x;
-        if (t < M.npairs && !same_group(M.keys, j, t, M.bS)) atomicMin(&s_end, (unsigned long long)t);
+        if (t < M.npairs && !same_group(M.keys, j, t, M.key_words)) atomicMin(&s_end, (unsigned long long)t);
         __syncthreads();
         if (s_end != M.npairs) break;
     }
@@ -285,7 +283,7 @@ static int opt_alloc(elp_ctx* c) {
 }
 
 // called by phase_markdup after pair_mark (npairs may be 0: then only the per-read counters run)
-int phase_optical(elp_ctx* c, uint64_t npairs, const uint64_t* sorted_keys, const uint32_t* sorted_vals, int bS) {
+int phase_optical(elp_ctx* c, uint64_t npairs, const uint64_t* sorted_keys, const uint32_t* sorted_vals, int key_words) {
     int rc = opt_alloc(c);
     if (rc) return rc;
     const uint64_t n = c->n;
@@ -304,7 +302,7 @@ int phase_optical(elp_ctx* c, uint64_t npairs, const uint64_t* sorted_keys, cons
         // scratch: keys_b (2n+4 u64) is free after pair_keys_kernel; npairs <= n/2, so five u32 arrays of npairs fit
         uint32_t* base = reinterpret_cast<uint32_t*>(c->keys_b.p);
         MemberArgs M{};
-        M.npairs = npairs; M.keys = sorted_keys; M.vals = sorted_vals; M.bS = bS; M.pair_a = c->pair_a.p; M.pair_b = c->pair_b.p;
+        M.npairs = npairs; M.keys = sorted_keys; M.vals = sorted_vals; M.key_words = key_words; M.pair_a = c->pair_a.p; M.pair_b = c->pair_b.p;
         M.flag = c->flag.p; M.rg = c->rg.p; M.rg_lib = c->d_rg_lib; M.n_rg = c->n_rg; M.qname_off = c->qname_off.p; M.qname = c->qname.p;
         M.m_t = reinterpret_cast<int32_t*>(base); M.m_x = reinterpret_cast<int32_t*>(base + npairs); M.m_y = reinterpret_cast<int32_t*>(base + 2 * npairs);
         M.m_info = base + 3 * npairs;

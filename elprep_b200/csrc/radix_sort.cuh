@@ -11,8 +11,8 @@
 //   rs_onesweep_kernel  per pass: warp-striped coalesced key loads, per-warp ranking with match.any,
 //                       chained-scan (decoupled look-back) across tiles for the global digit offsets, tile-local
 //                       reorder through shared memory so the scatter leaves in digit-contiguous runs.
-// Keys are compacted by the caller so that only `key_bits` low bits are significant; P = ceil(key_bits/8)
-// passes with balanced digit widths <= 8.
+// Keys are compacted by the caller; the sort orders by bits [lo_bit, lo_bit + key_bits) in P = ceil(key_bits/8) passes with
+// balanced digit widths <= 8.  Bits below lo_bit travel with the key unsorted (equal ranges keep arrival order).
 #pragma once
 #include "common.cuh"
 
@@ -28,11 +28,11 @@ struct Plan {
     int bits[MAX_PASSES];
 };
 
-inline Plan make_plan(int key_bits) {
+inline Plan make_plan(int key_bits, int lo_bit = 0) {
     Plan p{};
     if (key_bits < 1) key_bits = 1;
     p.n_passes = (key_bits + 7) / 8;
-    int base = key_bits / p.n_passes, extra = key_bits % p.n_passes, s = 0;
+    int base = key_bits / p.n_passes, extra = key_bits % p.n_passes, s = lo_bit;
     for (int i = 0; i < p.n_passes; i++) {
         p.bits[i] = base + (i < extra ? 1 : 0);
         p.shift[i] = s;

@@ -4,12 +4,13 @@
 namespace {
 
 template <class K>
-int radix_sort_impl(elp_ctx* c, K* ka, K* kb, uint32_t* va, uint32_t* vb, uint64_t n, int key_bits, bool* result_in_b, const char* tag) {
+int radix_sort_impl(elp_ctx* c, K* ka, K* kb, uint32_t* va, uint32_t* vb, uint64_t n, int key_bits, bool* result_in_b, const char* tag, int lo_bit) {
     using namespace rs;
     *result_in_b = false;
     if (n == 0) return E_OK;
     if (n >= (1ull << 30)) return c->fail(E_LIMIT, "radix sort: %llu keys exceed the 2^30 limit of the look-back status words", (unsigned long long)n);
-    Plan plan = make_plan(key_bits);
+    if (lo_bit < 0 || lo_bit + key_bits > (int)(8 * sizeof(K))) return c->fail(E_INVAL, "radix sort: bits [%d, %d) outside the key", lo_bit, lo_bit + key_bits);
+    Plan plan = make_plan(key_bits, lo_bit);
     Workspace& ws = c->ws;
     if (!ws.ghist) {
         CUDA_TRY(c, cudaMalloc(&ws.ghist, MAX_PASSES * RADIX * 4));
@@ -140,11 +141,11 @@ int scan_impl(elp_ctx* c, const TIn* in, uint64_t* out, uint64_t n, uint64_t bas
 
 }  // namespace
 
-int radix_sort_u64(elp_ctx* c, uint64_t* ka, uint64_t* kb, uint32_t* va, uint32_t* vb, uint64_t n, int key_bits, bool* result_in_b, const char* tag) {
-    return radix_sort_impl<rs::K64>(c, reinterpret_cast<rs::K64*>(ka), reinterpret_cast<rs::K64*>(kb), va, vb, n, key_bits, result_in_b, tag);
+int radix_sort_u64(elp_ctx* c, uint64_t* ka, uint64_t* kb, uint32_t* va, uint32_t* vb, uint64_t n, int key_bits, bool* result_in_b, const char* tag, int lo_bit) {
+    return radix_sort_impl<rs::K64>(c, reinterpret_cast<rs::K64*>(ka), reinterpret_cast<rs::K64*>(kb), va, vb, n, key_bits, result_in_b, tag, lo_bit);
 }
-int radix_sort_u128(elp_ctx* c, uint64_t* ka, uint64_t* kb, uint32_t* va, uint32_t* vb, uint64_t n, int key_bits, bool* result_in_b, const char* tag) {
-    return radix_sort_impl<rs::K128>(c, reinterpret_cast<rs::K128*>(ka), reinterpret_cast<rs::K128*>(kb), va, vb, n, key_bits, result_in_b, tag);
+int radix_sort_u128(elp_ctx* c, uint64_t* ka, uint64_t* kb, uint32_t* va, uint32_t* vb, uint64_t n, int key_bits, bool* result_in_b, const char* tag, int lo_bit) {
+    return radix_sort_impl<rs::K128>(c, reinterpret_cast<rs::K128*>(ka), reinterpret_cast<rs::K128*>(kb), va, vb, n, key_bits, result_in_b, tag, lo_bit);
 }
 int exclusive_scan_u32_to_u64(elp_ctx* c, const uint32_t* in, uint64_t* out, uint64_t n) { return scan_impl<uint32_t>(c, in, out, n, 0); }
 int exclusive_scan_u64_from_u32(elp_ctx* c, const uint32_t* in, uint64_t* out, uint64_t n, uint64_t base) { return scan_impl<uint32_t>(c, in, out, n, base); }
