@@ -12,7 +12,7 @@ SO_PATH = os.environ.get("ELPREP_B200_LIB", os.path.join(_HERE, "lib", "libelpre
 
 SO_KEEP, SO_UNKNOWN, SO_UNSORTED, SO_QUERYNAME, SO_COORDINATE = 0, 1, 2, 3, 4
 MARKDUP, MARKDUP_OPTICAL = 1, 2
-EINVAL, ELIMIT, EBAM, ESAM = -1, -15, -18, -20
+EINVAL, ELIMIT, ESTATE, EBAM, ESAM = -1, -15, -16, -18, -20
 FILTER_UNMAPPED, FILTER_UNMAPPED_STRICT, FILTER_NON_EXACT, FILTER_DUPLICATES, FILTER_NON_EXACT_STRICT, FILTER_TARGET_REGIONS = 1, 2, 4, 8, 16, 32
 
 
@@ -42,7 +42,7 @@ class ElpKernelStat(C.Structure):
 EXPORTS = ["elp_create", "elp_destroy", "elp_last_error", "elp_reserve", "elp_reset", "elp_set_reference", "elp_set_known_sites",
            "elp_fetch_opt_flags", "elp_set_target_regions", "elp_clean_sam", "elp_debug_cigar", "elp_comm_unique_id", "elp_comm_init", "elp_comm_set_partition", "elp_comm_destroy", "elp_bqsr_tables_allreduce", "elp_optical_allreduce", "elp_bqsr_tables_clear", "elp_bqsr_tables_write_elrecal", "elp_bqsr_tables_add_elrecal", "elp_optical_write_gob", "elp_optical_add_gob", "elp_append_batch", "elp_append_batch_async", "elp_append_wait", "elp_fetch_async", "elp_fetch_wait", "elp_append_bam", "elp_append_sam", "elp_set_ingest_filter", "elp_n_filtered", "elp_n_reads", "elp_sort_markdup", "elp_bqsr_gather", "elp_bqsr_tables_len", "elp_bqsr_n_cov",
            "elp_bqsr_cov_name", "elp_bqsr_tables_get", "elp_bqsr_tables_put", "elp_bqsr_tables_device", "elp_bqsr_finalize",
-           "elp_bqsr_empirical_get", "elp_bqsr_apply", "elp_fetch", "elp_fetch_qual_bytes", "elp_fetch_bam", "elp_fetch_bam_bytes", "elp_debug_adapt", "elp_launch_count",
+           "elp_bqsr_empirical_get", "elp_bqsr_apply", "elp_fetch", "elp_fetch_qual_bytes", "elp_fetch_bam", "elp_fetch_bam_bytes", "elp_fetch_sam", "elp_fetch_sam_bytes", "elp_debug_adapt", "elp_launch_count",
            "elp_kernel_stats", "elp_synchronize", "elp_reset_stats", "elp_timer_start", "elp_timer_stop", "elp_debug_sort_u64", "elp_debug_sort_u128",
            "elp_optical_n_libraries", "elp_optical_library_name", "elp_optical_metrics", "elp_optical_histogram", "elp_optical_merge",
            "elp_print_duplicates_metrics",
@@ -102,6 +102,9 @@ def load():
     L.elp_fetch_bam_bytes.restype = C.c_uint64
     L.elp_fetch_bam_bytes.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64]
     L.elp_fetch_bam.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p]
+    L.elp_fetch_sam_bytes.restype = C.c_uint64
+    L.elp_fetch_sam_bytes.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64]
+    L.elp_fetch_sam.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p]
     L.elp_set_ingest_filter.argtypes = [C.c_void_p, C.c_uint32, C.c_int32]
     L.elp_n_filtered.restype = C.c_uint64
     L.elp_n_filtered.argtypes = [C.c_void_p]

@@ -196,6 +196,7 @@ void elp_destroy(elp_ctx* c) {
     cudaSetDevice(c->device);
     if (c->stream) cudaStreamSynchronize(c->stream);
     sam_state_release(c);
+    sam_out_release(c);
     for (auto p : c->d_ref) if (p) cudaFree(p);
     for (auto p : c->d_refnib_raw) if (p) cudaFree(p);
     for (auto p : c->d_refhot_raw) if (p) cudaFree(p);
@@ -231,7 +232,7 @@ int elp_reset(elp_ctx* c) {
     if (c->copy_in) CUDA_TRY(c, cudaStreamSynchronize(c->copy_in));
     if (c->copy_out) CUDA_TRY(c, cudaStreamSynchronize(c->copy_out));
     CUDA_TRY(c, cudaStreamSynchronize(c->stream));
-    c->n = c->n_qname = c->n_cigar = 0; c->n_qual = c->n_seq = ARENA_FRONT_PAD; c->n_bam = c->bam_reads = 0; c->n_filtered = 0; c->n_cleaned = 0;
+    c->n = c->n_qname = c->n_cigar = 0; c->n_qual = c->n_seq = ARENA_FRONT_PAD; c->n_bam = c->bam_reads = 0; c->n_filtered = 0; c->n_cleaned = 0; c->n_sam_lost_names = 0;
     CUDA_TRY(c, cudaMemsetAsync(c->d_qpresent, 0, 16, c->stream));
     c->adapted = c->sorted = c->qual_out_valid = c->gathered = c->finalized = c->opt_valid = false;
     c->launches = 0;

@@ -14,6 +14,7 @@
 #include <thread>
 #include <vector>
 #include "../../include/elprep_b200.h"
+#include "pool.hpp"
 
 namespace {
 
@@ -52,15 +53,6 @@ int scan_blocks(const uint8_t* d, uint64_t n, std::vector<Block>& blocks, uint64
     }
     *total = out;
     return ELP_OK;
-}
-
-template <class F> void pool_for(size_t n, int threads, F f) {
-    threads = std::max(1, std::min<int>(threads, (int)std::max<size_t>(n, 1)));
-    if (threads == 1) { for (size_t i = 0; i < n; i++) f(i); return; }
-    std::atomic<size_t> next{0};
-    std::vector<std::thread> th;
-    for (int t = 0; t < threads; t++) th.emplace_back([&]() { for (;;) { const size_t i = next.fetch_add(16); if (i >= n) break; for (size_t k = i; k < std::min(n, i + 16); k++) f(k); } });
-    for (auto& x : th) x.join();
 }
 
 }  // namespace

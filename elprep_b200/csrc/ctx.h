@@ -110,6 +110,8 @@ struct elp_ctx {
     uint64_t n_cleaned = 0;                  // reads whose CIGAR elp_clean_sam rewrote
     bool has_contig_names = false;           // elp_config.contig_names was given (elp_append_sam resolves RNAME / RNEXT against it)
     struct SamState* sam = nullptr;          // device tables and staging of elp_append_sam (sam_ingest.cu)
+    uint64_t n_sam_lost_names = 0;           // reads of elp_append_sam whose RNAME / RNEXT text the stored record cannot reproduce (elp_fetch_sam refuses)
+    struct SamOutState* sam_out = nullptr;   // @SQ names and float staging of elp_fetch_sam (sam_format.cu)
     uint8_t* d_rg_names = nullptr; uint32_t* d_rg_name_off = nullptr; std::vector<std::string> rg_ids;   // @RG IDs for the RG:Z match
     DBuf<int32_t> lseq_stage;       // staging for l_seq of the batch being appended
     DBuf<uint64_t> off_stage;       // staging for batch-relative offsets
@@ -252,3 +254,4 @@ int exclusive_scan_u64_from_u32(elp_ctx* c, const uint32_t* in, uint64_t* out, u
 int qual_presence_update(elp_ctx* c, uint64_t first_byte, uint64_t n_bytes);   // api.cu: called by both ingest paths
 int bam_ingest_core(elp_ctx* c, uint64_t n_bytes, uint64_t nrec);   // bam_ingest.cu: records staged in bam_raw / bam_off -> reads (elp_append_bam, elp_append_sam)
 void sam_state_release(elp_ctx* c);   // sam_ingest.cu
+void sam_out_release(elp_ctx* c);     // sam_format.cu

@@ -22,8 +22,9 @@ struct SlowF { uint64_t text_off, out_off; uint32_t len, line; };   // one float
 struct SamState {
     DBuf<uint8_t> text; DBuf<uint32_t> cnt, len; DBuf<uint64_t> cnt_off, ls;
     DBuf<SlowF> slow; DBuf<uint64_t> patch_off; DBuf<uint32_t> patch_bits;
+    DBuf<uint8_t> lost;                       // per line: 1 if its RNAME / RNEXT text is lost in the record (see parse_line)
     uint8_t* d_names = nullptr; uint32_t* d_name_off = nullptr; int32_t* d_name_id = nullptr; int n_names = 0;
-    unsigned long long* d_small = nullptr;   // [0] first error (line << 8 | SamErr), [1] floats handed to the host
+    unsigned long long* d_small = nullptr;   // [0] first error (line << 8 | SamErr), [1] floats handed to the host, [2] lines with a lost name
     uint64_t h_last = 0;                      // source of the virtual line end of a final line without '\n'
 };
 
@@ -31,7 +32,7 @@ void sam_state_release(elp_ctx* c) {
     SamState* S = c->sam;
     if (!S) return;
     S->text.release(); S->cnt.release(); S->len.release(); S->cnt_off.release(); S->ls.release();
-    S->slow.release(); S->patch_off.release(); S->patch_bits.release();
+    S->slow.release(); S->patch_off.release(); S->patch_bits.release(); S->lost.release();
     void* singles[] = {S->d_names, S->d_name_off, S->d_name_id, S->d_small};
     for (void* p : singles) if (p) cudaFree(p);
     delete S;
@@ -117,6 +118,7 @@ struct SamArgs {
     const uint8_t* text; const uint64_t* ls; uint64_t n_lines;
     const uint8_t* names; const uint32_t* name_off; const int32_t* name_id; int n_names;   // "*" and @SQ SN, sorted, with their refid
     uint32_t* len;             // measure: BAM record length per line
+    uint8_t* lost;             // measure: 1 if the record loses the line's RNAME / RNEXT text
     const uint64_t* rec_off;   // emit: record offsets in out
     uint8_t* out;
     unsigned long long* small; SlowF* slow;
@@ -325,6 +327,10 @@ template <bool W> __device__ int parse_line(const SamArgs& A, uint64_t k, const 
     const int32_t refid = refid_of(A, p + e[1] + 1, e[2] - e[1] - 1);
     const bool rnext_eq = e[6] - e[5] - 1 == 1 && p[e[5] + 1] == '=';
     const int32_t nref = rnext_eq ? refid : refid_of(A, p + e[5] + 1, e[6] - e[5] - 1);
+    // names the record cannot give back to elp_fetch_sam: an RNAME that is neither "*" nor an @SQ name, likewise an RNEXT other than
+    // "=", and RNEXT "=" with an RNAME that resolves to -1 ("*" included; the reference's SAM -> SAM text keeps the '=')
+    const bool rname_star = e[2] - e[1] - 1 == 1 && p[e[1] + 1] == '*', rnext_star = e[6] - e[5] - 1 == 1 && p[e[5] + 1] == '*';
+    const bool lost = (refid < 0 && !rname_star) || (!rnext_eq && !rnext_star && nref < 0) || (rnext_eq && refid < 0);
     const uint64_t L = e[9] - e[8] - 1;
     if (e[10] - e[9] - 1 != L) return SE_QUAL;
     uint8_t* o = W ? A.out + A.rec_off[k] : nullptr;
@@ -388,7 +394,7 @@ template <bool W> __device__ int parse_line(const SamArgs& A, uint64_t k, const 
     }
     const uint64_t rec = otag + tsz;
     if (rec >= (1ull << 31)) return SE_RECORD_LIMIT;
-    if (!W) { if (lane == 0) A.len[k] = (uint32_t)rec; return 0; }
+    if (!W) { if (lane == 0) { A.len[k] = (uint32_t)rec; A.lost[k] = lost; if (lost) atomicAdd(A.small + 2, 1ull); } return 0; }
     // bin() (bam-files.go:443-468) in int32 arithmetic; an unmapped read spans [beg, beg]
     const int32_t beg = (int32_t)((uint32_t)pos - 1u);
     const int32_t end = (flag & 4) ? beg : (int32_t)((uint32_t)beg + refspan - 1u);
@@ -429,6 +435,16 @@ template <bool W> __global__ void __launch_bounds__(256) sam_line_kernel(SamArgs
     }
 }
 
+// lost-name lines among the records the ingest filters kept: kept[i] is the start of a kept record, line_off the starts of all lines
+__global__ void __launch_bounds__(256) sam_lost_kept_kernel(uint64_t nk, const uint64_t* __restrict__ kept, const uint64_t* __restrict__ line_off, uint64_t nl,
+                                                             const uint8_t* __restrict__ lost, unsigned long long* __restrict__ cnt) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= nk) return;
+    uint64_t lo = 0, hi = nl;
+    while (hi - lo > 1) { const uint64_t mid = (lo + hi) >> 1; if (line_off[mid] <= kept[i]) lo = mid; else hi = mid; }
+    if (lost[lo]) atomicAdd(cnt, 1ull);
+}
+
 __global__ void __launch_bounds__(256) sam_fpatch_kernel(uint64_t n, const uint64_t* __restrict__ off, const uint32_t* __restrict__ bits, uint8_t* __restrict__ out) {
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) for (int b = 0; b < 4; b++) out[off[i] + b] = (uint8_t)(bits[i] >> (8 * b));
@@ -451,7 +467,7 @@ int sam_tables(elp_ctx* c) {
     CUDA_TRY(c, cudaMemcpy(S.d_name_off, off.data(), off.size() * 4, cudaMemcpyHostToDevice));
     CUDA_TRY(c, cudaMemcpy(S.d_name_id, id.data(), id.size() * 4, cudaMemcpyHostToDevice));
     S.n_names = (int)id.size();
-    CUDA_TRY(c, cudaMalloc(&S.d_small, 16));
+    CUDA_TRY(c, cudaMalloc(&S.d_small, 24));
     return E_OK;
 }
 
@@ -493,7 +509,7 @@ extern "C" int elp_append_sam(elp_ctx* c, const char* text, uint64_t n_bytes) {
     const bool open_end = h[n_bytes - 1] != '\n';
     const uint64_t nl = n_nl + (open_end ? 1 : 0);   // lines
     if (c->n + nl >= (1ull << 32)) return c->fail(E_LIMIT, "more than 2^32-1 reads in one context");
-    TRY(grow(c, S.ls, nl + 2, 0)); TRY(grow(c, S.len, nl + 8, 0)); TRY(grow(c, c->bam_off, nl + 2, 0));
+    TRY(grow(c, S.ls, nl + 2, 0)); TRY(grow(c, S.len, nl + 8, 0)); TRY(grow(c, S.lost, nl + 8, 0)); TRY(grow(c, c->bam_off, nl + 2, 0));
     CUDA_TRY(c, cudaMemsetAsync(S.ls.p, 0, 8, s));
     c->begin("sam_lines", (double)n_bytes + 8.0 * (double)n_nl);
     sam_lines_kernel<<<nblk(n_chunks, 256), 256, 0, s>>>(S.text.p, n_chunks, S.cnt_off.p, S.ls.p);
@@ -504,14 +520,14 @@ extern "C" int elp_append_sam(elp_ctx* c, const char* text, uint64_t n_bytes) {
     SamArgs A{};
     A.text = S.text.p; A.ls = S.ls.p; A.n_lines = nl;
     A.names = S.d_names; A.name_off = S.d_name_off; A.name_id = S.d_name_id; A.n_names = S.n_names;
-    A.len = S.len.p; A.rec_off = c->bam_off.p; A.small = S.d_small;
-    CUDA_TRY(c, cudaMemsetAsync(S.d_small, 0xff, 8, s)); CUDA_TRY(c, cudaMemsetAsync(S.d_small + 1, 0, 8, s));
+    A.len = S.len.p; A.lost = S.lost.p; A.rec_off = c->bam_off.p; A.small = S.d_small;
+    CUDA_TRY(c, cudaMemsetAsync(S.d_small, 0xff, 8, s)); CUDA_TRY(c, cudaMemsetAsync(S.d_small + 1, 0, 16, s));
     c->begin("sam_measure", (double)n_bytes);
     sam_line_kernel<false><<<nblk(nl * 32, 256), 256, 0, s>>>(A);
     c->end(); LAUNCH_CHECK(c);
     TRY(exclusive_scan_u32_to_u64(c, S.len.p, c->bam_off.p, nl));
-    unsigned long long small[2]; uint64_t total = 0;
-    CUDA_TRY(c, cudaMemcpyAsync(small, S.d_small, 16, cudaMemcpyDeviceToHost, s));
+    unsigned long long small[3]; uint64_t total = 0;
+    CUDA_TRY(c, cudaMemcpyAsync(small, S.d_small, 24, cudaMemcpyDeviceToHost, s));
     CUDA_TRY(c, cudaMemcpyAsync(&total, c->bam_off.p + nl, 8, cudaMemcpyDeviceToHost, s));
     CUDA_TRY(c, cudaStreamSynchronize(s));
     if (small[0] != ~0ull) {
@@ -545,5 +561,16 @@ extern "C" int elp_append_sam(elp_ctx* c, const char* text, uint64_t n_bytes) {
         c->end(); LAUNCH_CHECK(c);
         CUDA_TRY(c, cudaStreamSynchronize(s));   // (po / pb are pageable host memory)
     }
-    return bam_ingest_core(c, total, nl);
+    const uint64_t n0 = c->n;
+    TRY(bam_ingest_core(c, total, nl));
+    uint64_t lost = small[2];
+    if (lost && (c->filter_mask || c->filter_min_mapq > 0)) {   // count only the lines the filters kept (bam_start: their record starts)
+        const uint64_t nk = c->n - n0;
+        CUDA_TRY(c, cudaMemsetAsync(S.d_small + 2, 0, 8, s));
+        if (nk) { sam_lost_kept_kernel<<<nblk(nk, 256), 256, 0, s>>>(nk, c->bam_start.p, c->bam_off.p, nl, S.lost.p, S.d_small + 2); c->launches++; LAUNCH_CHECK(c); }
+        CUDA_TRY(c, cudaMemcpyAsync(&lost, S.d_small + 2, 8, cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(c, cudaStreamSynchronize(s));
+    }
+    c->n_sam_lost_names += lost;
+    return ELP_OK;
 }

@@ -300,6 +300,15 @@ class Context:
         self._ck(self.L.elp_fetch_bam(self.h, first, n, _vp(out), out.size, _vp(off)))
         return out[:nb], off
 
+    def fetch_sam(self, first=0, n=None):
+        """-> (uint8 SAM text, uint64 line offsets [n+1]) of output records [first, first+n): FormatAlignment of each stored record with
+        FLAG and QUAL patched, one '\\n'-terminated alignment line per record, no header"""
+        n = self.n - first if n is None else n
+        nb = int(self.L.elp_fetch_sam_bytes(self.h, first, n)) if n else 0
+        out, off = np.empty(max(nb, 1), np.uint8), np.empty(n + 1, np.uint64)
+        self._ck(self.L.elp_fetch_sam(self.h, first, n, _vp(out), out.size, _vp(off)))
+        return out[:nb], off
+
     def debug_adapt(self):
         u, s = np.zeros(self.n, np.int32), np.zeros(self.n, np.int32)
         self._ck(self.L.elp_debug_adapt(self.h, _vp(u), _vp(s)))

@@ -267,6 +267,17 @@ int elp_fetch_wait(elp_ctx *ctx);
  * compresses the result.  record_off[n+1] may be NULL. */
 uint64_t elp_fetch_bam_bytes(elp_ctx *ctx, uint64_t first, uint64_t n);
 int elp_fetch_bam(elp_ctx *ctx, uint64_t first, uint64_t n, uint8_t *out, uint64_t capacity, uint64_t *record_off);
+/* The same as SAM text alignment lines (FormatAlignment, sam/sam-files.go:563-598, of parseBamAlignment of the record elp_fetch_bam returns):
+ * output records [first, first+n) as lines ending in '\n', with the context's FLAG and -- once elp_bqsr_apply has run -- QUAL; no header
+ * lines (the caller writes the header text).  line_off[n+1] (may be NULL): offset of every line in out.  The reference's quirks are kept:
+ * every integer tag prints as i, POS / PNEXT wrap in int32, RNEXT is '=' when its @SQ name equals RNAME's, f values print as Go's
+ * strconv 'g' shortest float32, H digits in lower case.  Refusals as elp_fetch_bam (ELP_ESTATE before elp_sort_markdup, for reads that did
+ * not come through elp_append_bam / elp_append_sam, after elp_clean_sam rewrote a CIGAR; ELP_EINVAL for a range past the reads or a buffer
+ * too small, nothing written), plus: ELP_EINVAL when a context with @SQ lines was created without elp_config.contig_names; ELP_ESTATE when
+ * elp_append_sam took a line whose RNAME or RNEXT the stored record cannot reproduce (a name that is not an @SQ name, or RNEXT '=' with
+ * such an RNAME; elp_last_error gives their number); ELP_EBAM for a CIGAR operation code above 8.  elp_fetch_sam_bytes returns 0 on error. */
+uint64_t elp_fetch_sam_bytes(elp_ctx *ctx, uint64_t first, uint64_t n);
+int elp_fetch_sam(elp_ctx *ctx, uint64_t first, uint64_t n, char *out, uint64_t capacity, uint64_t *line_off);
 int elp_debug_adapt(elp_ctx *ctx, int32_t *upos, int32_t *score);
 /* opt_flags of output records [first, first+n) (what filters.RemoveOptionalReads looks at when the worker writes its output) */
 int elp_fetch_opt_flags(elp_ctx *ctx, uint64_t first, uint64_t n, uint8_t *opt_flags);
