@@ -205,11 +205,11 @@ void elp_destroy(elp_ctx* c) {
     if (c->d_region_ptrs) cudaFree((void*)c->d_region_ptrs);
     if (c->d_n_regions) cudaFree(c->d_n_regions);
     void* singles[] = {c->d_rg_lib, c->d_rg_cov, c->d_contig_len, c->d_ranges, c->d_err, (void*)c->d_ref_ptrs, (void*)c->d_refnib_ptrs, (void*)c->d_refhot_ptrs, c->d_bq_small, c->d_qpresent, c->d_ref_len, (void*)c->d_site_ptrs, c->d_n_sites, c->d_tables,
-                       c->d_lut, c->d_clut, c->d_rowtab, c->d_cov_exists, c->d_opt_ctr, c->d_opt_hist, c->d_opt_ovf, c->d_opt_small, c->d_rg_names, c->d_rg_name_off, c->ws.ghist, c->ws.gofs, c->ws.counters, c->ws.status};
+                       c->d_lut, c->d_clut, c->d_rowtab, c->d_cov_exists, c->d_opt_ctr, c->d_opt_hist, c->d_opt_ovf, c->d_opt_small, c->d_rg_names, c->d_rg_name_off, c->d_out_drop, c->ws.ghist, c->ws.gofs, c->ws.counters, c->ws.status};
     for (void* p : singles) if (p) cudaFree(p);
     c->refid.release(); c->pos.release(); c->nref.release(); c->pnext.release(); c->tlen.release(); c->rg.release(); c->flag.release(); c->mapq.release(); c->optf.release(); c->s_optf.release();
     c->qname_off.release(); c->cigar_off.release(); c->qual_off.release(); c->seq_off.release(); c->qname.release(); c->seq.release(); c->qual.release(); c->cigar.release();
-    c->bam_raw.release(); c->bam_off.release(); c->bam_all.release(); c->bam_all_off.release(); c->bam_start.release(); c->lseq_stage.release(); c->off_stage.release(); c->upos.release(); c->score.release(); c->qhash.release(); c->keys_a.release(); c->keys_b.release();
+    c->bam_raw.release(); c->bam_off.release(); c->bam_all.release(); c->bam_all_off.release(); c->bam_start.release(); c->out_sel.release(); c->lseq_stage.release(); c->off_stage.release(); c->upos.release(); c->score.release(); c->qhash.release(); c->keys_a.release(); c->keys_b.release();
     c->bq_recs.release(); c->bq_segs.release(); c->vals_a.release(); c->vals_b.release(); c->mate.release(); c->pair_a.release(); c->pair_b.release(); c->pair_score.release(); c->tie_bits.release(); c->scan_tmp.release(); c->scan_blk.release(); c->bytes_tmp.release();
     c->perm.release(); c->s_refid.release(); c->s_pos.release(); c->s_nref.release(); c->s_pnext.release(); c->s_tlen.release(); c->s_rg.release(); c->s_lseq.release();
     c->s_flag.release(); c->s_mapq.release(); c->s_qual_off.release(); c->s_seq_off.release(); c->s_cigar_off.release(); c->s_out_off.release(); c->s_ncigar.release(); c->qual_out.release();
@@ -235,6 +235,7 @@ int elp_reset(elp_ctx* c) {
     c->n = c->n_qname = c->n_cigar = 0; c->n_qual = c->n_seq = ARENA_FRONT_PAD; c->n_bam = c->bam_reads = 0; c->n_filtered = 0; c->n_cleaned = 0; c->n_sam_lost_names = 0;
     CUDA_TRY(c, cudaMemsetAsync(c->d_qpresent, 0, 16, c->stream));
     c->adapted = c->sorted = c->qual_out_valid = c->gathered = c->finalized = c->opt_valid = false;
+    c->out_sel_valid = false; c->n_out = 0;   // (the output filter setting itself stays)
     c->launches = 0;
     CUDA_TRY(c, cudaMemsetAsync(c->d_err, 0, 4, c->stream));
     return ELP_OK;
@@ -395,6 +396,7 @@ int elp_sort_markdup(elp_ctx* c, int sorting_order, int mark_duplicates) {
     if (mark_duplicates != 0 && mark_duplicates != ELP_MARKDUP && mark_duplicates != ELP_MARKDUP_OPTICAL) return c->fail(E_INVAL, "elp_sort_markdup: mark_duplicates must be 0, ELP_MARKDUP or ELP_MARKDUP_OPTICAL");
     if (mark_duplicates) TRY(phase_markdup(c, mark_duplicates == ELP_MARKDUP_OPTICAL));
     TRY(phase_coordinate_sort(c, sorting_order == ELP_SO_COORDINATE ? 1 : (sorting_order == ELP_SO_QUERYNAME ? 2 : 0)));
+    c->out_sel_valid = false;   // the record filters' selection reads the new FLAG column (built on the first filtered fetch)
     return ELP_OK;
 }
 

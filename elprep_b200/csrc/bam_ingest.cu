@@ -14,6 +14,7 @@
 // an RG:Z value that is not an @RG ID of the header.
 #include <algorithm>
 #include "ctx.h"
+#include "tagwalk.cuh"
 #include "../../include/elprep_b200.h"
 
 namespace {
@@ -27,6 +28,7 @@ struct BamArgs {
     uint64_t n, n0;                       // records in this call, reads already in the context
     const uint8_t* raw; const uint64_t* start; uint64_t n_bytes;   // start[i]: offset of record i's block_size field
     int chained;                          // start[] has n + 1 entries and start[i + 1] must be the end of record i (no filter ran)
+    int clear_dup;                        // ClearDuplicateFlag: 0x400 cleared in the FLAG column (the stored record keeps its bytes)
     int32_t *refid, *pos, *nref, *pnext, *tlen, *rg; uint16_t* flag; uint8_t* mapq; uint8_t* optf;
     uint32_t *len_qname, *len_cigar, *len_seq, *len_qual;   // [n] lengths, scanned afterwards
     const uint8_t* rg_names; const uint32_t* rg_name_off; int n_rg; int n_contigs;
@@ -52,7 +54,7 @@ __global__ void __launch_bounds__(256) bam_fixed_kernel(BamArgs A) {
     const uint64_t var = (uint64_t)l_name + 4ull * n_cig + ((lsq + 1) >> 1) + lsq;
     if (l_name < 1 || l_seq < 0 || lsq > rec_len || BAM_FIXED + var > rec_len || refid >= A.n_contigs || nref >= A.n_contigs) bad = 1;
     const uint64_t k = A.n0 + i;
-    A.refid[k] = refid < 0 ? -1 : refid; A.pos[k] = pos + 1; A.flag[k] = (uint16_t)flag; A.mapq[k] = (uint8_t)mapq;
+    A.refid[k] = refid < 0 ? -1 : refid; A.pos[k] = pos + 1; A.flag[k] = (uint16_t)(A.clear_dup ? flag & ~(uint32_t)F_DUPLICATE : flag); A.mapq[k] = (uint8_t)mapq;
     A.nref[k] = nref < 0 ? -1 : nref; A.pnext[k] = pnext + 1; A.tlen[k] = tlen;
     int32_t rg = -1; uint8_t optf = 0;
     if (!bad) {
@@ -237,19 +239,21 @@ __global__ void __launch_bounds__(256) add_base_u64_kernel(uint64_t n, uint64_t*
 }
 
 // ---- egress ----
-__global__ void __launch_bounds__(256) bam_out_len_kernel(uint64_t n, const uint32_t* __restrict__ perm, const uint64_t* __restrict__ all_start, const uint8_t* __restrict__ all,
-                                                           uint32_t* __restrict__ len) {
-    const uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (k < n) len[k] = rd32(all + all_start[perm[k]]) + 4;
+// output record k of a call: first + kk, or sel[first + kk] when the record filters of elp_set_output_filter select the records
+__device__ __forceinline__ uint64_t out_pos(const uint32_t* __restrict__ sel, uint64_t first, uint64_t kk) { return sel ? sel[first + kk] : first + kk; }
+__global__ void __launch_bounds__(256) bam_out_len_kernel(uint64_t n, uint64_t first, const uint32_t* __restrict__ sel, const uint32_t* __restrict__ perm, const uint64_t* __restrict__ all_start,
+                                                           const uint8_t* __restrict__ all, uint32_t* __restrict__ len) {
+    const uint64_t kk = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (kk < n) len[kk] = rd32(all + all_start[perm[out_pos(sel, first, kk)]]) + 4;
 }
 // one warp per output record: copy the stored record, patch FLAG (bytes 18..19 of the record with its block_size) and QUAL
-__global__ void __launch_bounds__(256) bam_out_copy_kernel(uint64_t n, uint64_t first, const uint32_t* __restrict__ perm, const uint64_t* __restrict__ all_start,
+__global__ void __launch_bounds__(256) bam_out_copy_kernel(uint64_t n, uint64_t first, const uint32_t* __restrict__ sel, const uint32_t* __restrict__ perm, const uint64_t* __restrict__ all_start,
                                                             const uint8_t* __restrict__ all, const uint64_t* __restrict__ out_off, uint8_t* __restrict__ out,
                                                             const uint16_t* __restrict__ s_flag, const uint64_t* __restrict__ s_out_off, const uint8_t* __restrict__ qual_out) {
     const unsigned lane = threadIdx.x & 31;
     const uint64_t kk = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (kk >= n) return;
-    const uint64_t k = first + kk;
+    const uint64_t k = out_pos(sel, first, kk);
     const uint32_t i = perm[k];
     const uint8_t* r = all + all_start[i];
     const uint64_t len = (uint64_t)rd32(r) + 4;
@@ -264,6 +268,79 @@ __global__ void __launch_bounds__(256) bam_out_copy_kernel(uint64_t n, uint64_t 
         if (t == 18) v = (uint8_t)(f & 0xff); else if (t == 19) v = (uint8_t)(f >> 8);
         else if (nq && t >= q0 && t < q1) v = nq[t - q0];
         o[t] = v;
+    }
+}
+
+// ---- write-phase filters (elp_set_output_filter; cmd/filter.go:803-902) ----
+// keep[k] = 1 iff output record k passes RemoveDuplicateReads (the FLAG after marking) and RemoveOptionalReads (no sr tag)
+__global__ void __launch_bounds__(256) out_select_kernel(uint64_t n, uint32_t mask, const uint16_t* __restrict__ s_flag, const uint8_t* __restrict__ s_optf, uint32_t* __restrict__ keep) {
+    const uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n) return;
+    bool ok = true;
+    if ((mask & ELP_OUT_REMOVE_DUPLICATES) && (s_flag[k] & F_DUPLICATE)) ok = false;               // simple-filters.go:138-140
+    if ((mask & ELP_OUT_REMOVE_OPTIONAL_READS) && (s_optf[k] & ELP_OPT_SR)) ok = false;            // :146-152
+    keep[k] = ok ? 1u : 0u;
+}
+__global__ void __launch_bounds__(256) out_compact_kernel(uint64_t n, const uint32_t* __restrict__ keep, const uint64_t* __restrict__ slot, uint32_t* __restrict__ sel) {
+    const uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (k < n && keep[k]) sel[slot[k]] = (uint32_t)k;
+}
+
+// start of the optional fields of a stored record
+__device__ __forceinline__ uint64_t tags_start(const uint8_t* r) {
+    const uint64_t l_seq = rd32(r + 20);
+    return BAM_FIXED + (uint64_t)r[12] + 4ull * rd16(r + 16) + ((l_seq + 1) >> 1) + l_seq;
+}
+
+// RemoveOptionalFields / KeepOptionalFields (simple-filters.go:235-288) on BAM records, one warp per output record.
+// measure: the record's length without its dropped fields
+__global__ void __launch_bounds__(256) bam_out_fields_measure_kernel(uint64_t n, uint64_t first, const uint32_t* __restrict__ sel, const uint32_t* __restrict__ perm,
+                                                                     const uint64_t* __restrict__ all_start, const uint8_t* __restrict__ all, const uint32_t* __restrict__ drop,
+                                                                     uint32_t* __restrict__ len) {
+    const uint64_t kk = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (kk >= n) return;
+    const uint8_t* r = all + all_start[perm[out_pos(sel, first, kk)]];
+    const uint64_t rec = (uint64_t)rd32(r) + 4;
+    uint64_t t = tags_start(r), x = t;
+    while (t + 3 <= rec) {
+        const uint64_t fe = tagwalk::field_end(r, t, rec);
+        if (!tagwalk::dropped(drop, r[t], r[t + 1])) x += fe - t;
+        t = fe;
+    }
+    if ((threadIdx.x & 31) == 0) len[kk] = (uint32_t)x;
+}
+// emit: the fixed part and the variable fields with block_size, FLAG and QUAL patched, then the kept fields in their order
+__global__ void __launch_bounds__(256) bam_out_fields_emit_kernel(uint64_t n, uint64_t first, const uint32_t* __restrict__ sel, const uint32_t* __restrict__ perm,
+                                                                  const uint64_t* __restrict__ all_start, const uint8_t* __restrict__ all, const uint32_t* __restrict__ drop,
+                                                                  const uint64_t* __restrict__ out_off, uint8_t* __restrict__ out,
+                                                                  const uint16_t* __restrict__ s_flag, const uint64_t* __restrict__ s_out_off, const uint8_t* __restrict__ qual_out) {
+    const unsigned lane = threadIdx.x & 31;
+    const uint64_t kk = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (kk >= n) return;
+    const uint64_t k = out_pos(sel, first, kk);
+    const uint8_t* r = all + all_start[perm[k]];
+    const uint64_t rec = (uint64_t)rd32(r) + 4, t0 = tags_start(r);
+    uint8_t* o = out + out_off[kk];
+    const uint32_t bs = (uint32_t)(out_off[kk + 1] - out_off[kk] - 4);
+    const int32_t l_seq = (int32_t)rd32(r + 20);
+    const uint64_t q1 = t0, q0 = q1 - (uint64_t)l_seq;
+    const uint16_t f = s_flag[k];
+    const uint8_t* nq = qual_out ? qual_out + s_out_off[k] : nullptr;
+    for (uint64_t t = lane; t < t0; t += 32) {
+        uint8_t v = r[t];
+        if (t < 4) v = (uint8_t)(bs >> (8 * t));
+        else if (t == 18) v = (uint8_t)(f & 0xff); else if (t == 19) v = (uint8_t)(f >> 8);
+        else if (nq && t >= q0) v = nq[t - q0];
+        o[t] = v;
+    }
+    uint64_t t = t0, x = t0;
+    while (t + 3 <= rec) {
+        const uint64_t fe = tagwalk::field_end(r, t, rec);
+        if (!tagwalk::dropped(drop, r[t], r[t + 1])) {
+            for (uint64_t j = lane; j < fe - t; j += 32) o[x + j] = r[t + j];
+            x += fe - t;
+        }
+        t = fe;
     }
 }
 
@@ -360,7 +437,7 @@ int bam_ingest_core(elp_ctx* c, uint64_t n_bytes, uint64_t nrec) {
     TRY(grow(c, c->qname_off, n1 + 2, n0 + 1)); TRY(grow(c, c->cigar_off, n1 + 2, n0 + 1)); TRY(grow(c, c->qual_off, n1 + 2, n0 + 1)); TRY(grow(c, c->seq_off, n1 + 2, n0 + 1));
     TRY(grow(c, c->scan_tmp, 4 * (bn + 4) + 8, 0));   // (the keep flags above are dead by now)
     BamArgs A{};
-    A.n = bn; A.n0 = n0; A.raw = c->bam_raw.p; A.start = d_start; A.n_bytes = n_bytes; A.chained = d_start == c->bam_off.p;
+    A.n = bn; A.n0 = n0; A.raw = c->bam_raw.p; A.start = d_start; A.n_bytes = n_bytes; A.chained = d_start == c->bam_off.p; A.clear_dup = c->clear_dup;
     A.refid = c->refid.p; A.pos = c->pos.p; A.nref = c->nref.p; A.pnext = c->pnext.p; A.tlen = c->tlen.p; A.rg = c->rg.p; A.flag = c->flag.p; A.mapq = c->mapq.p; A.optf = c->optf.p;
     A.len_qname = c->scan_tmp.p; A.len_cigar = c->scan_tmp.p + (bn + 4); A.len_seq = c->scan_tmp.p + 2 * (bn + 4); A.len_qual = c->scan_tmp.p + 3 * (bn + 4);
     A.rg_names = c->d_rg_names; A.rg_name_off = c->d_rg_name_off; A.n_rg = c->n_rg; A.n_contigs = c->n_contigs; A.err = c->d_err;
@@ -405,12 +482,51 @@ int bam_ingest_core(elp_ctx* c, uint64_t n_bytes, uint64_t nrec) {
     return ELP_OK;
 }
 
-static int bam_out_prepare(elp_ctx* c, uint64_t first, uint64_t n, uint64_t* total) {
+// The selection of the record filters: sel[j] is the output position of the j-th record that passes (in output order).  Built once per
+// sort and setting, on the first filtered fetch; without record bits there is none (sel null, every record passes).
+int out_select(elp_ctx* c, const uint32_t** sel, uint64_t* n_out) {
+    *sel = nullptr; *n_out = c->n;
+    if (!c->out_mask) return E_OK;
+    if (!c->out_sel_valid) {
+        const uint64_t n = c->n;
+        uint64_t kept = 0;
+        if (n) {
+            cudaStream_t s = c->stream;
+            TRY(grow(c, c->scan_tmp, n + 8, 0)); TRY(grow(c, c->off_stage, n + 2, 0)); TRY(grow(c, c->out_sel, n + 1, 0));
+            c->begin("out_select", 7.0 * (double)n);
+            out_select_kernel<<<nblk(n, 256), 256, 0, s>>>(n, c->out_mask, c->s_flag.p, c->s_optf.p, c->scan_tmp.p);
+            c->end(); LAUNCH_CHECK(c);
+            TRY(exclusive_scan_u32_to_u64(c, c->scan_tmp.p, c->off_stage.p, n));
+            c->begin("out_select", 12.0 * (double)n + 4.0 * (double)n);
+            out_compact_kernel<<<nblk(n, 256), 256, 0, s>>>(n, c->scan_tmp.p, c->off_stage.p, c->out_sel.p);
+            c->end(); LAUNCH_CHECK(c);
+            CUDA_TRY(c, cudaMemcpyAsync(&kept, c->off_stage.p + n, 8, cudaMemcpyDeviceToHost, s));
+            CUDA_TRY(c, cudaStreamSynchronize(s));
+        }
+        c->n_out = kept; c->out_sel_valid = true;
+    }
+    *sel = c->out_sel.p; *n_out = c->n_out;
+    return E_OK;
+}
+
+// record lengths of the call (without dropped fields when a field filter is set) scanned into off_stage[0..n], *total bytes
+static int bam_out_prepare(elp_ctx* c, uint64_t first, uint64_t n, uint64_t* total, const uint32_t** sel) {
     if (!c->sorted) return c->fail(E_STATE, "elp_fetch_bam before elp_sort_markdup");
     if (c->bam_reads != c->n) return c->fail(E_STATE, "elp_fetch_bam: not every read of this context came in through elp_append_bam");
-    if (first + n > c->n) return c->fail(E_INVAL, "elp_fetch_bam: range [%llu,%llu) exceeds %llu reads", (unsigned long long)first, (unsigned long long)(first + n), (unsigned long long)c->n);
+    uint64_t n_out = 0;
+    TRY(out_select(c, sel, &n_out));
+    if (first + n > n_out) {
+        if (*sel) return c->fail(E_INVAL, "elp_fetch_bam: range [%llu,%llu) exceeds the %llu output records that pass the record filters (elp_n_output)", (unsigned long long)first, (unsigned long long)(first + n), (unsigned long long)n_out);
+        return c->fail(E_INVAL, "elp_fetch_bam: range [%llu,%llu) exceeds %llu reads", (unsigned long long)first, (unsigned long long)(first + n), (unsigned long long)c->n);
+    }
     TRY(grow(c, c->scan_tmp, n + 8, 0)); TRY(grow(c, c->off_stage, n + 2, 0));
-    bam_out_len_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(n, c->perm.p + first, c->bam_all_off.p, c->bam_all.p, c->scan_tmp.p); c->launches++;
+    if (c->out_fields) {
+        c->begin("bam_out_fields_measure", (double)c->n_bam * (double)n / (double)std::max<uint64_t>(c->n, 1) + 4.0 * (double)n);
+        bam_out_fields_measure_kernel<<<nblk(n * 32, 256), 256, 0, c->stream>>>(n, first, *sel, c->perm.p, c->bam_all_off.p, c->bam_all.p, c->d_out_drop, c->scan_tmp.p);
+        c->end();
+    } else {
+        bam_out_len_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(n, first, *sel, c->perm.p, c->bam_all_off.p, c->bam_all.p, c->scan_tmp.p); c->launches++;
+    }
     LAUNCH_CHECK(c);
     TRY(exclusive_scan_u32_to_u64(c, c->scan_tmp.p, c->off_stage.p, n));
     CUDA_TRY(c, cudaMemcpyAsync(total, c->off_stage.p + n, 8, cudaMemcpyDeviceToHost, c->stream));
@@ -421,8 +537,8 @@ static int bam_out_prepare(elp_ctx* c, uint64_t first, uint64_t n, uint64_t* tot
 extern "C" uint64_t elp_fetch_bam_bytes(elp_ctx* c, uint64_t first, uint64_t n) {
     if (!c || n == 0) return 0;
     cudaSetDevice(c->device);
-    uint64_t total = 0;
-    if (bam_out_prepare(c, first, n, &total)) return 0;
+    uint64_t total = 0; const uint32_t* sel = nullptr;
+    if (bam_out_prepare(c, first, n, &total, &sel)) return 0;
     return total;
 }
 
@@ -431,13 +547,19 @@ extern "C" int elp_fetch_bam(elp_ctx* c, uint64_t first, uint64_t n, uint8_t* ou
     if (!c || (!out && n)) return ELP_EINVAL;
     cudaSetDevice(c->device);
     if (n == 0) { if (record_off) record_off[0] = 0; return ELP_OK; }
-    uint64_t total = 0;
-    TRY(bam_out_prepare(c, first, n, &total));
+    uint64_t total = 0; const uint32_t* sel = nullptr;
+    TRY(bam_out_prepare(c, first, n, &total, &sel));
     if (total > capacity) return c->fail(E_INVAL, "elp_fetch_bam: output buffer too small (%llu > %llu)", (unsigned long long)total, (unsigned long long)capacity);
     TRY(grow(c, c->bam_raw, total + 64, 0));      // staging for the formatted records
-    c->begin("bam_format", 2.0 * (double)total);
-    bam_out_copy_kernel<<<nblk(n * 32, 256), 256, 0, c->stream>>>(n, first, c->perm.p, c->bam_all_off.p, c->bam_all.p, c->off_stage.p, c->bam_raw.p, c->s_flag.p, c->s_out_off.p,
-                                                                  c->qual_out_valid ? c->qual_out.p : nullptr);
+    if (c->out_fields) {
+        c->begin("bam_out_fields_emit", (double)c->n_bam * (double)n / (double)std::max<uint64_t>(c->n, 1) + (double)total);
+        bam_out_fields_emit_kernel<<<nblk(n * 32, 256), 256, 0, c->stream>>>(n, first, sel, c->perm.p, c->bam_all_off.p, c->bam_all.p, c->d_out_drop, c->off_stage.p, c->bam_raw.p,
+                                                                             c->s_flag.p, c->s_out_off.p, c->qual_out_valid ? c->qual_out.p : nullptr);
+    } else {
+        c->begin("bam_format", 2.0 * (double)total);
+        bam_out_copy_kernel<<<nblk(n * 32, 256), 256, 0, c->stream>>>(n, first, sel, c->perm.p, c->bam_all_off.p, c->bam_all.p, c->off_stage.p, c->bam_raw.p, c->s_flag.p, c->s_out_off.p,
+                                                                      c->qual_out_valid ? c->qual_out.p : nullptr);
+    }
     c->end(); LAUNCH_CHECK(c);
     CUDA_TRY(c, cudaMemcpyAsync(out, c->bam_raw.p, total, cudaMemcpyDeviceToHost, c->stream));
     if (record_off) CUDA_TRY(c, cudaMemcpyAsync(record_off, c->off_stage.p, (n + 1) * 8, cudaMemcpyDeviceToHost, c->stream));
@@ -467,8 +589,45 @@ extern "C" int elp_set_target_regions(elp_ctx* c, int32_t contig, const int32_t*
 
 extern "C" int elp_set_ingest_filter(elp_ctx* c, uint32_t mask, int32_t min_mapq) {
     if (!c) return ELP_EINVAL;
-    if (mask & ~(uint32_t)(ELP_FILTER_UNMAPPED | ELP_FILTER_UNMAPPED_STRICT | ELP_FILTER_NON_EXACT | ELP_FILTER_DUPLICATES | ELP_FILTER_NON_EXACT_STRICT | ELP_FILTER_TARGET_REGIONS)) return c->fail(E_INVAL, "elp_set_ingest_filter: unknown filter bits 0x%x", mask);
-    c->filter_mask = mask; c->filter_min_mapq = min_mapq;
+    if (mask & ~(uint32_t)(ELP_FILTER_UNMAPPED | ELP_FILTER_UNMAPPED_STRICT | ELP_FILTER_NON_EXACT | ELP_FILTER_DUPLICATES | ELP_FILTER_NON_EXACT_STRICT | ELP_FILTER_TARGET_REGIONS | ELP_FILTER_CLEAR_DUPLICATE_FLAG)) return c->fail(E_INVAL, "elp_set_ingest_filter: unknown filter bits 0x%x", mask);
+    c->filter_mask = mask & ~(uint32_t)ELP_FILTER_CLEAR_DUPLICATE_FLAG; c->filter_min_mapq = min_mapq;   // (the clear drops no record)
+    c->clear_dup = (mask & ELP_FILTER_CLEAR_DUPLICATE_FLAG) != 0;
     return ELP_OK;
+}
+
+// a 2-byte tag string as its index in the tag table; -1 for any other length (it matches no field, as an interned symbol would not)
+static int32_t tag_index(const char* s) { return (s && s[0] && s[1] && !s[2]) ? (int32_t)((uint8_t)s[0] | ((uint32_t)(uint8_t)s[1] << 8)) : -1; }
+
+extern "C" int elp_set_output_filter(elp_ctx* c, uint32_t mask, const char* const* remove_tags, int32_t n_remove, const char* const* keep_tags, int32_t n_keep) {
+    if (!c) return ELP_EINVAL;
+    cudaSetDevice(c->device);
+    if (mask & ~(uint32_t)(ELP_OUT_REMOVE_DUPLICATES | ELP_OUT_REMOVE_OPTIONAL_READS | ELP_OUT_KEEP_FIELDS)) return c->fail(E_INVAL, "elp_set_output_filter: unknown filter bits 0x%x", mask);
+    if (n_remove < 0 || n_keep < 0 || (n_remove && !remove_tags) || (n_keep && !keep_tags)) return c->fail(E_INVAL, "elp_set_output_filter: bad tag list");
+    if (n_keep && !(mask & ELP_OUT_KEEP_FIELDS)) return c->fail(E_INVAL, "elp_set_output_filter: keep_tags without ELP_OUT_KEEP_FIELDS");
+    // one decision per tag: RemoveOptionalFields(remove_tags), then KeepOptionalFields(keep_tags) -- dropped by either, dropped
+    std::vector<uint32_t> drop(2048, 0u);
+    for (int32_t i = 0; i < n_remove; i++) { const int32_t t = tag_index(remove_tags[i]); if (t >= 0) drop[t >> 5] |= 1u << (t & 31); }
+    if (mask & ELP_OUT_KEEP_FIELDS) {
+        std::vector<uint32_t> keep(2048, 0u);
+        for (int32_t i = 0; i < n_keep; i++) { const int32_t t = tag_index(keep_tags[i]); if (t >= 0) keep[t >> 5] |= 1u << (t & 31); }
+        for (int w = 0; w < 2048; w++) drop[w] |= ~keep[w];
+    }
+    bool any = false;
+    for (uint32_t w : drop) any |= w != 0;
+    if (any) {
+        if (!c->d_out_drop) CUDA_TRY(c, cudaMalloc(&c->d_out_drop, 2048 * 4));
+        CUDA_TRY(c, cudaMemcpyAsync(c->d_out_drop, drop.data(), 2048 * 4, cudaMemcpyHostToDevice, c->stream));
+        CUDA_TRY(c, cudaStreamSynchronize(c->stream));   // (drop is pageable host memory)
+    }
+    c->out_mask = mask & ~(uint32_t)ELP_OUT_KEEP_FIELDS; c->out_fields = any; c->out_sel_valid = false;
+    return ELP_OK;
+}
+
+extern "C" uint64_t elp_n_output(elp_ctx* c) {
+    if (!c || !c->sorted) return 0;
+    cudaSetDevice(c->device);
+    const uint32_t* sel = nullptr; uint64_t n_out = 0;
+    if (out_select(c, &sel, &n_out)) return 0;
+    return n_out;
 }
 extern "C" uint64_t elp_n_filtered(const elp_ctx* c) { return c ? c->n_filtered : 0; }

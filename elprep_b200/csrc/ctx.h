@@ -105,7 +105,12 @@ struct elp_ctx {
     DBuf<uint8_t> bam_raw; DBuf<uint64_t> bam_off;   // staging of elp_append_bam: raw records and their offsets
     DBuf<uint8_t> bam_all; DBuf<uint64_t> bam_all_off; uint64_t n_bam = 0, bam_reads = 0;   // all raw records (for elp_fetch_bam) and the start of every read's record
     DBuf<uint64_t> bam_start;                 // starts of the records that pass the ingest filters
-    uint32_t filter_mask = 0; int32_t filter_min_mapq = 0; uint64_t n_filtered = 0;   // elp_set_ingest_filter
+    uint32_t filter_mask = 0; int32_t filter_min_mapq = 0; uint64_t n_filtered = 0;   // elp_set_ingest_filter (record predicates)
+    bool clear_dup = false;                   // elp_set_ingest_filter ELP_FILTER_CLEAR_DUPLICATE_FLAG: 0x400 cleared in the FLAG column at ingest
+    // write-phase filters of elp_fetch_bam / elp_fetch_sam (elp_set_output_filter; survive elp_reset)
+    uint32_t out_mask = 0;                    // record bits (ELP_OUT_REMOVE_DUPLICATES, ELP_OUT_REMOVE_OPTIONAL_READS)
+    uint32_t* d_out_drop = nullptr; bool out_fields = false;   // 65 536-bit tag table (bit set: the field is dropped); out_fields: some bit is set
+    DBuf<uint32_t> out_sel; uint64_t n_out = 0; bool out_sel_valid = false;   // output positions of the records that pass, built on first use
     std::vector<int32_t*> d_regions; std::vector<uint64_t> n_regions; const int32_t** d_region_ptrs = nullptr; uint64_t* d_n_regions = nullptr; bool regions_dirty = true;   // target regions (BED) of RemoveNonOverlappingReads
     uint64_t n_cleaned = 0;                  // reads whose CIGAR elp_clean_sam rewrote
     bool has_contig_names = false;           // elp_config.contig_names was given (elp_append_sam resolves RNAME / RNEXT against it)
@@ -253,5 +258,6 @@ int spread_exchange_end(elp_ctx* c);
 int exclusive_scan_u64_from_u32(elp_ctx* c, const uint32_t* in, uint64_t* out, uint64_t n, uint64_t base);   // out[n+1], out[0] = base
 int qual_presence_update(elp_ctx* c, uint64_t first_byte, uint64_t n_bytes);   // api.cu: called by both ingest paths
 int bam_ingest_core(elp_ctx* c, uint64_t n_bytes, uint64_t nrec);   // bam_ingest.cu: records staged in bam_raw / bam_off -> reads (elp_append_bam, elp_append_sam)
+int out_select(elp_ctx* c, const uint32_t** sel, uint64_t* n_out);   // bam_ingest.cu: the record filters' selection (sel null and n_out = n without record bits)
 void sam_state_release(elp_ctx* c);   // sam_ingest.cu
 void sam_out_release(elp_ctx* c);     // sam_format.cu

@@ -16,6 +16,7 @@
 #include "ctx.h"
 #include "gofloat.hpp"
 #include "pool.hpp"
+#include "tagwalk.cuh"
 #include "../../include/elprep_b200.h"
 
 struct SamOutState {
@@ -48,7 +49,9 @@ enum { FM_MEASURE = 0, FM_LIST = 1, FM_EMIT = 2 };
 enum : unsigned long long { FE_CIGAR_OP = 1, FE_LINE_LIMIT = 2 };
 
 struct FmtArgs {
-    uint64_t n, first;                                                    // lines [first, first + n) of the output order
+    uint64_t n, first;                                                    // lines [first, first + n) of the output order (of sel when sel is set)
+    const uint32_t* sel;                                                  // output positions of the records the record filters keep, or null
+    const uint32_t* drop;                                                 // 65 536-bit tag table of the field filter, or null
     const uint32_t* perm; const uint64_t* all_start; const uint8_t* all;
     const uint16_t* flag; const uint64_t* qoff; const uint8_t* qual;      // qual: recalibrated QUAL in output order, or null (stored QUAL)
     const uint8_t* names; const uint32_t* name_off; const int32_t* canon; int n_contigs;   // canon[n_contigs]: the canon of "*" (-1 if no @SQ has that name)
@@ -106,16 +109,6 @@ template <class F> __device__ __forceinline__ void warp_map(uint8_t* dst, const 
     if (t0 + lane < n) dst[t0 + lane] = (uint8_t)f((uint32_t)src[t0 + lane]);
 }
 
-// first NUL at or after `from` (the ingest checked that there is one before n)
-__device__ __forceinline__ uint64_t find_nul(const uint8_t* p, uint64_t from, uint64_t n) {
-    const unsigned lane = threadIdx.x & 31;
-    for (uint64_t b = from; b < n; b += 32) {
-        const unsigned m = __ballot_sync(FULL_MASK, b + lane < n && p[b + lane] == 0);
-        if (m) return b + __ffs(m) - 1;
-    }
-    return n;
-}
-
 // name of contig id, or "*" for id < 0
 __device__ __forceinline__ const uint8_t* name_of(const FmtArgs& A, int32_t id, uint32_t* len) {
     if (id < 0) { *len = 1; return reinterpret_cast<const uint8_t*>("*"); }
@@ -136,7 +129,7 @@ template <int M> __device__ __forceinline__ int float_text(const FmtArgs& A, uin
 template <int M> __device__ void format_line(const FmtArgs& A, uint64_t kk, const uint8_t* tbl) {
     constexpr bool W = M == FM_EMIT;
     const unsigned lane = threadIdx.x & 31;
-    const uint64_t k = A.first + kk;
+    const uint64_t k = A.sel ? A.sel[A.first + kk] : A.first + kk;
     const uint8_t* r = A.all + A.all_start[A.perm[k]];
     const uint64_t rec = (uint64_t)rd32(r) + 4;
     const uint32_t l_name = r[12], mapq = r[13], ncig = rd16(r + 16), flag = A.flag[k];
@@ -204,6 +197,8 @@ template <int M> __device__ void format_line(const FmtArgs& A, uint64_t kk, cons
     uint64_t fj = 0;                                                      // float values of this line so far
     while (t + 3 <= rec) {
         const uint8_t t0 = r[t], t1 = r[t + 1], ty = r[t + 2];
+        const uint64_t fe = tagwalk::field_end(r, t, rec);
+        if (A.drop && tagwalk::dropped(A.drop, t0, t1)) { t = fe; continue; }   // no text, no float slot
         t += 3;
         const bool integer = ty == 'c' || ty == 'C' || ty == 's' || ty == 'S' || ty == 'i' || ty == 'I';
         if (W && lane == 0) { o[x] = '\t'; o[x + 1] = t0; o[x + 2] = t1; o[x + 3] = ':'; o[x + 4] = integer ? 'i' : ty; o[x + 5] = ':'; }
@@ -229,16 +224,16 @@ template <int M> __device__ void format_line(const FmtArgs& A, uint64_t kk, cons
             if (lane == 0) fl = float_text<M>(A, fb + fj, rd32(r + t), W ? o + x : nullptr);
             x += __shfl_sync(FULL_MASK, fl, 0); t += 4; fj++;
         } else if (ty == 'Z' || ty == 'H') {                              // H: the stored hex digits in lower case (AppendUint(b, 16))
-            const uint64_t e = find_nul(r, t, rec), n = e - t;
+            const uint64_t n = fe - 1 - t;
             if (W) { if (ty == 'Z') warp_map(o + x, r + t, n, Ident()); else warp_map(o + x, r + t, n, Lower()); }
-            x += n; t = e + 1;
+            x += n; t = fe;
         } else if (ty == 'B') {                                           // subtype, then ","value per element over the warp
             const uint8_t sub = r[t];
             const uint32_t cnt = rd32(r + t + 1);
             t += 5;
             if (W && lane == 0) o[x] = sub;
             x += 1;
-            const int es = (sub == 'c' || sub == 'C') ? 1 : ((sub == 's' || sub == 'S') ? 2 : 4);
+            const int es = tagwalk::elem_size(sub);
             for (uint32_t e0 = 0; e0 < cnt; e0 += 32) {
                 const uint32_t e = e0 + lane;
                 int len = 0; int64_t v = 0;
@@ -264,7 +259,7 @@ template <int M> __device__ void format_line(const FmtArgs& A, uint64_t kk, cons
                 x += tot;
             }
             if (sub == 'f') fj += cnt;
-            t += (uint64_t)es * cnt;
+            t = fe;
         } else break;                                                     // (the ingest accepted no other type)
     }
     x += 1;
@@ -317,25 +312,30 @@ int sam_out_tables(elp_ctx* c) {
     return E_OK;
 }
 
-// the refusals of elp_fetch_sam and elp_fetch_sam_bytes (no device work)
-int sam_out_check(elp_ctx* c, uint64_t first, uint64_t n) {
+// the refusals of elp_fetch_sam and elp_fetch_sam_bytes (no device work but the record filters' selection); *sel: that selection or null
+int sam_out_check(elp_ctx* c, uint64_t first, uint64_t n, const uint32_t** sel) {
     if (!c->sorted) return c->fail(E_STATE, "elp_fetch_sam before elp_sort_markdup");
     if (c->bam_reads != c->n) return c->fail(E_STATE, "elp_fetch_sam: not every read of this context came in through elp_append_bam or elp_append_sam");
     if (c->n_cleaned) return c->fail(E_STATE, "elp_fetch_sam: elp_clean_sam rewrote %llu CIGARs; the stored records still carry the old ones (use elp_fetch)", (unsigned long long)c->n_cleaned);
     if (c->n_contigs > 0 && !c->has_contig_names) return c->fail(E_INVAL, "elp_fetch_sam: the context was created without elp_config.contig_names, so RNAME / RNEXT cannot be written");
     if (c->n_sam_lost_names) return c->fail(E_STATE, "elp_fetch_sam: %llu SAM lines of this context have an RNAME or RNEXT that is not an @SQ name (or RNEXT '=' with such an RNAME); their stored records cannot reproduce it (use elp_fetch_bam)", (unsigned long long)c->n_sam_lost_names);
-    if (first + n > c->n) return c->fail(E_INVAL, "elp_fetch_sam: range [%llu,%llu) exceeds %llu reads", (unsigned long long)first, (unsigned long long)(first + n), (unsigned long long)c->n);
+    uint64_t n_out = 0;
+    TRY(out_select(c, sel, &n_out));
+    if (first + n > n_out) {
+        if (*sel) return c->fail(E_INVAL, "elp_fetch_sam: range [%llu,%llu) exceeds the %llu output records that pass the record filters (elp_n_output)", (unsigned long long)first, (unsigned long long)(first + n), (unsigned long long)n_out);
+        return c->fail(E_INVAL, "elp_fetch_sam: range [%llu,%llu) exceeds %llu reads", (unsigned long long)first, (unsigned long long)(first + n), (unsigned long long)c->n);
+    }
     return E_OK;
 }
 
 // measure (and the float step): line lengths scanned into off_stage[0..n], *total bytes; A is left ready for the emit pass
-int sam_out_prepare(elp_ctx* c, uint64_t first, uint64_t n, uint64_t* total, FmtArgs* Aout) {
+int sam_out_prepare(elp_ctx* c, uint64_t first, uint64_t n, const uint32_t* sel, uint64_t* total, FmtArgs* Aout) {
     TRY(sam_out_tables(c));
     SamOutState& S = *c->sam_out;
     cudaStream_t s = c->stream;
     TRY(grow(c, c->scan_tmp, n + 8, 0)); TRY(grow(c, c->off_stage, n + 2, 0)); TRY(grow(c, S.nf, n + 8, 0));
     FmtArgs A{};
-    A.n = n; A.first = first; A.perm = c->perm.p; A.all_start = c->bam_all_off.p; A.all = c->bam_all.p;
+    A.n = n; A.first = first; A.sel = sel; A.drop = c->out_fields ? c->d_out_drop : nullptr; A.perm = c->perm.p; A.all_start = c->bam_all_off.p; A.all = c->bam_all.p;
     A.flag = c->s_flag.p; A.qoff = c->s_out_off.p; A.qual = c->qual_out_valid ? c->qual_out.p : nullptr;
     A.names = S.d_names; A.name_off = S.d_name_off; A.canon = S.d_canon; A.n_contigs = c->n_contigs;
     A.len = c->scan_tmp.p; A.nf = S.nf.p; A.small = S.d_small;
@@ -389,19 +389,21 @@ int sam_out_prepare(elp_ctx* c, uint64_t first, uint64_t n, uint64_t* total, Fmt
 extern "C" uint64_t elp_fetch_sam_bytes(elp_ctx* c, uint64_t first, uint64_t n) {
     if (!c || n == 0) return 0;
     cudaSetDevice(c->device);
-    if (sam_out_check(c, first, n)) return 0;
+    const uint32_t* sel = nullptr;
+    if (sam_out_check(c, first, n, &sel)) return 0;
     uint64_t total = 0; FmtArgs A;
-    if (sam_out_prepare(c, first, n, &total, &A)) return 0;
+    if (sam_out_prepare(c, first, n, sel, &total, &A)) return 0;
     return total;
 }
 
 extern "C" int elp_fetch_sam(elp_ctx* c, uint64_t first, uint64_t n, char* out, uint64_t capacity, uint64_t* line_off) {
     if (!c || (!out && n)) return ELP_EINVAL;
     cudaSetDevice(c->device);
-    TRY(sam_out_check(c, first, n));
+    const uint32_t* sel = nullptr;
+    TRY(sam_out_check(c, first, n, &sel));
     if (n == 0) { if (line_off) line_off[0] = 0; return ELP_OK; }
     uint64_t total = 0; FmtArgs A;
-    TRY(sam_out_prepare(c, first, n, &total, &A));
+    TRY(sam_out_prepare(c, first, n, sel, &total, &A));
     if (total > capacity) return c->fail(E_INVAL, "elp_fetch_sam: output buffer too small (%llu > %llu)", (unsigned long long)total, (unsigned long long)capacity);
     TRY(grow(c, c->bam_raw, total + 64, 0));                              // staging of the text
     A.out = c->bam_raw.p;

@@ -115,6 +115,26 @@ class Context:
     def set_ingest_filter(self, mask=0, min_mapq=0):
         self._ck(self.L.elp_set_ingest_filter(self.h, mask, min_mapq))
 
+    def set_output_filter(self, mask=0, remove=(), keep=None):
+        """the write-phase filters of fetch_bam / fetch_sam (elp_set_output_filter): mask of _lib.OUT_REMOVE_DUPLICATES and
+        _lib.OUT_REMOVE_OPTIONAL_READS; remove: RemoveOptionalFields tags; keep: KeepOptionalFields tags ([] keeps none, None: no keep filter)"""
+        remove = [t.encode() if isinstance(t, str) else bytes(t) for t in remove]
+        if keep is not None:
+            mask |= _lib.OUT_KEEP_FIELDS
+        keep = [t.encode() if isinstance(t, str) else bytes(t) for t in (keep or ())]
+        ra, ka = (C.c_char_p * max(1, len(remove)))(*remove), (C.c_char_p * max(1, len(keep)))(*keep)
+        self._ck(self.L.elp_set_output_filter(self.h, mask, ra, len(remove), ka, len(keep)))
+
+    def n_output(self):
+        """output records fetch_bam / fetch_sam write (those that pass the record filters of set_output_filter); 0 before sort_markdup"""
+        return int(self.L.elp_n_output(self.h))
+
+    def _n_out(self, first):
+        k = self.n_output()
+        if k == 0 and self.L.elp_fetch_opt_flags(self.h, 0, 0, None) != 0:
+            k = self.n                                                    # before sort_markdup: the fetch reports the refusal
+        return k - first
+
     def set_target_regions(self, contig, start_end, already_flat=False):
         se = np.ascontiguousarray(start_end, dtype=np.int32).reshape(-1)
         self._ck(self.L.elp_set_target_regions(self.h, contig, _vp(se) if se.size else None, se.size // 2, int(already_flat)))
@@ -293,8 +313,9 @@ class Context:
         return idx, flag, qoff, qual
 
     def fetch_bam(self, first=0, n=None):
-        """-> (uint8 record bytes, uint64 record offsets [n+1]) of output records [first, first+n), FLAG and QUAL patched"""
-        n = self.n - first if n is None else n
+        """-> (uint8 record bytes, uint64 record offsets [n+1]) of output records [first, first+n) (of those that pass the output filter),
+        FLAG and QUAL patched"""
+        n = self._n_out(first) if n is None else n
         nb = int(self.L.elp_fetch_bam_bytes(self.h, first, n))
         out, off = np.empty(max(nb, 1), np.uint8), np.empty(n + 1, np.uint64)
         self._ck(self.L.elp_fetch_bam(self.h, first, n, _vp(out), out.size, _vp(off)))
@@ -302,8 +323,8 @@ class Context:
 
     def fetch_sam(self, first=0, n=None):
         """-> (uint8 SAM text, uint64 line offsets [n+1]) of output records [first, first+n): FormatAlignment of each stored record with
-        FLAG and QUAL patched, one '\\n'-terminated alignment line per record, no header"""
-        n = self.n - first if n is None else n
+        FLAG and QUAL patched, one '\\n'-terminated alignment line per record, no header (records as in fetch_bam)"""
+        n = self._n_out(first) if n is None else n
         nb = int(self.L.elp_fetch_sam_bytes(self.h, first, n)) if n else 0
         out, off = np.empty(max(nb, 1), np.uint8), np.empty(n + 1, np.uint64)
         self._ck(self.L.elp_fetch_sam(self.h, first, n, _vp(out), out.size, _vp(off)))

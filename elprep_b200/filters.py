@@ -145,6 +145,41 @@ def RemoveDuplicateReads(header):
     return lambda batch: _keep(batch, (batch.flag & sam.Duplicate) == 0)
 
 
+def ClearDuplicateFlag(header):
+    """filters.ClearDuplicateFlag (simple-filters.go:350-355): 0x400 cleared in every read, before marking.  With elp_append_bam /
+    elp_append_sam the device does it at ingest (_lib.FILTER_CLEAR_DUPLICATE_FLAG)."""
+    def flt(batch):
+        batch.flag = (batch.flag & ~np.uint16(sam.Duplicate)).astype(np.uint16)
+        return batch
+    return flt
+
+
+def write_phase_filters(removeDuplicates=False, removeOptionalFields="", keepOptionalFields="", header_has_sr=False):
+    """the write-phase flags of `elprep filter` as the arguments of Context.set_output_filter / elp_set_output_filter -> (mask, remove, keep),
+    as cmd/filter.go:803-902 builds them: RemoveOptionalReads iff the header has @sr (the caller drops @sr from the header it writes);
+    --remove-duplicates; --remove-optional-fields "all" is KeepOptionalFields(nil), else RemoveOptionalFields of the comma-split, trimmed list;
+    --keep-optional-fields "none" is KeepOptionalFields(nil), else KeepOptionalFields of the list.  "all" / "none" are compared untrimmed, as
+    there.  keep is None without a keep filter; mask carries _lib.OUT_KEEP_FIELDS when keep is a list.  Two keep filters in a row keep
+    what both keep, so remove "all" with any keep list keeps nothing."""
+    from . import _lib
+    mask, remove, keep = 0, [], None
+    if header_has_sr:
+        mask |= _lib.OUT_REMOVE_OPTIONAL_READS
+    if removeDuplicates:
+        mask |= _lib.OUT_REMOVE_DUPLICATES
+    if removeOptionalFields != "":
+        if removeOptionalFields == "all":
+            keep = []
+        else:
+            remove = [t.strip() for t in removeOptionalFields.split(",")]
+    if keepOptionalFields != "":
+        tags = [] if keepOptionalFields == "none" else [t.strip() for t in keepOptionalFields.split(",")]
+        keep = tags if keep is None else [t for t in keep if t in tags]
+    if keep is not None:
+        mask |= _lib.OUT_KEEP_FIELDS
+    return mask, remove, keep
+
+
 def MarkDuplicates(alsoOpticals):
     """filters.MarkDuplicates (filters/mark-duplicates.go:406-445). Returns (filter, fragments, pairs); the two maps live on
     the device and are only handles here."""

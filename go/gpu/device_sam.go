@@ -317,6 +317,21 @@ func (d *DeviceSam) PrintDuplicatesMetrics(path, commandLine, startedOn string) 
 	check(d.ctx, C.elp_print_duplicates_metrics(d.ctx, p, c, s))
 }
 
+// SetOutputFilter: the write-phase filters of elp_fetch_bam / elp_fetch_sam (filters2 of cmd/filter.go:803-902, and RemoveOptionalReads).
+// mask: C.ELP_OUT_REMOVE_DUPLICATES (--remove-duplicates), C.ELP_OUT_REMOVE_OPTIONAL_READS (the header has @sr; drop @sr from the header
+// written).  remove: the --remove-optional-fields tags; keep: the --keep-optional-fields tags, with keepFilter false for no keep filter
+// ("all" / "none" are keepFilter with an empty keep).  The columnar RunPipeline above runs filters2 on the host and ignores this setting.
+func (d *DeviceSam) SetOutputFilter(mask uint32, remove []string, keep []string, keepFilter bool) {
+	cRemove, f1 := cstrings(remove, nil)
+	cKeep, f2 := cstrings(keep, nil)
+	defer f1()
+	defer f2()
+	if keepFilter {
+		mask |= C.ELP_OUT_KEEP_FIELDS
+	}
+	check(d.ctx, C.elp_set_output_filter(d.ctx, C.uint32_t(mask), cRemove, C.int32_t(len(remove)), cKeep, C.int32_t(len(keep))))
+}
+
 // SetReference / SetKnownSites: the side inputs of filters.NewBaseRecalibrator (bqsr.go:424-443).
 func (d *DeviceSam) SetReference(contig int, bases []byte) {
 	check(d.ctx, C.elp_set_reference(d.ctx, C.int32_t(contig), (*C.uint8_t)(unsafe.Pointer(&bases[0])), C.uint64_t(len(bases))))

@@ -148,6 +148,9 @@ int elp_append_sam(elp_ctx *ctx, const char *text, uint64_t n_bytes);
 #define ELP_FILTER_DUPLICATES 8u
 #define ELP_FILTER_NON_EXACT_STRICT 16u   /* RemoveNonExactMappingReadsStrict (:115-136): optional fields X0 = 1, X1 = XM = XO = XG = 0 must all be present */
 #define ELP_FILTER_TARGET_REGIONS 32u     /* RemoveNonOverlappingReads (:310-328): keep reads whose [POS, End()] overlaps a region of elp_set_target_regions */
+#define ELP_FILTER_CLEAR_DUPLICATE_FLAG 64u   /* ClearDuplicateFlag (:350-355): 0x400 cleared in the FLAG column at ingest, before marking; drops no record.
+                                               * ELP_FILTER_DUPLICATES still tests the FLAG the record comes in with.  With elp_append_batch the
+                                               * marshaller clears the bit in the batch's FLAG column (filters.ClearDuplicateFlag), as for the other filters. */
 /* regions of one contig as (start, end) pairs, the Start / End of the BED records as the reference's bed parser stores them; sorted by
  * start and flattened inside unless already_flat (intervals.FromBed + ParallelSortByStart + ParallelFlatten, filters/simple-filters.go:311-315) */
 int elp_set_target_regions(elp_ctx *ctx, int32_t contig, const int32_t *start_end_pairs, uint64_t n_intervals, int already_flat);
@@ -278,6 +281,25 @@ int elp_fetch_bam(elp_ctx *ctx, uint64_t first, uint64_t n, uint8_t *out, uint64
  * such an RNAME; elp_last_error gives their number); ELP_EBAM for a CIGAR operation code above 8.  elp_fetch_sam_bytes returns 0 on error. */
 uint64_t elp_fetch_sam_bytes(elp_ctx *ctx, uint64_t first, uint64_t n);
 int elp_fetch_sam(elp_ctx *ctx, uint64_t first, uint64_t n, char *out, uint64_t capacity, uint64_t *line_off);
+/* Write-phase filters (the filters2 of `elprep filter`, cmd/filter.go:803-902, and RemoveOptionalReads): applied by elp_fetch_bam,
+ * elp_fetch_bam_bytes, elp_fetch_sam and elp_fetch_sam_bytes only.  elp_fetch, elp_fetch_async, elp_fetch_qual_bytes and elp_fetch_opt_flags
+ * are unchanged: a columnar caller owns its *Alignments and runs filters2 itself.
+ *  - Record selection.  With a record bit set, [first, first+n) of those four calls indexes the output records that pass, in output order
+ *    (elp_n_output of them); record_off / line_off describe the records written.  With no record bit the calls behave as without a filter.
+ *  - Field filter.  One decision per tag: remove_tags (RemoveOptionalFields, :235-257; active iff n_remove > 0) first, then keep_tags
+ *    (KeepOptionalFields, :261-288; active iff ELP_OUT_KEEP_FIELDS, n_keep == 0 drops every optional field), the order in which filters2
+ *    appends them.  A string matches the 2-byte tag when it equals it, case-sensitively; a string that is not 2 bytes long (also "") matches
+ *    no field.  Repeated tags are all dropped or all kept (SmallMap.DeleteIf).  The fields that remain keep their bytes and their order;
+ *    block_size is rewritten; FLAG and QUAL are patched as without a filter.  "all" / "none" and TrimSpace belong to the caller's flag parsing.
+ *  - Lifetime.  The setting survives elp_reset, like the ingest filter; the selection is rebuilt after elp_sort_markdup, elp_set_output_filter
+ *    or elp_reset.  Unknown mask bits, and keep_tags without ELP_OUT_KEEP_FIELDS, are ELP_EINVAL.  A range past elp_n_output is ELP_EINVAL and
+ *    nothing is written; the other refusals of the fetch calls still apply (before elp_sort_markdup, after elp_clean_sam, ...). */
+#define ELP_OUT_REMOVE_DUPLICATES     1u  /* RemoveDuplicateReads (filters/simple-filters.go:138-140) on the FLAG after elp_sort_markdup */
+#define ELP_OUT_REMOVE_OPTIONAL_READS 2u  /* RemoveOptionalReads (:146-152): reads with ELP_OPT_SR; the caller sets it iff the header has @sr (and drops @sr from the header it writes) */
+#define ELP_OUT_KEEP_FIELDS           4u  /* KeepOptionalFields(keep_tags) (:261-288); n_keep == 0 drops every optional field */
+int elp_set_output_filter(elp_ctx *ctx, uint32_t mask, const char *const *remove_tags, int32_t n_remove, const char *const *keep_tags, int32_t n_keep);
+/* after elp_sort_markdup: the number of output records that pass the record filters (elp_n_reads without them); 0 on error or before the sort */
+uint64_t elp_n_output(elp_ctx *ctx);
 int elp_debug_adapt(elp_ctx *ctx, int32_t *upos, int32_t *score);
 /* opt_flags of output records [first, first+n) (what filters.RemoveOptionalReads looks at when the worker writes its output) */
 int elp_fetch_opt_flags(elp_ctx *ctx, uint64_t first, uint64_t n, uint8_t *opt_flags);
