@@ -550,14 +550,28 @@ int elp_kernel_stats(elp_ctx* c, elp_kernel_stat* out, int cap) {
     return k;
 }
 
-int elp_debug_sort_u64(elp_ctx* c, uint64_t* keys, uint32_t* vals, uint64_t n, int key_bits) {
+int elp_debug_join_hash(elp_ctx* c, uint64_t* qhash) {
+    if (!c) return ELP_EINVAL;
+    cudaSetDevice(c->device);
+    TRY(phase_adapt(c));
+    if (qhash) CUDA_TRY(c, cudaMemcpyAsync(qhash, c->qhash.p, c->n * 8, cudaMemcpyDeviceToHost, c->stream));
+    CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+    return ELP_OK;
+}
+
+int elp_debug_sort_u64(elp_ctx* c, uint64_t* keys, uint32_t* vals, uint64_t n, int key_bits) { return elp_debug_sort_u64_range(c, keys, vals, n, 0, key_bits); }
+int elp_debug_sort_u128(elp_ctx* c, uint64_t* keys_hi, uint64_t* keys_lo, uint32_t* vals, uint64_t n, int key_bits) {
+    return elp_debug_sort_u128_range(c, keys_hi, keys_lo, vals, n, 0, key_bits);
+}
+
+int elp_debug_sort_u64_range(elp_ctx* c, uint64_t* keys, uint32_t* vals, uint64_t n, int lo_bit, int key_bits) {
     if (!c) return ELP_EINVAL;
     cudaSetDevice(c->device);
     TRY(grow(c, c->keys_a, n + 4, 0)); TRY(grow(c, c->keys_b, n + 4, 0)); TRY(grow(c, c->vals_a, n + 4, 0)); TRY(grow(c, c->vals_b, n + 4, 0));
     CUDA_TRY(c, cudaMemcpyAsync(c->keys_a.p, keys, n * 8, cudaMemcpyHostToDevice, c->stream));
     CUDA_TRY(c, cudaMemcpyAsync(c->vals_a.p, vals, n * 4, cudaMemcpyHostToDevice, c->stream));
     bool in_b = false;
-    TRY(radix_sort_u64(c, c->keys_a.p, c->keys_b.p, c->vals_a.p, c->vals_b.p, n, key_bits, &in_b, "u64"));
+    TRY(radix_sort_u64(c, c->keys_a.p, c->keys_b.p, c->vals_a.p, c->vals_b.p, n, key_bits, &in_b, "u64", lo_bit));
     CUDA_TRY(c, cudaMemcpyAsync(keys, in_b ? c->keys_b.p : c->keys_a.p, n * 8, cudaMemcpyDeviceToHost, c->stream));
     CUDA_TRY(c, cudaMemcpyAsync(vals, in_b ? c->vals_b.p : c->vals_a.p, n * 4, cudaMemcpyDeviceToHost, c->stream));
     CUDA_TRY(c, cudaStreamSynchronize(c->stream));
@@ -567,7 +581,7 @@ int elp_debug_sort_u64(elp_ctx* c, uint64_t* keys, uint32_t* vals, uint64_t n, i
     return ELP_OK;
 }
 
-int elp_debug_sort_u128(elp_ctx* c, uint64_t* keys_hi, uint64_t* keys_lo, uint32_t* vals, uint64_t n, int key_bits) {
+int elp_debug_sort_u128_range(elp_ctx* c, uint64_t* keys_hi, uint64_t* keys_lo, uint32_t* vals, uint64_t n, int lo_bit, int key_bits) {
     if (!c) return ELP_EINVAL;
     cudaSetDevice(c->device);
     TRY(grow(c, c->keys_a, 2 * n + 4, 0)); TRY(grow(c, c->keys_b, 2 * n + 4, 0)); TRY(grow(c, c->vals_a, n + 4, 0)); TRY(grow(c, c->vals_b, n + 4, 0));
@@ -576,7 +590,7 @@ int elp_debug_sort_u128(elp_ctx* c, uint64_t* keys_hi, uint64_t* keys_lo, uint32
     CUDA_TRY(c, cudaMemcpyAsync(c->keys_a.p, inter.data(), n * 16, cudaMemcpyHostToDevice, c->stream));
     CUDA_TRY(c, cudaMemcpyAsync(c->vals_a.p, vals, n * 4, cudaMemcpyHostToDevice, c->stream));
     bool in_b = false;
-    TRY(radix_sort_u128(c, c->keys_a.p, c->keys_b.p, c->vals_a.p, c->vals_b.p, n, key_bits, &in_b, "u128"));
+    TRY(radix_sort_u128(c, c->keys_a.p, c->keys_b.p, c->vals_a.p, c->vals_b.p, n, key_bits, &in_b, "u128", lo_bit));
     CUDA_TRY(c, cudaMemcpyAsync(inter.data(), in_b ? c->keys_b.p : c->keys_a.p, n * 16, cudaMemcpyDeviceToHost, c->stream));
     CUDA_TRY(c, cudaMemcpyAsync(vals, in_b ? c->vals_b.p : c->vals_a.p, n * 4, cudaMemcpyDeviceToHost, c->stream));
     CUDA_TRY(c, cudaStreamSynchronize(c->stream));

@@ -357,15 +357,28 @@ class Context:
         k = self.L.elp_kernel_stats(self.h, arr, 64)
         return {arr[i].name.decode(): dict(launches=int(arr[i].launches), ms=float(arr[i].ms), alg_bytes=float(arr[i].alg_bytes)) for i in range(k)}
 
-    def debug_sort_u64(self, keys, vals, key_bits):
+    def debug_join_hash(self):
+        """per read, the (library, QNAME) hash of the mate join (0 for reads that are not true pairs)"""
+        q = np.zeros(self.n, np.uint64)
+        self._ck(self.L.elp_debug_join_hash(self.h, _vp(q)))
+        return q
+
+    def debug_sort_u64(self, keys, vals, key_bits, lo_bit=None):
+        """stable sort by bits [lo_bit, lo_bit + key_bits) (lo_bit None: the call without a range)"""
         keys = np.ascontiguousarray(keys, dtype=np.uint64).copy()
         vals = np.ascontiguousarray(vals, dtype=np.uint32).copy()
-        self._ck(self.L.elp_debug_sort_u64(self.h, _vp(keys), _vp(vals), keys.size, key_bits))
+        if lo_bit is None:
+            self._ck(self.L.elp_debug_sort_u64(self.h, _vp(keys), _vp(vals), keys.size, key_bits))
+        else:
+            self._ck(self.L.elp_debug_sort_u64_range(self.h, _vp(keys), _vp(vals), keys.size, lo_bit, key_bits))
         return keys, vals
 
-    def debug_sort_u128(self, hi, lo, vals, key_bits):
+    def debug_sort_u128(self, hi, lo, vals, key_bits, lo_bit=None):
         hi = np.ascontiguousarray(hi, dtype=np.uint64).copy()
         lo = np.ascontiguousarray(lo, dtype=np.uint64).copy()
         vals = np.ascontiguousarray(vals, dtype=np.uint32).copy()
-        self._ck(self.L.elp_debug_sort_u128(self.h, _vp(hi), _vp(lo), _vp(vals), hi.size, key_bits))
+        if lo_bit is None:
+            self._ck(self.L.elp_debug_sort_u128(self.h, _vp(hi), _vp(lo), _vp(vals), hi.size, key_bits))
+        else:
+            self._ck(self.L.elp_debug_sort_u128_range(self.h, _vp(hi), _vp(lo), _vp(vals), hi.size, lo_bit, key_bits))
         return hi, lo, vals

@@ -301,6 +301,9 @@ int elp_set_output_filter(elp_ctx *ctx, uint32_t mask, const char *const *remove
 /* after elp_sort_markdup: the number of output records that pass the record filters (elp_n_reads without them); 0 on error or before the sort */
 uint64_t elp_n_output(elp_ctx *ctx);
 int elp_debug_adapt(elp_ctx *ctx, int32_t *upos, int32_t *score);
+/* per read, the 64-bit (library, QNAME) hash duplicate marking joins mates by (its low 31 bits are the join key); 0 for a read that is
+ * not a true pair (unmapped, secondary, supplementary, unpaired or mate unmapped) */
+int elp_debug_join_hash(elp_ctx *ctx, uint64_t *qhash);
 /* opt_flags of output records [first, first+n) (what filters.RemoveOptionalReads looks at when the worker writes its output) */
 int elp_fetch_opt_flags(elp_ctx *ctx, uint64_t first, uint64_t n, uint8_t *opt_flags);
 /* arrival-order CIGARs as the context holds them (after elp_clean_sam), for parity tests: cigar_off[n+1] relative to the first operation */
@@ -331,6 +334,10 @@ int elp_timer_stop(elp_ctx *ctx, double *elapsed_ms);    /* synchronizes */
  * stable LSD sort of n 64-bit keys (only the low key_bits are significant) carrying 32-bit values. Host buffers. ---- */
 int elp_debug_sort_u64(elp_ctx *ctx, uint64_t *keys, uint32_t *vals, uint64_t n, int key_bits);
 int elp_debug_sort_u128(elp_ctx *ctx, uint64_t *keys_hi, uint64_t *keys_lo, uint32_t *vals, uint64_t n, int key_bits);
+/* the same sorts over bits [lo_bit, lo_bit + key_bits) only: the bits below lo_bit travel with the key unsorted, and keys equal
+ * in the sorted range keep their input order (the fragment-group sort of duplicate marking uses such a range) */
+int elp_debug_sort_u64_range(elp_ctx *ctx, uint64_t *keys, uint32_t *vals, uint64_t n, int lo_bit, int key_bits);
+int elp_debug_sort_u128_range(elp_ctx *ctx, uint64_t *keys_hi, uint64_t *keys_lo, uint32_t *vals, uint64_t n, int lo_bit, int key_bits);
 
 #ifdef __cplusplus
 }

@@ -4,122 +4,13 @@ The fragment sort orders by the group bits only and the winner is found from the
 orders by the signature alone (64-bit keys when it fits, else 128-bit) with the pair scores kept beside it; the long-tie rounds
 skip chunks that are equal on every long-run element and sort the others over their differing bits only.  Every case compares
 FLAG, output order and the duplication metrics bit for bit with the oracle, and checks from kernel_stats() which sort widths
-ran and how many digit passes each took (a Python restatement of the key widths, below)."""
-import numpy as np
+ran and how many digit passes each took (markdup_check.py restates the key widths)."""
 import pytest
 
 from elprep_b200 import sam, synth
+from markdup_check import check as _check
 
 pytestmark = pytest.mark.gpu
-
-F_PAIRED, F_UNMAPPED, F_NEXTUNMAPPED, F_REVERSED, F_NEXTREVERSED = 0x1, 0x4, 0x8, 0x10, 0x20
-
-
-def _passes(bits):
-    return (max(bits, 1) + 7) // 8
-
-
-def _mod_flag(f):
-    f = f.copy()
-    f[(f & F_PAIRED) == 0] &= ~np.uint16(F_NEXTUNMAPPED | F_NEXTREVERSED)
-    f[(f & F_UNMAPPED) != 0] &= ~np.uint16(F_REVERSED)
-    f[(f & F_NEXTUNMAPPED) != 0] &= ~np.uint16(F_NEXTREVERSED)
-    return f.astype(np.uint64)
-
-
-def _tie_passes(b, n_contigs, bP):
-    """digit passes of the long-tie rounds: for every chunk of the secondary key, the bits that differ among the elements of runs
-    of more than 32 equal coordinate keys"""
-    refid = b.refid.astype(np.int64)
-    rr = np.where((refid < 0) | (refid >= n_contigs), n_contigs, refid).astype(np.uint64)
-    key = ((b.flag & F_REVERSED) != 0).astype(np.uint64) | (b.pos.astype(np.uint64) << np.uint64(1)) | (rr << np.uint64(1 + bP))
-    order = np.argsort(key, kind="stable")
-    ks = key[order]
-    starts = np.flatnonzero(np.r_[True, ks[1:] != ks[:-1]])
-    lens = np.diff(np.r_[starts, ks.size])
-    elems = np.concatenate([order[s:s + l] for s, l in zip(starts, lens) if l > 32] or [np.zeros(0, np.int64)])
-    if elems.size == 0:
-        return 0
-    qlen = np.diff(b.qname_off.astype(np.int64))
-    nq = max(1, (int(qlen.max()) + 7) // 8)
-    u32 = lambda v: (v.astype(np.int64) & 0xffffffff).astype(np.uint64) ^ np.uint64(0x80000000)
-    f = b.flag[elems]
-    chunks = [u32(b.tlen[elems]),
-              np.where((f & F_PAIRED) != 0, (u32(b.nref[elems]) << np.uint64(32)) | u32(b.pnext[elems]), np.uint64(0)),
-              (_mod_flag(f) << np.uint64(8)) | b.mapq[elems].astype(np.uint64)]
-    for k in range(nq):
-        qc = nq - 1 - k
-        col = np.zeros(elems.size, np.uint64)
-        for t, e in enumerate(elems):
-            name = bytes(b.qname[b.qname_off[e]:b.qname_off[e + 1]])[8 * qc:8 * qc + 8]
-            col[t] = int.from_bytes(name.ljust(8, b"\0"), "big")
-        chunks.append(col)
-    chunks.append(key[elems])
-    total = 0
-    for col in chunks:
-        diff = int(np.bitwise_or.reduce(col)) ^ int(np.bitwise_and.reduce(col))
-        if diff:
-            lo = (diff & -diff).bit_length() - 1
-            total += _passes(diff.bit_length() - lo)
-    return total
-
-
-def _expected_sorts(b, h):
-    """(u64 passes, u128 passes) of one elp_sort_markdup(coordinate, optical) over batch b, whose FLAG already carries the
-    duplicate bits (the coordinate sort runs after duplicate marking and its modFlag chunk sees them)"""
-    import oracle
-    n_contigs = len(h.SQ)
-    n_lib = len({rg["LB"] for rg in h.RG if rg.get("LB")})
-    bR, bL = n_contigs.bit_length(), (n_lib + 1).bit_length()
-    upos, _ = oracle.mark_duplicates(b.copy(), h, want_adapt=True)
-    entering = (b.flag & 0x904) == 0
-    true_pair = entering & ((b.flag & (F_PAIRED | F_NEXTUNMAPPED)) == F_PAIRED)
-    bU = int(upos[entering].max() - upos[entering].min()).bit_length() if entering.any() else 0
-    bP = int(max(0, b.pos.max())).bit_length()
-    u64 = _passes(1 + bP + bR) + _tie_passes(b, n_contigs, bP)
-    u128 = 0
-    if entering.any():
-        u64 += _passes(1 + bU + bR + bL)
-    if true_pair.sum() >= 2:
-        u64 += 4                                   # mate join: 32-bit keys
-        pair_bits = 2 * bU + 2 + 2 * bR + bL
-        if pair_bits <= 64:
-            u64 += _passes(pair_bits)
-        else:
-            u128 += _passes(pair_bits)
-    return u64, u128
-
-
-def _check(b, h, pixel=100):
-    """FLAG, order and duplication metrics against the oracle; the sort widths and pass counts against _expected_sorts"""
-    import oracle
-    from elprep_b200 import device, _lib
-    b1 = b.copy()
-    oracle.mark_duplicates(b1, h, n_threads=1)
-    perm = oracle.coordinate_sort(b1, n_threads=4)
-    b2 = b.copy()
-    om = oracle.markdup_optical(b2, h, order=perm, pixel_distance=pixel)
-    assert np.array_equal(b1.flag, b2.flag)
-    ctx = device.Context(h, optical_pixel_distance=pixel, profile=True)
-    try:
-        ctx.append(b)
-        ctx.sort_markdup(device.SO_COORDINATE, _lib.MARKDUP_OPTICAL)
-        idx, flag, _, _ = ctx.fetch()
-        assert np.array_equal(idx, perm.astype(np.uint64)), "output order differs"
-        assert np.array_equal(flag, b2.flag[perm]), "FLAG differs"
-        for slot, g in enumerate(ctx.optical_metrics()):
-            for k_g, k_o in zip(_lib.ElpDupMetrics.COUNTERS, oracle.COUNTERS):
-                assert g[k_g] == om.counters[slot][k_o], (slot, k_g)
-            assert g["hist"] == om.hist[slot], slot
-            assert g["estimated_library_size"] == om.library_size[slot]
-        stats = ctx.kernel_stats()
-    finally:
-        ctx.close()
-    u64, u128 = _expected_sorts(b2, h)
-    assert stats.get("radix_onesweep_u64", {}).get("launches", 0) == u64
-    assert stats.get("radix_onesweep_u128", {}).get("launches", 0) == u128
-    return b2.flag, stats
-
 
 H = sam.Header(sq=[{"SN": "chr1", "LN": 100000}, {"SN": "chr2", "LN": 50000}],
                rg=[{"ID": "rg1", "LB": "libA"}, {"ID": "rg2", "LB": "libA"}, {"ID": "rg3", "LB": "libB"}])
