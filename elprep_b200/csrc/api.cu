@@ -298,13 +298,25 @@ uint64_t elp_n_reads(const elp_ctx* c) { return c ? c->n : 0; }
 // elp_append_batch and its asynchronous form.  All host->device copies go to the context's ingest stream (`copy_in`), the small kernels
 // that turn batch-relative offsets into arena offsets follow on the compute stream behind an event, so a pipelined caller can overlap
 // the upload of one context with the kernels and the download of another (bench.py's e2e loop does exactly that with two contexts).
-static uint64_t sum_lengths(const int32_t* l, uint64_t n, uint64_t* seq_bytes) {
+// One host pass over the batch's fixed-width columns: the QUAL and SEQ byte counts, and the first read whose REFID or NextREFID lies
+// outside [-1, n_contigs) (n if none).  Such a value has no place in the coordinate key or in duplicate marking's packed refid + 1 field
+// (it would spill into the library bits), so the batch is refused; elp_append_bam maps negative ids to -1 and refuses the others itself.
+struct BatchScan { uint64_t bases, seq_bytes, bad_ref; };
+static BatchScan scan_batch(const elp_batch* b, uint64_t n, int n_contigs) {
     const unsigned nt = n > (1u << 20) ? std::min(8u, std::max(1u, std::thread::hardware_concurrency())) : 1u;
-    std::vector<uint64_t> a(nt, 0), b(nt, 0);
-    auto work = [&](unsigned t) { uint64_t x = 0, y = 0; for (uint64_t i = n * t / nt, e = n * (t + 1) / nt; i < e; i++) { const uint64_t v = (uint64_t)(uint32_t)l[i]; x += v; y += (v + 1) >> 1; } a[t] = x; b[t] = y; };
+    std::vector<uint64_t> a(nt, 0), s(nt, 0), bad(nt, n);
+    const uint32_t lim = (uint32_t)n_contigs;
+    auto work = [&](unsigned t) {
+        uint64_t x = 0, y = 0, e = n * (t + 1) / nt;
+        for (uint64_t i = n * t / nt; i < e; i++) { const uint64_t v = (uint64_t)(uint32_t)b->l_seq[i]; x += v; y += (v + 1) >> 1; }
+        for (uint64_t i = n * t / nt; i < e; i++)
+            if ((uint32_t)b->refid[i] + 1u > lim || (uint32_t)b->nref[i] + 1u > lim) { bad[t] = i; break; }   // -1 -> 0, -2 -> 2^32-1
+        a[t] = x; s[t] = y;
+    };
     if (nt == 1) work(0); else { std::vector<std::thread> th; for (unsigned t = 0; t < nt; t++) th.emplace_back(work, t); for (auto& x : th) x.join(); }
-    uint64_t x = 0, y = 0; for (unsigned t = 0; t < nt; t++) { x += a[t]; y += b[t]; }
-    *seq_bytes = y; return x;
+    BatchScan r{0, 0, n};
+    for (unsigned t = 0; t < nt; t++) { r.bases += a[t]; r.seq_bytes += s[t]; r.bad_ref = std::min(r.bad_ref, bad[t]); }
+    return r;
 }
 
 // Large host<->device copies go out whole by default.  (A copy engine serves its queue in order, so cutting a copy into pieces that are all
@@ -330,8 +342,11 @@ static int append_impl(elp_ctx* c, const elp_batch* b, bool wait) {
     const uint64_t n0 = c->n, n1 = n0 + bn;
     if (n1 >= (1ull << 32)) return c->fail(E_LIMIT, "more than 2^32-1 reads in one context");
     const uint64_t bq = b->qname_off[bn] - b->qname_off[0], bc = b->cigar_off[bn] - b->cigar_off[0];
-    uint64_t bseq = 0;
-    const uint64_t bbases = sum_lengths(b->l_seq, bn, &bseq);
+    const BatchScan sc = scan_batch(b, bn, c->n_contigs);
+    if (sc.bad_ref < bn)
+        return c->fail(E_INVAL, "elp_append_batch: read %llu of the batch has REFID %d, NextREFID %d; both must lie in [-1, %d)", (unsigned long long)sc.bad_ref,
+                       b->refid[sc.bad_ref], b->nref[sc.bad_ref], c->n_contigs);
+    const uint64_t bbases = sc.bases, bseq = sc.seq_bytes;
     // growing a buffer moves it: uploads of an earlier asynchronous append that are still in flight must land first
     if (c->copy_in && (n1 + 2 > c->flag.cap || n1 + 2 > c->qname_off.cap || c->n_qname + bq + 64 > c->qname.cap || c->n_cigar + bc + 16 > c->cigar.cap ||
                        c->n_qual + bbases + 64 > c->qual.cap || c->n_seq + bseq + 64 > c->seq.cap)) CUDA_TRY(c, cudaStreamSynchronize(c->copy_in));

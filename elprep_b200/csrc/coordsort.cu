@@ -4,8 +4,8 @@
 //  1. radix sort of the compact key (refid with -1 last | POS | strand)           -- the first three comparator clauses
 //  2. runs of equal keys are ordered by the remaining clauses (QNAME bytes, modFlag, MAPQ, [NextREFID signed, PNEXT] if
 //     both paired, TLEN): short runs by a per-run insertion sort, long runs (e.g. all unmapped reads) by a batched LSD
-//     radix sort over 64-bit chunks of the composite secondary key.  Everything is stable: fully equal records keep
-//     arrival order.
+//     radix sort over 64-bit chunks of the composite secondary key (layout at chunk_key).  Everything is stable: fully
+//     equal records keep arrival order.
 //  3. the fixed-width columns are gathered into output order once; the byte arenas (QNAME, CIGAR, SEQ, QUAL) stay where
 //     they are and are reached through the gathered offsets (the reference sorts pointers, too).
 // Deviation (malformed input only): an empty QNAME takes part in the comparison as the smallest string, whereas the
@@ -15,10 +15,20 @@
 namespace {
 
 constexpr int SHORT_RUN = 32;
+constexpr int QC0 = 4;          // chunk id of the last (least significant) QNAME chunk
+constexpr int FLAG_SLICE = 64;  // chunks tie_long_flag_kernel reduces per round through shared memory
 
 inline unsigned nblk(uint64_t n, int t) { return (unsigned)((n + t - 1) / t); }
 
 struct CoordLayout { int bP, bR; int n_contigs; int key_bits; };
+
+CoordLayout coord_layout(const elp_ctx* c) {   // after phase_adapt (pos_max)
+    CoordLayout L{}; L.n_contigs = c->n_contigs; L.bP = bits_for((uint64_t)c->h_ranges.pos_max); L.bR = bits_for((uint64_t)c->n_contigs);
+    L.key_bits = 1 + L.bP + L.bR;
+    return L;
+}
+
+int qname_chunks(const elp_ctx* c) { return std::max(1, (int)((c->h_ranges.qname_max + 7) / 8)); }   // longest QNAME, from the adapt kernel's range reduction
 
 __global__ void __launch_bounds__(256) coord_keys_kernel(uint64_t n, const int32_t* __restrict__ refid, const int32_t* __restrict__ pos, const uint16_t* __restrict__ flag,
                                                           CoordLayout L, uint64_t* __restrict__ keys, uint32_t* __restrict__ vals) {
@@ -79,16 +89,25 @@ __global__ void __launch_bounds__(128) tie_short_kernel(uint64_t n, const uint64
 }
 
 // chunk key of the composite secondary key; chunk ids (least significant first):
-//   0: TLEN   1: NextREFID|PNEXT (0 unless paired)   2: modFlag|MAPQ   3+k: QNAME bytes [8*(nq-1-k), +8) big-endian, zero padded
+//   0: TLEN   1: NextREFID|PNEXT (0 unless paired)   2: modFlag|MAPQ
+//   3: the number of trailing NUL bytes of the QNAME   QC0+k: QNAME bytes [8*(nq-1-k), +8), big-endian, zero padded
 //   last: the primary coordinate key itself (keeps the runs apart and in place)
+// The zero-padded QNAME chunks alone see "a" and "a\0" as equal.  Two names with equal padded bytes are one name without a trailing
+// NUL followed by different numbers of NULs, so chunk 3 orders them by length as qname_compare does; it is 0 for every name that does
+// not end in a NUL, and the tie rounds then skip it.
 __device__ __forceinline__ uint64_t chunk_key(uint32_t a, int chunk, int nq, const TieCols& c, const int32_t* __restrict__ refid, const int32_t* __restrict__ pos,
                                               const CoordLayout& L) {
     uint64_t key;
     if (chunk == 0) key = (uint64_t)((uint32_t)c.tlen[a] ^ 0x80000000u);
     else if (chunk == 1) key = (c.flag[a] & F_MULTIPLE) ? (((uint64_t)((uint32_t)c.nref[a] ^ 0x80000000u) << 32) | (uint64_t)((uint32_t)c.pnext[a] ^ 0x80000000u)) : 0ull;
     else if (chunk == 2) key = ((uint64_t)mod_flag(c.flag[a]) << 8) | c.mapq[a];
-    else if (chunk < 3 + nq) {
-        const int qc = nq - 1 - (chunk - 3);
+    else if (chunk == 3) {
+        const uint64_t q0 = c.qname_off[a], q1 = c.qname_off[a + 1];
+        uint64_t e = q1;
+        while (e > q0 && c.qname[e - 1] == 0) e--;
+        key = q1 - e;
+    } else if (chunk < QC0 + nq) {
+        const int qc = nq - 1 - (chunk - QC0);
         const uint64_t q0 = c.qname_off[a], q1 = c.qname_off[a + 1], lo = q0 + (uint64_t)qc * 8;
         key = 0;
         if (lo < q1) {
@@ -122,12 +141,12 @@ __global__ void __launch_bounds__(256) chunk_keys_kernel(uint64_t m, const uint3
 
 // flag[j] = 1 if j belongs to a run longer than SHORT_RUN (checked against the element SHORT_RUN places away on either side).
 // Over the elements of all long runs, bits[ch] accumulates the OR and bits[n_chunks + ch] the AND of chunk key ch: a bit
-// where the two differ is the only kind that can reorder anything in the tie rounds.
+// where the two differ is the only kind that can reorder anything in the tie rounds.  The chunks go through shared memory
+// FLAG_SLICE at a time, so the footprint does not grow with the longest QNAME.
 __global__ void __launch_bounds__(256) tie_long_flag_kernel(uint64_t n, const uint64_t* __restrict__ keys, const uint32_t* __restrict__ vals, uint32_t* __restrict__ long_flag,
                                                              int n_chunks, int nq, TieCols c, const int32_t* __restrict__ refid, const int32_t* __restrict__ pos,
                                                              CoordLayout L, unsigned long long* __restrict__ bits) {
-    extern __shared__ unsigned long long s_bits[];   // [n_chunks] OR, [n_chunks] AND
-    unsigned long long *s_or = s_bits, *s_and = s_bits + n_chunks;
+    __shared__ unsigned long long s_or[FLAG_SLICE], s_and[FLAG_SLICE];
     const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     bool lng = false;
     if (j < n) {
@@ -140,18 +159,22 @@ __global__ void __launch_bounds__(256) tie_long_flag_kernel(uint64_t n, const ui
         long_flag[j] = lng ? 1u : 0u;
     }
     if (!__syncthreads_or(lng)) return;
-    for (int ch = threadIdx.x; ch < n_chunks; ch += blockDim.x) { s_or[ch] = 0; s_and[ch] = ~0ull; }
-    __syncthreads();
     const uint32_t a = lng ? vals[j] : 0u;
     const unsigned lane = threadIdx.x & 31;
-    for (int ch = 0; ch < n_chunks; ch++) {
-        const uint64_t k = lng ? chunk_key(a, ch, nq, c, refid, pos, L) : 0ull;
-        uint64_t o = k, an = lng ? k : ~0ull;
-        for (int d = 16; d; d >>= 1) { o |= __shfl_xor_sync(FULL_MASK, o, d); an &= __shfl_xor_sync(FULL_MASK, an, d); }
-        if (lane == 0) { atomicOr(&s_or[ch], (unsigned long long)o); atomicAnd(&s_and[ch], (unsigned long long)an); }
+    for (int ch0 = 0; ch0 < n_chunks; ch0 += FLAG_SLICE) {
+        const int ns = min(FLAG_SLICE, n_chunks - ch0);
+        if ((int)threadIdx.x < ns) { s_or[threadIdx.x] = 0; s_and[threadIdx.x] = ~0ull; }
+        __syncthreads();
+        for (int s = 0; s < ns; s++) {
+            const uint64_t k = lng ? chunk_key(a, ch0 + s, nq, c, refid, pos, L) : 0ull;
+            uint64_t o = k, an = lng ? k : ~0ull;
+            for (int d = 16; d; d >>= 1) { o |= __shfl_xor_sync(FULL_MASK, o, d); an &= __shfl_xor_sync(FULL_MASK, an, d); }
+            if (lane == 0) { atomicOr(&s_or[s], (unsigned long long)o); atomicAnd(&s_and[s], (unsigned long long)an); }
+        }
+        __syncthreads();
+        if ((int)threadIdx.x < ns) { atomicOr(bits + ch0 + threadIdx.x, s_or[threadIdx.x]); atomicAnd(bits + n_chunks + ch0 + threadIdx.x, s_and[threadIdx.x]); }
+        __syncthreads();   // the next slice reuses the shared words
     }
-    __syncthreads();
-    for (int ch = threadIdx.x; ch < n_chunks; ch += blockDim.x) { atomicOr(bits + ch, s_or[ch]); atomicAnd(bits + n_chunks + ch, s_and[ch]); }
 }
 
 __global__ void __launch_bounds__(256) compact_long_kernel(uint64_t n, const uint32_t* __restrict__ long_flag, const uint64_t* __restrict__ slot,
@@ -223,8 +246,7 @@ int phase_coordinate_sort(elp_ctx* c, int order) {   // 0 keep, 1 coordinate, 2 
     if (sort && n > 1) {
         CUDA_TRY(c, c->keys_a.reserve(2 * n + 4, c->stream)); CUDA_TRY(c, c->keys_b.reserve(2 * n + 4, c->stream));
         CUDA_TRY(c, c->vals_a.reserve(n + 4, c->stream)); CUDA_TRY(c, c->vals_b.reserve(n + 4, c->stream));
-        CoordLayout L{}; L.n_contigs = c->n_contigs; L.bP = bits_for((uint64_t)c->h_ranges.pos_max); L.bR = bits_for((uint64_t)c->n_contigs);
-        L.key_bits = 1 + L.bP + L.bR;
+        const CoordLayout L = coord_layout(c);
         c->begin("coord_keys", (double)n * (4 + 4 + 2 + 8 + 4));
         coord_keys_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(n, c->refid.p, c->pos.p, c->flag.p, L, c->keys_a.p, c->vals_a.p);
         c->end(); LAUNCH_CHECK(c);
@@ -236,15 +258,15 @@ int phase_coordinate_sort(elp_ctx* c, int order) {   // 0 keep, 1 coordinate, 2 
         uint64_t* keys_free = in_b ? c->keys_a.p : c->keys_b.p;
 
         TieCols tc{c->flag.p, c->mapq.p, c->nref.p, c->pnext.p, c->tlen.p, c->qname_off.p, c->qname.p};
-        const int nq = std::max(1, (int)((c->h_ranges.qname_max + 7) / 8));   // longest QNAME, from the adapt kernel's range reduction
-        const int n_chunks = 3 + nq + 1;
+        const int nq = qname_chunks(c);
+        const int n_chunks = QC0 + nq + 1;
         // long runs first (flags computed from the keys only), then short runs in place
         CUDA_TRY(c, c->scan_tmp.reserve(n + 4, c->stream));
         CUDA_TRY(c, c->tie_bits.reserve(2 * n_chunks, c->stream));
         CUDA_TRY(c, cudaMemsetAsync(c->tie_bits.p, 0, n_chunks * 8, c->stream));
         CUDA_TRY(c, cudaMemsetAsync(c->tie_bits.p + n_chunks, 0xff, n_chunks * 8, c->stream));
         c->begin("tie_long_flag", (double)n * 12);
-        tie_long_flag_kernel<<<nblk(n, 256), 256, 2 * n_chunks * 8, c->stream>>>(n, keys, vals, c->scan_tmp.p, n_chunks, nq, tc, c->refid.p, c->pos.p, L,
+        tie_long_flag_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(n, keys, vals, c->scan_tmp.p, n_chunks, nq, tc, c->refid.p, c->pos.p, L,
                                                                   reinterpret_cast<unsigned long long*>(c->tie_bits.p));
         c->end(); LAUNCH_CHECK(c);
         uint64_t* slot = keys_free;   // n+1 u64
@@ -292,20 +314,22 @@ int phase_coordinate_sort(elp_ctx* c, int order) {   // 0 keep, 1 coordinate, 2 
 
     } else if (order == 2 && n > 1) {
         // By(QNAMELess).ParallelStableSort (sam/sam-types.go:479-481, sam/filter-pipeline.go:119-123): stable LSD radix sort over
-        // 8-byte big-endian chunks of the QNAME, last chunk first (names are zero padded: a prefix sorts before its extensions)
+        // 8-byte big-endian chunks of the QNAME, last chunk first (names are zero padded: a prefix sorts before its extensions),
+        // after a first pass over the number of trailing NUL bytes (chunk 3), which orders names that differ only by those
         CUDA_TRY(c, c->keys_a.reserve(2 * n + 4, c->stream)); CUDA_TRY(c, c->keys_b.reserve(2 * n + 4, c->stream));
         CUDA_TRY(c, c->vals_a.reserve(n + 4, c->stream)); CUDA_TRY(c, c->vals_b.reserve(n + 4, c->stream));
         TieCols tc{c->flag.p, c->mapq.p, c->nref.p, c->pnext.p, c->tlen.p, c->qname_off.p, c->qname.p};
         CoordLayout L{};
-        const int nq = std::max(1, (int)((c->h_ranges.qname_max + 7) / 8));
+        const int nq = qname_chunks(c);
         iota_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(n, c->vals_a.p); c->launches++; LAUNCH_CHECK(c);
         const uint32_t* elem = c->vals_a.p;
-        for (int ch = 0; ch < nq; ch++) {
+        for (int ch = QC0 - 1; ch < QC0 + nq; ch++) {
             c->begin("qname_chunk_keys", (double)n * 32);
-            chunk_keys_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(n, elem, 3 + ch, nq, tc, c->refid.p, c->pos.p, L, c->keys_a.p, c->vals_a.p);
+            chunk_keys_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(n, elem, ch, nq, tc, c->refid.p, c->pos.p, L, c->keys_a.p, c->vals_a.p);
             c->end(); LAUNCH_CHECK(c);
             bool b2 = false;
-            rc = radix_sort_u64(c, c->keys_a.p, c->keys_b.p, c->vals_a.p, c->vals_b.p, n, 64, &b2, "u64");
+            const int bits = ch < QC0 ? std::max(1, bits_for((uint64_t)c->h_ranges.qname_max)) : 64;   // trailing NULs <= the longest name
+            rc = radix_sort_u64(c, c->keys_a.p, c->keys_b.p, c->vals_a.p, c->vals_b.p, n, bits, &b2, "u64");
             if (rc) return rc;
             elem = b2 ? c->vals_b.p : c->vals_a.p;
         }
@@ -341,5 +365,25 @@ int phase_coordinate_sort(elp_ctx* c, int order) {   // 0 keep, 1 coordinate, 2 
     if (rc) return rc;
     c->sorted = true;
     c->qual_out_valid = false;
+    return E_OK;
+}
+
+// chunk_key of every read in arrival order, under the layout (nq, primary key widths) the coordinate sort would use
+extern "C" int elp_debug_coord_chunk_keys(elp_ctx* c, int chunk, uint64_t* keys) {
+    if (!c) return E_INVAL;
+    cudaSetDevice(c->device);
+    int rc = phase_adapt(c);
+    if (rc) return rc;
+    const uint64_t n = c->n;
+    const int nq = qname_chunks(c), n_chunks = QC0 + nq + 1;
+    if (chunk < 0 || chunk >= n_chunks) return c->fail(E_INVAL, "elp_debug_coord_chunk_keys: chunk %d outside [0, %d)", chunk, n_chunks);
+    if (n == 0) return E_OK;
+    CUDA_TRY(c, c->keys_a.reserve(n + 4, c->stream)); CUDA_TRY(c, c->vals_a.reserve(n + 4, c->stream)); CUDA_TRY(c, c->vals_b.reserve(n + 4, c->stream));
+    const TieCols tc{c->flag.p, c->mapq.p, c->nref.p, c->pnext.p, c->tlen.p, c->qname_off.p, c->qname.p};
+    iota_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(n, c->vals_a.p); c->launches++; LAUNCH_CHECK(c);
+    chunk_keys_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(n, c->vals_a.p, chunk, nq, tc, c->refid.p, c->pos.p, coord_layout(c), c->keys_a.p, c->vals_b.p);
+    c->launches++; LAUNCH_CHECK(c);
+    CUDA_TRY(c, cudaMemcpyAsync(keys, c->keys_a.p, n * 8, cudaMemcpyDeviceToHost, c->stream));
+    CUDA_TRY(c, cudaStreamSynchronize(c->stream));
     return E_OK;
 }

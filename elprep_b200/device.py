@@ -363,6 +363,12 @@ class Context:
         self._ck(self.L.elp_debug_join_hash(self.h, _vp(q)))
         return q
 
+    def debug_coord_chunk_keys(self, chunk):
+        """per read in arrival order, chunk `chunk` of the coordinate sort's long-tie key (layout in elp_debug_coord_chunk_keys)"""
+        k = np.zeros(self.n, np.uint64)
+        self._ck(self.L.elp_debug_coord_chunk_keys(self.h, chunk, _vp(k)))
+        return k
+
     def debug_sort_u64(self, keys, vals, key_bits, lo_bit=None):
         """stable sort by bits [lo_bit, lo_bit + key_bits) (lo_bit None: the call without a range)"""
         keys = np.ascontiguousarray(keys, dtype=np.uint64).copy()

@@ -70,7 +70,8 @@ typedef struct {
 
 /* One batch of sam.Alignment records in columnar form (sam/sam-types.go:289-331) -- what a
  * pipeline stage marshals from []*sam.Alignment (sam/filter-pipeline.go:92-104).
- * refid/nref are the REFID/NextREFID temps of filters.AddREFID (simple-filters.go:208-231);
+ * refid/nref are the REFID/NextREFID temps of filters.AddREFID (simple-filters.go:208-231), each in [-1, n_contigs): a batch
+ * with any other value is refused with ELP_EINVAL and nothing of it is appended;
  * rg is the index of the read's RG:Z tag in elp_config.rg_id, -1 if the read has no RG tag.
  * cigar: BAM encoding len<<4|op, op indexes "MIDNSHP=X" (sam/bam-files.go). seq: BAM nibbles, high nibble
  * first, each read byte-aligned, reads packed back to back ((l_seq+1)/2 bytes each). qual: phred bytes
@@ -304,6 +305,11 @@ int elp_debug_adapt(elp_ctx *ctx, int32_t *upos, int32_t *score);
 /* per read, the 64-bit (library, QNAME) hash duplicate marking joins mates by (its low 31 bits are the join key); 0 for a read that is
  * not a true pair (unmapped, secondary, supplementary, unpaired or mate unmapped) */
 int elp_debug_join_hash(elp_ctx *ctx, uint64_t *qhash);
+/* per read in arrival order, chunk `chunk` of the composite key by which the coordinate sort orders runs of more than 32 reads with
+ * equal (REFID, POS, strand), as that sort would compute it for the reads appended so far: 0 TLEN, 1 NextREFID|PNEXT (0 if unpaired),
+ * 2 modFlag|MAPQ, 3 the number of trailing NUL bytes of the QNAME, 4..3+nq the QNAME in 8-byte big-endian chunks (4 = the last),
+ * 4+nq the (REFID, POS, strand) key; nq = ceil(longest QNAME / 8), at least 1.  A chunk outside [0, 5+nq) is ELP_EINVAL. */
+int elp_debug_coord_chunk_keys(elp_ctx *ctx, int chunk, uint64_t *keys);
 /* opt_flags of output records [first, first+n) (what filters.RemoveOptionalReads looks at when the worker writes its output) */
 int elp_fetch_opt_flags(elp_ctx *ctx, uint64_t first, uint64_t n, uint8_t *opt_flags);
 /* arrival-order CIGARs as the context holds them (after elp_clean_sam), for parity tests: cigar_off[n+1] relative to the first operation */

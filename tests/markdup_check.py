@@ -6,56 +6,13 @@ import tempfile
 
 import numpy as np
 
-F_PAIRED, F_UNMAPPED, F_NEXTUNMAPPED, F_REVERSED, F_NEXTREVERSED = 0x1, 0x4, 0x8, 0x10, 0x20
-
-
-def _passes(bits):
-    return (max(bits, 1) + 7) // 8
-
-
-def _mod_flag(f):
-    f = f.copy()
-    f[(f & F_PAIRED) == 0] &= ~np.uint16(F_NEXTUNMAPPED | F_NEXTREVERSED)
-    f[(f & F_UNMAPPED) != 0] &= ~np.uint16(F_REVERSED)
-    f[(f & F_NEXTUNMAPPED) != 0] &= ~np.uint16(F_NEXTREVERSED)
-    return f.astype(np.uint64)
+from coordsort_ref import F_NEXTUNMAPPED, F_PAIRED, passes as _passes, tie_rounds
 
 
 def _tie_passes(b, n_contigs, bP):
-    """digit passes of the long-tie rounds: for every chunk of the secondary key, the bits that differ among the elements of runs
-    of more than 32 equal coordinate keys"""
-    refid = b.refid.astype(np.int64)
-    rr = np.where((refid < 0) | (refid >= n_contigs), n_contigs, refid).astype(np.uint64)
-    key = ((b.flag & F_REVERSED) != 0).astype(np.uint64) | (b.pos.astype(np.uint64) << np.uint64(1)) | (rr << np.uint64(1 + bP))
-    order = np.argsort(key, kind="stable")
-    ks = key[order]
-    starts = np.flatnonzero(np.r_[True, ks[1:] != ks[:-1]])
-    lens = np.diff(np.r_[starts, ks.size])
-    elems = np.concatenate([order[s:s + l] for s, l in zip(starts, lens) if l > 32] or [np.zeros(0, np.int64)])
-    if elems.size == 0:
-        return 0
-    qlen = np.diff(b.qname_off.astype(np.int64))
-    nq = max(1, (int(qlen.max()) + 7) // 8)
-    u32 = lambda v: (v.astype(np.int64) & 0xffffffff).astype(np.uint64) ^ np.uint64(0x80000000)
-    f = b.flag[elems]
-    chunks = [u32(b.tlen[elems]),
-              np.where((f & F_PAIRED) != 0, (u32(b.nref[elems]) << np.uint64(32)) | u32(b.pnext[elems]), np.uint64(0)),
-              (_mod_flag(f) << np.uint64(8)) | b.mapq[elems].astype(np.uint64)]
-    for k in range(nq):
-        qc = nq - 1 - k
-        col = np.zeros(elems.size, np.uint64)
-        for t, e in enumerate(elems):
-            name = bytes(b.qname[b.qname_off[e]:b.qname_off[e + 1]])[8 * qc:8 * qc + 8]
-            col[t] = int.from_bytes(name.ljust(8, b"\0"), "big")
-        chunks.append(col)
-    chunks.append(key[elems])
-    total = 0
-    for col in chunks:
-        diff = int(np.bitwise_or.reduce(col)) ^ int(np.bitwise_and.reduce(col))
-        if diff:
-            lo = (diff & -diff).bit_length() - 1
-            total += _passes(diff.bit_length() - lo)
-    return total
+    """digit passes of the long-tie rounds: for every chunk of the secondary key (coordsort_ref.chunk_keys), the bits that differ
+    among the elements of runs of more than 32 equal coordinate keys"""
+    return sum(_passes(bits) for _, _, bits in tie_rounds(b, n_contigs, bP))
 
 
 def _joined_pairs(b, h, true_pair):
