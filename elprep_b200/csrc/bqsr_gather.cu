@@ -290,8 +290,10 @@ __global__ void __launch_bounds__(128) bqsr_prep_kernel(GatherArgs A) {
                 if (fs <= fe) { d.skip[d.n_skip][0] = (uint16_t)fs; d.skip[d.n_skip][1] = (uint16_t)fe; d.n_skip++; }
             }
         } else {
+            // every read past the reserved slots is still counted: gather_general then reserves that many and runs this kernel again
             const uint32_t slot = atomicAdd(A.ovf_count, 1u);
-            if (slot >= A.ovf_cap) { atomicOr(A.err, DERR_READLEN_LIMIT); done(); return; }
+            d.flags |= DF_SKIP_OVF;
+            if (slot >= A.ovf_cap) { done(); return; }
             uint32_t bits[OVF_WORDS];
             for (int i = 0; i < OVF_WORDS; i++) bits[i] = 0;
             for (uint64_t s = s0; s < s1; s++) {
@@ -302,7 +304,7 @@ __global__ void __launch_bounds__(128) bqsr_prep_kernel(GatherArgs A) {
                 for (int i = fs; i <= fe; i++) bits[i >> 5] |= 1u << (i & 31);
             }
             for (int i = 0; i < OVF_WORDS; i++) A.ovf_bits[(size_t)slot * OVF_WORDS + i] = bits[i];
-            d.flags |= DF_SKIP_OVF; d.ovf = slot;
+            d.ovf = slot;
         }
     }
     // chunk kernel: one M run, every cycle inside --max-cycle (|cycle| <= L), inside the contig, fits the lanes of a read
@@ -821,18 +823,27 @@ int gather_general(elp_ctx* c, GatherArgs A, const uint32_t* in_list, uint32_t n
     CUDA_TRY(c, c->vals_b.reserve(2 * n + 16, c->stream));
     A.gen_list = c->vals_b.p; A.cg_list = c->vals_b.p + n + 8;
     A.desc = reinterpret_cast<ReadDesc*>(c->keys_a.p);
-    A.ovf_cap = (uint32_t)std::min<uint64_t>(n, (n >> 4) + 4096);
-    CUDA_TRY(c, c->vals_a.reserve((size_t)A.ovf_cap * OVF_WORDS + 8, c->stream));
-    A.ovf_bits = c->vals_a.p;
-    A.ovf_count = c->scan_tmp.p;   // three u32 (overflow slots, fallback reads, GEN chunk reads), zeroed below
+    A.ovf_count = c->scan_tmp.p;   // three u32 (overflow slots, fallback reads, GEN chunk reads), zeroed before each prep pass
     A.gen_count = c->scan_tmp.p + 1;
-    CUDA_TRY(c, cudaMemsetAsync(A.ovf_count, 0, 12, c->stream));
-    c->begin("bqsr_g_prep", (double)n_work * (4 * 7 + 2 + 1 + 8 + 8 + 4 + 48) + (double)c->n_cigar * 4 * ((double)n_work / (double)n));
-    bqsr_prep_kernel<<<(unsigned)((n_work + 127) / 128), 128, 0, c->stream>>>(A);
-    c->end(); LAUNCH_CHECK(c);
-    c->begin("bqsr_g_gen_list", (double)n_work * 20);
-    gen_list_kernel<<<(unsigned)((n_work + 255) / 256), 256, 0, c->stream>>>(A);
-    c->end(); LAUNCH_CHECK(c);
+    // a first guess of the reads with more than four known-site ranges; when more need a mask, the prep kernel still counts them,
+    // and a second pass runs with exactly that many slots (nothing has consumed the descriptors of the first pass yet)
+    A.ovf_cap = (uint32_t)std::min<uint64_t>(n, (n >> 4) + 4096);
+    uint32_t cnt3[3] = {0, 0, 0};
+    for (int pass = 0; pass < 2; pass++) {
+        CUDA_TRY(c, c->vals_a.reserve((size_t)A.ovf_cap * OVF_WORDS + 8, c->stream));
+        A.ovf_bits = c->vals_a.p;
+        CUDA_TRY(c, cudaMemsetAsync(A.ovf_count, 0, 12, c->stream));
+        c->begin("bqsr_g_prep", (double)n_work * (4 * 7 + 2 + 1 + 8 + 8 + 4 + 48) + (double)c->n_cigar * 4 * ((double)n_work / (double)n));
+        bqsr_prep_kernel<<<(unsigned)((n_work + 127) / 128), 128, 0, c->stream>>>(A);
+        c->end(); LAUNCH_CHECK(c);
+        c->begin("bqsr_g_gen_list", (double)n_work * 20);
+        gen_list_kernel<<<(unsigned)((n_work + 255) / 256), 256, 0, c->stream>>>(A);
+        c->end(); LAUNCH_CHECK(c);
+        CUDA_TRY(c, cudaMemcpyAsync(cnt3, A.ovf_count, 12, cudaMemcpyDeviceToHost, c->stream));
+        CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+        if (cnt3[0] <= A.ovf_cap) break;
+        A.ovf_cap = cnt3[0];
+    }
     const uint64_t rpw = 32 / A.lanes_per_read;
     CUDA_TRY(c, cudaFuncSetAttribute(bqsr_chunk_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(smem, 1024)));
     CUDA_TRY(c, cudaFuncSetAttribute(bqsr_chunk_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(smem, 1024)));
@@ -844,10 +855,7 @@ int gather_general(elp_ctx* c, GatherArgs A, const uint32_t* in_list, uint32_t n
         bqsr_chunk_kernel<false><<<(unsigned)grid, 256, smem, c->stream>>>(A, nullptr, 0);
         c->end(); LAUNCH_CHECK(c);
     }
-    uint32_t cnt2[2] = {0, 0};
-    CUDA_TRY(c, cudaMemcpyAsync(cnt2, A.gen_count, 8, cudaMemcpyDeviceToHost, c->stream));
-    CUDA_TRY(c, cudaStreamSynchronize(c->stream));
-    const uint32_t n_gen = cnt2[0], n_cg = cnt2[1];
+    const uint32_t n_gen = cnt3[1], n_cg = cnt3[2];
     if (n_cg) {
         const uint64_t steps_g = ((uint64_t)n_cg + rpw - 1) / rpw;
         const uint64_t grid_cg = std::min<uint64_t>((steps_g + 7) / 8, (uint64_t)sms * CHUNK_MINB);

@@ -9,8 +9,8 @@ import numpy as np
 import pytest
 
 from elprep_b200 import synth
-from util import (SYNTH_QUALS, apply_plan, bqsr_paths, fast_plan, gpu_phases, gpu_pipeline, oracle_pipeline, oracle_tables_dense,
-                  set_side_inputs, with_qual_alphabet)
+from util import (SYNTH_QUALS, apply_plan, bqsr_paths, compare_bqsr as _compare, fast_plan, gpu_phases, gpu_pipeline, oracle_pipeline,
+                  oracle_tables_dense, set_side_inputs, with_qual_alphabet)
 
 pytestmark = pytest.mark.gpu
 
@@ -33,17 +33,6 @@ ALPHABETS = [
 
 def _qid(v):
     return "q" + "-".join(str(x) for x in v)
-
-
-def _compare(g, o, max_cycle=500):
-    assert np.array_equal(g["perm"], o["perm"]), "output order differs"
-    assert np.array_equal(g["flag"], o["flag"]), "FLAG differs"
-    assert np.array_equal(g["qual_off"], o["qual_off"])
-    d, e = oracle_tables_dense(o["tables"], max_cycle)
-    assert np.array_equal(g["tables"], d), "BQSR table counters differ"
-    assert np.array_equal(g["emp"], e), "EmpiricalQuality differs"
-    assert g["report"] == o["report"], "recalibration report text differs"
-    assert np.array_equal(g["qual"], o["qual"]), "QUAL bytes differ"
 
 
 def _expected(values, n_cov, L, max_cycle=500):

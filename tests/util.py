@@ -28,6 +28,18 @@ def oracle_pipeline(w, bqsr=True, threads=4, max_cycle=500, quantize_levels=0, s
     return res
 
 
+def compare_bqsr(g, o, max_cycle=500):
+    """gpu_pipeline vs oracle_pipeline results, bit for bit: order, FLAG, table counters, EmpiricalQuality, report text, QUAL bytes"""
+    assert np.array_equal(g["perm"], o["perm"]), "output order differs"
+    assert np.array_equal(g["flag"], o["flag"]), "FLAG differs"
+    assert np.array_equal(g["qual_off"], o["qual_off"])
+    d, e = oracle_tables_dense(o["tables"], max_cycle)
+    assert np.array_equal(g["tables"], d), "BQSR table counters differ"
+    assert np.array_equal(g["emp"], e), "EmpiricalQuality differs"
+    assert g["report"] == o["report"], "recalibration report text differs"
+    assert np.array_equal(g["qual"], o["qual"]), "QUAL bytes differ"
+
+
 def oracle_tables_dense(t, max_cycle=500):
     """oracle tables -> the C ABI's dense layout [n_cov][94][1+(2mc+1)+16][2] (+ empirical [..][..][..])"""
     n_cov = t.n_cov
