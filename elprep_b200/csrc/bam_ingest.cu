@@ -9,7 +9,7 @@
 //   bam_copy_kernel   one warp per record: QNAME bytes (without the NUL), CIGAR words (already `len<<4|op`), SEQ nibbles
 //                     and QUAL bytes (phred without +33) are byte-for-byte the device layout -> four segmented copies
 // Offsets come from device prefix sums of the lengths.  The raw records stay in a device arena so that the write phase can
-// hand them back (elp_fetch_bam): output order, FLAG and QUAL patched, everything else -- names, CIGAR, tags -- untouched
+// hand them back (elp_fetch_bam): output order, MAPQ, FLAG and QUAL patched, everything else -- names, CIGAR, tags -- untouched
 // (the counterpart of formatting every *sam.Alignment again, sam/bam-files.go:635-735).  Not handled (error return): the CG:B long-CIGAR convention (:376-392),
 // an RG:Z value that is not an @RG ID of the header.
 #include <algorithm>
@@ -38,25 +38,24 @@ struct BamArgs {
 // fixed part: block_size(4) refID(4) pos(4) l_read_name(1) mapq(1) bin(2) n_cigar_op(2) flag(2) l_seq(4) next_refID(4) next_pos(4) tlen(4)
 constexpr int BAM_FIXED = 36;
 
-__global__ void __launch_bounds__(256) bam_fixed_kernel(BamArgs A) {
-    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= A.n) return;
-    const uint64_t st = A.start[i];
-    const uint8_t* r = A.raw + st;
+struct RgNames { const uint8_t* names; const uint32_t* off; int n; };
+
+// The structure of one record of rec_len >= BAM_FIXED bytes, as parseBamAlignment (sam/bam-files.go:314-400) reads it: the variable
+// lengths against block_size, contig ids, every optional field.  Returns 1 for a malformed record, else 2 for a well-formed one that
+// uses the CG:B long-CIGAR convention, else 0; *rg_out: the @RG index of RG:Z, -1 without one, -2 for a value that is no @RG ID;
+// *optf_out: the sr bit.  Every record of a call goes through it, whether the ingest filters keep it or not: a malformed record fails
+// the call whatever filters are set, as the reference parses a record before any filter sees it.  CG:B and an unknown RG:Z value are
+// well-formed (the reference reads them); they are refused only in the records that become reads, where the device cannot represent them.
+__device__ uint32_t check_record(const uint8_t* r, uint64_t rec_len, int n_contigs, RgNames G, int32_t* rg_out, uint8_t* optf_out) {
     uint32_t bad = 0;
-    const uint64_t rec_len = (st + 4 <= A.n_bytes) ? (uint64_t)rd32(r) + 4 : 0;      // block_size counts the bytes after itself
-    if (rec_len < BAM_FIXED || st + rec_len > A.n_bytes || (A.chained && A.start[i + 1] != st + rec_len)) { atomicOr(A.err, DERR_BAM); A.len_qname[i] = A.len_cigar[i] = A.len_seq[i] = A.len_qual[i] = 0; return; }
-    const int32_t refid = (int32_t)rd32(r + 4), pos = (int32_t)rd32(r + 8);
-    const uint32_t l_name = r[12], mapq = r[13], n_cig = rd16(r + 16), flag = rd16(r + 18);
-    const int32_t l_seq = (int32_t)rd32(r + 20), nref = (int32_t)rd32(r + 24), pnext = (int32_t)rd32(r + 28), tlen = (int32_t)rd32(r + 32);
+    const int32_t refid = (int32_t)rd32(r + 4);
+    const uint32_t l_name = r[12], n_cig = rd16(r + 16);
+    const int32_t l_seq = (int32_t)rd32(r + 20), nref = (int32_t)rd32(r + 24);
     // all lengths in 64 bits: a crafted l_seq near INT_MAX must not wrap (l_seq > rec_len is malformed whatever else the record says)
     const uint64_t lsq = l_seq < 0 ? 0ull : (uint64_t)(uint32_t)l_seq;
     const uint64_t var = (uint64_t)l_name + 4ull * n_cig + ((lsq + 1) >> 1) + lsq;
-    if (l_name < 1 || l_seq < 0 || lsq > rec_len || BAM_FIXED + var > rec_len || refid >= A.n_contigs || nref >= A.n_contigs) bad = 1;
-    const uint64_t k = A.n0 + i;
-    A.refid[k] = refid < 0 ? -1 : refid; A.pos[k] = pos + 1; A.flag[k] = (uint16_t)(A.clear_dup ? flag & ~(uint32_t)F_DUPLICATE : flag); A.mapq[k] = (uint8_t)mapq;
-    A.nref[k] = nref < 0 ? -1 : nref; A.pnext[k] = pnext + 1; A.tlen[k] = tlen;
-    int32_t rg = -1; uint8_t optf = 0;
+    if (l_name < 1 || l_seq < 0 || lsq > rec_len || BAM_FIXED + var > rec_len || refid >= n_contigs || nref >= n_contigs) bad = 1;
+    int32_t rg = -1; uint8_t optf = 0; bool cg = false;
     if (!bad) {
         // optional fields: tag[2] type[1] value (sam/bam-files.go:369-397)
         uint64_t x = BAM_FIXED + var;
@@ -75,7 +74,7 @@ __global__ void __launch_bounds__(256) bam_fixed_kernel(BamArgs A) {
                     const uint8_t sub = r[x]; const uint64_t cnt = rd32(r + x + 1);
                     const uint64_t es = (sub == 'c' || sub == 'C') ? 1 : ((sub == 's' || sub == 'S') ? 2 : ((sub == 'i' || sub == 'I' || sub == 'f') ? 4 : 0));
                     if (!es) bad = 1;
-                    if (t0 == 'C' && t1 == 'G') bad = 2;     // long-CIGAR convention: not supported here
+                    if (t0 == 'C' && t1 == 'G') cg = true;   // long-CIGAR convention: not supported here
                     if (cnt * es > rec_len) { bad = 1; break; }    // (cnt < 2^32, es <= 4: no overflow; bounded before it is added to x)
                     sz = 5 + cnt * es; break;
                 }
@@ -88,11 +87,11 @@ __global__ void __launch_bounds__(256) bam_fixed_kernel(BamArgs A) {
                 if (e >= rec_len) { bad = 1; break; }
                 if (t0 == 'R' && t1 == 'G' && ty == 'Z') {
                     rg = -2;                                   // present but (so far) unknown
-                    for (int g = 0; g < A.n_rg; g++) {
-                        const uint32_t a = A.rg_name_off[g], b = A.rg_name_off[g + 1];
+                    for (int g = 0; g < G.n; g++) {
+                        const uint32_t a = G.off[g], b = G.off[g + 1];
                         if ((uint64_t)(b - a) != e - x) continue;
                         bool same = true;
-                        for (uint32_t q = 0; q < b - a && same; q++) same = A.rg_names[a + q] == r[x + q];
+                        for (uint32_t q = 0; q < b - a && same; q++) same = G.names[a + q] == r[x + q];
                         if (same) { rg = g; break; }
                     }
                 }
@@ -101,8 +100,28 @@ __global__ void __launch_bounds__(256) bam_fixed_kernel(BamArgs A) {
         }
         if (x != rec_len && !bad) bad = 1;
     }
-    if (rg == -2) { atomicOr(A.err, DERR_BAM_RG); rg = -1; }
+    *rg_out = rg; *optf_out = optf;
+    return bad ? bad : (cg ? 2u : 0u);
+}
+
+__global__ void __launch_bounds__(256) bam_fixed_kernel(BamArgs A) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= A.n) return;
+    const uint64_t st = A.start[i];
+    const uint8_t* r = A.raw + st;
+    const uint64_t rec_len = (st + 4 <= A.n_bytes) ? (uint64_t)rd32(r) + 4 : 0;      // block_size counts the bytes after itself
+    if (rec_len < BAM_FIXED || st + rec_len > A.n_bytes || (A.chained && A.start[i + 1] != st + rec_len)) { atomicOr(A.err, DERR_BAM); A.len_qname[i] = A.len_cigar[i] = A.len_seq[i] = A.len_qual[i] = 0; return; }
+    const int32_t refid = (int32_t)rd32(r + 4), pos = (int32_t)rd32(r + 8);
+    const uint32_t l_name = r[12], mapq = r[13], n_cig = rd16(r + 16), flag = rd16(r + 18);
+    const int32_t l_seq = (int32_t)rd32(r + 20), nref = (int32_t)rd32(r + 24), pnext = (int32_t)rd32(r + 28), tlen = (int32_t)rd32(r + 32);
+    const uint64_t k = A.n0 + i;
+    A.refid[k] = refid < 0 ? -1 : refid; A.pos[k] = pos + 1; A.flag[k] = (uint16_t)(A.clear_dup ? flag & ~(uint32_t)F_DUPLICATE : flag); A.mapq[k] = (uint8_t)mapq;
+    A.nref[k] = nref < 0 ? -1 : nref; A.pnext[k] = pnext + 1; A.tlen[k] = tlen;
+    int32_t rg; uint8_t optf;
+    const uint32_t bad = check_record(r, rec_len, A.n_contigs, RgNames{A.rg_names, A.rg_name_off, A.n_rg}, &rg, &optf);
+    if (rg == -2) atomicOr(A.err, DERR_BAM_RG);
     if (bad) atomicOr(A.err, bad == 2 ? DERR_BAM_CG : DERR_BAM);
+    if (rg == -2) rg = -1;
     A.rg[k] = rg; A.optf[k] = optf;
     A.len_qname[i] = bad ? 0 : l_name - 1; A.len_cigar[i] = bad ? 0 : n_cig;
     A.len_seq[i] = bad ? 0 : (uint32_t)((l_seq + 1) >> 1); A.len_qual[i] = bad ? 0 : (uint32_t)l_seq;
@@ -112,12 +131,13 @@ __global__ void __launch_bounds__(256) bam_fixed_kernel(BamArgs A) {
 // keep[i] = 1 iff record i passes every requested predicate; also checks that the caller's offsets follow the block_size chain
 // intervals.Overlap (intervals/intervals.go:146-164) over one contig's flattened, start-sorted (start, end) pairs
 __device__ bool overlap_any(const int32_t* __restrict__ iv, uint64_t n, int32_t start, int32_t end) {
+    const int32_t end_1 = (int32_t)((uint32_t)end - 1u), start_1 = (int32_t)((uint32_t)start - 1u);   // end-1, start-1 in Go's int32: they wrap
     int64_t left = 0, right = (int64_t)n - 1;
     while (left <= right) {
         const int64_t mid = (left + right) / 2;
         const int32_t is = iv[2 * mid], ie = iv[2 * mid + 1];
-        if (is > end - 1) right = mid - 1;
-        else if (ie <= start - 1) left = mid + 1;
+        if (is > end_1) right = mid - 1;
+        else if (ie <= start_1) left = mid + 1;
         else return true;
     }
     return false;
@@ -137,36 +157,40 @@ __device__ __forceinline__ bool tag_int(const uint8_t* r, uint64_t x, uint8_t ty
 
 __global__ void __launch_bounds__(256) bam_keep_kernel(uint64_t n, const uint8_t* __restrict__ raw, const uint64_t* __restrict__ rec_off, uint64_t n_bytes,
                                                         uint32_t mask, int32_t min_mapq, const int32_t* const* __restrict__ regions, const uint64_t* __restrict__ n_regions, int n_contigs,
-                                                        uint32_t* __restrict__ keep, uint32_t* __restrict__ err) {
+                                                        RgNames G, uint32_t* __restrict__ keep, uint32_t* __restrict__ err) {
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const uint64_t st = rec_off[i], len = rec_off[i + 1] - st;
     const uint8_t* r = raw + st;
     if (len < BAM_FIXED || (uint64_t)rd32(r) + 4 != len) { atomicOr(err, DERR_BAM); keep[i] = 0; return; }
-    const int32_t refid = (int32_t)rd32(r + 4), pos = (int32_t)rd32(r + 8) + 1;
+    {   // the reference parses a record before any filter sees it: a malformed record fails the call even when a filter would drop it.
+        // (CG:B and an unknown RG:Z are left to bam_fixed_kernel, which sees the records that are kept.)
+        int32_t rg; uint8_t optf;
+        if (check_record(r, len, n_contigs, G, &rg, &optf) == 1) { atomicOr(err, DERR_BAM); keep[i] = 0; return; }
+    }
+    // from here on the record is well-formed: every length fits in len
+    const int32_t refid = (int32_t)rd32(r + 4), pos = (int32_t)(rd32(r + 8) + 1u);                                 // int32 + 1 wraps as in Go
     const uint32_t l_name = r[12], mapq = r[13], n_cig = rd16(r + 16), flag = rd16(r + 18);
     bool k = true;
     if ((mask & ELP_FILTER_UNMAPPED) && (flag & F_UNMAPPED)) k = false;                                           // RemoveUnmappedReads :73-75
     if ((mask & ELP_FILTER_UNMAPPED_STRICT) && ((flag & F_UNMAPPED) || pos == 0 || refid < 0)) k = false;          // RemoveUnmappedReadsStrict :79-83
-    if ((int32_t)mapq < min_mapq) k = false;                                                                      // RemoveMappingQualityLessThan :332-347
+    if ((int32_t)mapq < min_mapq) k = false;                                                                      // RemoveMappingQualityLessThan :332-347 (min_mapq as elp_set_ingest_filter stores it)
     if (k && (mask & ELP_FILTER_NON_EXACT)) {                                                                     // RemoveNonExactMappingReads :90-99: only M and S
         const uint64_t c0 = BAM_FIXED + (uint64_t)l_name;
-        if (c0 + 4ull * n_cig > len) { atomicOr(err, DERR_BAM); keep[i] = 0; return; }
         for (uint32_t q = 0; q < n_cig; q++) { const uint32_t o = r[c0 + 4 * q] & 15u; if (o != 0 && o != 4) { k = false; break; } }
     }
     if ((mask & ELP_FILTER_DUPLICATES) && (flag & F_DUPLICATE)) k = false;                                        // RemoveDuplicateReads :131-133 (flags of the input)
     if (k && (mask & (ELP_FILTER_NON_EXACT_STRICT | ELP_FILTER_TARGET_REGIONS))) {
-        const int32_t l_seq = (int32_t)rd32(r + 20);
-        const uint64_t c0 = BAM_FIXED + (uint64_t)l_name, lsq = l_seq < 0 ? 0ull : (uint64_t)(uint32_t)l_seq;
+        const uint64_t lsq = rd32(r + 20);
+        const uint64_t c0 = BAM_FIXED + (uint64_t)l_name;
         const uint64_t tags0 = c0 + 4ull * n_cig + ((lsq + 1) >> 1) + lsq;
-        if (l_seq < 0 || tags0 > len) { atomicOr(err, DERR_BAM); keep[i] = 0; return; }
         if (mask & ELP_FILTER_TARGET_REGIONS) {                                                                   // RemoveNonOverlappingReads :310-328
             int32_t a_end = pos;
             if (!(flag & F_UNMAPPED)) {
-                int32_t rl = 0, fl = 0;
-                for (uint32_t q = 0; q < n_cig; q++) { const uint32_t op = rd32(r + c0 + 4 * q); const uint32_t o = op & 15u; const int32_t ln = (int32_t)(op >> 4);
+                uint32_t rl = 0, fl = 0;                                                                          // int32 sums of Go, wrapping: kept unsigned
+                for (uint32_t q = 0; q < n_cig; q++) { const uint32_t op = rd32(r + c0 + 4 * q); const uint32_t o = op & 15u; const uint32_t ln = op >> 4;
                     if (o == 0 || o == 1 || o == 4 || o == 7 || o == 8) rl += ln; if (o == 0 || o == 2 || o == 3 || o == 7 || o == 8) fl += ln; }
-                if (rl > 0) a_end = pos + fl - 1;                                                                 // aln.End(), sam/sam-types.go:769-775
+                if ((int32_t)rl > 0) a_end = (int32_t)((uint32_t)pos + fl - 1u);                                  // aln.End(), sam/sam-types.go:769-775
             }
             if (refid < 0 || refid >= n_contigs || !regions || !overlap_any(regions[refid], n_regions[refid], pos, a_end)) k = false;   // no regions for RNAME: Overlap(nil) is false
         }
@@ -184,9 +208,9 @@ __global__ void __launch_bounds__(256) bam_keep_kernel(uint64_t n, const uint8_t
                     case 's': case 'S': sz = 2; break;
                     case 'i': case 'I': case 'f': sz = 4; break;
                     case 'Z': case 'H': { uint64_t e = x; while (e < len && r[e] != 0) e++; sz = e - x + 1; break; }
-                    case 'B': { if (x + 5 > len) { sz = len; break; } const uint8_t sub = r[x]; const uint64_t cnt = rd32(r + x + 1);
+                    case 'B': { const uint8_t sub = r[x]; const uint64_t cnt = rd32(r + x + 1);
                                 sz = 5 + cnt * ((sub == 'c' || sub == 'C') ? 1 : ((sub == 's' || sub == 'S') ? 2 : 4)); break; }
-                    default: sz = len;                                                                            // malformed: bam_fixed_kernel reports it
+                    default: sz = len;                                                                            // (check_record refused the record)
                 }
                 if (x + sz > len) break;
                 if (which >= 0 && !(seen & (1u << which))) {                                                      // (TAGS.Get returns the first occurrence)
@@ -246,10 +270,11 @@ __global__ void __launch_bounds__(256) bam_out_len_kernel(uint64_t n, uint64_t f
     const uint64_t kk = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (kk < n) len[kk] = rd32(all + all_start[perm[out_pos(sel, first, kk)]]) + 4;
 }
-// one warp per output record: copy the stored record, patch FLAG (bytes 18..19 of the record with its block_size) and QUAL
+// one warp per output record: copy the stored record, patch MAPQ (byte 13 of the record with its block_size; elp_clean_sam sets it to 0
+// for unmapped reads, otherwise it equals the stored byte), FLAG (bytes 18..19) and QUAL
 __global__ void __launch_bounds__(256) bam_out_copy_kernel(uint64_t n, uint64_t first, const uint32_t* __restrict__ sel, const uint32_t* __restrict__ perm, const uint64_t* __restrict__ all_start,
                                                             const uint8_t* __restrict__ all, const uint64_t* __restrict__ out_off, uint8_t* __restrict__ out,
-                                                            const uint16_t* __restrict__ s_flag, const uint64_t* __restrict__ s_out_off, const uint8_t* __restrict__ qual_out) {
+                                                            const uint16_t* __restrict__ s_flag, const uint8_t* __restrict__ s_mapq, const uint64_t* __restrict__ s_out_off, const uint8_t* __restrict__ qual_out) {
     const unsigned lane = threadIdx.x & 31;
     const uint64_t kk = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (kk >= n) return;
@@ -262,6 +287,7 @@ __global__ void __launch_bounds__(256) bam_out_copy_kernel(uint64_t n, uint64_t 
     const int32_t l_seq = (int32_t)rd32(r + 20);
     const uint64_t q0 = BAM_FIXED + (uint64_t)l_name + 4ull * n_cig + (uint64_t)((l_seq + 1) >> 1), q1 = q0 + (uint64_t)l_seq;
     const uint16_t f = s_flag[k];
+    const uint8_t mq = s_mapq[k];
     const uint8_t* nq = qual_out ? qual_out + s_out_off[k] : nullptr;
     for (uint64_t t = lane; t < len; t += 32) {
         uint8_t v = r[t];
@@ -269,6 +295,7 @@ __global__ void __launch_bounds__(256) bam_out_copy_kernel(uint64_t n, uint64_t 
         else if (nq && t >= q0 && t < q1) v = nq[t - q0];
         o[t] = v;
     }
+    if (lane == 13) o[13] = mq;                  // (this lane copied byte 13 in its first step: outside the per-byte loop, no extra compare there)
 }
 
 // ---- write-phase filters (elp_set_output_filter; cmd/filter.go:803-902) ----
@@ -309,11 +336,11 @@ __global__ void __launch_bounds__(256) bam_out_fields_measure_kernel(uint64_t n,
     }
     if ((threadIdx.x & 31) == 0) len[kk] = (uint32_t)x;
 }
-// emit: the fixed part and the variable fields with block_size, FLAG and QUAL patched, then the kept fields in their order
+// emit: the fixed part and the variable fields with block_size, MAPQ, FLAG and QUAL patched, then the kept fields in their order
 __global__ void __launch_bounds__(256) bam_out_fields_emit_kernel(uint64_t n, uint64_t first, const uint32_t* __restrict__ sel, const uint32_t* __restrict__ perm,
                                                                   const uint64_t* __restrict__ all_start, const uint8_t* __restrict__ all, const uint32_t* __restrict__ drop,
                                                                   const uint64_t* __restrict__ out_off, uint8_t* __restrict__ out,
-                                                                  const uint16_t* __restrict__ s_flag, const uint64_t* __restrict__ s_out_off, const uint8_t* __restrict__ qual_out) {
+                                                                  const uint16_t* __restrict__ s_flag, const uint8_t* __restrict__ s_mapq, const uint64_t* __restrict__ s_out_off, const uint8_t* __restrict__ qual_out) {
     const unsigned lane = threadIdx.x & 31;
     const uint64_t kk = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (kk >= n) return;
@@ -325,6 +352,7 @@ __global__ void __launch_bounds__(256) bam_out_fields_emit_kernel(uint64_t n, ui
     const int32_t l_seq = (int32_t)rd32(r + 20);
     const uint64_t q1 = t0, q0 = q1 - (uint64_t)l_seq;
     const uint16_t f = s_flag[k];
+    const uint8_t mq = s_mapq[k];
     const uint8_t* nq = qual_out ? qual_out + s_out_off[k] : nullptr;
     for (uint64_t t = lane; t < t0; t += 32) {
         uint8_t v = r[t];
@@ -333,6 +361,7 @@ __global__ void __launch_bounds__(256) bam_out_fields_emit_kernel(uint64_t n, ui
         else if (nq && t >= q0) v = nq[t - q0];
         o[t] = v;
     }
+    if (lane == 13) o[13] = mq;                  // (as in bam_out_copy_kernel)
     uint64_t t = t0, x = t0;
     while (t + 3 <= rec) {
         const uint64_t fe = tagwalk::field_end(r, t, rec);
@@ -405,11 +434,21 @@ int bam_ingest_core(elp_ctx* c, uint64_t n_bytes, uint64_t nrec) {
     cudaStream_t s = c->stream;
     TRY(grow(c, c->bam_start, nrec + 2, 0));
     const uint64_t* d_start = c->bam_off.p;                   // without filters: record i is read n0 + i
+    // @RG ID strings for the RG:Z match
+    if (!c->d_rg_names && c->n_rg) {
+        std::vector<uint8_t> names; std::vector<uint32_t> off(1, 0);
+        for (auto& id : c->rg_ids) { names.insert(names.end(), id.begin(), id.end()); off.push_back((uint32_t)names.size()); }
+        CUDA_TRY(c, cudaMalloc(&c->d_rg_names, std::max<size_t>(names.size(), 1)));
+        CUDA_TRY(c, cudaMalloc(&c->d_rg_name_off, off.size() * 4));
+        CUDA_TRY(c, cudaMemcpy(c->d_rg_names, names.data(), names.size(), cudaMemcpyHostToDevice));
+        CUDA_TRY(c, cudaMemcpy(c->d_rg_name_off, off.data(), off.size() * 4, cudaMemcpyHostToDevice));
+    }
     if (c->filter_mask || c->filter_min_mapq > 0) {
         TRY(grow(c, c->scan_tmp, nrec + 8, 0)); TRY(grow(c, c->off_stage, nrec + 2, 0));
         c->begin("bam_keep", (double)nrec * 48);
         if (c->filter_mask & ELP_FILTER_TARGET_REGIONS) { int rcr = upload_regions(c); if (rcr) return rcr; }
-        bam_keep_kernel<<<nblk(nrec, 256), 256, 0, s>>>(nrec, c->bam_raw.p, c->bam_off.p, n_bytes, c->filter_mask, c->filter_min_mapq, c->d_region_ptrs, c->d_n_regions, c->n_contigs, c->scan_tmp.p, c->d_err);
+        bam_keep_kernel<<<nblk(nrec, 256), 256, 0, s>>>(nrec, c->bam_raw.p, c->bam_off.p, n_bytes, c->filter_mask, c->filter_min_mapq, c->d_region_ptrs, c->d_n_regions, c->n_contigs,
+                                                        RgNames{c->d_rg_names, c->d_rg_name_off, c->n_rg}, c->scan_tmp.p, c->d_err);
         c->end(); LAUNCH_CHECK(c);
         TRY(exclusive_scan_u32_to_u64(c, c->scan_tmp.p, c->off_stage.p, nrec));
         bam_compact_kernel<<<nblk(nrec, 256), 256, 0, s>>>(nrec, c->scan_tmp.p, c->off_stage.p, c->bam_off.p, c->bam_start.p); c->launches++;
@@ -423,15 +462,6 @@ int bam_ingest_core(elp_ctx* c, uint64_t n_bytes, uint64_t nrec) {
         if (bn == 0) return ELP_OK;
     }
     const uint64_t n1 = n0 + bn;
-    // @RG ID strings for the RG:Z match
-    if (!c->d_rg_names && c->n_rg) {
-        std::vector<uint8_t> names; std::vector<uint32_t> off(1, 0);
-        for (auto& id : c->rg_ids) { names.insert(names.end(), id.begin(), id.end()); off.push_back((uint32_t)names.size()); }
-        CUDA_TRY(c, cudaMalloc(&c->d_rg_names, std::max<size_t>(names.size(), 1)));
-        CUDA_TRY(c, cudaMalloc(&c->d_rg_name_off, off.size() * 4));
-        CUDA_TRY(c, cudaMemcpy(c->d_rg_names, names.data(), names.size(), cudaMemcpyHostToDevice));
-        CUDA_TRY(c, cudaMemcpy(c->d_rg_name_off, off.data(), off.size() * 4, cudaMemcpyHostToDevice));
-    }
     TRY(grow(c, c->refid, n1 + 1, n0)); TRY(grow(c, c->pos, n1 + 1, n0)); TRY(grow(c, c->nref, n1 + 1, n0)); TRY(grow(c, c->pnext, n1 + 1, n0)); TRY(grow(c, c->tlen, n1 + 1, n0));
     TRY(grow(c, c->rg, n1 + 1, n0)); TRY(grow(c, c->flag, n1 + 2, n0)); TRY(grow(c, c->mapq, n1 + 1, n0)); TRY(grow(c, c->optf, n1 + 1, n0));
     TRY(grow(c, c->qname_off, n1 + 2, n0 + 1)); TRY(grow(c, c->cigar_off, n1 + 2, n0 + 1)); TRY(grow(c, c->qual_off, n1 + 2, n0 + 1)); TRY(grow(c, c->seq_off, n1 + 2, n0 + 1));
@@ -554,10 +584,10 @@ extern "C" int elp_fetch_bam(elp_ctx* c, uint64_t first, uint64_t n, uint8_t* ou
     if (c->out_fields) {
         c->begin("bam_out_fields_emit", (double)c->n_bam * (double)n / (double)std::max<uint64_t>(c->n, 1) + (double)total);
         bam_out_fields_emit_kernel<<<nblk(n * 32, 256), 256, 0, c->stream>>>(n, first, sel, c->perm.p, c->bam_all_off.p, c->bam_all.p, c->d_out_drop, c->off_stage.p, c->bam_raw.p,
-                                                                             c->s_flag.p, c->s_out_off.p, c->qual_out_valid ? c->qual_out.p : nullptr);
+                                                                             c->s_flag.p, c->s_mapq.p, c->s_out_off.p, c->qual_out_valid ? c->qual_out.p : nullptr);
     } else {
         c->begin("bam_format", 2.0 * (double)total);
-        bam_out_copy_kernel<<<nblk(n * 32, 256), 256, 0, c->stream>>>(n, first, sel, c->perm.p, c->bam_all_off.p, c->bam_all.p, c->off_stage.p, c->bam_raw.p, c->s_flag.p, c->s_out_off.p,
+        bam_out_copy_kernel<<<nblk(n * 32, 256), 256, 0, c->stream>>>(n, first, sel, c->perm.p, c->bam_all_off.p, c->bam_all.p, c->off_stage.p, c->bam_raw.p, c->s_flag.p, c->s_mapq.p, c->s_out_off.p,
                                                                       c->qual_out_valid ? c->qual_out.p : nullptr);
     }
     c->end(); LAUNCH_CHECK(c);
@@ -590,7 +620,9 @@ extern "C" int elp_set_target_regions(elp_ctx* c, int32_t contig, const int32_t*
 extern "C" int elp_set_ingest_filter(elp_ctx* c, uint32_t mask, int32_t min_mapq) {
     if (!c) return ELP_EINVAL;
     if (mask & ~(uint32_t)(ELP_FILTER_UNMAPPED | ELP_FILTER_UNMAPPED_STRICT | ELP_FILTER_NON_EXACT | ELP_FILTER_DUPLICATES | ELP_FILTER_NON_EXACT_STRICT | ELP_FILTER_TARGET_REGIONS | ELP_FILTER_CLEAR_DUPLICATE_FLAG)) return c->fail(E_INVAL, "elp_set_ingest_filter: unknown filter bits 0x%x", mask);
-    c->filter_mask = mask & ~(uint32_t)ELP_FILTER_CLEAR_DUPLICATE_FLAG; c->filter_min_mapq = min_mapq;   // (the clear drops no record)
+    c->filter_mask = mask & ~(uint32_t)ELP_FILTER_CLEAR_DUPLICATE_FLAG;   // (the clear drops no record)
+    // RemoveMappingQualityLessThan(mq int): 0 no filter, above 255 every read dropped, else MAPQ >= byte(mq) -- so -1 keeps MAPQ 255 only
+    c->filter_min_mapq = min_mapq == 0 ? 0 : (min_mapq > 255 ? 256 : (int32_t)((uint32_t)min_mapq & 255u));
     c->clear_dup = (mask & ELP_FILTER_CLEAR_DUPLICATE_FLAG) != 0;
     return ELP_OK;
 }

@@ -11,6 +11,9 @@ namespace {
 inline unsigned nblk(uint64_t n, int t) { return (unsigned)((n + t - 1) / t); }
 __device__ __forceinline__ int cons_read(uint32_t o) { return o == 0 || o == 1 || o == 4 || o == 7 || o == 8; }
 __device__ __forceinline__ int cons_ref(uint32_t o) { return o == 0 || o == 2 || o == 3 || o == 7 || o == 8; }
+// int32 addition as Go does it: wraps (`pos += endPos` doubles pos, so a long CIGAR overflows it)
+__device__ __forceinline__ int32_t wadd(int32_t a, int32_t b) { return (int32_t)((uint32_t)a + (uint32_t)b); }
+__device__ __forceinline__ int32_t wsub(int32_t a, int32_t b) { return (int32_t)((uint32_t)a - (uint32_t)b); }
 
 // walks one read; out == nullptr: only counts.  returns the new number of operations, or -1 if the read keeps its CIGAR
 __device__ int clean_one(const uint32_t* __restrict__ cg, int nc, int32_t pos, int32_t refid, uint16_t flag, const int32_t* __restrict__ contig_len, int n_contigs,
@@ -18,29 +21,29 @@ __device__ int clean_one(const uint32_t* __restrict__ cg, int nc, int32_t pos, i
     if (flag & F_UNMAPPED) return -1;
     const int32_t length = (refid >= 0 && refid < n_contigs) ? contig_len[refid] : 0;       // referenceSequenceTable[aln.RNAME]: 0 for a name that is not an @SQ
     int32_t reflen = 0, readlen = 0;
-    for (int i = 0; i < nc; i++) { const uint32_t o = cg[i] & 15u; const int32_t l = (int32_t)(cg[i] >> 4); reflen += cons_ref(o) * l; readlen += cons_read(o) * l; }
-    if (!(pos + reflen - 1 > length)) return -1;                                                // aln.End() > length
-    int32_t clipFrom = length - pos + 1;
+    for (int i = 0; i < nc; i++) { const uint32_t o = cg[i] & 15u; const int32_t l = (int32_t)(cg[i] >> 4); reflen = wadd(reflen, cons_ref(o) * l); readlen = wadd(readlen, cons_read(o) * l); }
+    if (!(wsub(wadd(pos, reflen), 1) > length)) return -1;                                     // aln.End() > length
+    int32_t clipFrom = wadd(wsub(length, pos), 1);
     // softClipEndOfRead
-    int32_t p = 0; clipFrom--;
+    int32_t p = 0; clipFrom = wsub(clipFrom, 1);
     int no = 0;
     for (int i = 0; i < nc; i++) {
         const uint32_t o = cg[i] & 15u; const int32_t l = (int32_t)(cg[i] >> 4);
-        const int32_t endPos = p + cons_read(o) * l;
+        const int32_t endPos = wadd(p, cons_read(o) * l);
         if (endPos < clipFrom) { if (out) out[no] = cg[i]; no++; }
         else {
-            int32_t clipped = readlen + clipFrom;
-            const int32_t rel = clipFrom - p;
+            int32_t clipped = wadd(readlen, clipFrom);
+            const int32_t rel = wsub(clipFrom, p);
             // elementStradlessClippedRead
             if (cons_read(o)) {
                 if (cons_ref(o)) { if (rel > 0) { if (out) out[no] = ((uint32_t)rel << 4) | o; no++; } }
-                else clipped += rel;
+                else clipped = wadd(clipped, rel);
             } else if (rel != 0) atomicOr(err, DERR_CLEANSAM);
             if (out) out[no] = ((uint32_t)clipped << 4) | 4u;
             no++;
             break;
         }
-        p += endPos;
+        p = wadd(p, endPos);
     }
     return no;
 }

@@ -2,7 +2,7 @@
 // with formatSamTag :485-546 and cigarToString :548-557, applied to parseBamAlignment, sam/bam-files.go:317-400, of every record a
 // BAM-in or SAM-in run writes to a SAM file).
 //
-// Line k is FormatAlignment(parseBamAlignment(stored record of perm[k])) with the context's FLAG and, once elp_bqsr_apply has run, the
+// Line k is FormatAlignment(parseBamAlignment(stored record of perm[k])) with the context's FLAG and MAPQ and, once elp_bqsr_apply has run, the
 // recalibrated QUAL: the bytes elp_fetch_bam returns, written as text.  One warp per line; one device function (format_line) in three modes:
 //   sam_out_measure  byte length of every line, number of float values (f fields and B:f elements) in it
 //   sam_out_float    only when a line holds a float value: the float bits into one list (the host formats them, gofloat.hpp), then the
@@ -53,7 +53,8 @@ struct FmtArgs {
     const uint32_t* sel;                                                  // output positions of the records the record filters keep, or null
     const uint32_t* drop;                                                 // 65 536-bit tag table of the field filter, or null
     const uint32_t* perm; const uint64_t* all_start; const uint8_t* all;
-    const uint16_t* flag; const uint64_t* qoff; const uint8_t* qual;      // qual: recalibrated QUAL in output order, or null (stored QUAL)
+    const uint16_t* flag; const uint8_t* mapq;                            // in output order: FLAG after marking, MAPQ after elp_clean_sam
+    const uint64_t* qoff; const uint8_t* qual;                            // qual: recalibrated QUAL in output order, or null (stored QUAL)
     const uint8_t* names; const uint32_t* name_off; const int32_t* canon; int n_contigs;   // canon[n_contigs]: the canon of "*" (-1 if no @SQ has that name)
     uint32_t* len; uint32_t* nf;                                          // measure: line length, float values per line
     const uint64_t* fbase; uint32_t* fbits;                               // list: slot of a line's first float value, float bits
@@ -132,7 +133,7 @@ template <int M> __device__ void format_line(const FmtArgs& A, uint64_t kk, cons
     const uint64_t k = A.sel ? A.sel[A.first + kk] : A.first + kk;
     const uint8_t* r = A.all + A.all_start[A.perm[k]];
     const uint64_t rec = (uint64_t)rd32(r) + 4;
-    const uint32_t l_name = r[12], mapq = r[13], ncig = rd16(r + 16), flag = A.flag[k];
+    const uint32_t l_name = r[12], mapq = A.mapq[k], ncig = rd16(r + 16), flag = A.flag[k];
     const int32_t refid = (int32_t)rd32(r + 4), nref = (int32_t)rd32(r + 24), tlen = (int32_t)rd32(r + 32);
     const int32_t pos1 = (int32_t)(rd32(r + 8) + 1u), pnext1 = (int32_t)(rd32(r + 28) + 1u);   // int32(x) + 1 wraps as in Go
     const uint64_t L = rd32(r + 20);                                      // l_seq >= 0 (checked at ingest)
@@ -336,7 +337,7 @@ int sam_out_prepare(elp_ctx* c, uint64_t first, uint64_t n, const uint32_t* sel,
     TRY(grow(c, c->scan_tmp, n + 8, 0)); TRY(grow(c, c->off_stage, n + 2, 0)); TRY(grow(c, S.nf, n + 8, 0));
     FmtArgs A{};
     A.n = n; A.first = first; A.sel = sel; A.drop = c->out_fields ? c->d_out_drop : nullptr; A.perm = c->perm.p; A.all_start = c->bam_all_off.p; A.all = c->bam_all.p;
-    A.flag = c->s_flag.p; A.qoff = c->s_out_off.p; A.qual = c->qual_out_valid ? c->qual_out.p : nullptr;
+    A.flag = c->s_flag.p; A.mapq = c->s_mapq.p; A.qoff = c->s_out_off.p; A.qual = c->qual_out_valid ? c->qual_out.p : nullptr;
     A.names = S.d_names; A.name_off = S.d_name_off; A.canon = S.d_canon; A.n_contigs = c->n_contigs;
     A.len = c->scan_tmp.p; A.nf = S.nf.p; A.small = S.d_small;
     CUDA_TRY(c, cudaMemsetAsync(S.d_small, 0, 16, s));

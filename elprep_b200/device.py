@@ -314,7 +314,7 @@ class Context:
 
     def fetch_bam(self, first=0, n=None):
         """-> (uint8 record bytes, uint64 record offsets [n+1]) of output records [first, first+n) (of those that pass the output filter),
-        FLAG and QUAL patched"""
+        FLAG, MAPQ and QUAL patched"""
         n = self._n_out(first) if n is None else n
         nb = int(self.L.elp_fetch_bam_bytes(self.h, first, n))
         out, off = np.empty(max(nb, 1), np.uint8), np.empty(n + 1, np.uint64)
@@ -323,7 +323,7 @@ class Context:
 
     def fetch_sam(self, first=0, n=None):
         """-> (uint8 SAM text, uint64 line offsets [n+1]) of output records [first, first+n): FormatAlignment of each stored record with
-        FLAG and QUAL patched, one '\\n'-terminated alignment line per record, no header (records as in fetch_bam)"""
+        FLAG, MAPQ and QUAL patched, one '\\n'-terminated alignment line per record, no header (records as in fetch_bam)"""
         n = self._n_out(first) if n is None else n
         nb = int(self.L.elp_fetch_sam_bytes(self.h, first, n)) if n else 0
         out, off = np.empty(max(nb, 1), np.uint8), np.empty(n + 1, np.uint64)

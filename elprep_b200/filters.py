@@ -134,10 +134,14 @@ def CleanSam(header):
 
 
 def RemoveMappingQualityLessThan(mq):
-    """filters.RemoveMappingQualityLessThan (simple-filters.go:332-347) -> Filter"""
+    """filters.RemoveMappingQualityLessThan (simple-filters.go:332-347) -> Filter: nil for 0, every read dropped above 255, else MAPQ
+    compared against byte(mq) -- so -1 keeps MAPQ 255 only and -256 keeps every read (elp_set_ingest_filter applies the same rule)"""
     if mq == 0:
         return None
-    return lambda header: (lambda batch: _keep(batch, batch.mapq.astype(np.int64) >= mq))
+    if mq > 255:
+        return lambda header: (lambda batch: _keep(batch, np.zeros(batch.n, bool)))
+    mapq = int(mq) & 255
+    return lambda header: (lambda batch: _keep(batch, batch.mapq.astype(np.int64) >= mapq))
 
 
 def RemoveDuplicateReads(header):

@@ -141,8 +141,13 @@ int elp_append_sam(elp_ctx *ctx, const char *text, uint64_t n_bytes);
 /* Per-record filters fused into elp_append_bam (SURVEY.md 8f row 4): a record that fails a requested predicate never becomes a read
  * of the context (later calls; elp_n_filtered counts them).  filters/simple-filters.go: RemoveUnmappedReads (:73-75),
  * RemoveUnmappedReadsStrict (:79-83: FLAG 0x4, POS 0 or RNAME *), RemoveNonExactMappingReads (:90-99: only M and S operations),
- * RemoveMappingQualityLessThan (:332-347: keeps MAPQ >= min_mapq), RemoveDuplicateReads (:131-133, on the FLAG the record comes
- * in with).  With elp_append_batch the caller's marshaller applies its filters to the []*Alignment before building columns. */
+ * RemoveMappingQualityLessThan (:332-347, min_mapq as the reference's `mq int`: 0 keeps every read, more than 255 drops every read,
+ * anything else keeps MAPQ >= (min_mapq & 255), so -1 keeps MAPQ 255 only and -256 keeps every read), RemoveDuplicateReads (:131-133, on
+ * the FLAG the record comes in with).  Every record of a call is checked for structure whether a filter drops it or not: a malformed
+ * record fails the call (ELP_EBAM) with any filter mask, as the reference parses a record before any filter sees it.  The two
+ * well-formed records the device cannot hold -- an RG:Z value that is not an @RG ID, the CG:B long-CIGAR convention -- are refused
+ * only when they pass the filters; a record a filter drops never needs them, so the call gives the reference's result.  With
+ * elp_append_batch the caller's marshaller applies its filters to the []*Alignment before building columns. */
 #define ELP_FILTER_UNMAPPED 1u
 #define ELP_FILTER_UNMAPPED_STRICT 2u
 #define ELP_FILTER_NON_EXACT 4u
@@ -160,8 +165,9 @@ uint64_t elp_n_filtered(const elp_ctx *ctx);
 uint64_t elp_n_reads(const elp_ctx *ctx);
 /* filters.CleanSam (filters/simple-filters.go:292-306, softClipEndOfRead filters/utils.go:82-119) over the reads appended so far (either ingest
  * path; call before elp_sort_markdup): MAPQ of unmapped reads becomes 0; a read that runs past the end of its contig gets its CIGAR soft-clipped
- * there.  Returns the number of rewritten CIGARs in *n_rewritten (may be NULL).  After a rewrite elp_fetch_bam is refused (the stored records
- * still carry the old CIGAR); the columnar elp_fetch is unaffected. */
+ * there.  Returns the number of rewritten CIGARs in *n_rewritten (may be NULL).  The new MAPQ reaches both byte outputs (elp_fetch_bam and
+ * elp_fetch_sam write the MAPQ column); only a CIGAR rewrite makes them refuse (the stored records still carry the old CIGAR); the columnar
+ * elp_fetch is unaffected. */
 int elp_clean_sam(elp_ctx *ctx, uint64_t *n_rewritten);
 
 /* filters.MarkDuplicates (filters/mark-duplicates.go:406-445) + By(CoordinateLess).ParallelStableSort in the
@@ -266,13 +272,13 @@ int elp_fetch_async(elp_ctx *ctx, uint64_t first, uint64_t n, uint32_t *record_i
 int elp_fetch_wait(elp_ctx *ctx);
 /* per-read temps of adaptAlignment (filters/mark-duplicates.go:153-156), arrival order; for parity tests */
 /* The same as BAM alignment records (only if every read came in through elp_append_bam or elp_append_sam): output records [first, first+n) are
- * the stored records with FLAG and -- once elp_bqsr_apply has run -- QUAL replaced; names, CIGAR and optional fields are the
+ * the stored records with FLAG, MAPQ and -- once elp_bqsr_apply has run -- QUAL replaced; names, CIGAR and optional fields are the
  * input bytes.  This stands in for formatting every *sam.Alignment again (sam/bam-files.go:635-735); the caller BGZF-
  * compresses the result.  record_off[n+1] may be NULL. */
 uint64_t elp_fetch_bam_bytes(elp_ctx *ctx, uint64_t first, uint64_t n);
 int elp_fetch_bam(elp_ctx *ctx, uint64_t first, uint64_t n, uint8_t *out, uint64_t capacity, uint64_t *record_off);
 /* The same as SAM text alignment lines (FormatAlignment, sam/sam-files.go:563-598, of parseBamAlignment of the record elp_fetch_bam returns):
- * output records [first, first+n) as lines ending in '\n', with the context's FLAG and -- once elp_bqsr_apply has run -- QUAL; no header
+ * output records [first, first+n) as lines ending in '\n', with the context's FLAG, MAPQ and -- once elp_bqsr_apply has run -- QUAL; no header
  * lines (the caller writes the header text).  line_off[n+1] (may be NULL): offset of every line in out.  The reference's quirks are kept:
  * every integer tag prints as i, POS / PNEXT wrap in int32, RNEXT is '=' when its @SQ name equals RNAME's, f values print as Go's
  * strconv 'g' shortest float32, H digits in lower case.  Refusals as elp_fetch_bam (ELP_ESTATE before elp_sort_markdup, for reads that did
@@ -291,7 +297,7 @@ int elp_fetch_sam(elp_ctx *ctx, uint64_t first, uint64_t n, char *out, uint64_t 
  *    (KeepOptionalFields, :261-288; active iff ELP_OUT_KEEP_FIELDS, n_keep == 0 drops every optional field), the order in which filters2
  *    appends them.  A string matches the 2-byte tag when it equals it, case-sensitively; a string that is not 2 bytes long (also "") matches
  *    no field.  Repeated tags are all dropped or all kept (SmallMap.DeleteIf).  The fields that remain keep their bytes and their order;
- *    block_size is rewritten; FLAG and QUAL are patched as without a filter.  "all" / "none" and TrimSpace belong to the caller's flag parsing.
+ *    block_size is rewritten; FLAG, MAPQ and QUAL are patched as without a filter.  "all" / "none" and TrimSpace belong to the caller's flag parsing.
  *  - Lifetime.  The setting survives elp_reset, like the ingest filter; the selection is rebuilt after elp_sort_markdup, elp_set_output_filter
  *    or elp_reset.  Unknown mask bits, and keep_tags without ELP_OUT_KEEP_FIELDS, are ELP_EINVAL.  A range past elp_n_output is ELP_EINVAL and
  *    nothing is written; the other refusals of the fetch calls still apply (before elp_sort_markdup, after elp_clean_sam, ...). */

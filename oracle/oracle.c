@@ -689,10 +689,11 @@ int64_t orc_flatten(int32_t *se, int64_t len) {
     return len;
 }
 int orc_overlap(const int32_t *se, int64_t n, int32_t start, int32_t end) {
+    const int32_t e1 = (int32_t)((uint32_t)end - 1u), s1 = (int32_t)((uint32_t)start - 1u);   /* end-1, start-1 in Go's int32: they wrap */
     for (int64_t left = 0, right = n - 1; left <= right;) {
         int64_t mid = (left + right) / 2;
         int32_t is = se[2 * mid], ie = se[2 * mid + 1];
-        if (is > end - 1) right = mid - 1; else if (ie <= start - 1) left = mid + 1; else return 1;
+        if (is > e1) right = mid - 1; else if (ie <= s1) left = mid + 1; else return 1;
     }
     return 0;
 }

@@ -7,44 +7,11 @@ import numpy as np
 import pytest
 
 from elprep_b200 import device, filters, synth, _lib
+from ingestfilter_ref import clean_cigar as _ref_clean_cigar
 from util import encode_bam
 
 pytestmark = pytest.mark.gpu
 SMALL = [("chr20", 300_000), ("chr21", 200_000)]
-
-
-def _ref_clean_cigar(ops, pos, length, unmapped):
-    """CleanSam's CIGAR rewrite, operation by operation as the reference does it (incl. `pos += endPos` and the clipped length)"""
-    cr = lambda o: 1 if o in (0, 1, 4, 7, 8) else 0
-    cf = lambda o: 1 if o in (0, 2, 3, 7, 8) else 0
-    if unmapped:
-        return list(ops)
-    reflen = sum(cf(o & 15) * (o >> 4) for o in ops)
-    if not (pos + reflen - 1 > length):
-        return list(ops)
-    clip_from = length - pos + 1
-    p, new = 0, []
-    clip_from -= 1
-    readlen = sum(cr(o & 15) * (o >> 4) for o in ops)
-    for op in ops:
-        o, l = op & 15, op >> 4
-        end = p + cr(o) * l
-        if end < clip_from:
-            new.append(op)
-        else:
-            clipped, rel = readlen + clip_from, clip_from - p
-            if cr(o):
-                if cf(o):
-                    if rel > 0:
-                        new.append((rel << 4) | o)
-                else:
-                    clipped += rel
-            elif rel != 0:
-                raise AssertionError("Unexpected non-0 relative clipping position in CleanSam.")
-            new.append((clipped << 4) | 4)
-            break
-        p += end
-    return new
 
 
 def test_clean_sam_matches_reference_rule():

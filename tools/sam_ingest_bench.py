@@ -1,7 +1,8 @@
 """Ingest rate of SAM text (elp_append_sam) against BAM records (elp_append_bam) of the same reads, in one process.
 Whole-call time: host clock around the appends of one context, ending in a device synchronise, the two paths alternated.
 Device-kernel time: CUDA events of every kernel of the appends (kernel_stats), in separate runs with profiling on.
-usage: python tools/sam_ingest_bench.py [n_pairs] [reps]   -> one JSON line on stdout"""
+With an ingest filter (mask and min_mapq of elp_set_ingest_filter), both paths run the fused filter on every append.
+usage: python tools/sam_ingest_bench.py [n_pairs] [reps] [filter_mask] [min_mapq]   -> one JSON line on stdout"""
 import json
 import os
 import subprocess
@@ -18,6 +19,8 @@ from samtext import sam_text
 
 n_pairs = int(sys.argv[1]) if len(sys.argv) > 1 else 5_000_000
 reps = int(sys.argv[2]) if len(sys.argv) > 2 else 3
+filter_mask = int(sys.argv[3]) if len(sys.argv) > 3 else 0
+min_mapq = int(sys.argv[4]) if len(sys.argv) > 4 else 0
 CH = 8                                                          # appends per pass, cut at line / record boundaries
 
 
@@ -55,6 +58,7 @@ def run_bam(ctx):
 
 paths = {"sam": run_sam, "bam": run_bam}
 ctx = device.Context(w.header)
+ctx.set_ingest_filter(filter_mask, min_mapq)
 wall = {k: [] for k in paths}
 for rep in range(reps + 1):                                     # rep 0 warms up every shape and allocation
     for k, f in paths.items():
@@ -63,12 +67,14 @@ for rep in range(reps + 1):                                     # rep 0 warms up
         f(ctx)
         ctx.synchronize()
         dt = time.perf_counter() - t0
-        assert ctx.n == n
+        assert ctx.n + ctx.n_filtered() == n and (ctx.n == n or filter_mask or min_mapq)
+        kept = ctx.n
         if rep:
             wall[k].append(dt)
 ctx.close()
 
 prof = device.Context(w.header, profile=True)
+prof.set_ingest_filter(filter_mask, min_mapq)
 kern = {}
 for k, f in paths.items():
     for rep in range(2):
@@ -80,7 +86,8 @@ prof.close()
 
 name, power = card()
 out = {"tool": "sam_ingest_bench", "gpu": name, "power_limit_w": power, "reads": n, "read_length": 150, "appends_per_pass": CH,
-       "sam_text_bytes": int(text.size), "bam_record_bytes": int(raw.size), "reps": reps}
+       "sam_text_bytes": int(text.size), "bam_record_bytes": int(raw.size), "reps": reps,
+       "filter_mask": filter_mask, "min_mapq": min_mapq, "reads_kept": kept}
 for k in paths:
     best, med = min(wall[k]), float(np.median(wall[k]))
     kms = sum(v["ms"] for v in kern[k].values())
