@@ -46,7 +46,7 @@ EXPORTS = ["elp_create", "elp_destroy", "elp_last_error", "elp_reserve", "elp_re
            "elp_bqsr_cov_name", "elp_bqsr_tables_get", "elp_bqsr_tables_put", "elp_bqsr_tables_device", "elp_bqsr_finalize",
            "elp_bqsr_empirical_get", "elp_bqsr_apply", "elp_fetch", "elp_fetch_qual_bytes", "elp_fetch_bam", "elp_fetch_bam_bytes", "elp_fetch_sam", "elp_fetch_sam_bytes", "elp_set_output_filter", "elp_n_output", "elp_debug_adapt", "elp_launch_count",
            "elp_kernel_stats", "elp_synchronize", "elp_reset_stats", "elp_timer_start", "elp_timer_stop", "elp_debug_sort_u64", "elp_debug_sort_u128",
-           "elp_debug_sort_u64_range", "elp_debug_sort_u128_range", "elp_debug_join_hash", "elp_debug_coord_chunk_keys",
+           "elp_debug_sort_u64_range", "elp_debug_sort_u128_range", "elp_debug_sort_u32_range", "elp_debug_scan_u32", "elp_debug_join_hash", "elp_debug_coord_chunk_keys",
            "elp_optical_n_libraries", "elp_optical_library_name", "elp_optical_metrics", "elp_optical_histogram", "elp_optical_merge",
            "elp_print_duplicates_metrics",
            "elp_bgzf_inflate_bound", "elp_bgzf_inflate", "elp_bgzf_deflate_bound", "elp_bgzf_deflate", "elp_bam_header_size"]
@@ -134,6 +134,8 @@ def load():
     L.elp_debug_sort_u128.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_int]
     L.elp_debug_sort_u64_range.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_int]
     L.elp_debug_sort_u128_range.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_int]
+    L.elp_debug_sort_u32_range.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_int]
+    L.elp_debug_scan_u32.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64]
     L.elp_debug_join_hash.argtypes = [C.c_void_p, C.c_void_p]
     L.elp_debug_coord_chunk_keys.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
     L.elp_optical_n_libraries.argtypes = [C.c_void_p]

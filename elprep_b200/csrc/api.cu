@@ -596,6 +596,33 @@ int elp_debug_sort_u64_range(elp_ctx* c, uint64_t* keys, uint32_t* vals, uint64_
     return ELP_OK;
 }
 
+int elp_debug_sort_u32_range(elp_ctx* c, uint32_t* keys, uint32_t* vals, uint64_t n, int lo_bit, int key_bits) {
+    if (!c) return ELP_EINVAL;
+    cudaSetDevice(c->device);
+    TRY(grow(c, c->keys_a, n / 2 + 4, 0)); TRY(grow(c, c->keys_b, n / 2 + 4, 0)); TRY(grow(c, c->vals_a, n + 4, 0)); TRY(grow(c, c->vals_b, n + 4, 0));
+    uint32_t* ka = reinterpret_cast<uint32_t*>(c->keys_a.p);
+    uint32_t* kb = reinterpret_cast<uint32_t*>(c->keys_b.p);
+    CUDA_TRY(c, cudaMemcpyAsync(ka, keys, n * 4, cudaMemcpyHostToDevice, c->stream));
+    CUDA_TRY(c, cudaMemcpyAsync(c->vals_a.p, vals, n * 4, cudaMemcpyHostToDevice, c->stream));
+    bool in_b = false;
+    TRY(radix_sort_u32(c, ka, kb, c->vals_a.p, c->vals_b.p, n, key_bits, &in_b, "u32", lo_bit));
+    CUDA_TRY(c, cudaMemcpyAsync(keys, in_b ? kb : ka, n * 4, cudaMemcpyDeviceToHost, c->stream));
+    CUDA_TRY(c, cudaMemcpyAsync(vals, in_b ? c->vals_b.p : c->vals_a.p, n * 4, cudaMemcpyDeviceToHost, c->stream));
+    CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+    return ELP_OK;
+}
+
+int elp_debug_scan_u32(elp_ctx* c, const uint32_t* in, uint64_t* out, uint64_t n, uint64_t base) {
+    if (!c) return ELP_EINVAL;
+    cudaSetDevice(c->device);
+    TRY(grow(c, c->scan_tmp, n + 4, 0)); TRY(grow(c, c->keys_a, n + 4, 0));
+    if (n) CUDA_TRY(c, cudaMemcpyAsync(c->scan_tmp.p, in, n * 4, cudaMemcpyHostToDevice, c->stream));
+    TRY(exclusive_scan_u64_from_u32(c, c->scan_tmp.p, c->keys_a.p, n, base));
+    CUDA_TRY(c, cudaMemcpyAsync(out, c->keys_a.p, (n + 1) * 8, cudaMemcpyDeviceToHost, c->stream));
+    CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+    return ELP_OK;
+}
+
 int elp_debug_sort_u128_range(elp_ctx* c, uint64_t* keys_hi, uint64_t* keys_lo, uint32_t* vals, uint64_t n, int lo_bit, int key_bits) {
     if (!c) return ELP_EINVAL;
     cudaSetDevice(c->device);

@@ -235,6 +235,7 @@ struct elp_ctx {
 
 // ---- internal phase entry points (implemented in the .cu files) ----
 // stable sort by key bits [lo_bit, lo_bit + key_bits); the bits below lo_bit do not take part in the order
+int radix_sort_u32(elp_ctx* c, uint32_t* keys_a, uint32_t* keys_b, uint32_t* vals_a, uint32_t* vals_b, uint64_t n, int key_bits, bool* result_in_b, const char* tag, int lo_bit = 0);
 int radix_sort_u64(elp_ctx* c, uint64_t* keys_a, uint64_t* keys_b, uint32_t* vals_a, uint32_t* vals_b, uint64_t n, int key_bits, bool* result_in_b, const char* tag, int lo_bit = 0);
 int radix_sort_u128(elp_ctx* c, uint64_t* keys_a, uint64_t* keys_b, uint32_t* vals_a, uint32_t* vals_b, uint64_t n, int key_bits, bool* result_in_b, const char* tag, int lo_bit = 0);
 int exclusive_scan_u32_to_u64(elp_ctx* c, const uint32_t* in, uint64_t* out, uint64_t n);   // out[n+1]

@@ -1,4 +1,4 @@
-// radix_sort.cuh -- hand-written onesweep LSD radix sort for sm_90a (keys u64 or u128, u32 payload).
+// radix_sort.cuh -- hand-written onesweep LSD radix sort for sm_90a (keys u32, u64 or u128, u32 payload).
 //
 // Replaces pargo sort.StableSort as used by By(CoordinateLess).ParallelStableSort (sam/sam-types.go:599-641)
 // and the sharded-map grouping of filters/mark-duplicates.go:210-396 (sort-by-key + segmented scan instead of
@@ -41,6 +41,11 @@ inline Plan make_plan(int key_bits, int lo_bit = 0) {
     return p;
 }
 
+struct K32 {
+    uint32_t v;
+    __device__ __forceinline__ static K32 load(const K32* p) { K32 k; k.v = ld_stream_u32(reinterpret_cast<const uint32_t*>(p)); return k; }
+    __device__ __forceinline__ uint32_t digit(int shift, uint32_t mask) const { return (v >> shift) & mask; }
+};
 struct K64 {
     uint64_t v;
     __device__ __forceinline__ static K64 load(const K64* p) { K64 k; k.v = ld_stream_u64(reinterpret_cast<const uint64_t*>(p)); return k; }
@@ -111,12 +116,14 @@ __global__ void __launch_bounds__(THREADS, MIN_CTAS) rs_onesweep_kernel(const K*
                                                               uint64_t n, int shift, int bits, const uint32_t* __restrict__ gofs,
                                                               uint32_t* __restrict__ status, uint32_t* __restrict__ tile_counter) {
     constexpr int WARPS = THREADS / 32, TILE = THREADS * ITEMS;
+    static_assert(THREADS >= RADIX && THREADS % 32 == 0, "one look-back thread per digit");
+    static_assert(TILE % 4 == 0, "tiles start 16-byte aligned in the payload");
     extern __shared__ __align__(16) unsigned char smem_raw[];
     uint32_t* warp_hist = reinterpret_cast<uint32_t*>(smem_raw);                // [WARPS][RADIX]
     K* sk = reinterpret_cast<K*>(smem_raw + (size_t)WARPS * RADIX * 4);         // [TILE]; reused for the payload
     uint32_t* sv = reinterpret_cast<uint32_t*>(sk);
     uint32_t* stage_v = reinterpret_cast<uint32_t*>(smem_raw + (size_t)WARPS * RADIX * 4 + (size_t)TILE * sizeof(K));   // [TILE] payload in arrival order
-    __shared__ uint32_t s_tile, digit_start[RADIX], gbase[RADIX], wsum[8];
+    __shared__ uint32_t s_tile, digit_start[RADIX], gbase[RADIX], wsum[RADIX / 32];
 
     const unsigned tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const uint32_t mask = (1u << bits) - 1;
@@ -169,13 +176,16 @@ __global__ void __launch_bounds__(THREADS, MIN_CTAS) rs_onesweep_kernel(const K*
     __syncthreads();
     RS_STAMP(2);
 
-    // per digit: exclusive scan over warps, tile total, then exclusive scan over digits
+    // per digit: exclusive scan over warps, tile total (published at once for the successors' look-back), then exclusive
+    // scan over digits
     uint32_t total = 0;
+    uint32_t* my = status + (uint64_t)tile * RADIX + tid;
     if (tid < RADIX) {
         uint32_t run = 0;
 #pragma unroll
         for (int w = 0; w < WARPS; w++) { uint32_t c = warp_hist[w * RADIX + tid]; warp_hist[w * RADIX + tid] = run; run += c; }
         total = run;
+        if (tile > 0) st_relaxed_u32(my, total | ST_PARTIAL);
         uint32_t x = total;
 #pragma unroll
         for (int o = 1; o < 32; o <<= 1) { uint32_t y = __shfl_up_sync(FULL_MASK, x, o); if (lane >= (unsigned)o) x += y; }
@@ -192,14 +202,12 @@ __global__ void __launch_bounds__(THREADS, MIN_CTAS) rs_onesweep_kernel(const K*
     constexpr int LB = RS_LB;
     uint32_t lb_first[LB];
     uint32_t dstart = 0;
-    uint32_t* my = status + (uint64_t)tile * RADIX + tid;
     if (tid < RADIX) {
         uint32_t add = 0;
         for (unsigned i = 0; i < warp; i++) add += wsum[i];
         dstart = digit_start[tid] + add;
         digit_start[tid] = dstart;
         if (tile > 0) {
-            st_relaxed_u32(my, total | ST_PARTIAL);
 #pragma unroll
             for (int j = 0; j < LB; j++) lb_first[j] = ((int64_t)tile - 1 - j >= 0) ? ld_relaxed_u32(status + (uint64_t)(tile - 1 - j) * RADIX + tid) : ST_INCLUSIVE;
         }
@@ -282,11 +290,19 @@ struct Workspace {
 };
 
 template <class K> struct Cfg;
+// 384 x 16 keys per tile, 2 CTAs per SM: on an H100 (tools/sort_roofline.py) this beat 256 x 12 at 4 CTAs (the look-back
+// wait dominated), 256 x 24 at 2, and 384 x 24 / 384 x 30 / 512 x 16 at 1 CTA per SM (ranking latency with 12-16 warps per SM)
 #ifndef RS64_THREADS
-#define RS64_THREADS 256
-#define RS64_ITEMS 12
-#define RS64_MINCTAS 4
+#define RS64_THREADS 384
+#define RS64_ITEMS 16
+#define RS64_MINCTAS 2
 #endif
+#ifndef RS32_THREADS
+#define RS32_THREADS 384
+#define RS32_ITEMS 16
+#define RS32_MINCTAS 2
+#endif
+template <> struct Cfg<K32> { static constexpr int THREADS = RS32_THREADS, ITEMS = RS32_ITEMS, MIN_CTAS = RS32_MINCTAS; };
 template <> struct Cfg<K64> { static constexpr int THREADS = RS64_THREADS, ITEMS = RS64_ITEMS, MIN_CTAS = RS64_MINCTAS; };
 template <> struct Cfg<K128> { static constexpr int THREADS = 256, ITEMS = 8, MIN_CTAS = 4; };
 

@@ -63,84 +63,118 @@ int radix_sort_impl(elp_ctx* c, K* ka, K* kb, uint32_t* va, uint32_t* vb, uint64
     return E_OK;
 }
 
-// ---- 3-kernel exclusive scan (block reduce -> scan of block sums -> downsweep) ----
-constexpr int SCAN_T = 512, SCAN_ITEMS = 8, SCAN_TILE = SCAN_T * SCAN_ITEMS;
+// ---- single-pass exclusive scan (decoupled look-back over ticketed tiles) ----
+// A tile loads SCAN_TILE inputs warp-striped (coalesced), transposes them through shared memory so that each thread scans
+// SCAN_ITEMS consecutive values, publishes its aggregate, looks back over its predecessors with one warp (32 tiles per
+// step) and stores the exclusive prefixes warp-striped again.  Tiles take tickets in start order, so a tile only ever
+// waits on tiles that are already running.  Status per tile: flag (0 none, 1 aggregate, 2 inclusive prefix) released
+// after the value it guards; aggregate and inclusive prefix live in separate words so a reader never pairs a flag with
+// the other value.
+constexpr int SCAN_T = 256, SCAN_ITEMS = 16, SCAN_TILE = SCAN_T * SCAN_ITEMS;
+__device__ __forceinline__ int scan_pad(int i) { return i + (i >> 4); }   // one pad word per 16: blocked reads are conflict-free
+
+__device__ __forceinline__ uint64_t ld_relaxed_u64(const uint64_t* p) {
+    uint64_t r;
+    asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(r) : "l"(p) : "memory");
+    return r;
+}
 
 template <class TIn>
-__global__ void __launch_bounds__(SCAN_T) scan_reduce_kernel(const TIn* __restrict__ in, uint64_t n, uint64_t* __restrict__ blk) {
-    __shared__ uint64_t ws[SCAN_T / 32];
-    uint64_t base = (uint64_t)blockIdx.x * SCAN_TILE, s = 0;
-    for (int k = 0; k < SCAN_ITEMS; k++) { uint64_t i = base + (uint64_t)k * SCAN_T + threadIdx.x; if (i < n) s += (uint64_t)in[i]; }
-    for (int o = 16; o; o >>= 1) s += __shfl_down_sync(FULL_MASK, s, o);
-    if ((threadIdx.x & 31) == 0) ws[threadIdx.x >> 5] = s;
+__global__ void __launch_bounds__(SCAN_T) scan_kernel(const TIn* __restrict__ in, uint64_t n, uint64_t base, uint64_t* __restrict__ out,
+                                                     uint64_t* __restrict__ agg, uint64_t* __restrict__ incl, uint32_t* __restrict__ flag,
+                                                     uint32_t* __restrict__ counter) {
+    constexpr int WARPS = SCAN_T / 32;
+    __shared__ uint64_t sh[SCAN_TILE + SCAN_TILE / 16];
+    __shared__ uint64_t wofs[WARPS];
+    __shared__ uint64_t s_excl;
+    __shared__ uint32_t s_tile;
+    const unsigned tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if (tid == 0) s_tile = atomicAdd(counter, 1u);
     __syncthreads();
-    if (threadIdx.x == 0) { uint64_t t = 0; for (int i = 0; i < SCAN_T / 32; i++) t += ws[i]; blk[blockIdx.x] = t; }
-}
-__global__ void __launch_bounds__(1024) scan_blocks_kernel(uint64_t* __restrict__ blk, uint64_t nblk, uint64_t base) {
-    __shared__ uint64_t ws[32];
-    __shared__ uint64_t carry;
-    if (threadIdx.x == 0) carry = base;
-    __syncthreads();
-    for (uint64_t b0 = 0; b0 < nblk; b0 += 1024) {
-        uint64_t i = b0 + threadIdx.x;
-        uint64_t v = i < nblk ? blk[i] : 0, x = v;
-        unsigned lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-        for (int o = 1; o < 32; o <<= 1) { uint64_t y = __shfl_up_sync(FULL_MASK, x, o); if (lane >= (unsigned)o) x += y; }
-        if (lane == 31) ws[w] = x;
-        __syncthreads();
-        uint64_t add = carry;
-        for (unsigned k = 0; k < w; k++) add += ws[k];
-        if (i < nblk) blk[i] = x - v + add;
-        __syncthreads();
-        if (threadIdx.x == 1023) carry = x + add;
-        __syncthreads();
+    const uint32_t tile = s_tile;
+    const uint64_t t0 = (uint64_t)tile * SCAN_TILE;
+    const uint32_t n_valid = (uint32_t)((n - t0) < (uint64_t)SCAN_TILE ? (n - t0) : (uint64_t)SCAN_TILE);
+#pragma unroll
+    for (int j = 0; j < SCAN_ITEMS; j++) {
+        const int s = j * SCAN_T + tid;
+        sh[scan_pad(s)] = (uint32_t)s < n_valid ? (uint64_t)in[t0 + s] : 0;
     }
-}
-template <class TIn>
-__global__ void __launch_bounds__(SCAN_T) scan_down_kernel(const TIn* __restrict__ in, uint64_t n, const uint64_t* __restrict__ blk, uint64_t* __restrict__ out) {
-    __shared__ uint64_t ws[SCAN_T / 32];
-    uint64_t base = (uint64_t)blockIdx.x * SCAN_TILE + (uint64_t)threadIdx.x * SCAN_ITEMS;   // blocked arrangement
-    uint64_t v[SCAN_ITEMS], s = 0;
-    for (int k = 0; k < SCAN_ITEMS; k++) { uint64_t i = base + k; v[k] = i < n ? (uint64_t)in[i] : 0; s += v[k]; }
-    uint64_t x = s;
-    unsigned lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    for (int o = 1; o < 32; o <<= 1) { uint64_t y = __shfl_up_sync(FULL_MASK, x, o); if (lane >= (unsigned)o) x += y; }
-    if (lane == 31) ws[w] = x;
     __syncthreads();
-    uint64_t add = blk[blockIdx.x];
-    for (unsigned k = 0; k < w; k++) add += ws[k];
-    uint64_t run = x - s + add;
-    for (int k = 0; k < SCAN_ITEMS; k++) { uint64_t i = base + k; if (i < n) out[i] = run; run += v[k]; }
-    if (base <= n && n < base + SCAN_ITEMS) {   // the thread owning position n writes the total
-        uint64_t r2 = x - s + add;
-        for (int k = 0; k < SCAN_ITEMS && base + k < n; k++) r2 += v[k];
-        out[n] = r2;
+    uint64_t v[SCAN_ITEMS], sum = 0;
+#pragma unroll
+    for (int j = 0; j < SCAN_ITEMS; j++) { v[j] = sh[scan_pad(tid * SCAN_ITEMS + j)]; sum += v[j]; }
+    uint64_t x = sum;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { uint64_t y = __shfl_up_sync(FULL_MASK, x, o); if (lane >= (unsigned)o) x += y; }
+    if (lane == 31) wofs[warp] = x;
+    __syncthreads();
+    if (warp == 0) {
+        const uint64_t wt = lane < WARPS ? wofs[lane] : 0;
+        uint64_t wx = wt;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) { uint64_t y = __shfl_up_sync(FULL_MASK, wx, o); if (lane >= (unsigned)o) wx += y; }
+        const uint64_t total = __shfl_sync(FULL_MASK, wx, WARPS - 1);
+        if (lane < WARPS) wofs[lane] = wx - wt;
+        uint64_t excl = 0;
+        if (tile == 0) {
+            if (lane == 0) { incl[0] = total; st_release_u32(flag, 2u); }
+        } else {
+            if (lane == 0) { agg[tile] = total; st_release_u32(flag + tile, 1u); }
+            // lane l inspects tile t - l; the walk stops at the nearest tile that has its inclusive prefix
+            for (int64_t t = (int64_t)tile - 1;; t -= 32) {
+                const int64_t tt = t - (int64_t)lane;
+                uint32_t f = tt >= 0 ? ld_acquire_u32(flag + tt) : 2u;
+                while (__any_sync(FULL_MASK, f == 0)) { if (f == 0) f = ld_acquire_u32(flag + tt); }
+                const unsigned stop_mask = __ballot_sync(FULL_MASK, f == 2);
+                const unsigned stop = stop_mask ? (unsigned)(__ffs(stop_mask) - 1) : 31u;
+                uint64_t val = 0;
+                if (lane <= stop && tt >= 0) val = f == 2 ? ld_relaxed_u64(incl + tt) : ld_relaxed_u64(agg + tt);
+#pragma unroll
+                for (int o = 16; o; o >>= 1) val += __shfl_xor_sync(FULL_MASK, val, o);
+                excl += val;
+                if (stop_mask) break;
+            }
+            if (lane == 0) { incl[tile] = excl + total; st_release_u32(flag + tile, 2u); }
+        }
+        if (lane == 0) {
+            s_excl = excl;
+            if (t0 + n_valid == n) out[n] = base + excl + total;   // the last tile writes the total
+        }
+    }
+    __syncthreads();
+    uint64_t run = base + s_excl + wofs[warp] + x - sum;
+#pragma unroll
+    for (int j = 0; j < SCAN_ITEMS; j++) { sh[scan_pad(tid * SCAN_ITEMS + j)] = run; run += v[j]; }
+    __syncthreads();
+#pragma unroll
+    for (int j = 0; j < SCAN_ITEMS; j++) {
+        const int s = j * SCAN_T + tid;
+        if ((uint32_t)s < n_valid) out[t0 + s] = sh[scan_pad(s)];
     }
 }
 
 template <class TIn>
 int scan_impl(elp_ctx* c, const TIn* in, uint64_t* out, uint64_t n, uint64_t base) {
     if (n == 0) { CUDA_TRY(c, cudaMemcpyAsync(out, &base, 8, cudaMemcpyHostToDevice, c->stream)); cudaStreamSynchronize(c->stream); return E_OK; }
-    uint64_t nblk = (n + SCAN_TILE - 1) / SCAN_TILE;
-    // position n may fall into block index n/SCAN_TILE == nblk when n is a multiple of the tile: launch one more block for it
-    uint64_t nblk_down = n / SCAN_TILE + 1;
-    CUDA_TRY(c, c->scan_blk.reserve((nblk_down + 1) * 2, c->stream));   // u32 buffer reused as u64 storage
-    uint64_t* blk = reinterpret_cast<uint64_t*>(c->scan_blk.p);
-    CUDA_TRY(c, cudaMemsetAsync(blk, 0, (nblk_down + 1) * 8, c->stream));
-    c->begin("scan_reduce", (double)n * sizeof(TIn));
-    scan_reduce_kernel<TIn><<<(unsigned)nblk, SCAN_T, 0, c->stream>>>(in, n, blk);
-    c->end(); LAUNCH_CHECK(c);
-    c->begin("scan_blocks", 0);
-    scan_blocks_kernel<<<1, 1024, 0, c->stream>>>(blk, nblk_down, base);
-    c->end(); LAUNCH_CHECK(c);
-    c->begin("scan_down", (double)n * (sizeof(TIn) + 8));
-    scan_down_kernel<TIn><<<(unsigned)nblk_down, SCAN_T, 0, c->stream>>>(in, n, blk, out);
+    const uint64_t tiles = (n + SCAN_TILE - 1) / SCAN_TILE;
+    if (tiles >= (1ull << 31)) return c->fail(E_LIMIT, "exclusive scan: %llu values exceed the tile count limit", (unsigned long long)n);
+    // u32 buffer: [agg u64 x tiles][incl u64 x tiles][flag u32 x tiles][ticket counter]
+    CUDA_TRY(c, c->scan_blk.reserve(tiles * 5 + 2, c->stream));
+    uint64_t* agg = reinterpret_cast<uint64_t*>(c->scan_blk.p);
+    uint64_t* incl = agg + tiles;
+    uint32_t* flag = reinterpret_cast<uint32_t*>(incl + tiles);
+    CUDA_TRY(c, cudaMemsetAsync(flag, 0, (tiles + 1) * 4, c->stream));
+    c->begin("prefix_scan", (double)n * (sizeof(TIn) + 8));
+    scan_kernel<TIn><<<(unsigned)tiles, SCAN_T, 0, c->stream>>>(in, n, base, out, agg, incl, flag, flag + tiles);
     c->end(); LAUNCH_CHECK(c);
     return E_OK;
 }
 
 }  // namespace
 
+int radix_sort_u32(elp_ctx* c, uint32_t* ka, uint32_t* kb, uint32_t* va, uint32_t* vb, uint64_t n, int key_bits, bool* result_in_b, const char* tag, int lo_bit) {
+    return radix_sort_impl<rs::K32>(c, reinterpret_cast<rs::K32*>(ka), reinterpret_cast<rs::K32*>(kb), va, vb, n, key_bits, result_in_b, tag, lo_bit);
+}
 int radix_sort_u64(elp_ctx* c, uint64_t* ka, uint64_t* kb, uint32_t* va, uint32_t* vb, uint64_t n, int key_bits, bool* result_in_b, const char* tag, int lo_bit) {
     return radix_sort_impl<rs::K64>(c, reinterpret_cast<rs::K64*>(ka), reinterpret_cast<rs::K64*>(kb), va, vb, n, key_bits, result_in_b, tag, lo_bit);
 }

@@ -379,6 +379,20 @@ class Context:
             self._ck(self.L.elp_debug_sort_u64_range(self.h, _vp(keys), _vp(vals), keys.size, lo_bit, key_bits))
         return keys, vals
 
+    def debug_sort_u32(self, keys, vals, key_bits, lo_bit=0):
+        """stable sort of 32-bit keys by bits [lo_bit, lo_bit + key_bits)"""
+        keys = np.ascontiguousarray(keys, dtype=np.uint32).copy()
+        vals = np.ascontiguousarray(vals, dtype=np.uint32).copy()
+        self._ck(self.L.elp_debug_sort_u32_range(self.h, _vp(keys), _vp(vals), keys.size, lo_bit, key_bits))
+        return keys, vals
+
+    def debug_scan_u32(self, values, base=0):
+        """exclusive prefix sum of u32 values into u64, plus base; n + 1 entries (the last one is base + the total)"""
+        values = np.ascontiguousarray(values, dtype=np.uint32)
+        out = np.zeros(values.size + 1, np.uint64)
+        self._ck(self.L.elp_debug_scan_u32(self.h, _vp(values), _vp(out), values.size, base))
+        return out
+
     def debug_sort_u128(self, hi, lo, vals, key_bits, lo_bit=None):
         hi = np.ascontiguousarray(hi, dtype=np.uint64).copy()
         lo = np.ascontiguousarray(lo, dtype=np.uint64).copy()

@@ -350,6 +350,10 @@ int elp_debug_sort_u128(elp_ctx *ctx, uint64_t *keys_hi, uint64_t *keys_lo, uint
  * in the sorted range keep their input order (the fragment-group sort of duplicate marking uses such a range) */
 int elp_debug_sort_u64_range(elp_ctx *ctx, uint64_t *keys, uint32_t *vals, uint64_t n, int lo_bit, int key_bits);
 int elp_debug_sort_u128_range(elp_ctx *ctx, uint64_t *keys_hi, uint64_t *keys_lo, uint32_t *vals, uint64_t n, int lo_bit, int key_bits);
+/* the 32-bit-key sort (the mate join's), over bits [lo_bit, lo_bit + key_bits) with lo_bit + key_bits <= 32 */
+int elp_debug_sort_u32_range(elp_ctx *ctx, uint32_t *keys, uint32_t *vals, uint64_t n, int lo_bit, int key_bits);
+/* the device prefix sum: out[i] = base + in[0] + ... + in[i-1] for i <= n (out has n + 1 entries, out[n] the total). Host buffers. */
+int elp_debug_scan_u32(elp_ctx *ctx, const uint32_t *in, uint64_t *out, uint64_t n, uint64_t base);
 
 #ifdef __cplusplus
 }
