@@ -205,7 +205,7 @@ void elp_destroy(elp_ctx* c) {
     if (c->d_region_ptrs) cudaFree((void*)c->d_region_ptrs);
     if (c->d_n_regions) cudaFree(c->d_n_regions);
     void* singles[] = {c->d_rg_lib, c->d_rg_cov, c->d_contig_len, c->d_ranges, c->d_err, (void*)c->d_ref_ptrs, (void*)c->d_refnib_ptrs, (void*)c->d_refhot_ptrs, c->d_bq_small, c->d_qpresent, c->d_ref_len, (void*)c->d_site_ptrs, c->d_n_sites, c->d_tables,
-                       c->d_lut, c->d_clut, c->d_rowtab, c->d_cov_exists, c->d_opt_ctr, c->d_opt_hist, c->d_opt_ovf, c->d_opt_small, c->d_rg_names, c->d_rg_name_off, c->d_out_drop, c->ws.ghist, c->ws.gofs, c->ws.counters, c->ws.status};
+                       c->d_lut, c->d_clut, c->d_rowtab, c->d_cov_exists, c->d_unobs,c->d_opt_ctr, c->d_opt_hist, c->d_opt_ovf, c->d_opt_small, c->d_rg_names, c->d_rg_name_off, c->d_out_drop, c->ws.ghist, c->ws.gofs, c->ws.counters, c->ws.status};
     for (void* p : singles) if (p) cudaFree(p);
     c->refid.release(); c->pos.release(); c->nref.release(); c->pnext.release(); c->tlen.release(); c->rg.release(); c->flag.release(); c->mapq.release(); c->optf.release(); c->s_optf.release();
     c->qname_off.release(); c->cigar_off.release(); c->qual_off.release(); c->seq_off.release(); c->qname.release(); c->seq.release(); c->qual.release(); c->cigar.release();

@@ -35,6 +35,7 @@ struct ApplyArgs {
     const uint8_t *seq, *qual; uint8_t* out;
     const int32_t* rg_cov; int n_rg; const uint8_t* cov_exists;
     const uint8_t* lut; int lut_maxcyc, max_cycle;
+    const uint8_t* unobs;                                  // [n_cov] the byte of a QUAL value without table rows (QUAL > 93)
     int lanes_per_read;
     uint32_t* err;
 };
@@ -59,13 +60,14 @@ __global__ void __launch_bounds__(WARPS * 32, APPLY_MINB) bqsr_apply_kernel(Appl
     const uint64_t kb0 = (uint64_t)blockIdx.x * WARPS * (uint64_t)rpw, kb1 = min(A.n, kb0 + (uint64_t)(WARPS * rpw));
     const uint64_t o0 = A.out_off[kb0], o1 = A.out_off[kb1];               // the block's slice [o0, o1) of the output stream
     const uint32_t phase = (uint32_t)(o0 & 15);
-    bool recal = valid && A.lut != nullptr && L > 0;
+    bool recal = valid && A.lut != nullptr;
     int cov = 0;
-    if (recal) {
+    if (recal) {   // every read, empty ones included: the reference looks up the read group before it looks at SEQ (bqsr.go:949)
         const int g = A.rg[k];
         if (g < 0 || g >= A.n_rg) { errbits |= DERR_NORG; recal = false; }                 // readGroupCovariate panics, bqsr.go:38
         else { cov = A.rg_cov[g]; if (!A.cov_exists[cov]) recal = false; }                  // no recalibration, bqsr table empty (:950-953)
     }
+    recal = recal && L > 0;
     const int i0 = c * CHUNK, nb = min(max(L - i0, 0), CHUNK);
     // ---- 1. loads and word-parallel covariates ----
     uint32_t Q[4] = {0, 0, 0, 0};
@@ -105,35 +107,40 @@ __global__ void __launch_bounds__(WARPS * 32, APPLY_MINB) bqsr_apply_kernel(Appl
 #pragma unroll
         for (int wq = 0; wq < 4; wq++) { const int keep = nb - 4 * wq; if (keep < 4) Q[wq] = keep <= 0 ? 0u : (Q[wq] & (0xffffffffu >> (8 * (4 - keep)))); }
         if (max(cyc_a, cyc_b) > A.max_cycle || min(cyc_a, cyc_b) < -A.max_cycle) {
-            // checkCycleCovariate (:364-369) fails somewhere in this chunk: an error if one of those bases is recalibrated
+            // checkCycleCovariate (:364-369) fails somewhere in this chunk: an error if one of those bases is recalibrated; the bases
+            // inside --max-cycle are recalibrated as usual (a base past it with QUAL < 6 is no error).  Reads reach here only when they
+            // are longer than --max-cycle, and then the table covers every cycle the check lets through (lut_maxcyc = max_cycle).
             int cyc = cyc_a;
 #pragma unroll
             for (int j = 0; j < CHUNK; j++) {
                 const uint32_t q = (Q[j >> 2] >> (8 * (j & 3))) & 0xffu;
-                if (q >= 6) errbits |= q > 93 ? DERR_QUAL_RANGE : ((cyc > A.max_cycle || cyc < -A.max_cycle) ? DERR_CYCLE : 0u);
+                if (q >= 6u) {
+                    if (cyc > A.max_cycle || cyc < -A.max_cycle) errbits |= DERR_CYCLE;
+                    else {
+                        const uint32_t nib = (ctx_w[j >> 3] >> (4 * (j & 7))) & 15u;
+                        const uint32_t ctx = ((okc_w[j >> 3] >> (4 * (j & 7))) & 1u) ? nib : 16u;
+                        const uint32_t t = __ldg(lut_cov + min(q, 93u) * ncyc17 + (uint32_t)(cyc + A.lut_maxcyc) * 17u + ctx);
+                        const uint32_t v = q <= 93u ? t : (uint32_t)__ldg(A.unobs + cov);
+                        Q[j >> 2] = __byte_perm(Q[j >> 2], v, (j & 3) == 0 ? 0x3214 : ((j & 3) == 1 ? 0x3240 : ((j & 3) == 2 ? 0x3410 : 0x4210)));
+                    }
+                }
                 cyc += inc;
             }
         } else {
             uint32_t idx = (uint32_t)(cyc_a + A.lut_maxcyc) * 17u;
             const uint32_t step = (uint32_t)(inc * 17);
-            uint32_t over = 0;
 #pragma unroll
             for (int j = 0; j < CHUNK; j++) {
                 const uint32_t q = (Q[j >> 2] >> (8 * (j & 3))) & 0xffu;
                 const uint32_t nib = (ctx_w[j >> 3] >> (4 * (j & 7))) & 15u;
                 const uint32_t ctx = ((okc_w[j >> 3] >> (4 * (j & 7))) & 1u) ? nib : 16u;   // 16 = no context (key -1)
-                over |= q;
-                if (q - 6u <= 87u) {                                                        // minInterestingQual <= q <= 93
-                    const uint32_t v = __ldg(lut_cov + q * ncyc17 + idx + ctx);
+                if (q >= 6u) {                                                              // minInterestingQual (bqsr.go:969)
+                    // QUAL 94..255 has no table entry anywhere: the read group's estimate alone (bqsr.go:973-995, map misses)
+                    const uint32_t t = __ldg(lut_cov + min(q, 93u) * ncyc17 + idx + ctx);      // (row clamped: the load stays inside the table)
+                    const uint32_t v = q <= 93u ? t : (uint32_t)__ldg(A.unobs + cov);
                     Q[j >> 2] = __byte_perm(Q[j >> 2], v, (j & 3) == 0 ? 0x3214 : ((j & 3) == 1 ? 0x3240 : ((j & 3) == 2 ? 0x3410 : 0x4210)));
                 }
                 idx += step;
-            }
-            // a QUAL above 93 (any byte with bit 7, or 94..127) is an error for a recalibrated base
-            if (over & 0x80u) errbits |= DERR_QUAL_RANGE;
-            else if (over >= 94u) {
-#pragma unroll
-                for (int wq = 0; wq < 4; wq++) { const uint32_t v = Q[wq]; if ((((v & 0x7f7f7f7fu) + 0x22222222u) | v) & 0x80808080u) errbits |= DERR_QUAL_RANGE; }
             }
         }
     }
@@ -172,7 +179,8 @@ struct Apply2Args {
     const uint8_t *seq, *qual; uint8_t* out;
     const int32_t* rg_cov; int n_rg; const uint8_t* cov_exists;
     const uint8_t* clut; uint32_t clut_bytes, blk, Lc;     // compact table [2 Lc + 1 + 64 margin cycles][blk]; blk = n_cov * S * 17 rounded up to odd
-    const uint16_t* rowtab;                                // [256] byte offset of the slot of a QUAL value inside a covariate's part of a block (0xffff: none)
+    const uint16_t* rowtab;                                // [256] byte offset of the slot of a QUAL value inside a covariate's part of a block (0: slot 0 for
+                                                           // values without a slot; QUAL 94..255 share the last slot when any of them occurs)
     uint32_t S17;                                          // S * 17: bytes of one covariate inside a block
     int lpr, rpw;
     uint32_t* err;
@@ -235,14 +243,15 @@ __global__ void __launch_bounds__(AP2_WARPS * 32, 2) bqsr_apply2_kernel(Apply2Ar
             lanes::align_nibbles32<true>(V, (uint32_t)(reinterpret_cast<uintptr_t>(sp) & 15), (uint32_t)(ni & 1), N);
         }
         // (bytes past the read end are whatever follows in the arena: they index valid table rows, are never stored, and are masked where it
-        //  matters -- the tail search below and the range check in its slow path)
+        //  matters -- the tail search below)
         const uint32_t f = fg & 0xffffu; const int g = (int)(fg >> 16) - 1;
-        bool recal = A.clut != nullptr && nb > 0;
+        bool recal = A.clut != nullptr && lane_used && p * rpw + (uint64_t)r < A.n;
         int cov = 0;
-        if (recal) {
+        if (recal) {   // every read, empty ones included: the reference looks up the read group before it looks at SEQ (bqsr.go:949)
             if (g < 0 || g >= A.n_rg) { errbits |= DERR_NORG; recal = false; }                 // readGroupCovariate panics, bqsr.go:38
             else { cov = A.rg_cov[g]; if (!A.cov_exists[cov]) recal = false; }                  // no recalibration, bqsr table empty (:950-953)
         }
+        recal = recal && nb > 0;
         const bool rev = (f & F_REVERSED) != 0;
         // ---- word-parallel covariates (stored order; nibble k of word w <-> base 8 w + k) ----
         const uint32_t M1 = 0x11111111u;
@@ -310,7 +319,6 @@ __global__ void __launch_bounds__(AP2_WARPS * 32, 2) bqsr_apply2_kernel(Apply2Ar
             if (L > (int)A.Lc) errbits |= DERR_CYCLE;                                             // (the host only selects this kernel when every cycle fits)
             const uint32_t cbase = lut_s + (uint32_t)(cyc0 + (int)A.Lc + 32) * A.blk + (uint32_t)cov * A.S17;
             const int stepb = step * (int)A.blk;
-            uint32_t over = 0;
 #pragma unroll
             for (int j = 0; j < 32; j++) {
                 const uint32_t q = (Q[j >> 2] >> (8 * (j & 3))) & 0xffu;
@@ -319,17 +327,7 @@ __global__ void __launch_bounds__(AP2_WARPS * 32, 2) bqsr_apply2_kernel(Apply2Ar
                 uint32_t v; asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(cbase + (uint32_t)(j * stepb) + (row & 0x7fffu) + ctx));
                 R[j >> 2] = __byte_perm(R[j >> 2], v, (j & 3) == 0 ? 0x3214 : ((j & 3) == 1 ? 0x3240 : ((j & 3) == 2 ? 0x3410 : 0x4210)));
             }
-            // QUAL > 93 is an error (bqsr.go:968 indexes a 94-entry table): any byte >= 64 sends the lane through the exact, masked check
-#pragma unroll
-            for (int w = 0; w < 8; w++) over |= Q[w];
-            if (over & 0xc0c0c0c0u) {
-#pragma unroll
-                for (int w = 0; w < 8; w++) {
-                    const int keep = nb - 4 * w;
-                    const uint32_t v = keep >= 4 ? Q[w] : (keep <= 0 ? 0u : (Q[w] & (0xffffffffu >> (8 * (4 - keep)))));
-                    if ((((v & 0x7f7f7f7fu) + 0x22222222u) | v) & 0x80808080u) errbits |= DERR_QUAL_RANGE;
-                }
-            }
+            // (QUAL 94..255 read the slot build_compact_lut fills with the read group's estimate: no table has entries for them, bqsr.go:973-995)
             // bases without a context take column 16
 #pragma unroll
             for (int i = 0; i < 8; i++) {
@@ -343,7 +341,7 @@ __global__ void __launch_bounds__(AP2_WARPS * 32, 2) bqsr_apply2_kernel(Apply2Ar
                     R[i] = (R[i] & ~(0xffu << (8 * b))) | (v << (8 * b));
                 }
             }
-            // QUAL values below 6 (and values without a table row) stay as they are (bqsr.go:968)
+            // QUAL values below 6 stay as they are (bqsr.go:969)
 #pragma unroll
             for (int w = 0; w < 8; w++) {
                 const uint32_t x = Q[w];
@@ -389,6 +387,9 @@ __global__ void __launch_bounds__(256) qual_copy_kernel(uint64_t n, const int32_
 
 int run_apply_kernel(elp_ctx* c, bool with_lut) {
     const uint64_t n = c->n;
+    // until this call succeeds the output stream may hold a mix of recalibrated and original bytes: a fetch after a failed apply
+    // materialises the original QUAL again instead of returning it
+    c->qual_out_valid = false;
     uint64_t total = 0;
     if (n) {
         CUDA_TRY(c, cudaMemcpyAsync(&total, c->s_out_off.p + n, 8, cudaMemcpyDeviceToHost, c->stream));
@@ -407,7 +408,7 @@ int run_apply_kernel(elp_ctx* c, bool with_lut) {
         ApplyArgs A{};
         A.n = n; A.flag = c->s_flag.p; A.rg = c->s_rg.p; A.lseq = c->s_lseq.p; A.qual_off = c->s_qual_off.p; A.seq_off = c->s_seq_off.p; A.out_off = c->s_out_off.p;
         A.seq = c->seq.p; A.qual = c->qual.p; A.out = c->qual_out.p; A.rg_cov = c->d_rg_cov; A.n_rg = c->n_rg; A.cov_exists = c->d_cov_exists;
-        A.lut = with_lut ? c->d_lut : nullptr; A.lut_maxcyc = c->lut_maxcyc; A.max_cycle = c->max_cycle; A.err = c->d_err;
+        A.lut = with_lut ? c->d_lut : nullptr; A.lut_maxcyc = c->lut_maxcyc; A.max_cycle = c->max_cycle; A.unobs = c->d_unobs; A.err = c->d_err;
         const double bytes = (double)n * (2 + 4 + 4 + 8 + 8 + 8) + (double)c->n_seq + 2.0 * (double)c->n_qual;
         // second-generation kernel: whenever the compact table fits shared memory and every cycle is inside it
         const char* force = getenv("ELPREP_B200_APPLY");

@@ -279,13 +279,16 @@ int build_apply_lut(elp_ctx* c, int Lc) {
     if (have_stat) stat = static_quantized(c->sqq);
     const int ncyc = 2 * Lc + 1;
     std::vector<uint8_t> lut((size_t)g.n_cov * 94 * ncyc * 17, 0);
-    std::vector<uint8_t> cov_exists(g.n_cov, 0);
+    std::vector<uint8_t> cov_exists(g.n_cov, 0), unobs(g.n_cov, 0);
     std::vector<double> dGv(g.n_cov, 0.0);
+    auto final_q = [&](double est) { int r = (int)gomath::Round(est); r = std::max(1, std::min(r, 93)); uint8_t nq = quant[r]; if (have_stat) nq = stat[nq]; return nq; };
     for (int cv = 0; cv < g.n_cov; cv++) {
         if (!comb[cv].exists) continue;
         cov_exists[cv] = 1;
         // globalQualityScorePrior = -1 -> epsilon is always the read group's reportedQuality (:959-964)
         dGv[cv] = (double)Entry(comb[cv].obs, comb[cv].mis).empirical(comb[cv].reported) - comb[cv].reported;
+        // a QUAL value without any table entry (never observed, or above 93): only the read-group term (:901-919 with three map misses)
+        unobs[cv] = final_q(0.0 + dGv[cv] + comb[cv].reported);
     }
     host_parallel_for(g.n_cov * 88, [&](int job) {
         const int cv = job / 88, q = 6 + job % 88;
@@ -294,7 +297,6 @@ int build_apply_lut(elp_ctx* c, int Lc) {
         double dQ = 0;
         if (T.obs(cv, q, 0) > 0) dQ = (double)Entry(T.obs(cv, q, 0), T.mis(cv, q, 0)).empirical(dG + eps) - dG - eps;
         const double cp = dQ + dG + eps;
-        auto final_q = [&](double est) { int r = (int)gomath::Round(est); r = std::max(1, std::min(r, 93)); uint8_t nq = quant[r]; if (have_stat) nq = stat[nq]; return nq; };
         uint8_t* row = &lut[((size_t)cv * 94 + q) * ncyc * 17];
         if (T.obs(cv, q, 0) <= 0) { std::memset(row, final_q(cp + 0.0), (size_t)ncyc * 17); return; }   // QUAL never observed: no cycle/context entries either
         double dctx[17]; bool hctx[17];
@@ -321,6 +323,9 @@ int build_apply_lut(elp_ctx* c, int Lc) {
     { int rcu = upload_small(c, c->d_lut, lut.data(), lut.size()); if (rcu) return rcu; }
     if (!c->d_cov_exists) CUDA_TRY(c, cudaMalloc(&c->d_cov_exists, std::max(1, g.n_cov)));
     { int rcu = upload_small(c, c->d_cov_exists, cov_exists.data(), g.n_cov); if (rcu) return rcu; }
+    if (!c->d_unobs) CUDA_TRY(c, cudaMalloc(&c->d_unobs, std::max(1, g.n_cov)));
+    { int rcu = upload_small(c, c->d_unobs, unobs.data(), g.n_cov); if (rcu) return rcu; }
+    c->h_unobs.swap(unobs);
     CUDA_TRY(c, cudaStreamSynchronize(c->stream));
     c->lut_maxcyc = Lc;
     c->h_lut.swap(lut);            // kept for the compact shared-memory table (build_compact_lut)
@@ -330,7 +335,9 @@ int build_apply_lut(elp_ctx* c, int Lc) {
 
 // The apply table compacted for bqsr_apply2_kernel: only the QUAL values >= 6 that occur in the QUAL arena get rows ("slots"); layout
 // [cycle + Lc + 32][covariate][slot][17] with 32 zero cycles of margin on both sides (lanes index up to 31 bases past a read's end) and an
-// odd number of bytes per cycle (bank spread).  Rebuilt whenever the full table or the set of QUAL values changes.
+// odd number of bytes per cycle (bank spread).  When some QUAL above 93 occurs (presence bits 94..127; bit 127 stands for 128..255), one more
+// slot holds every covariate's "unobserved QUAL" byte and QUAL 94..255 map to it.  Rebuilt whenever the full table or the set of QUAL
+// values changes.
 int build_compact_lut(elp_ctx* c) {
     uint32_t present[4] = {0, 0, 0, 0};
     CUDA_TRY(c, cudaMemcpyAsync(present, c->d_qpresent, 16, cudaMemcpyDeviceToHost, c->stream));
@@ -340,15 +347,20 @@ int build_compact_lut(elp_ctx* c) {
     c->clut_Lc = 0; c->clut_bytes = 0;
     std::vector<int> slots;
     for (int q = 6; q < 94; q++) if ((present[q >> 5] >> (q & 31)) & 1u) slots.push_back(q);
-    const int S = (int)slots.size(), Lc = c->lut_maxcyc, ncyc = 2 * Lc + 1, n_cov = c->geom.n_cov;
+    const bool above93 = (present[2] >> 30) != 0 || present[3] != 0;   // bits 94..127
+    const int S = (int)slots.size() + (above93 ? 1 : 0), Lc = c->lut_maxcyc, ncyc = 2 * Lc + 1, n_cov = c->geom.n_cov;
     if (S == 0 || n_cov == 0 || c->h_lut.empty()) return E_OK;
     uint32_t blk = (uint32_t)(n_cov * S * 17); if (!(blk & 1)) blk++;
     const size_t bytes = ((size_t)(ncyc + 64) * blk + 15) / 16 * 16;
     if (bytes > 80 * 1024) return E_OK;                               // too large for two CTAs per SM: the global-memory kernel serves
     std::vector<uint8_t> t(bytes, 0); std::vector<uint16_t> rowtab(256, 0);
-    for (int sl = 0; sl < S; sl++) rowtab[slots[sl]] = (uint16_t)(sl * 17);
-    for (int cy = 0; cy < ncyc; cy++) for (int cv = 0; cv < n_cov; cv++) for (int sl = 0; sl < S; sl++)
-        memcpy(&t[(size_t)(cy + 32) * blk + (size_t)(cv * S + sl) * 17], &c->h_lut[(((size_t)cv * 94 + slots[sl]) * ncyc + cy) * 17], 17);
+    for (int sl = 0; sl < (int)slots.size(); sl++) rowtab[slots[sl]] = (uint16_t)(sl * 17);
+    if (above93) for (int q = 94; q < 256; q++) rowtab[q] = (uint16_t)((S - 1) * 17);
+    for (int cy = 0; cy < ncyc; cy++) for (int cv = 0; cv < n_cov; cv++) {
+        for (int sl = 0; sl < (int)slots.size(); sl++)
+            memcpy(&t[(size_t)(cy + 32) * blk + (size_t)(cv * S + sl) * 17], &c->h_lut[(((size_t)cv * 94 + slots[sl]) * ncyc + cy) * 17], 17);
+        if (above93) memset(&t[(size_t)(cy + 32) * blk + (size_t)(cv * S + S - 1) * 17], c->h_unobs[cv], 17);
+    }
     if (c->clut_cap < bytes) { if (c->d_clut) cudaFree(c->d_clut); c->d_clut = nullptr; CUDA_TRY(c, cudaMalloc(&c->d_clut, bytes)); c->clut_cap = bytes; }
     if (!c->d_rowtab) CUDA_TRY(c, cudaMalloc(&c->d_rowtab, 512));
     { int rcu = upload_small(c, c->d_clut, t.data(), bytes); if (rcu) return rcu; }

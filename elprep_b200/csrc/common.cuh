@@ -120,4 +120,5 @@ struct DeviceRanges {            // filled by the adapt kernel, read back by the
     int32_t pos_max, upos_min, upos_max, score_max, lseq_max, qname_max;
     uint32_t qual_present[4];    // bit q set if QUAL value q (0..127) occurs
     uint32_t n_entering, n_true_pairs;
+    uint32_t qual_invalid;       // some read entering duplicate marking has a QUAL byte computePhredScore refuses (an error only when marking runs)
 };

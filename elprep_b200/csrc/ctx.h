@@ -165,6 +165,8 @@ struct elp_ctx {
     int lut_maxcyc = 0;
     size_t lut_cap = 0;
     uint8_t* d_cov_exists = nullptr;          // [n_cov]
+    uint8_t* d_unobs = nullptr;               // [n_cov] recalibrated byte of a QUAL value without table entries (QUAL 94..255)
+    std::vector<uint8_t> h_unobs;
     uint8_t* d_clut = nullptr; uint16_t* d_rowtab = nullptr;   // compact apply table for the shared-memory kernel: [cycle][covariate][slot][17], QUAL -> slot offset
     uint32_t clut_bytes = 0, clut_blk = 0, clut_S17 = 0; int clut_Lc = 0; size_t clut_cap = 0; uint32_t clut_present[4] = {0, 0, 0, 0};
     std::vector<uint8_t> h_lut;               // the full apply table [n_cov][94][2*lut_maxcyc+1][17] on the host

@@ -219,6 +219,9 @@ __global__ void __launch_bounds__(AD_T, 1) adapt_kernel(AdaptArgs A) {
         atomicMax(&A.ranges->score_max, sh_i[0][3]); atomicMax(&A.ranges->lseq_max, sh_i[0][4]); atomicMax(&A.ranges->qname_max, sh_i[0][6]);
         atomicAdd(&A.ranges->n_entering, sh_u[0][0]); atomicAdd(&A.ranges->n_true_pairs, sh_u[0][1]);
         if (sh_i[0][5] < 0) sh_u[0][2] |= DERR_QUAL_RANGE;   // negative POS: not representable in the compact sort key
+        // an invalid QUAL is an error of MarkDuplicates alone (computePhredScore): phase_markdup raises it, a sort or BQSR does not
+        if (sh_u[0][2] & DERR_QUAL) atomicOr(&A.ranges->qual_invalid, 1u);
+        sh_u[0][2] &= ~DERR_QUAL;
         if (sh_u[0][2]) atomicOr(A.err, sh_u[0][2]);
     }
 }
@@ -523,6 +526,7 @@ static int mark_pairs(elp_ctx* c, bool optical, uint64_t nt, uint64_t n_true_pai
 int phase_markdup(elp_ctx* c, bool optical) {
     int rc = phase_adapt(c);
     if (rc) return rc;
+    if (c->h_ranges.qual_invalid) return c->fail(E_QUAL, "Invalid QUAL character in a read entering duplicate marking");
     // several GPUs (comm.cu): common key ranges, then the visiting mates of cross-group pairs arrive as ghost reads n .. n + n_ghost - 1.
     // Every rank makes the same collective calls in the same order, whatever its own reads look like.
     rc = comm_allreduce_ranges(c);

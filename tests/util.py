@@ -102,8 +102,9 @@ def fast_plan(values, n_cov, lseq_max):
 
 def apply_plan(values, n_cov, lseq_max, max_cycle=500):
     """Which apply kernel elp_bqsr_apply picks (run_apply_kernel / build_compact_lut): "v2" (bqsr_apply2_kernel, compact table in
-    shared memory) when the table of the QUAL values >= 6 present fits 80 KB, else "gmem" (bqsr_apply_kernel, global table)"""
-    S = sum(1 for q in set(values) if q >= 6)
+    shared memory) when the table of the QUAL values >= 6 present fits 80 KB, else "gmem" (bqsr_apply_kernel, global table).  Values 6..93
+    have a slot each; all values above 93 share one more."""
+    S = sum(1 for q in set(values) if 6 <= q <= 93) + (1 if any(q > 93 for q in values) else 0)
     Lc = max(1, min(max_cycle, lseq_max))
     blk = n_cov * S * 17
     blk += 1 - (blk & 1)
