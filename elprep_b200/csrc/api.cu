@@ -201,9 +201,7 @@ void elp_destroy(elp_ctx* c) {
     for (auto p : c->d_refnib_raw) if (p) cudaFree(p);
     for (auto p : c->d_refhot_raw) if (p) cudaFree(p);
     for (auto p : c->d_sites) if (p) cudaFree(p);
-    for (auto p : c->d_regions) if (p) cudaFree(p);
-    if (c->d_region_ptrs) cudaFree((void*)c->d_region_ptrs);
-    if (c->d_n_regions) cudaFree(c->d_n_regions);
+    region_release(c->regions); region_release(c->bqsr_regions);
     void* singles[] = {c->d_rg_lib, c->d_rg_cov, c->d_contig_len, c->d_ranges, c->d_err, (void*)c->d_ref_ptrs, (void*)c->d_refnib_ptrs, (void*)c->d_refhot_ptrs, c->d_bq_small, c->d_qpresent, c->d_ref_len, (void*)c->d_site_ptrs, c->d_n_sites, c->d_tables,
                        c->d_lut, c->d_clut, c->d_rowtab, c->d_cov_exists, c->d_unobs,c->d_opt_ctr, c->d_opt_hist, c->d_opt_ovf, c->d_opt_small, c->d_rg_names, c->d_rg_name_off, c->d_out_drop, c->ws.ghist, c->ws.gofs, c->ws.counters, c->ws.status};
     for (void* p : singles) if (p) cudaFree(p);
@@ -232,7 +230,7 @@ int elp_reset(elp_ctx* c) {
     if (c->copy_in) CUDA_TRY(c, cudaStreamSynchronize(c->copy_in));
     if (c->copy_out) CUDA_TRY(c, cudaStreamSynchronize(c->copy_out));
     CUDA_TRY(c, cudaStreamSynchronize(c->stream));
-    c->n = c->n_qname = c->n_cigar = 0; c->n_qual = c->n_seq = ARENA_FRONT_PAD; c->n_bam = c->bam_reads = 0; c->n_filtered = 0; c->n_cleaned = 0; c->n_sam_lost_names = 0;
+    c->n = c->n_sorted = c->n_qname = c->n_cigar = 0; c->n_qual = c->n_seq = ARENA_FRONT_PAD; c->n_bam = c->bam_reads = 0; c->n_filtered = 0; c->n_cleaned = 0; c->n_sam_lost_names = 0;
     CUDA_TRY(c, cudaMemsetAsync(c->d_qpresent, 0, 16, c->stream));
     c->adapted = c->sorted = c->qual_out_valid = c->gathered = c->finalized = c->opt_valid = false;
     c->out_sel_valid = false; c->n_out = 0;   // (the output filter setting itself stays)
@@ -456,7 +454,7 @@ int elp_bqsr_empirical_get(elp_ctx* c, uint8_t* emp, uint64_t n) {
 }
 
 uint64_t elp_fetch_qual_bytes(elp_ctx* c, uint64_t first, uint64_t n) {
-    if (!c || !c->sorted || first + n > c->n) return 0;
+    if (!c || !c->sorted || first + n > c->n_sorted) return 0;
     cudaSetDevice(c->device);
     uint64_t v[2] = {0, 0};
     cudaMemcpyAsync(&v[0], c->s_out_off.p + first, 8, cudaMemcpyDeviceToHost, c->stream);
@@ -468,7 +466,7 @@ uint64_t elp_fetch_qual_bytes(elp_ctx* c, uint64_t first, uint64_t n) {
 static int fetch_impl(elp_ctx* c, uint64_t first, uint64_t n, uint64_t* record_index, uint32_t* record_index32, uint16_t* flag, uint64_t* qual_off, uint8_t* qual, uint64_t qual_capacity, bool wait) {
     cudaSetDevice(c->device);
     if (!c->sorted) return c->fail(E_STATE, "elp_fetch before elp_sort_markdup");
-    if (first + n > c->n) return c->fail(E_INVAL, "elp_fetch: range [%llu,%llu) exceeds %llu reads", (unsigned long long)first, (unsigned long long)(first + n), (unsigned long long)c->n);
+    if (first + n > c->n_sorted) return c->fail(E_INVAL, "elp_fetch: range [%llu,%llu) exceeds %llu reads", (unsigned long long)first, (unsigned long long)(first + n), (unsigned long long)c->n_sorted);
     if (n == 0) { if (qual_off) qual_off[0] = 0; return ELP_OK; }
     cudaStream_t s = c->stream;
     if (!c->copy_out) { CUDA_TRY(c, cudaStreamCreateWithFlags(&c->copy_out, cudaStreamNonBlocking)); CUDA_TRY(c, cudaEventCreateWithFlags(&c->ev_out, cudaEventDisableTiming)); }
@@ -476,7 +474,7 @@ static int fetch_impl(elp_ctx* c, uint64_t first, uint64_t n, uint64_t* record_i
     uint64_t v[2] = {0, 0};
     if (qual) {
         if (!c->qual_out_valid) TRY(run_apply_kernel(c, false));   // no BQSR: just the QUAL bytes in output order
-        if (first == 0 && n == c->n) { v[0] = 0; v[1] = c->qual_out_total; }
+        if (first == 0 && n == c->n_sorted) { v[0] = 0; v[1] = c->qual_out_total; }
         else {
             CUDA_TRY(c, cudaMemcpyAsync(&v[0], c->s_out_off.p + first, 8, cudaMemcpyDeviceToHost, s));
             CUDA_TRY(c, cudaMemcpyAsync(&v[1], c->s_out_off.p + first + n, 8, cudaMemcpyDeviceToHost, s));
@@ -517,7 +515,7 @@ int elp_fetch_opt_flags(elp_ctx* c, uint64_t first, uint64_t n, uint8_t* opt_fla
     if (!c || (!opt_flags && n)) return ELP_EINVAL;
     cudaSetDevice(c->device);
     if (!c->sorted) return c->fail(E_STATE, "elp_fetch_opt_flags before elp_sort_markdup");
-    if (first + n > c->n) return c->fail(E_INVAL, "elp_fetch_opt_flags: range exceeds %llu reads", (unsigned long long)c->n);
+    if (first + n > c->n_sorted) return c->fail(E_INVAL, "elp_fetch_opt_flags: range exceeds %llu reads", (unsigned long long)c->n_sorted);
     if (n) { CUDA_TRY(c, cudaMemcpyAsync(opt_flags, c->s_optf.p + first, n, cudaMemcpyDeviceToHost, c->stream)); CUDA_TRY(c, cudaStreamSynchronize(c->stream)); }
     return ELP_OK;
 }

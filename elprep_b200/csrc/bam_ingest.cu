@@ -14,6 +14,7 @@
 // an RG:Z value that is not an @RG ID of the header.
 #include <algorithm>
 #include "ctx.h"
+#include "regions.cuh"
 #include "tagwalk.cuh"
 #include "../../include/elprep_b200.h"
 
@@ -129,19 +130,7 @@ __global__ void __launch_bounds__(256) bam_fixed_kernel(BamArgs A) {
 
 // ---- fused per-record filters of the ingest (SURVEY.md 8f row 4; filters/simple-filters.go:71-103,332-347) ----
 // keep[i] = 1 iff record i passes every requested predicate; also checks that the caller's offsets follow the block_size chain
-// intervals.Overlap (intervals/intervals.go:146-164) over one contig's flattened, start-sorted (start, end) pairs
-__device__ bool overlap_any(const int32_t* __restrict__ iv, uint64_t n, int32_t start, int32_t end) {
-    const int32_t end_1 = (int32_t)((uint32_t)end - 1u), start_1 = (int32_t)((uint32_t)start - 1u);   // end-1, start-1 in Go's int32: they wrap
-    int64_t left = 0, right = (int64_t)n - 1;
-    while (left <= right) {
-        const int64_t mid = (left + right) / 2;
-        const int32_t is = iv[2 * mid], ie = iv[2 * mid + 1];
-        if (is > end_1) right = mid - 1;
-        else if (ie <= start_1) left = mid + 1;
-        else return true;
-    }
-    return false;
-}
+// (overlap_any: regions.cuh)
 // integer value of an optional field at r[x] (x behind tag and type), by BAM type; false for a non-integer type
 __device__ __forceinline__ bool tag_int(const uint8_t* r, uint64_t x, uint8_t ty, int64_t* v) {
     switch (ty) {
@@ -382,17 +371,45 @@ template <class T> int grow(elp_ctx* c, DBuf<T>& b, size_t need, size_t keep) {
 
 }  // namespace
 
-static int upload_regions(elp_ctx* c) {
-    if (!c->regions_dirty && c->d_region_ptrs) return E_OK;
+// ---- region tables (RegionTable, ctx.h): the ingest filter's and the one of elp_filter_target_regions ----
+int region_upload(elp_ctx* c, RegionTable& t) {
+    if (!t.dirty && t.d_ptrs) return E_OK;
     const int nc = std::max(1, c->n_contigs);
-    if ((int)c->d_regions.size() != c->n_contigs) { c->d_regions.assign(c->n_contigs, nullptr); c->n_regions.assign(c->n_contigs, 0); }
-    if (!c->d_region_ptrs) { CUDA_TRY(c, cudaMalloc(&c->d_region_ptrs, nc * sizeof(void*))); CUDA_TRY(c, cudaMalloc(&c->d_n_regions, nc * 8)); }
+    if ((int)t.d.size() != c->n_contigs) { t.d.assign(c->n_contigs, nullptr); t.n.assign(c->n_contigs, 0); }
+    if (!t.d_ptrs) { CUDA_TRY(c, cudaMalloc(&t.d_ptrs, nc * sizeof(void*))); CUDA_TRY(c, cudaMalloc(&t.d_n, nc * 8)); }
     if (c->n_contigs) {
-        CUDA_TRY(c, cudaMemcpy(c->d_region_ptrs, c->d_regions.data(), c->n_contigs * sizeof(void*), cudaMemcpyHostToDevice));
-        CUDA_TRY(c, cudaMemcpy(c->d_n_regions, c->n_regions.data(), c->n_contigs * 8, cudaMemcpyHostToDevice));
+        CUDA_TRY(c, cudaMemcpy(t.d_ptrs, t.d.data(), c->n_contigs * sizeof(void*), cudaMemcpyHostToDevice));
+        CUDA_TRY(c, cudaMemcpy(t.d_n, t.n.data(), c->n_contigs * 8, cudaMemcpyHostToDevice));
     }
-    c->regions_dirty = false;
+    t.dirty = false;
     return E_OK;
+}
+
+// one contig's regions: sorted by start and flattened unless already_flat (intervals.ParallelSortByStart + ParallelFlatten, intervals/intervals.go:88-117)
+int region_set(elp_ctx* c, RegionTable& t, const char* who, int32_t contig, const int32_t* se, uint64_t n_intervals, int already_flat) {
+    if (contig < 0 || contig >= c->n_contigs) return c->fail(E_INVAL, "%s: contig %d out of range", who, contig);
+    if (n_intervals && !se) return c->fail(E_INVAL, "%s: null interval array", who);
+    if ((int)t.d.size() != c->n_contigs) { t.d.assign(c->n_contigs, nullptr); t.n.assign(c->n_contigs, 0); }
+    std::vector<std::pair<int32_t, int32_t>> iv(n_intervals);
+    for (uint64_t i = 0; i < n_intervals; i++) iv[i] = {se[2 * i], se[2 * i + 1]};
+    uint64_t n = n_intervals;
+    if (!already_flat && n > 1) {
+        std::stable_sort(iv.begin(), iv.end(), [](const std::pair<int32_t, int32_t>& a, const std::pair<int32_t, int32_t>& b) { return a.first < b.first; });
+        uint64_t m = 0;
+        for (uint64_t i = 0; i < n; i++) { if (m > 0 && iv[i].first <= iv[m - 1].second) { if (iv[i].second > iv[m - 1].second) iv[m - 1].second = iv[i].second; } else iv[m++] = iv[i]; }
+        n = m;
+    }
+    if (t.d[contig]) { cudaFree(t.d[contig]); t.d[contig] = nullptr; }
+    if (n) { CUDA_TRY(c, cudaMalloc(&t.d[contig], n * 8)); CUDA_TRY(c, cudaMemcpy(t.d[contig], iv.data(), n * 8, cudaMemcpyHostToDevice)); }
+    t.n[contig] = n; t.dirty = true;
+    return ELP_OK;
+}
+
+void region_release(RegionTable& t) {
+    for (auto p : t.d) if (p) cudaFree(p);
+    if (t.d_ptrs) cudaFree((void*)t.d_ptrs);
+    if (t.d_n) cudaFree(t.d_n);
+    t.d.clear(); t.n.clear(); t.d_ptrs = nullptr; t.d_n = nullptr; t.dirty = true;
 }
 
 extern "C" int elp_append_bam(elp_ctx* c, const uint8_t* records, uint64_t n_bytes, const uint64_t* record_off, uint64_t n_records) {
@@ -446,8 +463,8 @@ int bam_ingest_core(elp_ctx* c, uint64_t n_bytes, uint64_t nrec) {
     if (c->filter_mask || c->filter_min_mapq > 0) {
         TRY(grow(c, c->scan_tmp, nrec + 8, 0)); TRY(grow(c, c->off_stage, nrec + 2, 0));
         c->begin("bam_keep", (double)nrec * 48);
-        if (c->filter_mask & ELP_FILTER_TARGET_REGIONS) { int rcr = upload_regions(c); if (rcr) return rcr; }
-        bam_keep_kernel<<<nblk(nrec, 256), 256, 0, s>>>(nrec, c->bam_raw.p, c->bam_off.p, n_bytes, c->filter_mask, c->filter_min_mapq, c->d_region_ptrs, c->d_n_regions, c->n_contigs,
+        if (c->filter_mask & ELP_FILTER_TARGET_REGIONS) { int rcr = region_upload(c, c->regions); if (rcr) return rcr; }
+        bam_keep_kernel<<<nblk(nrec, 256), 256, 0, s>>>(nrec, c->bam_raw.p, c->bam_off.p, n_bytes, c->filter_mask, c->filter_min_mapq, c->regions.d_ptrs, c->regions.d_n, c->n_contigs,
                                                         RgNames{c->d_rg_names, c->d_rg_name_off, c->n_rg}, c->scan_tmp.p, c->d_err);
         c->end(); LAUNCH_CHECK(c);
         TRY(exclusive_scan_u32_to_u64(c, c->scan_tmp.p, c->off_stage.p, nrec));
@@ -515,10 +532,10 @@ int bam_ingest_core(elp_ctx* c, uint64_t n_bytes, uint64_t nrec) {
 // The selection of the record filters: sel[j] is the output position of the j-th record that passes (in output order).  Built once per
 // sort and setting, on the first filtered fetch; without record bits there is none (sel null, every record passes).
 int out_select(elp_ctx* c, const uint32_t** sel, uint64_t* n_out) {
-    *sel = nullptr; *n_out = c->n;
+    *sel = nullptr; *n_out = c->n_sorted;
     if (!c->out_mask) return E_OK;
     if (!c->out_sel_valid) {
-        const uint64_t n = c->n;
+        const uint64_t n = c->n_sorted;
         uint64_t kept = 0;
         if (n) {
             cudaStream_t s = c->stream;
@@ -547,7 +564,7 @@ static int bam_out_prepare(elp_ctx* c, uint64_t first, uint64_t n, uint64_t* tot
     TRY(out_select(c, sel, &n_out));
     if (first + n > n_out) {
         if (*sel) return c->fail(E_INVAL, "elp_fetch_bam: range [%llu,%llu) exceeds the %llu output records that pass the record filters (elp_n_output)", (unsigned long long)first, (unsigned long long)(first + n), (unsigned long long)n_out);
-        return c->fail(E_INVAL, "elp_fetch_bam: range [%llu,%llu) exceeds %llu reads", (unsigned long long)first, (unsigned long long)(first + n), (unsigned long long)c->n);
+        return c->fail(E_INVAL, "elp_fetch_bam: range [%llu,%llu) exceeds %llu reads", (unsigned long long)first, (unsigned long long)(first + n), (unsigned long long)n_out);
     }
     TRY(grow(c, c->scan_tmp, n + 8, 0)); TRY(grow(c, c->off_stage, n + 2, 0));
     if (c->out_fields) {
@@ -600,21 +617,7 @@ extern "C" int elp_fetch_bam(elp_ctx* c, uint64_t first, uint64_t n, uint8_t* ou
 extern "C" int elp_set_target_regions(elp_ctx* c, int32_t contig, const int32_t* se, uint64_t n_intervals, int already_flat) {
     if (!c) return ELP_EINVAL;
     cudaSetDevice(c->device);
-    if (contig < 0 || contig >= c->n_contigs) return c->fail(E_INVAL, "elp_set_target_regions: contig %d out of range", contig);
-    if ((int)c->d_regions.size() != c->n_contigs) { c->d_regions.assign(c->n_contigs, nullptr); c->n_regions.assign(c->n_contigs, 0); }
-    std::vector<std::pair<int32_t, int32_t>> iv(n_intervals);
-    for (uint64_t i = 0; i < n_intervals; i++) iv[i] = {se[2 * i], se[2 * i + 1]};
-    uint64_t n = n_intervals;
-    if (!already_flat && n > 1) {   // intervals.ParallelSortByStart + ParallelFlatten (intervals/intervals.go:88-117)
-        std::stable_sort(iv.begin(), iv.end(), [](const std::pair<int32_t, int32_t>& a, const std::pair<int32_t, int32_t>& b) { return a.first < b.first; });
-        uint64_t m = 0;
-        for (uint64_t i = 0; i < n; i++) { if (m > 0 && iv[i].first <= iv[m - 1].second) { if (iv[i].second > iv[m - 1].second) iv[m - 1].second = iv[i].second; } else iv[m++] = iv[i]; }
-        n = m;
-    }
-    if (c->d_regions[contig]) { cudaFree(c->d_regions[contig]); c->d_regions[contig] = nullptr; }
-    if (n) { CUDA_TRY(c, cudaMalloc(&c->d_regions[contig], n * 8)); CUDA_TRY(c, cudaMemcpy(c->d_regions[contig], iv.data(), n * 8, cudaMemcpyHostToDevice)); }
-    c->n_regions[contig] = n; c->regions_dirty = true;
-    return ELP_OK;
+    return region_set(c, c->regions, "elp_set_target_regions", contig, se, n_intervals, already_flat);
 }
 
 extern "C" int elp_set_ingest_filter(elp_ctx* c, uint32_t mask, int32_t min_mapq) {

@@ -386,7 +386,7 @@ __global__ void __launch_bounds__(256) qual_copy_kernel(uint64_t n, const int32_
 }  // namespace
 
 int run_apply_kernel(elp_ctx* c, bool with_lut) {
-    const uint64_t n = c->n;
+    const uint64_t n = c->n_sorted;                       // the output order: every read, or those elp_filter_target_regions kept
     // until this call succeeds the output stream may hold a mix of recalibrated and original bytes: a fetch after a failed apply
     // materialises the original QUAL again instead of returning it
     c->qual_out_valid = false;
@@ -409,7 +409,7 @@ int run_apply_kernel(elp_ctx* c, bool with_lut) {
         A.n = n; A.flag = c->s_flag.p; A.rg = c->s_rg.p; A.lseq = c->s_lseq.p; A.qual_off = c->s_qual_off.p; A.seq_off = c->s_seq_off.p; A.out_off = c->s_out_off.p;
         A.seq = c->seq.p; A.qual = c->qual.p; A.out = c->qual_out.p; A.rg_cov = c->d_rg_cov; A.n_rg = c->n_rg; A.cov_exists = c->d_cov_exists;
         A.lut = with_lut ? c->d_lut : nullptr; A.lut_maxcyc = c->lut_maxcyc; A.max_cycle = c->max_cycle; A.unobs = c->d_unobs; A.err = c->d_err;
-        const double bytes = (double)n * (2 + 4 + 4 + 8 + 8 + 8) + (double)c->n_seq + 2.0 * (double)c->n_qual;
+        const double bytes = (double)n * (2 + 4 + 4 + 8 + 8 + 8) + ((double)c->n_seq + 2.0 * (double)c->n_qual) * ((double)n / (double)c->n);
         // second-generation kernel: whenever the compact table fits shared memory and every cycle is inside it
         const char* force = getenv("ELPREP_B200_APPLY");
         const bool want_v2 = !(force && std::string(force) == "v1") && (!with_lut || (c->d_clut && c->clut_bytes && c->clut_Lc == c->lut_maxcyc && c->h_ranges.lseq_max <= c->clut_Lc)) && c->h_ranges.lseq_max <= 1024;
@@ -435,7 +435,7 @@ int run_apply_kernel(elp_ctx* c, bool with_lut) {
             return E_OK;
         }
         if (!with_lut && c->h_ranges.lseq_max > CHUNK * 32) {      // longer than either tiled kernel handles: plain per-read copy
-            c->begin("qual_materialize", 2.0 * (double)c->n_qual + (double)n * 20);
+            c->begin("qual_materialize", 2.0 * (double)c->n_qual * ((double)n / (double)c->n) + (double)n * 20);
             qual_copy_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, c->stream>>>(n, c->s_lseq.p, c->s_qual_off.p, c->s_out_off.p, c->qual.p, c->qual_out.p);
             c->end(); LAUNCH_CHECK(c);
             c->qual_out_valid = true;

@@ -789,7 +789,7 @@ namespace {
 // the general kernels (prep -> descriptors -> chunk / warp-per-read kernels with shared-memory counters) over all reads (in_list == nullptr)
 // or over the list bqsr_prep2_kernel left for them
 int gather_general(elp_ctx* c, GatherArgs A, const uint32_t* in_list, uint32_t n_in, double bytes) {
-    const uint64_t n = c->n;
+    const uint64_t n = c->n_sorted;
     const uint64_t n_work = in_list ? (uint64_t)n_in : n;
     if (!n_work) return E_OK;
     const int Lc = std::max(1, std::min(c->max_cycle, c->h_ranges.lseq_max));
@@ -928,7 +928,7 @@ int phase_bqsr_gather(elp_ctx* c) {
     if (rc) return rc;
     const size_t cells = c->geom.cells();
     CUDA_TRY(c, cudaMemsetAsync(c->d_tables, 0, cells * 2 * sizeof(int64_t), c->stream));
-    const uint64_t n = c->n;
+    const uint64_t n = c->n_sorted;                       // the output order: every read, or those elp_filter_target_regions kept
     c->gather_eligible = 0;
     if (n) {
         GatherArgs A{};
@@ -940,7 +940,7 @@ int phase_bqsr_gather(elp_ctx* c) {
         A.refnib = c->d_refnib_ptrs;
         uint64_t ref_bytes = 0; for (auto l : c->ref_len) ref_bytes += l;
         // SURVEY.md 8d: N_eligible * (19 + 4 + 4 c + L/2 + L) + genome bytes once; per-read averages of the arenas stand in for c and L
-        const double per_read = 23.0 + ((double)c->n_cigar * 4 + (double)(c->n_seq - ARENA_FRONT_PAD) + (double)(c->n_qual - ARENA_FRONT_PAD)) / (double)n;
+        const double per_read = 23.0 + ((double)c->n_cigar * 4 + (double)(c->n_seq - ARENA_FRONT_PAD) + (double)(c->n_qual - ARENA_FRONT_PAD)) / (double)c->n;
         uint32_t present[4] = {0, 0, 0, 0};
         CUDA_TRY(c, cudaMemcpyAsync(present, c->d_qpresent, 16, cudaMemcpyDeviceToHost, c->stream));
         CUDA_TRY(c, cudaStreamSynchronize(c->stream));

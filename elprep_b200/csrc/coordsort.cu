@@ -338,34 +338,42 @@ int phase_coordinate_sort(elp_ctx* c, int order) {   // 0 keep, 1 coordinate, 2 
         iota_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(n, c->perm.p);
         c->launches++; LAUNCH_CHECK(c);
     }
-    // gather the fixed-width columns into output order
-    CUDA_TRY(c, c->s_refid.reserve(n + 4, c->stream)); CUDA_TRY(c, c->s_pos.reserve(n + 4, c->stream)); CUDA_TRY(c, c->s_nref.reserve(n + 4, c->stream));
-    CUDA_TRY(c, c->s_pnext.reserve(n + 4, c->stream)); CUDA_TRY(c, c->s_tlen.reserve(n + 4, c->stream)); CUDA_TRY(c, c->s_rg.reserve(n + 4, c->stream));
-    CUDA_TRY(c, c->s_lseq.reserve(n + 4, c->stream)); CUDA_TRY(c, c->s_flag.reserve(n + 4, c->stream)); CUDA_TRY(c, c->s_mapq.reserve(n + 4, c->stream)); CUDA_TRY(c, c->s_optf.reserve(n + 4, c->stream));
-    CUDA_TRY(c, c->s_qual_off.reserve(n + 4, c->stream)); CUDA_TRY(c, c->s_seq_off.reserve(n + 4, c->stream)); CUDA_TRY(c, c->s_cigar_off.reserve(n + 4, c->stream));
-    CUDA_TRY(c, c->s_ncigar.reserve(n + 4, c->stream)); CUDA_TRY(c, c->s_out_off.reserve(n + 4, c->stream));
-    if (n) {
+    rc = build_output_columns(c, c->perm.p, n, false);
+    if (rc) return rc;
+    c->sorted = true;
+    c->n_sorted = n;
+    c->qual_out_valid = false;
+    return E_OK;
+}
+
+// The fixed-width columns of the output records perm[0, n_out) gathered into output order, and the offsets of the output QUAL stream.
+// The rows are packed for every read of the context (perm indexes arrival order).  refilter: launched by elp_filter_target_regions,
+// which rebuilds the columns of the reads it keeps (its own stats names).
+int build_output_columns(elp_ctx* c, const uint32_t* perm, uint64_t n_out, bool refilter) {
+    const uint64_t n = c->n;
+    CUDA_TRY(c, c->s_refid.reserve(n_out + 4, c->stream)); CUDA_TRY(c, c->s_pos.reserve(n_out + 4, c->stream)); CUDA_TRY(c, c->s_nref.reserve(n_out + 4, c->stream));
+    CUDA_TRY(c, c->s_pnext.reserve(n_out + 4, c->stream)); CUDA_TRY(c, c->s_tlen.reserve(n_out + 4, c->stream)); CUDA_TRY(c, c->s_rg.reserve(n_out + 4, c->stream));
+    CUDA_TRY(c, c->s_lseq.reserve(n_out + 4, c->stream)); CUDA_TRY(c, c->s_flag.reserve(n_out + 4, c->stream)); CUDA_TRY(c, c->s_mapq.reserve(n_out + 4, c->stream)); CUDA_TRY(c, c->s_optf.reserve(n_out + 4, c->stream));
+    CUDA_TRY(c, c->s_qual_off.reserve(n_out + 4, c->stream)); CUDA_TRY(c, c->s_seq_off.reserve(n_out + 4, c->stream)); CUDA_TRY(c, c->s_cigar_off.reserve(n_out + 4, c->stream));
+    CUDA_TRY(c, c->s_ncigar.reserve(n_out + 4, c->stream)); CUDA_TRY(c, c->s_out_off.reserve(n_out + 4, c->stream));
+    if (n_out) {
         GatherCols g{c->refid.p, c->pos.p, c->nref.p, c->pnext.p, c->tlen.p, c->rg.p, c->flag.p, c->mapq.p, c->qual_off.p, c->seq_off.p, c->cigar_off.p,
                      c->s_refid.p, c->s_pos.p, c->s_nref.p, c->s_pnext.p, c->s_tlen.p, c->s_rg.p, c->s_lseq.p, c->s_flag.p, c->s_mapq.p,
                      c->s_qual_off.p, c->s_seq_off.p, c->s_cigar_off.p, c->s_ncigar.p, c->optf.p, c->s_optf.p};
         // rows live in the key scratch (free here): 4 x uint4 per read
         CUDA_TRY(c, c->keys_a.reserve(8 * n + 8, c->stream));
         uint4* rows = reinterpret_cast<uint4*>(c->keys_a.p);
-        c->begin("pack_rows", (double)n * (27 + 24 + 64));
+        c->begin(refilter ? "target_pack_rows" : "pack_rows", (double)n * (27 + 24 + 64));
         pack_rows_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(n, g, rows);
         c->end(); LAUNCH_CHECK(c);
-        c->begin("gather_cols", (double)n * (4 + 27 + 24 + 27 + 28 + 8));
-        gather_cols_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(n, c->perm.p, g, rows);
+        c->begin(refilter ? "target_gather_cols" : "gather_cols", (double)n_out * (4 + 27 + 24 + 27 + 28 + 8));
+        gather_cols_kernel<<<nblk(n_out, 256), 256, 0, c->stream>>>(n_out, perm, g, rows);
         c->end(); LAUNCH_CHECK(c);
-        CUDA_TRY(c, c->scan_tmp.reserve(n + 4, c->stream));
-        lseq_u32_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(n, c->s_lseq.p, c->scan_tmp.p);
+        CUDA_TRY(c, c->scan_tmp.reserve(n_out + 4, c->stream));
+        lseq_u32_kernel<<<nblk(n_out, 256), 256, 0, c->stream>>>(n_out, c->s_lseq.p, c->scan_tmp.p);
         c->launches++; LAUNCH_CHECK(c);
     }
-    rc = exclusive_scan_u32_to_u64(c, c->scan_tmp.p, c->s_out_off.p, n);
-    if (rc) return rc;
-    c->sorted = true;
-    c->qual_out_valid = false;
-    return E_OK;
+    return exclusive_scan_u32_to_u64(c, c->scan_tmp.p, c->s_out_off.p, n_out);
 }
 
 // chunk_key of every read in arrival order, under the layout (nq, primary key widths) the coordinate sort would use

@@ -39,6 +39,13 @@ struct DupCounters { int64_t ctr[7] = {0, 0, 0, 0, 0, 0, 0}; std::map<int64_t, i
 #define OPT_HBINS 1024
 #define OPT_OVF_CAP (1 << 16)
 
+// target regions of RemoveNonOverlappingReads (filters/simple-filters.go:310-328) on the device: per contig, the flattened, start-sorted
+// (start, end) pairs, and the two device arrays of pointers and counts the kernels index by REFID (region_set / region_upload, bam_ingest.cu)
+struct RegionTable {
+    std::vector<int32_t*> d; std::vector<uint64_t> n;
+    const int32_t** d_ptrs = nullptr; uint64_t* d_n = nullptr; bool dirty = true;
+};
+
 struct KernelStat { uint64_t launches = 0; double ms = 0, alg_bytes = 0; };
 struct PendingEvent { std::string name; cudaEvent_t a, b; double alg_bytes; };
 
@@ -111,7 +118,8 @@ struct elp_ctx {
     uint32_t out_mask = 0;                    // record bits (ELP_OUT_REMOVE_DUPLICATES, ELP_OUT_REMOVE_OPTIONAL_READS)
     uint32_t* d_out_drop = nullptr; bool out_fields = false;   // 65 536-bit tag table (bit set: the field is dropped); out_fields: some bit is set
     DBuf<uint32_t> out_sel; uint64_t n_out = 0; bool out_sel_valid = false;   // output positions of the records that pass, built on first use
-    std::vector<int32_t*> d_regions; std::vector<uint64_t> n_regions; const int32_t** d_region_ptrs = nullptr; uint64_t* d_n_regions = nullptr; bool regions_dirty = true;   // target regions (BED) of RemoveNonOverlappingReads
+    RegionTable regions;                     // --filter-non-overlapping-reads: the ingest filter ELP_FILTER_TARGET_REGIONS (elp_set_target_regions)
+    RegionTable bqsr_regions;                // --target-regions: elp_filter_target_regions after marking (elp_set_bqsr_target_regions); both survive elp_reset
     uint64_t n_cleaned = 0;                  // reads whose CIGAR elp_clean_sam rewrote
     bool has_contig_names = false;           // elp_config.contig_names was given (elp_append_sam resolves RNAME / RNEXT against it)
     struct SamState* sam = nullptr;          // device tables and staging of elp_append_sam (sam_ingest.cu)
@@ -144,7 +152,8 @@ struct elp_ctx {
 
     // ---- output order ----
     bool sorted = false;                      // columns below valid
-    DBuf<uint32_t> perm;                      // [n] arrival index of k-th output record
+    uint64_t n_sorted = 0;                    // records in output order: n after the sort, the kept reads after elp_filter_target_regions
+    DBuf<uint32_t> perm;                      // [n_sorted] arrival index of k-th output record
     DBuf<int32_t> s_refid, s_pos, s_nref, s_pnext, s_tlen, s_rg, s_lseq;
     DBuf<uint16_t> s_flag;
     DBuf<uint8_t> s_mapq, s_optf;
@@ -261,6 +270,11 @@ int spread_exchange_end(elp_ctx* c);
 int exclusive_scan_u64_from_u32(elp_ctx* c, const uint32_t* in, uint64_t* out, uint64_t n, uint64_t base);   // out[n+1], out[0] = base
 int qual_presence_update(elp_ctx* c, uint64_t first_byte, uint64_t n_bytes);   // api.cu: called by both ingest paths
 int bam_ingest_core(elp_ctx* c, uint64_t n_bytes, uint64_t nrec);   // bam_ingest.cu: records staged in bam_raw / bam_off -> reads (elp_append_bam, elp_append_sam)
-int out_select(elp_ctx* c, const uint32_t** sel, uint64_t* n_out);   // bam_ingest.cu: the record filters' selection (sel null and n_out = n without record bits)
+int out_select(elp_ctx* c, const uint32_t** sel, uint64_t* n_out);   // bam_ingest.cu: the record filters' selection (sel null and n_out = n_sorted without record bits)
+int region_set(elp_ctx* c, RegionTable& t, const char* who, int32_t contig, const int32_t* se, uint64_t n_intervals, int already_flat);   // bam_ingest.cu
+int region_upload(elp_ctx* c, RegionTable& t);
+void region_release(RegionTable& t);
+int build_output_columns(elp_ctx* c, const uint32_t* perm, uint64_t n_out, bool refilter);   // coordsort.cu: s_* columns and s_out_off of perm[0, n_out)
+int phase_target_filter(elp_ctx* c, uint64_t* n_removed);   // target_regions.cu
 void sam_state_release(elp_ctx* c);   // sam_ingest.cu
 void sam_out_release(elp_ctx* c);     // sam_format.cu

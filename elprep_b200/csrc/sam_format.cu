@@ -324,7 +324,7 @@ int sam_out_check(elp_ctx* c, uint64_t first, uint64_t n, const uint32_t** sel) 
     TRY(out_select(c, sel, &n_out));
     if (first + n > n_out) {
         if (*sel) return c->fail(E_INVAL, "elp_fetch_sam: range [%llu,%llu) exceeds the %llu output records that pass the record filters (elp_n_output)", (unsigned long long)first, (unsigned long long)(first + n), (unsigned long long)n_out);
-        return c->fail(E_INVAL, "elp_fetch_sam: range [%llu,%llu) exceeds %llu reads", (unsigned long long)first, (unsigned long long)(first + n), (unsigned long long)c->n);
+        return c->fail(E_INVAL, "elp_fetch_sam: range [%llu,%llu) exceeds %llu reads", (unsigned long long)first, (unsigned long long)(first + n), (unsigned long long)n_out);
     }
     return E_OK;
 }

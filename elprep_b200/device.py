@@ -105,7 +105,7 @@ class Context:
 
     def fetch_async(self, out, first=0, n=None):
         """out = (record_index u32[n], flag u16[n], qual_off u64[n+1] or None, qual u8[]) page-locked; complete after fetch_wait()"""
-        n = self.n - first if n is None else n
+        n = self.n_sorted - first if n is None else n
         idx, flag, qoff, qual = out
         self._ck(self.L.elp_fetch_async(self.h, first, n, _vp(idx), _vp(flag), _vp(qoff), _vp(qual), qual.size if qual is not None else 0))
 
@@ -132,12 +132,28 @@ class Context:
     def _n_out(self, first):
         k = self.n_output()
         if k == 0 and self.L.elp_fetch_opt_flags(self.h, 0, 0, None) != 0:
-            k = self.n                                                    # before sort_markdup: the fetch reports the refusal
+            k = self.n_sorted                                             # before sort_markdup: the fetch reports the refusal
         return k - first
 
     def set_target_regions(self, contig, start_end, already_flat=False):
         se = np.ascontiguousarray(start_end, dtype=np.int32).reshape(-1)
         self._ck(self.L.elp_set_target_regions(self.h, contig, _vp(se) if se.size else None, se.size // 2, int(already_flat)))
+
+    def set_bqsr_target_regions(self, contig, start_end, already_flat=False):
+        """`--target-regions`: one contig's regions for filter_target_regions (a table separate from set_target_regions')"""
+        se = np.ascontiguousarray(start_end, dtype=np.int32).reshape(-1)
+        self._ck(self.L.elp_set_bqsr_target_regions(self.h, contig, _vp(se) if se.size else None, se.size // 2, int(already_flat)))
+
+    def filter_target_regions(self):
+        """RemoveNonOverlappingReads over the output order, after sort_markdup and before bqsr_gather; returns the number of records dropped"""
+        k = C.c_uint64()
+        self._ck(self.L.elp_filter_target_regions(self.h, C.byref(k)))
+        return int(k.value)
+
+    @property
+    def n_sorted(self):
+        """records in output order: n until filter_target_regions drops some, the kept count afterwards"""
+        return int(self.L.elp_n_sorted(self.h))
 
     def clean_sam(self):
         """filters.CleanSam over the reads appended so far; returns the number of rewritten CIGARs"""
@@ -146,7 +162,7 @@ class Context:
         return int(k.value)
 
     def fetch_opt_flags(self, first=0, n=None):
-        n = self.n - first if n is None else n
+        n = self.n_sorted - first if n is None else n
         out = np.zeros(n, np.uint8)
         self._ck(self.L.elp_fetch_opt_flags(self.h, first, n, _vp(out)))
         return out
@@ -304,7 +320,7 @@ class Context:
 
     def fetch(self, first=0, n=None, want_qual=True, out=None):
         """returns (record_index u64[n], flag u16[n], qual_off u64[n+1], qual u8[]) for output records [first, first+n)."""
-        n = self.n - first if n is None else n
+        n = self.n_sorted - first if n is None else n
         if out is None:
             qb = int(self.L.elp_fetch_qual_bytes(self.h, first, n)) if want_qual else 0
             out = (np.empty(n, np.uint64), np.empty(n, np.uint16), np.empty(n + 1, np.uint64), np.empty(max(qb, 1), np.uint8))

@@ -12,6 +12,15 @@ Same names, argument meaning and error behaviour as the Go API, so that the pari
     reads.RunPipeline(reads, [tables.ApplyBQSR(0, [], 500)], sam.Keep)                           # phase 5
     reads.RunPipeline(out, [], sam.Keep)                                                         # phase 6
 
+With `--target-regions` (bedRegions) the reference filters the marked reads before the gather, in the full run
+(runBestPracticesPipelineIntermediateSam, cmd/filter.go:171-180) and in the `--bqsr-tables-only` worker (:288-296) alike:
+
+    InputBatches(header, batches).RunPipeline(reads, [filters.AddREFID, md], sam.Coordinate)   # phase 1: mark every read
+    metrics = filters.MarkOpticalDuplicates(reads, pairs, 100)                                   # optical duplicates, on every read
+    filters.FilterTargetRegions(reads, bedRegions)                                               # RemoveNonOverlappingReads on the device
+    tables = recal.Recalibrate(reads, 500)                                                       # the gather sees the kept reads only
+    tables.PrintBQSRTablesToIntermediateFile("w.elrecal")   # tables-only worker; the full run finalizes and applies as above
+
 Differences forced by the columnar representation: an ``AlignmentFilter`` here receives a whole ``AlignmentBatch``
 (the reference calls it once per ``*sam.Alignment``), and operators that run on the device (MarkDuplicates, ApplyBQSR)
 return marker filters -- the work happens in the ``Finalize`` of ``DeviceSam.AddNodes`` / in ``DeviceSam.RunPipeline``,
@@ -123,8 +132,16 @@ def RemoveNonOverlappingReads(regions):
                 r = int(batch.refid[i])
                 keep[i] = 0 <= r < len(flat) and overlap(flat[r], pos, end)
             return _keep(batch, keep)
+        flt.regions = flat          # DeviceSam.RunPipeline runs the filter on the device instead (elp_filter_target_regions)
         return flt
     return make
+
+
+def FilterTargetRegions(reads, bedRegions):
+    """The `--target-regions` phase, "Filtering out reads not in target regions." (cmd/filter.go:171-180, 288-296): after duplicate
+    marking and the duplication metrics, before the gather, filteredReads.RunPipeline(filteredReads, [RemoveNonOverlappingReads(bedRegions)]).
+    reads: a DeviceSam after phase 1; bedRegions: per-contig (k,2) Start / End arrays.  Returns the number of reads dropped."""
+    return reads.RunPipeline(reads, [RemoveNonOverlappingReads(bedRegions)], sam.Keep)
 
 
 def CleanSam(header):
@@ -268,13 +285,18 @@ class DeviceSam:
     # -- PipelineInput.RunPipeline (sam/filter-pipeline.go:242-279): the Sam is the source of a later phase
     def RunPipeline(self, output, hdr_filters, sorting_order):
         alns = compose_filters(self.Header, hdr_filters)
+        removed = 0
         for a in alns:
             if isinstance(a, _DeviceOp) and a.kind == "apply":
                 self.ctx.bqsr_apply()
             elif isinstance(a, _DeviceOp):
                 raise ValueError(f"operator {a.kind} cannot run in this phase")
+            elif getattr(a, "regions", None) is not None:        # RemoveNonOverlappingReads over the reads in output order
+                for ci in range(len(self.Header.SQ)):
+                    self.ctx.set_bqsr_target_regions(ci, a.regions[ci] if ci < len(a.regions) else np.zeros((0, 2), np.int32), already_flat=True)
+                removed += self.ctx.filter_target_regions()
         if output is self:
-            return
+            return removed
         idx, flag, qoff, qual = self.ctx.fetch()
         output.AddResult(self.Header, self._batches, idx, flag, qoff, qual)
 

@@ -69,6 +69,22 @@ def make_header(contigs, n_rg=4):
     return sam.Header(sq=[{"SN": n, "LN": int(ln)} for n, ln in contigs], rg=rg, so=sam.Unsorted)
 
 
+def exome_regions(contigs, seed=20260924, pad=0):
+    """The exons make_workload(..., exome=True) places its fragments around (synth.cpp: 300 bases every 15 kbp at a seeded offset), as
+    per-contig (k, 2) int32 (start, end) arrays widened by ``pad`` on both sides -- a target-regions BED for that workload."""
+    def mix(z):
+        M = (1 << 64) - 1
+        z = (z + 0x9E3779B97F4A7C15) & M
+        z = ((z ^ (z >> 30)) * 0xBF58476D1CE4E5B9) & M
+        z = ((z ^ (z >> 27)) * 0x94D049BB133111EB) & M
+        return z ^ (z >> 31)
+    out = []
+    for c, (_, ln) in enumerate(contigs):
+        starts = [1000 + ex * 15000 + mix(int(seed) ^ (c << 32) ^ ex) % 5000 for ex in range(max(1, int(ln) // 15000))]
+        out.append(np.array([(s - pad, s + 300 + pad) for s in starts], dtype=np.int32).reshape(-1, 2))
+    return out
+
+
 def make_workload(n_pairs, contigs, seed=20260924, L=150, dup_frac=0.10, optical_frac=0.20, unmapped_frac=0.01,
                   mate_unmapped_frac=0.005, secondary_frac=0.005, supplementary_frac=0.005, cross_contig_frac=0.01,
                   n_rg=4, wide_quals=False, exome=False, threads=None, want_reference=True, home=None, pair_id_base=0, genome_seed=None, reference_for=None):

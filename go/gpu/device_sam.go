@@ -268,7 +268,7 @@ func (d *DeviceSam) AddNodes(p *pipeline.Pipeline, header *sam.Header, sortingOr
 
 // RunPipeline: the source side of the write phase (sam/filter-pipeline.go:242-279): output order, FLAG and QUAL come from the device.
 func (d *DeviceSam) RunPipeline(output sam.PipelineOutput, hdrFilters []sam.Filter, sortingOrder sam.SortingOrder) {
-	n := uint64(C.elp_n_reads(d.ctx))
+	n := uint64(C.elp_n_sorted(d.ctx)) // the output order: fewer than the reads held after FilterTargetRegions
 	const chunk = uint64(1 << 18)
 	idx := make([]C.uint64_t, chunk)
 	flag := make([]C.uint16_t, chunk)
@@ -345,6 +345,21 @@ func (d *DeviceSam) SetKnownSites(contig int, startEnd []int32) {
 }
 
 // Recalibrate: (*BaseRecalibrator).Recalibrate (bqsr.go:467-551).  The tables stay on the device.
+// --target-regions: RemoveNonOverlappingReads(bedRegions) over the marked reads, before Recalibrate (cmd/filter.go:171-180, 288-296).
+// SetTargetRegions takes one contig's BED Start / End pairs (sorted and flattened inside); FilterTargetRegions returns the reads dropped.
+func (d *DeviceSam) SetTargetRegions(contig int, startEnd []int32) {
+	var p *C.int32_t
+	if len(startEnd) > 0 {
+		p = (*C.int32_t)(unsafe.Pointer(&startEnd[0]))
+	}
+	check(d.ctx, C.elp_set_bqsr_target_regions(d.ctx, C.int32_t(contig), p, C.uint64_t(len(startEnd)/2), 0))
+}
+func (d *DeviceSam) FilterTargetRegions() uint64 {
+	var removed C.uint64_t
+	check(d.ctx, C.elp_filter_target_regions(d.ctx, &removed))
+	return uint64(removed)
+}
+
 func (d *DeviceSam) Recalibrate() { check(d.ctx, C.elp_bqsr_gather(d.ctx)) }
 
 // FinalizeBQSRTables + PrintBQSRTables (bqsr.go:677-694, print-bqsr.go:269-298); recalFile may be "".

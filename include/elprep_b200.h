@@ -153,7 +153,9 @@ int elp_append_sam(elp_ctx *ctx, const char *text, uint64_t n_bytes);
 #define ELP_FILTER_NON_EXACT 4u
 #define ELP_FILTER_DUPLICATES 8u
 #define ELP_FILTER_NON_EXACT_STRICT 16u   /* RemoveNonExactMappingReadsStrict (:115-136): optional fields X0 = 1, X1 = XM = XO = XG = 0 must all be present */
-#define ELP_FILTER_TARGET_REGIONS 32u     /* RemoveNonOverlappingReads (:310-328): keep reads whose [POS, End()] overlaps a region of elp_set_target_regions */
+#define ELP_FILTER_TARGET_REGIONS 32u     /* RemoveNonOverlappingReads (:310-328): keep reads whose [POS, End()] overlaps a region of elp_set_target_regions.
+                                           * This is `--filter-non-overlapping-reads` (a phase-1 filter, before duplicate marking).  `--target-regions`
+                                           * filters after marking instead: elp_set_bqsr_target_regions + elp_filter_target_regions. */
 #define ELP_FILTER_CLEAR_DUPLICATE_FLAG 64u   /* ClearDuplicateFlag (:350-355): 0x400 cleared in the FLAG column at ingest, before marking; drops no record.
                                                * ELP_FILTER_DUPLICATES still tests the FLAG the record comes in with.  With elp_append_batch the
                                                * marshaller clears the bit in the batch's FLAG column (filters.ClearDuplicateFlag), as for the other filters. */
@@ -204,6 +206,26 @@ int elp_optical_merge(elp_ctx *ctx, int32_t slot, const int64_t *counters7, int3
 /* PrintDuplicatesMetrics (:601-699). The reference prints libraries in Go map order; here ascending by name.
  * started_on replaces time.Now().Format(...) so that the output is reproducible. */
 int elp_print_duplicates_metrics(elp_ctx *ctx, const char *path, const char *command_line, const char *started_on);
+
+/* ---- between phases 2 and 3: `--target-regions` (runBestPracticesPipelineIntermediateSam, cmd/filter.go:171-180, and the tables-only
+ * worker, :288-296): RemoveNonOverlappingReads(bedRegions) (filters/simple-filters.go:308-328) over the reads in output order, after
+ * duplicate marking and the duplication metrics, before the BQSR gather.  Its regions are a table of their own, so that
+ * `--filter-non-overlapping-reads A.bed --target-regions B.bed` works in one context.
+ *  - elp_set_bqsr_target_regions: one contig's regions, with the conventions of elp_set_target_regions (BED Start / End as the reference's
+ *    parser stores them; sorted by start and flattened inside unless already_flat).  The regions survive elp_reset.
+ *  - elp_filter_target_regions: keeps output record k iff intervals.Overlap(regions[RNAME], POS, alnEnd), alnEnd = End() for a mapped read
+ *    whose CIGAR has read bases and POS otherwise, on the CIGAR the context holds now (after elp_clean_sam).  RNAME * and contigs without
+ *    regions never overlap; without any regions every read is dropped (an empty BED file).  The kept records keep their relative order and
+ *    their FLAG, whether or not their mates were dropped; duplication metrics already computed are unchanged.  *n_removed (may be NULL):
+ *    the records dropped by this call.  ELP_ESTATE before elp_sort_markdup and after elp_bqsr_gather, elp_bqsr_tables_put or elp_bqsr_apply;
+ *    a second call drops what the regions set then drop.  Later phases see only the kept records: the BQSR gather and apply, and every fetch.
+ *  - elp_n_sorted: the records in output order -- elp_n_reads until elp_filter_target_regions drops some, the kept count afterwards.
+ *    elp_fetch, elp_fetch_async, elp_fetch_qual_bytes, elp_fetch_opt_flags, elp_fetch_bam(_bytes) and elp_fetch_sam(_bytes) index
+ *    [0, elp_n_sorted) (through the record filters of elp_set_output_filter for the byte outputs); elp_n_reads stays the number of reads
+ *    the context holds. ---- */
+int elp_set_bqsr_target_regions(elp_ctx *ctx, int32_t contig, const int32_t *start_end_pairs, uint64_t n_intervals, int already_flat);
+int elp_filter_target_regions(elp_ctx *ctx, uint64_t *n_removed);
+uint64_t elp_n_sorted(const elp_ctx *ctx);
 
 /* ---- phase 3: (*BaseRecalibrator).Recalibrate (filters/bqsr.go:467-551) ---- */
 int elp_bqsr_gather(elp_ctx *ctx);
@@ -305,7 +327,8 @@ int elp_fetch_sam(elp_ctx *ctx, uint64_t first, uint64_t n, char *out, uint64_t 
 #define ELP_OUT_REMOVE_OPTIONAL_READS 2u  /* RemoveOptionalReads (:146-152): reads with ELP_OPT_SR; the caller sets it iff the header has @sr (and drops @sr from the header it writes) */
 #define ELP_OUT_KEEP_FIELDS           4u  /* KeepOptionalFields(keep_tags) (:261-288); n_keep == 0 drops every optional field */
 int elp_set_output_filter(elp_ctx *ctx, uint32_t mask, const char *const *remove_tags, int32_t n_remove, const char *const *keep_tags, int32_t n_keep);
-/* after elp_sort_markdup: the number of output records that pass the record filters (elp_n_reads without them); 0 on error or before the sort */
+/* after elp_sort_markdup: the number of records of the output order (elp_n_sorted) that pass the record filters (elp_n_sorted without them);
+ * 0 on error or before the sort */
 uint64_t elp_n_output(elp_ctx *ctx);
 int elp_debug_adapt(elp_ctx *ctx, int32_t *upos, int32_t *score);
 /* per read, the 64-bit (library, QNAME) hash duplicate marking joins mates by (its low 31 bits are the join key); 0 for a read that is

@@ -140,6 +140,10 @@ class DeviceSam {
 
     void SetReference(int contig, const std::string& bases) { check(elp_set_reference(ctx_, contig, reinterpret_cast<const uint8_t*>(bases.data()), bases.size())); }
     void SetKnownSites(int contig, const std::vector<int32_t>& startEnd) { check(elp_set_known_sites(ctx_, contig, startEnd.empty() ? nullptr : startEnd.data(), startEnd.size() / 2, 0)); }
+    // `--target-regions`: RemoveNonOverlappingReads(bedRegions) after marking, before Recalibrate (cmd/filter.go:171-180, 288-296); one
+    // contig's BED Start / End pairs per call, sorted and flattened inside.  FilterTargetRegions returns the number of reads dropped.
+    void SetTargetRegions(int contig, const std::vector<int32_t>& startEnd) { check(elp_set_bqsr_target_regions(ctx_, contig, startEnd.empty() ? nullptr : startEnd.data(), startEnd.size() / 2, 0)); }
+    uint64_t FilterTargetRegions() { uint64_t removed = 0; check(elp_filter_target_regions(ctx_, &removed)); return removed; }
     void Recalibrate() { check(elp_bqsr_gather(ctx_)); }
     void FinalizeBQSRTables(const std::string& recalFile = "") { check(elp_bqsr_finalize(ctx_, recalFile.empty() ? nullptr : recalFile.c_str())); }
     void ApplyBQSR() { check(elp_bqsr_apply(ctx_)); }
@@ -164,7 +168,7 @@ class DeviceSam {
 
     // the source side of the write phase: the alignments in output order with the FLAG and QUAL the device computed
     void RunPipeline(const std::function<void(const Alignment&)>& sink, uint64_t chunk = 1u << 18) {
-        const uint64_t n = elp_n_reads(ctx_);
+        const uint64_t n = elp_n_sorted(ctx_);                            // the output order: fewer than Len() after FilterTargetRegions
         std::vector<uint64_t> idx(chunk), off(chunk + 1); std::vector<uint16_t> flag(chunk); std::vector<uint8_t> qual;
         for (uint64_t first = 0; first < n; first += chunk) {
             const uint64_t m = std::min(chunk, n - first);
