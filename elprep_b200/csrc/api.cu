@@ -112,15 +112,11 @@ int qual_presence_update(elp_ctx* c, uint64_t first_byte, uint64_t n_bytes) {
 int upload_side_inputs(elp_ctx* c) {
     if (!c->side_dirty) return E_OK;
     const int nc = c->n_contigs;
-    std::vector<const uint8_t*> rp(nc), np(nc), hp(nc); std::vector<const int32_t*> sp(nc);
-    for (int i = 0; i < nc; i++) { rp[i] = c->d_ref[i]; np[i] = c->d_refnib_raw[i] ? c->d_refnib_raw[i] + 32 : nullptr; hp[i] = c->d_refhot_raw[i] ? c->d_refhot_raw[i] + REFHOT_PAD : nullptr; sp[i] = c->d_sites[i]; }
+    std::vector<const uint8_t*> hp(nc);
+    for (int i = 0; i < nc; i++) hp[i] = c->d_refhot_raw[i] ? c->d_refhot_raw[i] + REFHOT_PAD : nullptr;
     if (nc) {
-        CUDA_TRY(c, cudaMemcpyAsync(c->d_ref_ptrs, rp.data(), nc * sizeof(void*), cudaMemcpyHostToDevice, c->stream));
-        CUDA_TRY(c, cudaMemcpyAsync(c->d_refnib_ptrs, np.data(), nc * sizeof(void*), cudaMemcpyHostToDevice, c->stream));
         CUDA_TRY(c, cudaMemcpyAsync(c->d_refhot_ptrs, hp.data(), nc * sizeof(void*), cudaMemcpyHostToDevice, c->stream));
         CUDA_TRY(c, cudaMemcpyAsync(c->d_ref_len, c->ref_len.data(), nc * 8, cudaMemcpyHostToDevice, c->stream));
-        CUDA_TRY(c, cudaMemcpyAsync(c->d_site_ptrs, sp.data(), nc * sizeof(void*), cudaMemcpyHostToDevice, c->stream));
-        CUDA_TRY(c, cudaMemcpyAsync(c->d_n_sites, c->n_sites.data(), nc * 8, cudaMemcpyHostToDevice, c->stream));
         CUDA_TRY(c, cudaStreamSynchronize(c->stream));
     }
     c->side_dirty = false;
@@ -173,9 +169,8 @@ int elp_create(const elp_config* cfg, elp_ctx** out) {
     const int nc = std::max(1, c->n_contigs), nr = std::max(1, c->n_rg);
     bool ok = cudaMalloc(&c->d_rg_lib, nr * 4) == cudaSuccess && cudaMalloc(&c->d_rg_cov, nr * 4) == cudaSuccess && cudaMalloc(&c->d_contig_len, nc * 4) == cudaSuccess &&
               cudaMalloc(&c->d_ranges, sizeof(DeviceRanges)) == cudaSuccess && cudaMalloc(&c->d_err, 4) == cudaSuccess &&
-              cudaMalloc(&c->d_ref_ptrs, nc * sizeof(void*)) == cudaSuccess && cudaMalloc(&c->d_refnib_ptrs, nc * sizeof(void*)) == cudaSuccess && cudaMalloc(&c->d_refhot_ptrs, nc * sizeof(void*)) == cudaSuccess &&
+              cudaMalloc(&c->d_refhot_ptrs, nc * sizeof(void*)) == cudaSuccess &&
               cudaMalloc(&c->d_bq_small, 512 * 4) == cudaSuccess && cudaMalloc(&c->d_qpresent, 16) == cudaSuccess && cudaMalloc(&c->d_ref_len, nc * 8) == cudaSuccess &&
-              cudaMalloc(&c->d_site_ptrs, nc * sizeof(void*)) == cudaSuccess && cudaMalloc(&c->d_n_sites, nc * 8) == cudaSuccess &&
               cudaMalloc(&c->d_tables, std::max<size_t>(16, c->geom.cells() * 2 * sizeof(int64_t))) == cudaSuccess;
     if (!ok) { c->err = "device allocation failed in elp_create"; return bail(ELP_ENOMEM); }
     if (c->n_rg) { cudaMemcpy(c->d_rg_lib, c->rg_lib.data(), c->n_rg * 4, cudaMemcpyHostToDevice); cudaMemcpy(c->d_rg_cov, c->rg_cov.data(), c->n_rg * 4, cudaMemcpyHostToDevice); }
@@ -184,8 +179,7 @@ int elp_create(const elp_config* cfg, elp_ctx** out) {
     cudaMemset(c->d_qpresent, 0, 16);
     c->n_qual = c->n_seq = ARENA_FRONT_PAD;
     cudaMemset(c->d_tables, 0, std::max<size_t>(16, c->geom.cells() * 2 * sizeof(int64_t)));
-    c->d_ref.assign(c->n_contigs, nullptr); c->d_refnib_raw.assign(c->n_contigs, nullptr); c->d_refhot_raw.assign(c->n_contigs, nullptr); c->ref_len.assign(c->n_contigs, 0);
-    c->d_sites.assign(c->n_contigs, nullptr); c->n_sites.assign(c->n_contigs, 0);
+    c->d_refhot_raw.assign(c->n_contigs, nullptr); c->ref_len.assign(c->n_contigs, 0);
     if ((e = cudaGetLastError()) != cudaSuccess) { c->err = std::string("elp_create: ") + cudaGetErrorString(e); return bail(ELP_ECUDA); }
     *out = c;
     return ELP_OK;
@@ -197,12 +191,9 @@ void elp_destroy(elp_ctx* c) {
     if (c->stream) cudaStreamSynchronize(c->stream);
     sam_state_release(c);
     sam_out_release(c);
-    for (auto p : c->d_ref) if (p) cudaFree(p);
-    for (auto p : c->d_refnib_raw) if (p) cudaFree(p);
     for (auto p : c->d_refhot_raw) if (p) cudaFree(p);
-    for (auto p : c->d_sites) if (p) cudaFree(p);
-    region_release(c->regions); region_release(c->bqsr_regions);
-    void* singles[] = {c->d_rg_lib, c->d_rg_cov, c->d_contig_len, c->d_ranges, c->d_err, (void*)c->d_ref_ptrs, (void*)c->d_refnib_ptrs, (void*)c->d_refhot_ptrs, c->d_bq_small, c->d_qpresent, c->d_ref_len, (void*)c->d_site_ptrs, c->d_n_sites, c->d_tables,
+    region_release(c->regions); region_release(c->bqsr_regions); region_release(c->known_sites);
+    void* singles[] = {c->d_rg_lib, c->d_rg_cov, c->d_contig_len, c->d_ranges, c->d_err, (void*)c->d_refhot_ptrs, c->d_bq_small, c->d_qpresent, c->d_ref_len, c->d_tables,
                        c->d_lut, c->d_clut, c->d_rowtab, c->d_cov_exists, c->d_unobs,c->d_opt_ctr, c->d_opt_hist, c->d_opt_ovf, c->d_opt_small, c->d_rg_names, c->d_rg_name_off, c->d_out_drop, c->ws.ghist, c->ws.gofs, c->ws.counters, c->ws.status};
     for (void* p : singles) if (p) cudaFree(p);
     c->refid.release(); c->pos.release(); c->nref.release(); c->pnext.release(); c->tlen.release(); c->rg.release(); c->flag.release(); c->mapq.release(); c->optf.release(); c->s_optf.release();
@@ -256,39 +247,14 @@ int elp_set_reference(elp_ctx* c, int32_t contig, const uint8_t* bases, uint64_t
     if (!c) return ELP_EINVAL;
     cudaSetDevice(c->device);
     if (contig < 0 || contig >= c->n_contigs) return c->fail(E_INVAL, "elp_set_reference: contig %d out of range", contig);
-    if (c->d_ref[contig]) { cudaFree(c->d_ref[contig]); c->d_ref[contig] = nullptr; }
-    CUDA_TRY(c, cudaMalloc(&c->d_ref[contig], n + 16));
-    CUDA_TRY(c, cudaMemcpy(c->d_ref[contig], bases, n, cudaMemcpyHostToDevice));
     c->ref_len[contig] = n; c->side_dirty = true;
-    return pack_reference(c, contig);
+    return pack_reference(c, contig, bases);
 }
 
 int elp_set_known_sites(elp_ctx* c, int32_t contig, const int32_t* se, uint64_t n_intervals, int already_flat) {
     if (!c) return ELP_EINVAL;
     cudaSetDevice(c->device);
-    if (contig < 0 || contig >= c->n_contigs) return c->fail(E_INVAL, "elp_set_known_sites: contig %d out of range", contig);
-    std::vector<int32_t> v(se, se + 2 * n_intervals);
-    uint64_t n = n_intervals;
-    if (!already_flat && n > 1) {
-        // stable sort by start (intervals.ParallelSortByStart) then Flatten (intervals/intervals.go:88-117): merge while next.Start <= cur.End
-        std::vector<std::pair<int32_t, int32_t>> iv(n);
-        for (uint64_t i = 0; i < n; i++) iv[i] = {v[2 * i], v[2 * i + 1]};
-        std::stable_sort(iv.begin(), iv.end(), [](const std::pair<int32_t, int32_t>& a, const std::pair<int32_t, int32_t>& b) { return a.first < b.first; });
-        uint64_t m = 0;
-        for (uint64_t i = 0; i < n; i++) {
-            if (m > 0 && iv[i].first <= iv[m - 1].second) { if (iv[i].second > iv[m - 1].second) iv[m - 1].second = iv[i].second; }
-            else iv[m++] = iv[i];
-        }
-        n = m;
-        for (uint64_t i = 0; i < n; i++) { v[2 * i] = iv[i].first; v[2 * i + 1] = iv[i].second; }
-    }
-    if (c->d_sites[contig]) { cudaFree(c->d_sites[contig]); c->d_sites[contig] = nullptr; }
-    if (n) {
-        CUDA_TRY(c, cudaMalloc(&c->d_sites[contig], n * 8));
-        CUDA_TRY(c, cudaMemcpy(c->d_sites[contig], v.data(), n * 8, cudaMemcpyHostToDevice));
-    }
-    c->n_sites[contig] = n; c->side_dirty = true;
-    return ELP_OK;
+    return region_set(c, c->known_sites, "elp_set_known_sites", contig, se, n_intervals, already_flat);
 }
 
 uint64_t elp_n_reads(const elp_ctx* c) { return c ? c->n : 0; }

@@ -371,15 +371,18 @@ template <class T> int grow(elp_ctx* c, DBuf<T>& b, size_t need, size_t keep) {
 
 }  // namespace
 
-// ---- region tables (RegionTable, ctx.h): the ingest filter's and the one of elp_filter_target_regions ----
+// ---- region tables (RegionTable, ctx.h): the ingest filter's, the one of elp_filter_target_regions and the BQSR known sites ----
+// Uploads go on the context's stream and are waited for: a pageable cudaMemcpy may return before its DMA has landed, and the
+// (non-blocking) stream of the kernels that read the table does not wait for it.
 int region_upload(elp_ctx* c, RegionTable& t) {
     if (!t.dirty && t.d_ptrs) return E_OK;
     const int nc = std::max(1, c->n_contigs);
     if ((int)t.d.size() != c->n_contigs) { t.d.assign(c->n_contigs, nullptr); t.n.assign(c->n_contigs, 0); }
     if (!t.d_ptrs) { CUDA_TRY(c, cudaMalloc(&t.d_ptrs, nc * sizeof(void*))); CUDA_TRY(c, cudaMalloc(&t.d_n, nc * 8)); }
     if (c->n_contigs) {
-        CUDA_TRY(c, cudaMemcpy(t.d_ptrs, t.d.data(), c->n_contigs * sizeof(void*), cudaMemcpyHostToDevice));
-        CUDA_TRY(c, cudaMemcpy(t.d_n, t.n.data(), c->n_contigs * 8, cudaMemcpyHostToDevice));
+        CUDA_TRY(c, cudaMemcpyAsync(t.d_ptrs, t.d.data(), c->n_contigs * sizeof(void*), cudaMemcpyHostToDevice, c->stream));
+        CUDA_TRY(c, cudaMemcpyAsync(t.d_n, t.n.data(), c->n_contigs * 8, cudaMemcpyHostToDevice, c->stream));
+        CUDA_TRY(c, cudaStreamSynchronize(c->stream));
     }
     t.dirty = false;
     return E_OK;
@@ -400,7 +403,11 @@ int region_set(elp_ctx* c, RegionTable& t, const char* who, int32_t contig, cons
         n = m;
     }
     if (t.d[contig]) { cudaFree(t.d[contig]); t.d[contig] = nullptr; }
-    if (n) { CUDA_TRY(c, cudaMalloc(&t.d[contig], n * 8)); CUDA_TRY(c, cudaMemcpy(t.d[contig], iv.data(), n * 8, cudaMemcpyHostToDevice)); }
+    if (n) {
+        CUDA_TRY(c, cudaMalloc(&t.d[contig], n * 8));
+        CUDA_TRY(c, cudaMemcpyAsync(t.d[contig], iv.data(), n * 8, cudaMemcpyHostToDevice, c->stream));
+        CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+    }
     t.n[contig] = n; t.dirty = true;
     return ELP_OK;
 }

@@ -180,11 +180,10 @@ struct GatherArgs {
     const uint32_t* cigar; const uint8_t *seq, *qual;
     const int32_t* rg_cov; int n_rg;
     const int32_t* contig_len; int n_contigs;
-    const uint8_t* const* ref; const uint64_t* ref_len;
+    const uint8_t* const* refhot; const uint64_t* ref_len;   // per contig: one-hot reference nibbles (pack_reference), low nibble first
     const int32_t* const* sites; const uint64_t* n_sites;
     TableGeom geom; unsigned long long* tables; uint32_t* err;
     ReadDesc* desc; uint32_t* ovf_bits; uint32_t* ovf_count; uint32_t ovf_cap;
-    const uint8_t* const* refnib;    // per contig: reference base codes, 4 bits per base, low nibble first
     uint32_t* gen_list; uint32_t* gen_count;   // [0]: reads for the warp-per-read fallback kernel, list grows up from gen_list[0]
     uint32_t* cg_list;                         // [1] of gen_count: insertion/deletion reads for the chunk kernel's GEN variant
     int lanes_per_read;              // chunk kernel: lanes (16-base chunks) reserved per read
@@ -193,6 +192,21 @@ struct GatherArgs {
     int ncols_s, ctx_col_s;          // chunk kernel rows: skewed cycle cells [0, ctx_col_s), then 16 context cells
     const uint32_t* in_list; uint32_t n_in;   // when set: only these reads (the general path behind bqsr_prep2_kernel); they all go through the per-lane CIGAR walk
 };
+
+// ---------------------------------------------------------------- rules shared by the two prep kernels (bqsr_prep_kernel, bqsr_prep2_kernel)
+// recalibrateAln, bqsr.go:225-244, with alignmentAgreesWithHeader, utils.go:130-138
+__device__ __forceinline__ bool recal_eligible(const GatherArgs& A, uint64_t k, uint16_t f, int32_t refid, int32_t pos0, int32_t g, int32_t L0) {
+    const uint8_t mq = A.mapq[k];
+    return !(A.optf[k] & 1u) &&       // the `sr` tag: a group-file copy of a spread read is never recalibrated (bqsr.go:225-229)
+           (mq > 0 && mq < 255) && !(f & (F_SECONDARY | F_DUPLICATE | F_QCFAILED)) && !((f & F_UNMAPPED) || refid < 0 || pos0 == 0) && pos0 > 0 && L0 > 0 &&
+           g >= 0 && g < A.n_rg && refid < A.n_contigs && pos0 <= A.contig_len[refid];
+}
+// intervals.Intersect, intervals/intervals.go:166-173: the first of the ns sorted, flattened sites sv whose end is >= start
+__device__ __forceinline__ uint64_t first_site_from(const int32_t* sv, uint64_t ns, int32_t start) {
+    uint64_t lo = 0, hi = ns;
+    while (lo < hi) { const uint64_t m = (lo + hi) >> 1; if (!(__ldg(sv + 2 * m + 1) >= start)) lo = m + 1; else hi = m; }
+    return lo;
+}
 
 // ---------------------------------------------------------------- kernel A: one thread per read
 __global__ void __launch_bounds__(128) bqsr_prep_kernel(GatherArgs A) {
@@ -207,16 +221,10 @@ __global__ void __launch_bounds__(128) bqsr_prep_kernel(GatherArgs A) {
         const uint4* src = reinterpret_cast<const uint4*>(&d); uint4* dst = reinterpret_cast<uint4*>(out);
         dst[0] = src[0]; dst[1] = src[1]; dst[2] = src[2];
     };
-    // ---- recalibrateAln, bqsr.go:225-244 ----
     const uint16_t f = A.flag[k];
-    const uint8_t mq = A.mapq[k];
     const int32_t refid = A.refid[k], pos0 = A.pos[k], g = A.rg[k], L0 = A.lseq[k];
     const int nc0 = (int)A.ncigar[k];
-    bool elig = !(A.optf[k] & 1u) &&       // the `sr` tag: a group-file copy of a spread read is never recalibrated (bqsr.go:225-229)
-                (mq > 0 && mq < 255) && !(f & (F_SECONDARY | F_DUPLICATE | F_QCFAILED)) && !((f & F_UNMAPPED) || refid < 0 || pos0 == 0) && pos0 > 0 && L0 > 0 &&
-                g >= 0 && g < A.n_rg && refid < A.n_contigs;
-    if (elig && pos0 > A.contig_len[refid]) elig = false;            // alignmentAgreesWithHeader, utils.go:130-138
-    if (!elig) { done(); return; }
+    if (!recal_eligible(A, k, f, refid, pos0, g, L0)) { done(); return; }
     if (nc0 > MAXC) { atomicOr(A.err, DERR_CIGAR_LIMIT); done(); return; }
     uint32_t cg[MAXC + 4], tmp[MAXC + 4];
     const uint64_t coff = A.cigar_off[k];
@@ -275,10 +283,7 @@ __global__ void __launch_bounds__(128) bqsr_prep_kernel(GatherArgs A) {
         int refl = 0;
         for (int i = 0; i < a.nc; i++) refl += cons_ref(op_of(a.cg[i])) * len_of(a.cg[i]);
         const int ss = a.pos, se = a.pos + refl - 1;
-        // intervals.Intersect, intervals/intervals.go:166-173
-        uint64_t lo = 0, hi = ns;
-        while (lo < hi) { const uint64_t m = (lo + hi) >> 1; if (!(sv[2 * m + 1] >= ss)) lo = m + 1; else hi = m; }
-        const uint64_t s0 = lo;
+        const uint64_t s0 = first_site_from(sv, ns, ss);
         uint64_t s1 = s0;
         while (s1 < ns && sv[2 * s1] <= se) s1++;
         if (s1 - s0 <= 4) {
@@ -340,7 +345,7 @@ __device__ __forceinline__ void reds_add(uint32_t a, uint32_t v) { asm volatile(
 // reads per step; lane (r, c) owns bases [16c, 16c+16) of read r.  Everything per base is SIMD inside 32/64-bit words:
 //   QUAL    16 bytes  (unaligned 16-byte window out of two aligned 128-bit loads)
 //   SEQ     16 BAM nibbles -> base codes 0..3 / 8 by bit arithmetic, 4 bits per base
-//   REF     16 nibbles of pre-packed reference codes (pack_reference): mismatch = XOR
+//   REF     16 one-hot reference nibbles (pack_reference): mismatch = XOR with the read's SEQ nibbles, which are one-hot for ACGT too
 //   context previous base in sequencing direction by shifting the code word one nibble (edge nibble from the neighbour lane)
 //   masks   counted / context-valid / mismatch / known-site flags as one bit per nibble
 // leaving ~14 instructions per base for the two shared-memory increments (cycle, context).  The cycle column of a
@@ -410,18 +415,18 @@ __global__ void __launch_bounds__(256, CHUNK_MINB) bqsr_chunk_kernel(GatherArgs 
         const bool rev = flags & DF_REVERSED;
         // ---- loads ----
         uint32_t Q[4] = {0, 0, 0, 0};
-        unsigned long long C = 0, R = 0, pastf = 0;
+        unsigned long long C = 0, X = 0, pastf = 0;   // X: the read's SEQ nibbles XOR the reference's one-hot nibbles
         if (nb > 0) {
             const uint64_t qloc = ((uint64_t)loc.y << 32) | loc.x, nl = ((uint64_t)loc.w << 32) | loc.z;
             const uint32_t refid = (uint32_t)(qloc >> 40);
             load16_unaligned(A.qual + (qloc & ((1ull << 40) - 1)) + (uint64_t)i0, Q);
-            const unsigned long long nibs = load16_nibbles_bam(A.seq, nl + (uint64_t)i0);
-            C = (unsigned long long)codes_of((uint32_t)nibs) | ((unsigned long long)codes_of((uint32_t)(nibs >> 32)) << 32);
-            if (!GEN) R = load16_nibbles_le(A.refnib[refid], (uint64_t)((int64_t)(int32_t)sc.x - 1 + i0));
+            const unsigned long long N = load16_nibbles_bam(A.seq, nl + (uint64_t)i0);
+            unsigned long long R = 0;
+            if (!GEN) R = load16_nibbles_le(A.refhot[refid], (uint64_t)((int64_t)(int32_t)sc.x - 1 + i0));
             else {
                 // computeSnpEvents (bqsr.go:254-285) over the ORIGINAL alignment (kept bases keep their positions under hard
                 // clipping): find the operation holding the chunk's first base; a chunk inside one M run is one window load,
-                // a chunk that touches an insertion / deletion takes its reference codes base by base
+                // a chunk that touches an insertion / deletion takes its reference nibbles base by base
                 const uint64_t coff = A.cigar_off[kcur]; const int nc = (int)A.ncigar[kcur];
                 const int oi0 = (int)(sc.y & 0xffff) + i0;                    // read offset in the stored (unclipped) read
                 int ri = 0, ci = 0, oplen = 0, opk = -1; int64_t j = (int64_t)A.pos[kcur] - 1;
@@ -432,9 +437,9 @@ __global__ void __launch_bounds__(256, CHUNK_MINB) bqsr_chunk_kernel(GatherArgs 
                 }
                 const int64_t reflen = (int64_t)A.ref_len[refid];
                 const bool mtype = opk == 0 || opk == 7 || opk == 8;
-                if (mtype && oi0 + nb <= ri + oplen && j + (oi0 - ri) + nb <= reflen) R = load16_nibbles_le(A.refnib[refid], (uint64_t)(j + (oi0 - ri)));
+                if (mtype && oi0 + nb <= ri + oplen && j + (oi0 - ri) + nb <= reflen) R = load16_nibbles_le(A.refhot[refid], (uint64_t)(j + (oi0 - ri)));
                 else {
-                    const uint8_t* rn = A.refnib[refid];
+                    const uint8_t* rn = A.refhot[refid];
                     int rem = opk < 0 ? 0 : ri + oplen - oi0;                   // bases left in the current operation
                     int64_t jj = j + (mtype ? (oi0 - ri) : 0);
                     bool m = mtype;
@@ -445,7 +450,7 @@ __global__ void __launch_bounds__(256, CHUNK_MINB) bqsr_chunk_kernel(GatherArgs 
                             if (o == 2 || o == 3) { jj += ln; continue; }
                             if (cons_read(o)) { rem = ln; m = (o == 0 || o == 7 || o == 8); }
                         }
-                        unsigned long long rc = (C >> (4 * b)) & 15ull;         // no reference base (insertion): never a mismatch
+                        unsigned long long rc = (N >> (4 * b)) & 15ull;         // no reference base (insertion): never a mismatch
                         if (m) {
                             if (jj >= reflen) pastf |= 1ull << (4 * b);
                             else rc = (unsigned long long)((__ldg(rn + (jj >> 1)) >> (4 * (int)(jj & 1))) & 15u);
@@ -456,6 +461,8 @@ __global__ void __launch_bounds__(256, CHUNK_MINB) bqsr_chunk_kernel(GatherArgs 
                     }
                 }
             }
+            X = N ^ R;   // one-hot: a counted base differs from the reference iff any bit does
+            C = (unsigned long long)codes_of((uint32_t)N) | ((unsigned long long)codes_of((uint32_t)(N >> 32)) << 32);
         }
         if (nb < CHUNK) { const unsigned long long inlen = range16(0, nb - 1); C = (C & (inlen * 15ull)) | ((ONES & ~inlen) << 3); }   // codes past the read end: 8
         // ---- low-quality tails (computeStrandedClippedSeq, bqsr.go:312-331): first / last base with QUAL > 2 ----
@@ -484,7 +491,6 @@ __global__ void __launch_bounds__(256, CHUNK_MINB) bqsr_chunk_kernel(GatherArgs 
         }
         const unsigned long long counted = ~(C >> 3) & ONES & ~skipf;                             // ACGT, inside the read, not a known site (QUAL >= 6 via the slot table)
         const unsigned long long okc = counted & ~((Pn | C) >> 3) & range16(wlo - i0, whi - i0);
-        const unsigned long long X = C ^ R;
         const unsigned long long snpf = (X | (X >> 1) | (X >> 2) | (X >> 3)) & counted;         // computeSnpEvents, bqsr.go:254-285
         if (GEN && (pastf & counted)) errbits |= DERR_REFEND;                                   // a counted base beyond the end of its contig
         if (counted) {
@@ -551,20 +557,6 @@ __global__ void __launch_bounds__(256, CHUNK_MINB) bqsr_chunk_kernel(GatherArgs 
     }
 }
 
-// reference bases -> 4-bit codes (baseToIntMap, bqsr.go:247-252: A/a/* C/c G/g T/t -> 0..3, everything else 8), low nibble first
-__global__ void __launch_bounds__(256) ref_pack_kernel(const uint8_t* __restrict__ ref, uint64_t n, uint8_t* __restrict__ out, uint64_t n_out) {
-    const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= n_out) return;
-    uint32_t v = 0;
-#pragma unroll
-    for (int h = 0; h < 2; h++) {
-        const uint64_t j = 2 * t + h; uint32_t cd = 8;
-        if (j < n) { const uint8_t b = ref[j]; if (b == 'A' || b == 'a' || b == '*') cd = 0; else if (b == 'C' || b == 'c') cd = 1; else if (b == 'G' || b == 'g') cd = 2; else if (b == 'T' || b == 't') cd = 3; }
-        v |= cd << (4 * h);
-    }
-    out[t] = (uint8_t)v;
-}
-
 // work lists of the eligible reads that are not DF_LEAN: DF_CHUNKG reads (insertions / deletions) for the chunk kernel's GEN
 // variant, everything else for the warp-per-read fallback.  One global atomic per block and list.
 __global__ void __launch_bounds__(256) gen_list_kernel(GatherArgs A) {
@@ -596,7 +588,6 @@ __global__ void __launch_bounds__(256) gen_list_kernel(GatherArgs A) {
 // (insertions / deletions, cycles beyond --max-cycle, > 4 known-site ranges, reads running off their contig)
 __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32, 2048 / (WARPS_PER_BLOCK * 32 * 2)) bqsr_general_kernel(GatherArgs A, uint32_t n_gen) {
     extern __shared__ uint32_t sm_tab[];
-    __shared__ uint8_t sm_refcode[256];   // baseToIntMap (bqsr.go:247-252): A/a/* C/c G/g T/t -> 0..3, everything else 8
     __shared__ int8_t sm_qslot[256];      // QUAL -> shared-memory slot, -1 = none (and for QUAL > 93)
     const unsigned lane = lane_id(), w = threadIdx.x >> 5;
     const int Lc = A.Lc, ncols_s = 2 * Lc + 1 + 16, max_cycle = A.geom.max_cycle;    // this kernel's rows are not skewed
@@ -604,9 +595,7 @@ __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32, 2048 / (WARPS_PER_BLOCK 
     uint32_t* sm_mis = sm_tab + cells;
     for (int i = threadIdx.x; i < 2 * cells; i += blockDim.x) sm_tab[i] = 0;
     {
-        const int b = threadIdx.x; uint8_t c = 8;
-        if (b == 'A' || b == 'a' || b == '*') c = 0; else if (b == 'C' || b == 'c') c = 1; else if (b == 'G' || b == 'g') c = 2; else if (b == 'T' || b == 't') c = 3;
-        sm_refcode[b] = c;
+        const int b = threadIdx.x;
         sm_qslot[b] = b < 94 ? A.qslot[b] : (int8_t)-1;
     }
     __syncthreads();
@@ -624,7 +613,7 @@ __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32, 2048 / (WARPS_PER_BLOCK 
         const int32_t refid = A.refid[k];
         const uint8_t* qualp = A.qual + A.qual_off[k] + c_s0;
         const uint8_t* seqp = A.seq + A.seq_off[k];
-        const uint8_t* ref = A.ref[refid]; const int64_t reflen = (int64_t)A.ref_len[refid];
+        const uint8_t* ref = A.refhot[refid]; const int64_t reflen = (int64_t)A.ref_len[refid];
         const int nit = (L + 31) >> 5;
         // ---- general path: insertions / deletions, or a cycle beyond --max-cycle somewhere in the read ----
         // low-quality tails (computeStrandedClippedSeq, bqsr.go:312-331): first / last base with QUAL > 2
@@ -688,7 +677,7 @@ __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32, 2048 / (WARPS_PER_BLOCK 
             uint32_t snp = 0;
             if (counted && jj >= 0) {
                 if (jj >= reflen) { errbits |= DERR_REFEND; }
-                else snp = sm_refcode[ref[jj]] != code;
+                else snp = nib_code((uint32_t)(ref[jj >> 1] >> (4 * (int)(jj & 1))) & 15u) != code;
             }
             const int cyc = cf + ic * inc;
             const bool badc = (cyc > max_cycle) | (cyc < -max_cycle);                     // checkCycleCovariate :364-369
@@ -758,29 +747,26 @@ __global__ void derive_q_kernel(TableGeom geom, long long* tables) {
 
 }  // namespace
 
-// nibble-packed reference codes of one contig (read by the chunk kernel); 32 bytes of padding on both sides because the
-// kernel reads aligned 16-byte windows around the bases it needs
-int pack_reference(elp_ctx* c, int contig) {
+// the device's only copy of one contig: one-hot nibbles, low nibble first, read by every gather kernel. REFHOT_PAD bytes in front
+// (windows of reads at the start of a contig and the shifted window of an insertion start before base 0), 64 behind (the aligned
+// window loads past the last base). The n host bases pass through a temporary device buffer that is freed before the return; the copy
+// goes on the context's stream, since a pageable cudaMemcpy may return before its DMA has landed and the stream does not wait for it.
+int pack_reference(elp_ctx* c, int contig, const uint8_t* bases) {
     const uint64_t n = c->ref_len[contig], n_out = (n + 1) / 2;
-    if (c->d_refnib_raw[contig]) { cudaFree(c->d_refnib_raw[contig]); c->d_refnib_raw[contig] = nullptr; }
-    CUDA_TRY(c, cudaMalloc(&c->d_refnib_raw[contig], n_out + 64));
-    CUDA_TRY(c, cudaMemsetAsync(c->d_refnib_raw[contig], 0x88, n_out + 64, c->stream));
-    if (n_out) {
-        c->launches++;
-        ref_pack_kernel<<<(unsigned)((n_out + 255) / 256), 256, 0, c->stream>>>(c->d_ref[contig], n, c->d_refnib_raw[contig] + 32, n_out);
-        LAUNCH_CHECK(c);
-    }
-    // one-hot nibbles for the count kernel (bqsr_count.inl); REFHOT_PAD bytes in front (windows of reads at the start of a contig and
-    // the shifted window of an insertion start before base 0), 64 behind
     if (c->d_refhot_raw[contig]) { cudaFree(c->d_refhot_raw[contig]); c->d_refhot_raw[contig] = nullptr; }
     CUDA_TRY(c, cudaMalloc(&c->d_refhot_raw[contig], n_out + REFHOT_PAD + 64));
     CUDA_TRY(c, cudaMemsetAsync(c->d_refhot_raw[contig], 0, n_out + REFHOT_PAD + 64, c->stream));
-    if (n_out) {
+    uint8_t* d_bases = nullptr;
+    cudaError_t e = n ? cudaMalloc(&d_bases, n) : cudaSuccess;
+    if (e == cudaSuccess && n) e = cudaMemcpyAsync(d_bases, bases, n, cudaMemcpyHostToDevice, c->stream);
+    if (e == cudaSuccess && n) {
         c->launches++;
-        ref_pack_hot_kernel<<<(unsigned)((n_out + 255) / 256), 256, 0, c->stream>>>(c->d_ref[contig], n, c->d_refhot_raw[contig] + REFHOT_PAD, n_out);
-        LAUNCH_CHECK(c);
+        ref_pack_hot_kernel<<<(unsigned)((n_out + 255) / 256), 256, 0, c->stream>>>(d_bases, n, c->d_refhot_raw[contig] + REFHOT_PAD, n_out);
+        e = cudaGetLastError();
     }
-    CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+    if (d_bases) cudaFree(d_bases);
+    CUDA_TRY(c, e);
     return E_OK;
 }
 
@@ -925,6 +911,7 @@ template <int S> int launch_count(elp_ctx* c, CountArgs K, bool indel, unsigned 
 int phase_bqsr_gather(elp_ctx* c) {
     if (!c->sorted) return c->fail(E_STATE, "elp_bqsr_gather called before elp_sort_markdup");
     int rc = upload_side_inputs(c);
+    if (!rc) rc = region_upload(c, c->known_sites);
     if (rc) return rc;
     const size_t cells = c->geom.cells();
     CUDA_TRY(c, cudaMemsetAsync(c->d_tables, 0, cells * 2 * sizeof(int64_t), c->stream));
@@ -935,9 +922,8 @@ int phase_bqsr_gather(elp_ctx* c) {
         A.n = n; A.refid = c->s_refid.p; A.pos = c->s_pos.p; A.nref = c->s_nref.p; A.pnext = c->s_pnext.p; A.tlen = c->s_tlen.p; A.rg = c->s_rg.p; A.lseq = c->s_lseq.p;
         A.flag = c->s_flag.p; A.mapq = c->s_mapq.p; A.optf = c->s_optf.p; A.qual_off = c->s_qual_off.p; A.seq_off = c->s_seq_off.p; A.cigar_off = c->s_cigar_off.p; A.ncigar = c->s_ncigar.p;
         A.cigar = c->cigar.p; A.seq = c->seq.p; A.qual = c->qual.p; A.rg_cov = c->d_rg_cov; A.n_rg = c->n_rg; A.contig_len = c->d_contig_len; A.n_contigs = c->n_contigs;
-        A.ref = c->d_ref_ptrs; A.ref_len = c->d_ref_len; A.sites = c->d_site_ptrs; A.n_sites = c->d_n_sites;
+        A.refhot = c->d_refhot_ptrs; A.ref_len = c->d_ref_len; A.sites = c->known_sites.d_ptrs; A.n_sites = c->known_sites.d_n;
         A.geom = c->geom; A.tables = reinterpret_cast<unsigned long long*>(c->d_tables); A.err = c->d_err;
-        A.refnib = c->d_refnib_ptrs;
         uint64_t ref_bytes = 0; for (auto l : c->ref_len) ref_bytes += l;
         // SURVEY.md 8d: N_eligible * (19 + 4 + 4 c + L/2 + L) + genome bytes once; per-read averages of the arenas stand in for c and L
         const double per_read = 23.0 + ((double)c->n_cigar * 4 + (double)(c->n_seq - ARENA_FRONT_PAD) + (double)(c->n_qual - ARENA_FRONT_PAD)) / (double)c->n;

@@ -39,8 +39,9 @@ struct DupCounters { int64_t ctr[7] = {0, 0, 0, 0, 0, 0, 0}; std::map<int64_t, i
 #define OPT_HBINS 1024
 #define OPT_OVF_CAP (1 << 16)
 
-// target regions of RemoveNonOverlappingReads (filters/simple-filters.go:310-328) on the device: per contig, the flattened, start-sorted
-// (start, end) pairs, and the two device arrays of pointers and counts the kernels index by REFID (region_set / region_upload, bam_ingest.cu)
+// per-contig interval table on the device (the ingest filter's target regions, elp_filter_target_regions' regions and the BQSR known
+// sites): per contig, the flattened, start-sorted (start, end) pairs, and the two device arrays of pointers and counts the kernels
+// index by REFID (region_set / region_upload, bam_ingest.cu)
 struct RegionTable {
     std::vector<int32_t*> d; std::vector<uint64_t> n;
     const int32_t** d_ptrs = nullptr; uint64_t* d_n = nullptr; bool dirty = true;
@@ -86,19 +87,12 @@ struct elp_ctx {
     int32_t* d_contig_len = nullptr; // [n_contigs]
 
     // ---- reference genome + known sites (device) ----
-    std::vector<uint8_t*> d_ref;          // per contig
     std::vector<uint64_t> ref_len;
-    const uint8_t** d_ref_ptrs = nullptr; // [n_contigs] device array of pointers
-    std::vector<uint8_t*> d_refnib_raw;   // per contig: 4-bit reference codes (bqsr_gather.cu pack_reference), payload at +32
-    const uint8_t** d_refnib_ptrs = nullptr;
-    std::vector<uint8_t*> d_refhot_raw;   // per contig: one-hot reference nibbles for the count kernel (bqsr_count.inl), payload at +REFHOT_PAD
-    const uint8_t** d_refhot_ptrs = nullptr;
+    std::vector<uint8_t*> d_refhot_raw;   // per contig: the reference as one-hot nibbles (bqsr_gather.cu pack_reference), payload at +REFHOT_PAD
+    const uint8_t** d_refhot_ptrs = nullptr;   // [n_contigs] device array of the payload pointers
     uint64_t* d_ref_len = nullptr;
-    std::vector<int32_t*> d_sites;        // per contig, (start,end) pairs
-    std::vector<uint64_t> n_sites;
-    const int32_t** d_site_ptrs = nullptr;
-    uint64_t* d_n_sites = nullptr;
     bool side_dirty = true;
+    RegionTable known_sites;                 // elp_set_known_sites (survives elp_reset)
 
     // ---- reads, arrival order (SoA columns) ----
     uint64_t n = 0, n_qname = 0, n_cigar = 0, n_qual = 0, n_seq = 0;
@@ -261,7 +255,7 @@ int phase_bqsr_apply(elp_ctx* c);
 int build_apply_lut(elp_ctx* c, int Lc);   // bqsr_finalize.cu
 int build_compact_lut(elp_ctx* c);
 int upload_side_inputs(elp_ctx* c);
-int pack_reference(elp_ctx* c, int contig);
+int pack_reference(elp_ctx* c, int contig, const uint8_t* bases);   // bases: ref_len[contig] host bytes
 int check_device_errors(elp_ctx* c);
 int upload_small(elp_ctx* c, void* dst, const void* src, size_t bytes);   // api.cu: host -> device without the copy engine
 int comm_allreduce_ranges(elp_ctx* c);   // comm.cu

@@ -181,7 +181,7 @@ def test_raw_site_lists(values):
 
 
 def test_sites_replaced_across_reset():
-    """one context, two gathers: the second list is uploaded again after elp_reset (side_dirty), and the tables follow it"""
+    """one context, two gathers: the second list is uploaded again after elp_reset (the table is dirty), and the tables follow it"""
     from elprep_b200 import device
     values = (2, 11, 25, 37, 40)
     w = with_qual_alphabet(synth.make_workload(3_000, CONTIGS, seed=70, L=151), values)
