@@ -258,7 +258,7 @@ int upload_side_inputs(elp_ctx* c);
 int pack_reference(elp_ctx* c, int contig, const uint8_t* bases);   // bases: ref_len[contig] host bytes
 int check_device_errors(elp_ctx* c);
 int upload_small(elp_ctx* c, void* dst, const void* src, size_t bytes);   // api.cu: host -> device without the copy engine
-int comm_allreduce_ranges(elp_ctx* c);   // comm.cu
+int comm_allreduce_ranges(elp_ctx* c, int local_rc);   // comm.cu: returns local_rc, or a peer's error code
 int spread_exchange_begin(elp_ctx* c);
 int spread_exchange_end(elp_ctx* c);
 int exclusive_scan_u64_from_u32(elp_ctx* c, const uint32_t* in, uint64_t* out, uint64_t n, uint64_t base);   // out[n+1], out[0] = base

@@ -525,11 +525,11 @@ static int mark_pairs(elp_ctx* c, bool optical, uint64_t nt, uint64_t n_true_pai
 
 int phase_markdup(elp_ctx* c, bool optical) {
     int rc = phase_adapt(c);
-    if (rc) return rc;
-    if (c->h_ranges.qual_invalid) return c->fail(E_QUAL, "Invalid QUAL character in a read entering duplicate marking");
+    if (!rc && c->h_ranges.qual_invalid) rc = c->fail(E_QUAL, "Invalid QUAL character in a read entering duplicate marking");
     // several GPUs (comm.cu): common key ranges, then the visiting mates of cross-group pairs arrive as ghost reads n .. n + n_ghost - 1.
-    // Every rank makes the same collective calls in the same order, whatever its own reads look like.
-    rc = comm_allreduce_ranges(c);
+    // Every rank makes the same collective calls in the same order, whatever its own reads look like; an error of one rank before marking
+    // rides along in them (comm.cu), so that every rank returns before any FLAG changes.
+    rc = comm_allreduce_ranges(c, rc);
     if (rc) return rc;
     rc = spread_exchange_begin(c);
     if (rc) return rc;

@@ -264,7 +264,11 @@ int elp_optical_add_gob(elp_ctx *ctx, const char *path);
  * the smaller REFID together with its own pairs, and their 0x400 bits are sent back.  elp_bqsr_tables_allreduce is LoadAndCombineBQSRTables
  * (filters/print-bqsr.go:310-329) as one ncclAllReduce(sum, int64) between elp_bqsr_gather and elp_bqsr_finalize; elp_optical_allreduce is
  * mergeDuplicatesCtrMaps (filters/mark-optical-duplicates.go:451-466) over the ranks.  Output order = the ranks' outputs concatenated in
- * contig-group order (MergeSortedFilesSplitPerChromosome, sam/split-merge.go:465-547). */
+ * contig-group order (MergeSortedFilesSplitPerChromosome, sam/split-merge.go:465-547).
+ * A read of a cross-group pair may have a QNAME of at most 92 bytes (a longer one is ELP_ELIMIT; one context has no such limit).  An error
+ * of elp_sort_markdup on one rank before marking (an invalid QUAL, a negative POS, that QNAME limit, a failed allocation for the exchange)
+ * is returned by every rank: the others with the same code and "on rank r" in elp_last_error, and no rank changes FLAG.  A device fault
+ * (a sticky CUDA error) is not agreed. */
 int elp_comm_unique_id(uint8_t id[128]);
 int elp_comm_init(elp_ctx *ctx, const uint8_t id[128], int rank, int world);
 int elp_comm_set_partition(elp_ctx *ctx, const int32_t *contig_owner);
