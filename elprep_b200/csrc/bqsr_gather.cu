@@ -10,8 +10,8 @@
 //                      (:376-387) and 2-mer context (:64-146,312-362) covariates, and the table updates.  Observation
 //                      counters of the frequent QUAL values are privatised in shared memory per CTA (persistent CTAs,
 //                      flushed once with 64-bit atomics); mismatches (rare) and infrequent QUAL values go to the global table.
-// Kept bases keep their original alignment under hard clipping, so reference positions come from the ORIGINAL CIGAR
-// offset by the clip start; only the known-sites mask needs the clipped CIGAR (its coordinate mapping has quirks).
+// Kept bases keep the reference steps of the stored alignment under hard clipping, so reference positions come from the STORED
+// CIGAR placed at the clipped POS; only the known-sites mask needs the clipped CIGAR (its coordinate mapping has quirks).
 // Table layout: dense int64 [n_cov][94][1 + (2*max_cycle+1) + 16][2] = (observations, mismatches); the
 // QualityScores column is derived as the row sum of the Cycles columns (every counted base updates both).
 #include <algorithm>
@@ -160,11 +160,26 @@ __device__ void hard_clip(Clip& a, int start, int stop) {
     if (start == 0) a.pos += shift;
 }
 
+// reference index (POS - 1 based) that the stored alignment gives read base r: its own for an M/=/X base, the next reference base's for
+// an inserted one.  The clipped alignment keeps the stored one's reference steps between kept bases, but not always its origin:
+// clean_hard_clipped folds a leading D into H without moving POS when the clip is on the right (utils.go:473-504), and
+// computeSnpEvents (bqsr.go:254-285) then compares against the reference from POS.  The kernels that walk the stored CIGAR therefore
+// start from c_pos - 1 - orig_ref_offset(first kept base), c_pos being where the clipped alignment reaches its first kept base.
+__device__ int64_t orig_ref_offset(const uint32_t* cigar, int nc, int r) {
+    int ri = 0; int64_t j = 0;
+    for (int i = 0; i < nc; i++) {
+        const uint32_t op = __ldg(cigar + i); const int o = op_of(op), ln = len_of(op);
+        if (cons_read(o)) { if (r < ri + ln) return j + ((o == 0 || o == 7 || o == 8) ? r - ri : 0); ri += ln; }
+        if (cons_ref(o)) j += ln;
+    }
+    return j;
+}
+
 // ---------------------------------------------------------------- per-read descriptor written by the prep kernel
 struct __align__(16) ReadDesc {
     uint64_t qloc;            // QUAL arena offset of the first kept base | refid << 40
     uint64_t nloc;            // SEQ nibble index of the first kept base (2 * seq_off + c_s0)
-    int32_t c_pos;            // POS after clipping (1-based)
+    int32_t c_pos;            // 1-based reference position the clipped alignment reaches at its first kept base: POS after clipping + leading D
     uint16_t c_s0, c_len;     // kept bases [c_s0, c_s0 + c_len) of the original read; c_len == 0: not recalibrated
     uint8_t flags, cov, n_skip, pad;
     uint32_t ovf;             // slot of the 512-bit skip bitmask when more than 4 known-site ranges hit the read
@@ -267,12 +282,22 @@ __global__ void __launch_bounds__(128) bqsr_prep_kernel(GatherArgs A) {
     }
     if (a.err) { atomicOr(A.err, DERR_CLIP); done(); return; }
     if (a.slen <= 0) { done(); return; }
+    {
+        // computeSnpEvents (bqsr.go:254-285) reads the reference at every M/=/X base of the clipped alignment, counted or not: a read whose
+        // last such base lies past the contig is the reference's index-out-of-range error even when no base past the end would be counted
+        // (QUAL < 6, N, a known site).  Trailing deletions do not read the reference.
+        int64_t j = (int64_t)a.pos - 1, m_end = j;
+        for (int i = 0; i < a.nc; i++) { const int o = op_of(a.cg[i]); if (cons_ref(o)) j += len_of(a.cg[i]); if (o == 0 || o == 7 || o == 8) m_end = j; }
+        if (m_end > (int64_t)A.ref_len[refid]) { atomicOr(A.err, DERR_REFEND); done(); return; }
+    }
     if (a.slen > 32 * MAXIT) { atomicOr(A.err, DERR_READLEN_LIMIT); done(); return; }
     const int L = a.slen;
     // is the clipped CIGAR a single M-type operation (plus hard clips)?
     int n_m = 0, n_other = 0;
     for (int i = 0; i < a.nc; i++) { const int o = op_of(a.cg[i]); if (o == 0 || o == 7 || o == 8) n_m++; else if (o != 5) n_other++; }
-    d.c_pos = a.pos; d.c_s0 = (uint16_t)a.s0; d.c_len = (uint16_t)L; d.cov = (uint8_t)A.rg_cov[g];
+    int lead_d = 0;                                                  // deletions before the first kept base (a read not clipped at all)
+    for (int i = 0; i < a.nc && !cons_read(op_of(a.cg[i])); i++) lead_d += cons_ref(op_of(a.cg[i])) * len_of(a.cg[i]);
+    d.c_pos = a.pos + lead_d; d.c_s0 = (uint16_t)a.s0; d.c_len = (uint16_t)L; d.cov = (uint8_t)A.rg_cov[g];
     d.qloc = (A.qual_off[k] + (uint64_t)a.s0) | ((uint64_t)(uint32_t)refid << 40);
     d.nloc = A.seq_off[k] * 2 + (uint64_t)a.s0;
     d.flags = ((f & F_REVERSED) ? DF_REVERSED : 0) | ((f & F_LAST) ? DF_LAST : 0) | ((n_m == 1 && n_other == 0) ? DF_SINGLE_M : 0);
@@ -424,12 +449,13 @@ __global__ void __launch_bounds__(256, CHUNK_MINB) bqsr_chunk_kernel(GatherArgs 
             unsigned long long R = 0;
             if (!GEN) R = load16_nibbles_le(A.refhot[refid], (uint64_t)((int64_t)(int32_t)sc.x - 1 + i0));
             else {
-                // computeSnpEvents (bqsr.go:254-285) over the ORIGINAL alignment (kept bases keep their positions under hard
-                // clipping): find the operation holding the chunk's first base; a chunk inside one M run is one window load,
-                // a chunk that touches an insertion / deletion takes its reference nibbles base by base
+                // computeSnpEvents (bqsr.go:254-285) over the stored CIGAR, placed at the clipped POS (orig_ref_offset): find the
+                // operation holding the chunk's first base; a chunk inside one M run is one window load, a chunk that touches an
+                // insertion / deletion takes its reference nibbles base by base
                 const uint64_t coff = A.cigar_off[kcur]; const int nc = (int)A.ncigar[kcur];
                 const int oi0 = (int)(sc.y & 0xffff) + i0;                    // read offset in the stored (unclipped) read
-                int ri = 0, ci = 0, oplen = 0, opk = -1; int64_t j = (int64_t)A.pos[kcur] - 1;
+                int ri = 0, ci = 0, oplen = 0, opk = -1;
+                int64_t j = (int64_t)(int32_t)sc.x - 1 - orig_ref_offset(A.cigar + coff, nc, (int)(sc.y & 0xffff));
                 for (; ci < nc; ci++) {
                     const uint32_t op = __ldg(A.cigar + coff + ci); const int o = op_of(op), ln = len_of(op);
                     if (cons_read(o)) { if (oi0 < ri + ln) { opk = o; oplen = ln; break; } ri += ln; }
@@ -633,9 +659,9 @@ __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32, 2048 / (WARPS_PER_BLOCK 
         const uint32_t row0 = cov * (uint32_t)A.n_slots;
         const bool single_m = (flags & DF_SINGLE_M) != 0;
         const int64_t j0 = (int64_t)c_pos - 1;
-        // general CIGAR: reference positions from the ORIGINAL alignment (kept bases keep their positions under hard clipping)
+        // general CIGAR: reference positions from the stored CIGAR, placed at the clipped POS (orig_ref_offset)
         int32_t pos_orig = 0; uint64_t coff = 0; int nc = 0;
-        if (!single_m) { pos_orig = A.pos[k]; coff = A.cigar_off[k]; nc = (int)A.ncigar[k]; }
+        if (!single_m) { coff = A.cigar_off[k]; nc = (int)A.ncigar[k]; pos_orig = c_pos - (int32_t)orig_ref_offset(A.cigar + coff, nc, c_s0); }
         uint32_t errbits = 0;
         uint32_t carry = 8;   // code of the base just before this iteration's first lane, in sequencing direction
         for (int t = 0; t < nit; t++) {
