@@ -12,7 +12,7 @@ SO_PATH = os.environ.get("ELPREP_B200_LIB", os.path.join(_HERE, "lib", "libelpre
 
 SO_KEEP, SO_UNKNOWN, SO_UNSORTED, SO_QUERYNAME, SO_COORDINATE = 0, 1, 2, 3, 4
 MARKDUP, MARKDUP_OPTICAL = 1, 2
-EINVAL, ELIMIT, ESTATE, EBAM, ESAM = -1, -15, -16, -18, -20
+EINVAL, ELIMIT, ESTATE, EBAM, EBGZF, ESAM = -1, -15, -16, -18, -19, -20
 FILTER_UNMAPPED, FILTER_UNMAPPED_STRICT, FILTER_NON_EXACT, FILTER_DUPLICATES, FILTER_NON_EXACT_STRICT, FILTER_TARGET_REGIONS = 1, 2, 4, 8, 16, 32
 FILTER_CLEAR_DUPLICATE_FLAG = 64
 OUT_REMOVE_DUPLICATES, OUT_REMOVE_OPTIONAL_READS, OUT_KEEP_FIELDS = 1, 2, 4
@@ -49,7 +49,8 @@ EXPORTS = ["elp_create", "elp_destroy", "elp_last_error", "elp_reserve", "elp_re
            "elp_debug_sort_u64_range", "elp_debug_sort_u128_range", "elp_debug_sort_u32_range", "elp_debug_scan_u32", "elp_debug_join_hash", "elp_debug_coord_chunk_keys",
            "elp_optical_n_libraries", "elp_optical_library_name", "elp_optical_metrics", "elp_optical_histogram", "elp_optical_merge",
            "elp_print_duplicates_metrics",
-           "elp_bgzf_inflate_bound", "elp_bgzf_inflate", "elp_bgzf_deflate_bound", "elp_bgzf_deflate", "elp_bam_header_size"]
+           "elp_bgzf_inflate_bound", "elp_bgzf_inflate", "elp_bgzf_deflate_bound", "elp_bgzf_deflate", "elp_bam_header_size",
+           "elp_append_bgzf", "elp_append_bgzf_end", "elp_debug_inflate"]
 
 _lib = None
 
@@ -158,5 +159,8 @@ def load():
     L.elp_bgzf_deflate.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64), C.c_int, C.c_int, C.c_int]
     L.elp_bam_header_size.restype = C.c_int64
     L.elp_bam_header_size.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(C.c_int32)]
+    L.elp_append_bgzf.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64]
+    L.elp_append_bgzf_end.argtypes = [C.c_void_p]
+    L.elp_debug_inflate.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
     _lib = L
     return L

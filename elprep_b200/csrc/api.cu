@@ -191,6 +191,7 @@ void elp_destroy(elp_ctx* c) {
     if (c->stream) cudaStreamSynchronize(c->stream);
     sam_state_release(c);
     sam_out_release(c);
+    bgzf_release(c);
     for (auto p : c->d_refhot_raw) if (p) cudaFree(p);
     region_release(c->regions); region_release(c->bqsr_regions); region_release(c->known_sites);
     void* singles[] = {c->d_rg_lib, c->d_rg_cov, c->d_contig_len, c->d_ranges, c->d_err, (void*)c->d_refhot_ptrs, c->d_bq_small, c->d_qpresent, c->d_ref_len, c->d_tables,
@@ -226,6 +227,7 @@ int elp_reset(elp_ctx* c) {
     c->adapted = c->sorted = c->qual_out_valid = c->gathered = c->finalized = c->opt_valid = false;
     c->out_sel_valid = false; c->n_out = 0;   // (the output filter setting itself stays)
     c->launches = 0;
+    bgzf_stream_reset(c);
     CUDA_TRY(c, cudaMemsetAsync(c->d_err, 0, 4, c->stream));
     return ELP_OK;
 }
@@ -303,6 +305,7 @@ static int append_impl(elp_ctx* c, const elp_batch* b, bool wait) {
     const uint64_t bn = b->n;
     if (bn == 0) return ELP_OK;
     if (c->sorted) return c->fail(E_STATE, "elp_append_batch after elp_sort_markdup (call elp_reset first)");
+    if (c->bgzf_open) return c->fail(E_STATE, "elp_append_batch while a BGZF file is open (elp_append_bgzf_end first)");
     const uint64_t n0 = c->n, n1 = n0 + bn;
     if (n1 >= (1ull << 32)) return c->fail(E_LIMIT, "more than 2^32-1 reads in one context");
     const uint64_t bq = b->qname_off[bn] - b->qname_off[0], bc = b->cigar_off[bn] - b->cigar_off[0];
@@ -372,6 +375,7 @@ int elp_sort_markdup(elp_ctx* c, int sorting_order, int mark_duplicates) {
     if (!c) return ELP_EINVAL;
     cudaSetDevice(c->device);
     if (c->sorted) return c->fail(E_STATE, "elp_sort_markdup called twice (call elp_reset first)");
+    if (c->bgzf_open) return c->fail(E_STATE, "elp_sort_markdup while a BGZF file is open (elp_append_bgzf_end first)");
     if (mark_duplicates != 0 && mark_duplicates != ELP_MARKDUP && mark_duplicates != ELP_MARKDUP_OPTICAL) return c->fail(E_INVAL, "elp_sort_markdup: mark_duplicates must be 0, ELP_MARKDUP or ELP_MARKDUP_OPTICAL");
     if (mark_duplicates) TRY(phase_markdup(c, mark_duplicates == ELP_MARKDUP_OPTICAL));
     TRY(phase_coordinate_sort(c, sorting_order == ELP_SO_COORDINATE ? 1 : (sorting_order == ELP_SO_QUERYNAME ? 2 : 0)));

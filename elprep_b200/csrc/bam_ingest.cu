@@ -424,6 +424,7 @@ extern "C" int elp_append_bam(elp_ctx* c, const uint8_t* records, uint64_t n_byt
     cudaSetDevice(c->device);
     std::lock_guard<std::mutex> lk(c->append_mu);
     if (c->sorted) return c->fail(E_STATE, "elp_append_bam after elp_sort_markdup (call elp_reset first)");
+    if (c->bgzf_open) return c->fail(E_STATE, "elp_append_bam while a BGZF file is open (elp_append_bgzf_end first)");
     // record offsets: given, or found by walking the block_size chain
     std::vector<uint64_t> walked;
     if (!record_off) {

@@ -14,46 +14,16 @@
 #include <thread>
 #include <vector>
 #include "../../include/elprep_b200.h"
+#include "bgzf_scan.hpp"
 #include "pool.hpp"
 
 namespace {
 
 constexpr uint64_t BGZF_IN = 0xff00;          // uncompressed bytes per block written
-constexpr int BGZF_HDR = 18, BGZF_TRL = 8;
+constexpr int BGZF_HDR = 18;
 
-inline uint32_t rd16(const uint8_t* p) { return (uint32_t)p[0] | ((uint32_t)p[1] << 8); }
-inline uint32_t rd32(const uint8_t* p) { return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24); }
 inline void wr16(uint8_t* p, uint32_t v) { p[0] = v & 255; p[1] = (v >> 8) & 255; }
 inline void wr32(uint8_t* p, uint32_t v) { p[0] = v & 255; p[1] = (v >> 8) & 255; p[2] = (v >> 16) & 255; p[3] = v >> 24; }
-
-struct Block { uint64_t in_off, cdata_off, cdata_len, out_off; uint32_t isize, crc; };
-
-// block boundaries of a BGZF byte run (utils/bgzf/bgzf-files.go:95-127): gzip member header with FEXTRA, subfield 'B','C',2
-int scan_blocks(const uint8_t* d, uint64_t n, std::vector<Block>& blocks, uint64_t* total) {
-    uint64_t x = 0, out = 0;
-    while (x < n) {
-        if (n - x < (uint64_t)BGZF_HDR + BGZF_TRL) return ELP_EBGZF;
-        const uint8_t* h = d + x;
-        if (h[0] != 31 || h[1] != 139 || h[2] != 8 || !(h[3] & 4)) return ELP_EBGZF;
-        const uint32_t xlen = rd16(h + 10);
-        if (n - x < 12ull + xlen + BGZF_TRL) return ELP_EBGZF;
-        uint32_t bsize = 0; bool found = false;
-        for (uint32_t i = 0; i + 4 <= xlen;) {
-            const uint8_t* e = h + 12 + i; const uint32_t slen = rd16(e + 2);
-            if (e[0] == 66 && e[1] == 67 && slen == 2 && i + 6 <= xlen) { bsize = rd16(e + 4) + 1; found = true; break; }
-            i += 4 + slen;
-        }
-        if (!found) return ELP_EBGZF;                                  // "missing BC extra subfield in BGZF header"
-        if (bsize < 12 + xlen + BGZF_TRL || x + bsize > n) return ELP_EBGZF;
-        Block b; b.in_off = x; b.cdata_off = x + 12 + xlen; b.cdata_len = bsize - 12 - xlen - BGZF_TRL;
-        b.crc = rd32(d + x + bsize - 8); b.isize = rd32(d + x + bsize - 4); b.out_off = out;
-        if (b.isize > 65536) return ELP_EBGZF;
-        out += b.isize; x += bsize;
-        blocks.push_back(b);
-    }
-    *total = out;
-    return ELP_OK;
-}
 
 }  // namespace
 
@@ -61,20 +31,20 @@ extern "C" {
 
 int64_t elp_bgzf_inflate_bound(const uint8_t* data, uint64_t n) {
     if (!data && n) return ELP_EINVAL;
-    std::vector<Block> blocks; uint64_t total = 0;
+    std::vector<BgzfBlock> blocks; uint64_t total = 0;
     const int rc = scan_blocks(data, n, blocks, &total);
     return rc ? rc : (int64_t)total;
 }
 
 int elp_bgzf_inflate(const uint8_t* data, uint64_t n, uint8_t* out, uint64_t capacity, uint64_t* out_n, int n_threads) {
     if ((!data && n) || !out_n) return ELP_EINVAL;
-    std::vector<Block> blocks; uint64_t total = 0;
+    std::vector<BgzfBlock> blocks; uint64_t total = 0;
     int rc = scan_blocks(data, n, blocks, &total);
     if (rc) return rc;
     if (total > capacity || (!out && total)) return ELP_EINVAL;
     std::atomic<int> err{0};
     pool_for(blocks.size(), n_threads, [&](size_t i) {
-        const Block& b = blocks[i];
+        const BgzfBlock& b = blocks[i];
         if (b.isize == 0) { if (b.crc != 0) err = 1; return; }
         z_stream zs; std::memset(&zs, 0, sizeof zs);
         if (inflateInit2(&zs, -15) != Z_OK) { err = 1; return; }

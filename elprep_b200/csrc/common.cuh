@@ -22,6 +22,7 @@
 #define E_LIMIT (-15)
 #define E_TILE (-17)
 #define E_BAM (-18)
+#define E_BGZF (-19)
 #define E_SAM (-20)
 #define E_STATE (-16)
 

@@ -119,6 +119,9 @@ struct elp_ctx {
     struct SamState* sam = nullptr;          // device tables and staging of elp_append_sam (sam_ingest.cu)
     uint64_t n_sam_lost_names = 0;           // reads of elp_append_sam whose RNAME / RNEXT text the stored record cannot reproduce (elp_fetch_sam refuses)
     struct SamOutState* sam_out = nullptr;   // @SQ names and float staging of elp_fetch_sam (sam_format.cu)
+    struct BgzfStream* bgzf = nullptr;       // carried bytes and device staging of elp_append_bgzf / elp_debug_inflate (bgzf_inflate.cu)
+    bool bgzf_open = false;                  // a BGZF file is open (elp_append_bgzf until elp_append_bgzf_end or elp_reset): the other appends
+                                             // and elp_sort_markdup refuse, as the file's records are not all in yet
     uint8_t* d_rg_names = nullptr; uint32_t* d_rg_name_off = nullptr; std::vector<std::string> rg_ids;   // @RG IDs for the RG:Z match
     DBuf<int32_t> lseq_stage;       // staging for l_seq of the batch being appended
     DBuf<uint64_t> off_stage;       // staging for batch-relative offsets
@@ -272,3 +275,5 @@ int build_output_columns(elp_ctx* c, const uint32_t* perm, uint64_t n_out, bool 
 int phase_target_filter(elp_ctx* c, uint64_t* n_removed);   // target_regions.cu
 void sam_state_release(elp_ctx* c);   // sam_ingest.cu
 void sam_out_release(elp_ctx* c);     // sam_format.cu
+void bgzf_stream_reset(elp_ctx* c);   // bgzf_inflate.cu: forget the open file (elp_reset)
+void bgzf_release(elp_ctx* c);

@@ -192,6 +192,24 @@ class Context:
             t = np.ascontiguousarray(text, dtype=np.uint8)
             self._ck(self.L.elp_append_sam(self.h, C.cast(_vp(t), C.c_char_p), t.size))
 
+    def append_bgzf(self, data):
+        """the next bytes of a BGZF-compressed BAM file (bytes or a uint8 array), cut anywhere; inflated, framed and ingested on the device"""
+        d = np.frombuffer(data, dtype=np.uint8) if isinstance(data, (bytes, bytearray, memoryview)) else np.ascontiguousarray(data, dtype=np.uint8)
+        self._ck(self.L.elp_append_bgzf(self.h, _vp(d) if d.size else None, d.size))
+
+    def append_bgzf_end(self):
+        """ends the file of append_bgzf: it must end in the EOF marker block, with no block or record bytes left"""
+        self._ck(self.L.elp_append_bgzf_end(self.h))
+
+    def debug_inflate(self, data):
+        """whole BGZF blocks -> uint8 array of the inflated bytes, decoded on the device (the contract of bgzf.inflate)"""
+        d = np.frombuffer(data, dtype=np.uint8) if isinstance(data, (bytes, bytearray, memoryview)) else np.ascontiguousarray(data, dtype=np.uint8)
+        bound = int(self.L.elp_bgzf_inflate_bound(_vp(d) if d.size else None, d.size))
+        out = np.empty(max(bound, 1), np.uint8)
+        n = C.c_uint64()
+        self._ck(self.L.elp_debug_inflate(self.h, _vp(d) if d.size else None, d.size, _vp(out), max(bound, 0), C.byref(n)))
+        return out[:int(n.value)]
+
     @property
     def n(self):
         return int(self.L.elp_n_reads(self.h))

@@ -240,6 +240,25 @@ func (d *DeviceSam) appendBatch(batch []*sam.Alignment) {
 	check(d.ctx, rc)
 }
 
+// AppendBgzf hands over the next bytes of a BGZF-compressed BAM file as they come off disk, cut anywhere; the device inflates them,
+// walks the header and frames and ingests the records (elp_append_bgzf).  AppendBgzfEnd ends the file (EOF marker, no bytes left).
+func (d *DeviceSam) AppendBgzf(chunk []byte) {
+	if len(chunk) == 0 {
+		return
+	}
+	d.mu.Lock()
+	rc := C.elp_append_bgzf(d.ctx, (*C.uint8_t)(unsafe.Pointer(&chunk[0])), C.uint64_t(len(chunk)))
+	d.mu.Unlock()
+	check(d.ctx, rc)
+}
+
+func (d *DeviceSam) AppendBgzfEnd() {
+	d.mu.Lock()
+	rc := C.elp_append_bgzf_end(d.ctx)
+	d.mu.Unlock()
+	check(d.ctx, rc)
+}
+
 // AddNodes: the receiving end of phase 1 (sam/filter-pipeline.go:108-128).  The Finalize runs what By(CoordinateLess).ParallelStableSort
 // (sam/sam-types.go:599-641) and filters.MarkDuplicates (+ MarkOpticalDuplicates) do in the reference.
 func (d *DeviceSam) AddNodes(p *pipeline.Pipeline, header *sam.Header, sortingOrder sam.SortingOrder) {

@@ -360,6 +360,29 @@ uint64_t elp_bgzf_deflate_bound(uint64_t n);
 int elp_bgzf_deflate(const uint8_t *data, uint64_t n, uint8_t *out, uint64_t capacity, uint64_t *out_n, int level, int n_threads, int write_eof);
 int64_t elp_bam_header_size(const uint8_t *bam, uint64_t n, int32_t *n_ref_out);  /* -1 if malformed or truncated */
 
+/* ---- a BGZF-compressed BAM file straight into a context (SURVEY.md 8f row 2; utils/bgzf/bgzf-files.go:95-127,164-221 and the header part
+ * of sam/bam-files.go), inflated on the device:
+ *  - elp_append_bgzf: the file's bytes, handed over in order and cut anywhere (mid gzip header, mid block, mid record); the file's first
+ *    call starts at byte 0 of the file.  An incomplete trailing BGZF block (host side, < 64 KiB) and an incomplete trailing record (device
+ *    side) are carried to the next call.  The BAM header is walked on the device and checked against elp_config: n_ref must equal
+ *    n_contigs, every l_ref contig_lengths and, when contig_names were given, every name (ELP_EINVAL otherwise; ELP_EBAM for bytes that are
+ *    not a BAM header); a header may span several blocks and calls.  The complete records are ingested exactly as by elp_append_bam:
+ *    ingest filters, RG:Z, the sr bit, and the arena of elp_fetch_bam / elp_fetch_sam; CG:B is ELP_ELIMIT.
+ *  - Validity.  A block is valid exactly when elp_bgzf_inflate accepts it: magic, FEXTRA, a BC subfield, bsize, ISIZE <= 65536; the DEFLATE
+ *    stream ends with exactly ISIZE bytes out; the CRC-32 matches; an empty block has CRC 0.  Anything else is ELP_EBGZF.
+ *  - Atomic calls.  Nothing of a failing call is appended; the reads of earlier calls stay.  After an error the stream is poisoned:
+ *    elp_append_bgzf and elp_append_bgzf_end return ELP_ESTATE until elp_reset (the reference panics at that point).
+ *  - Ordering.  While a file is open (from its first elp_append_bgzf to its elp_append_bgzf_end, or an error) elp_append_bam,
+ *    elp_append_sam, elp_append_batch and elp_sort_markdup return ELP_ESTATE.  elp_reset discards the stream.  One caller per stream:
+ *    the calls serialise like the other appends, but only the caller knows the byte order.
+ *  - elp_append_bgzf_end ends the file: ELP_EBGZF if block bytes remain or the last block was not the EOF marker (bgzf-files.go:111-115),
+ *    ELP_EBAM if header or record bytes remain, ELP_ESTATE without an open file; afterwards a new file may start.
+ *  - elp_debug_inflate: whole BGZF blocks -> inflated bytes, with the contract of elp_bgzf_inflate but decoded on the device (tests,
+ *    micro-benchmark); it does not touch an open stream. ---- */
+int elp_append_bgzf(elp_ctx *ctx, const uint8_t *data, uint64_t n_bytes);
+int elp_append_bgzf_end(elp_ctx *ctx);
+int elp_debug_inflate(elp_ctx *ctx, const uint8_t *data, uint64_t n, uint8_t *out, uint64_t capacity, uint64_t *out_n);
+
 /* ---- measurement ---- */
 uint64_t elp_launch_count(const elp_ctx *ctx);           /* kernels launched by this library since create/reset */
 int elp_kernel_stats(elp_ctx *ctx, elp_kernel_stat *out, int cap); /* returns number of entries; profile must be on */

@@ -135,6 +135,10 @@ class DeviceSam {
         check(elp_append_batch(ctx_, &b));
         alns_.insert(alns_.end(), batch.begin(), batch.end());
     }
+    // a BGZF-compressed BAM file instead of AddNodes: its bytes in order, cut anywhere, inflated and parsed on the device (elp_append_bgzf);
+    // AppendBgzfEnd after the last bytes.  RunPipeline's alignments then come from elp_fetch_bam / elp_fetch_sam, not from AddNodes.
+    void AppendBgzf(const uint8_t* data, size_t n) { check(elp_append_bgzf(ctx_, data, n)); }
+    void AppendBgzfEnd() { check(elp_append_bgzf_end(ctx_)); }
     // the Finalize of AddNodes: By(CoordinateLess / QNAMELess).ParallelStableSort + filters.MarkDuplicates (+ MarkOpticalDuplicates)
     void Finalize(SortingOrder order) { check(elp_sort_markdup(ctx_, (int)order, opts_.MarkDuplicates ? (opts_.AlsoOpticals ? ELP_MARKDUP_OPTICAL : ELP_MARKDUP) : 0)); }
 
