@@ -50,7 +50,7 @@ EXPORTS = ["elp_create", "elp_destroy", "elp_last_error", "elp_reserve", "elp_re
            "elp_optical_n_libraries", "elp_optical_library_name", "elp_optical_metrics", "elp_optical_histogram", "elp_optical_merge",
            "elp_print_duplicates_metrics",
            "elp_bgzf_inflate_bound", "elp_bgzf_inflate", "elp_bgzf_deflate_bound", "elp_bgzf_deflate", "elp_bam_header_size",
-           "elp_append_bgzf", "elp_append_bgzf_end", "elp_debug_inflate"]
+           "elp_append_bgzf", "elp_append_bgzf_end", "elp_debug_inflate", "elp_fetch_bgzf", "elp_debug_deflate"]
 
 _lib = None
 
@@ -162,5 +162,7 @@ def load():
     L.elp_append_bgzf.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64]
     L.elp_append_bgzf_end.argtypes = [C.c_void_p]
     L.elp_debug_inflate.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
+    L.elp_fetch_bgzf.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, C.c_uint64, C.c_int, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
+    L.elp_debug_deflate.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
     _lib = L
     return L

@@ -192,6 +192,7 @@ void elp_destroy(elp_ctx* c) {
     sam_state_release(c);
     sam_out_release(c);
     bgzf_release(c);
+    bgzf_deflate_release(c);
     for (auto p : c->d_refhot_raw) if (p) cudaFree(p);
     region_release(c->regions); region_release(c->bqsr_regions); region_release(c->known_sites);
     void* singles[] = {c->d_rg_lib, c->d_rg_cov, c->d_contig_len, c->d_ranges, c->d_err, (void*)c->d_refhot_ptrs, c->d_bq_small, c->d_qpresent, c->d_ref_len, c->d_tables,

@@ -589,6 +589,21 @@ static int bam_out_prepare(elp_ctx* c, uint64_t first, uint64_t n, uint64_t* tot
     return E_OK;
 }
 
+// the records of the call (bam_out_prepare ran: off_stage holds their offsets, total their bytes) formatted at dst
+static int bam_out_format(elp_ctx* c, uint64_t first, uint64_t n, const uint32_t* sel, uint64_t total, uint8_t* dst) {
+    if (c->out_fields) {
+        c->begin("bam_out_fields_emit", (double)c->n_bam * (double)n / (double)std::max<uint64_t>(c->n, 1) + (double)total);
+        bam_out_fields_emit_kernel<<<nblk(n * 32, 256), 256, 0, c->stream>>>(n, first, sel, c->perm.p, c->bam_all_off.p, c->bam_all.p, c->d_out_drop, c->off_stage.p, dst,
+                                                                             c->s_flag.p, c->s_mapq.p, c->s_out_off.p, c->qual_out_valid ? c->qual_out.p : nullptr);
+    } else {
+        c->begin("bam_format", 2.0 * (double)total);
+        bam_out_copy_kernel<<<nblk(n * 32, 256), 256, 0, c->stream>>>(n, first, sel, c->perm.p, c->bam_all_off.p, c->bam_all.p, c->off_stage.p, dst, c->s_flag.p, c->s_mapq.p, c->s_out_off.p,
+                                                                      c->qual_out_valid ? c->qual_out.p : nullptr);
+    }
+    c->end(); LAUNCH_CHECK(c);
+    return E_OK;
+}
+
 extern "C" uint64_t elp_fetch_bam_bytes(elp_ctx* c, uint64_t first, uint64_t n) {
     if (!c || n == 0) return 0;
     cudaSetDevice(c->device);
@@ -606,20 +621,27 @@ extern "C" int elp_fetch_bam(elp_ctx* c, uint64_t first, uint64_t n, uint8_t* ou
     TRY(bam_out_prepare(c, first, n, &total, &sel));
     if (total > capacity) return c->fail(E_INVAL, "elp_fetch_bam: output buffer too small (%llu > %llu)", (unsigned long long)total, (unsigned long long)capacity);
     TRY(grow(c, c->bam_raw, total + 64, 0));      // staging for the formatted records
-    if (c->out_fields) {
-        c->begin("bam_out_fields_emit", (double)c->n_bam * (double)n / (double)std::max<uint64_t>(c->n, 1) + (double)total);
-        bam_out_fields_emit_kernel<<<nblk(n * 32, 256), 256, 0, c->stream>>>(n, first, sel, c->perm.p, c->bam_all_off.p, c->bam_all.p, c->d_out_drop, c->off_stage.p, c->bam_raw.p,
-                                                                             c->s_flag.p, c->s_mapq.p, c->s_out_off.p, c->qual_out_valid ? c->qual_out.p : nullptr);
-    } else {
-        c->begin("bam_format", 2.0 * (double)total);
-        bam_out_copy_kernel<<<nblk(n * 32, 256), 256, 0, c->stream>>>(n, first, sel, c->perm.p, c->bam_all_off.p, c->bam_all.p, c->off_stage.p, c->bam_raw.p, c->s_flag.p, c->s_mapq.p, c->s_out_off.p,
-                                                                      c->qual_out_valid ? c->qual_out.p : nullptr);
-    }
-    c->end(); LAUNCH_CHECK(c);
+    TRY(bam_out_format(c, first, n, sel, total, c->bam_raw.p));
     CUDA_TRY(c, cudaMemcpyAsync(out, c->bam_raw.p, total, cudaMemcpyDeviceToHost, c->stream));
     if (record_off) CUDA_TRY(c, cudaMemcpyAsync(record_off, c->off_stage.p, (n + 1) * 8, cudaMemcpyDeviceToHost, c->stream));
     CUDA_TRY(c, cudaStreamSynchronize(c->stream));
     return ELP_OK;
+}
+
+// the records of elp_fetch_bam(first, n) behind the caller's prefix in bam_raw, deflated there (bgzf_deflate.cu): the records never leave the
+// device uncompressed
+extern "C" int elp_fetch_bgzf(elp_ctx* c, uint64_t first, uint64_t n, const uint8_t* prefix, uint64_t n_prefix, int write_eof, uint8_t* out, uint64_t capacity, uint64_t* out_n) {
+    if (c && c->n_cleaned) return c->fail(E_STATE, "elp_fetch_bgzf: elp_clean_sam rewrote %llu CIGARs; the stored records still carry the old ones (use elp_fetch)", (unsigned long long)c->n_cleaned);
+    if (!c || !out || !out_n || (!prefix && n_prefix)) return ELP_EINVAL;
+    cudaSetDevice(c->device);
+    uint64_t total = 0; const uint32_t* sel = nullptr;
+    if (n) TRY(bam_out_prepare(c, first, n, &total, &sel));
+    const uint64_t all = n_prefix + total, need = elp_bgzf_deflate_bound(all);
+    if (capacity < need) return c->fail(E_INVAL, "elp_fetch_bgzf: output buffer too small (%llu < elp_bgzf_deflate_bound = %llu)", (unsigned long long)capacity, (unsigned long long)need);
+    TRY(grow(c, c->bam_raw, all + 64, 0));
+    if (n_prefix) CUDA_TRY(c, cudaMemcpyAsync(c->bam_raw.p, prefix, n_prefix, cudaMemcpyHostToDevice, c->stream));
+    if (n) TRY(bam_out_format(c, first, n, sel, total, c->bam_raw.p + n_prefix));
+    return bgzf_deflate_run(c, c->bam_raw.p, all, write_eof, out, out_n);
 }
 
 extern "C" int elp_set_target_regions(elp_ctx* c, int32_t contig, const int32_t* se, uint64_t n_intervals, int already_flat) {

@@ -59,9 +59,7 @@ __global__ void __launch_bounds__(256) bgzf_crc_kernel(const BlockDesc* __restri
     const uint64_t b = (uint64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
     if (b >= nb || status[b]) return;
     const BlockDesc d = tab[b];
-    const uint32_t chunk = (d.isize + 31) / 32, a = min(d.isize, lane * chunk), e = min(d.isize, a + chunk);
-    uint32_t v = dfl::crc_shift(x2n.v, dfl::crc_bytes(ctab, 0, out + d.out_off + a, e - a), d.isize - e);
-    for (int o = 16; o; o >>= 1) v ^= __shfl_xor_sync(FULL_MASK, v, o);
+    const uint32_t v = dfl::warp_crc(ctab, x2n.v, out + d.out_off, d.isize, lane);
     if (lane == 0 && v != d.crc) status[b] = dfl::E_CRC;
 }
 

@@ -120,6 +120,7 @@ struct elp_ctx {
     uint64_t n_sam_lost_names = 0;           // reads of elp_append_sam whose RNAME / RNEXT text the stored record cannot reproduce (elp_fetch_sam refuses)
     struct SamOutState* sam_out = nullptr;   // @SQ names and float staging of elp_fetch_sam (sam_format.cu)
     struct BgzfStream* bgzf = nullptr;       // carried bytes and device staging of elp_append_bgzf / elp_debug_inflate (bgzf_inflate.cu)
+    struct DeflateState* bgzf_out = nullptr;  // device scratch of elp_fetch_bgzf / elp_debug_deflate (bgzf_deflate.cu)
     bool bgzf_open = false;                  // a BGZF file is open (elp_append_bgzf until elp_append_bgzf_end or elp_reset): the other appends
                                              // and elp_sort_markdup refuse, as the file's records are not all in yet
     uint8_t* d_rg_names = nullptr; uint32_t* d_rg_name_off = nullptr; std::vector<std::string> rg_ids;   // @RG IDs for the RG:Z match
@@ -277,3 +278,5 @@ void sam_state_release(elp_ctx* c);   // sam_ingest.cu
 void sam_out_release(elp_ctx* c);     // sam_format.cu
 void bgzf_stream_reset(elp_ctx* c);   // bgzf_inflate.cu: forget the open file (elp_reset)
 void bgzf_release(elp_ctx* c);
+int bgzf_deflate_run(elp_ctx* c, const uint8_t* in, uint64_t n, int write_eof, uint8_t* out, uint64_t* out_n);   // bgzf_deflate.cu: in[0, n) on the device -> BGZF at out
+void bgzf_deflate_release(elp_ctx* c);

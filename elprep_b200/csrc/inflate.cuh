@@ -267,4 +267,15 @@ INF_HD uint32_t crc_shift(const uint32_t* x2n, uint32_t crc, uint64_t n_bytes) {
     return multmodp(p, crc);
 }
 
+#ifdef __CUDACC__
+// crc32 of p[0, n) by one warp: lane k takes the k-th 1/32 slice, shifts its crc past the bytes after the slice, and the slices fold by XOR
+// (ctab: crc_table_entry, x2n: x2n_table); every lane returns the whole crc
+__device__ __forceinline__ uint32_t warp_crc(const uint32_t* ctab, const uint32_t* x2n, const uint8_t* p, uint32_t n, unsigned lane) {
+    const uint32_t chunk = (n + 31) / 32, a = min(n, lane * chunk), e = min(n, a + chunk);
+    uint32_t v = crc_shift(x2n, crc_bytes(ctab, 0, p + a, e - a), n - e);
+    for (int o = 16; o; o >>= 1) v ^= __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+#endif
+
 }  // namespace dfl

@@ -210,6 +210,14 @@ class Context:
         self._ck(self.L.elp_debug_inflate(self.h, _vp(d) if d.size else None, d.size, _vp(out), max(bound, 0), C.byref(n)))
         return out[:int(n.value)]
 
+    def debug_deflate(self, data, eof=True):
+        """bytes or a uint8 array -> uint8 array of BGZF blocks (0xff00 input bytes each, the EOF marker when eof), deflated on the device"""
+        d = np.frombuffer(data, dtype=np.uint8) if isinstance(data, (bytes, bytearray, memoryview)) else np.ascontiguousarray(data, dtype=np.uint8)
+        out = np.empty(int(self.L.elp_bgzf_deflate_bound(d.size)), np.uint8)
+        n = C.c_uint64()
+        self._ck(self.L.elp_debug_deflate(self.h, _vp(d) if d.size else None, d.size, int(bool(eof)), _vp(out), out.size, C.byref(n)))
+        return out[:int(n.value)]
+
     @property
     def n(self):
         return int(self.L.elp_n_reads(self.h))
@@ -354,6 +362,17 @@ class Context:
         out, off = np.empty(max(nb, 1), np.uint8), np.empty(n + 1, np.uint64)
         self._ck(self.L.elp_fetch_bam(self.h, first, n, _vp(out), out.size, _vp(off)))
         return out[:nb], off
+
+    def fetch_bgzf(self, first=0, n=None, prefix=b"", eof=True):
+        """-> uint8 array: the BGZF blocks of prefix + the records fetch_bam(first, n) returns (the EOF marker when eof), deflated on the
+        device; outputs of consecutive ranges, eof on the last only, concatenate to one BGZF file"""
+        n = self._n_out(first) if n is None else n
+        p = np.frombuffer(prefix, dtype=np.uint8) if isinstance(prefix, (bytes, bytearray, memoryview)) else np.ascontiguousarray(prefix, dtype=np.uint8)
+        nb = int(self.L.elp_fetch_bam_bytes(self.h, first, n)) if n else 0
+        out = np.empty(int(self.L.elp_bgzf_deflate_bound(nb + p.size)), np.uint8)
+        got = C.c_uint64()
+        self._ck(self.L.elp_fetch_bgzf(self.h, first, n, _vp(p) if p.size else None, p.size, int(bool(eof)), _vp(out), out.size, C.byref(got)))
+        return out[:int(got.value)]
 
     def fetch_sam(self, first=0, n=None):
         """-> (uint8 SAM text, uint64 line offsets [n+1]) of output records [first, first+n): FormatAlignment of each stored record with

@@ -259,6 +259,29 @@ func (d *DeviceSam) AppendBgzfEnd() {
 	check(d.ctx, rc)
 }
 
+// FetchBgzf: output records [first, first+n) of elp_fetch_bam behind prefix (the BAM header on a file's first call) as BGZF blocks,
+// deflated on the device (elp_fetch_bgzf), with the EOF marker when eof.  The bytes go to the file as they are, with no bgzf.Writer;
+// the outputs of consecutive ranges, eof on the last only, make one file.
+func (d *DeviceSam) FetchBgzf(first, n uint64, prefix []byte, eof bool) []byte {
+	var records uint64
+	if n > 0 {
+		records = uint64(C.elp_fetch_bam_bytes(d.ctx, C.uint64_t(first), C.uint64_t(n))) // (0 on a refusal, which elp_fetch_bgzf then reports)
+	}
+	out := make([]byte, uint64(C.elp_bgzf_deflate_bound(C.uint64_t(records+uint64(len(prefix))))))
+	var pp *C.uint8_t
+	if len(prefix) > 0 {
+		pp = (*C.uint8_t)(unsafe.Pointer(&prefix[0]))
+	}
+	e := C.int(0)
+	if eof {
+		e = 1
+	}
+	var got C.uint64_t
+	check(d.ctx, C.elp_fetch_bgzf(d.ctx, C.uint64_t(first), C.uint64_t(n), pp, C.uint64_t(len(prefix)), e, (*C.uint8_t)(unsafe.Pointer(&out[0])),
+		C.uint64_t(len(out)), &got))
+	return out[:uint64(got)]
+}
+
 // AddNodes: the receiving end of phase 1 (sam/filter-pipeline.go:108-128).  The Finalize runs what By(CoordinateLess).ParallelStableSort
 // (sam/sam-types.go:599-641) and filters.MarkDuplicates (+ MarkOpticalDuplicates) do in the reference.
 func (d *DeviceSam) AddNodes(p *pipeline.Pipeline, header *sam.Header, sortingOrder sam.SortingOrder) {

@@ -383,6 +383,30 @@ int elp_append_bgzf(elp_ctx *ctx, const uint8_t *data, uint64_t n_bytes);
 int elp_append_bgzf_end(elp_ctx *ctx);
 int elp_debug_inflate(elp_ctx *ctx, const uint8_t *data, uint64_t n, uint8_t *out, uint64_t capacity, uint64_t *out_n);
 
+/* ---- the output records as a BGZF-compressed BAM file, deflated on the device (SURVEY.md 8f row 2; the writer of
+ * utils/bgzf/bgzf-files.go:324-431): the records never cross to the host uncompressed.
+ *  - elp_fetch_bgzf writes the BGZF blocks of prefix || elp_fetch_bam(first, n) to out and their length to *out_n.  prefix (n_prefix
+ *    bytes, may be NULL when 0) is typically the BAM header -- magic, text and reference list, which only the caller can format -- on the
+ *    first call of a file.  The records are exactly those of elp_fetch_bam: output order, FLAG, MAPQ and QUAL patched, the record and field
+ *    filters of elp_set_output_filter, the kept records after elp_filter_target_regions; [first, first+n) indexes elp_n_output.  n == 0
+ *    is allowed (prefix only, EOF marker only, or nothing).
+ *  - Blocks.  The bytes are cut into blocks of 0xff00 bytes, the last one partial, as elp_bgzf_deflate cuts them (so both writers give the
+ *    same ISIZE sequence), each one gzip member with the BC subfield and one final DEFLATE block: dynamic Huffman codes, or stored when
+ *    that is smaller, so every block is at most 65536 bytes.  The bytes out depend only on the bytes in.  write_eof != 0 appends the
+ *    28-byte EOF marker.  Not byte-identical to zlib or Go's compress/flate; any inflater decodes the same bytes.
+ *  - Calls compose.  Every call ends its own last block: the outputs of consecutive ranges, concatenated with write_eof on the last call
+ *    only, are a valid BGZF file that inflates to the same bytes as one call over the whole range (the block layouts differ).  Several
+ *    ranks' outputs, concatenated in contig-group order, make one file the same way.
+ *  - Refusals, with nothing written to out: those of elp_fetch_bam with its codes (ELP_ESTATE before elp_sort_markdup, for reads that did
+ *    not all come in as BAM, SAM or BGZF, after elp_clean_sam rewrote a CIGAR; ELP_EINVAL for a range past elp_n_output), and ELP_EINVAL
+ *    when capacity < elp_bgzf_deflate_bound(elp_fetch_bam_bytes(ctx, first, n) + n_prefix).
+ *  - elp_debug_deflate: host bytes in, the same kernels, BGZF out (capacity >= elp_bgzf_deflate_bound(n)); the counterpart of
+ *    elp_debug_inflate, for tests and the micro-benchmark. ---- */
+int elp_fetch_bgzf(elp_ctx *ctx, uint64_t first, uint64_t n, const uint8_t *prefix, uint64_t n_prefix, int write_eof,
+                   uint8_t *out, uint64_t capacity, uint64_t *out_n);
+int elp_debug_deflate(elp_ctx *ctx, const uint8_t *data, uint64_t n, int write_eof,
+                      uint8_t *out, uint64_t capacity, uint64_t *out_n);
+
 /* ---- measurement ---- */
 uint64_t elp_launch_count(const elp_ctx *ctx);           /* kernels launched by this library since create/reset */
 int elp_kernel_stats(elp_ctx *ctx, elp_kernel_stat *out, int cap); /* returns number of entries; profile must be on */

@@ -139,6 +139,16 @@ class DeviceSam {
     // AppendBgzfEnd after the last bytes.  RunPipeline's alignments then come from elp_fetch_bam / elp_fetch_sam, not from AddNodes.
     void AppendBgzf(const uint8_t* data, size_t n) { check(elp_append_bgzf(ctx_, data, n)); }
     void AppendBgzfEnd() { check(elp_append_bgzf_end(ctx_)); }
+    // the write side: output records [first, first+n) of elp_fetch_bam behind prefix (the BAM header on a file's first call), as BGZF blocks
+    // deflated on the device (elp_fetch_bgzf), with the EOF marker when eof; the bytes go to the file as they are
+    std::vector<uint8_t> FetchBgzf(uint64_t first, uint64_t n, const std::vector<uint8_t>& prefix = {}, bool eof = true) {
+        const uint64_t records = n ? elp_fetch_bam_bytes(ctx_, first, n) : 0;   // (0 on a refusal, which elp_fetch_bgzf then reports)
+        std::vector<uint8_t> out(elp_bgzf_deflate_bound(records + prefix.size()));
+        uint64_t got = 0;
+        check(elp_fetch_bgzf(ctx_, first, n, prefix.empty() ? nullptr : prefix.data(), prefix.size(), eof ? 1 : 0, out.data(), out.size(), &got));
+        out.resize(got);
+        return out;
+    }
     // the Finalize of AddNodes: By(CoordinateLess / QNAMELess).ParallelStableSort + filters.MarkDuplicates (+ MarkOpticalDuplicates)
     void Finalize(SortingOrder order) { check(elp_sort_markdup(ctx_, (int)order, opts_.MarkDuplicates ? (opts_.AlsoOpticals ? ELP_MARKDUP_OPTICAL : ELP_MARKDUP) : 0)); }
 
