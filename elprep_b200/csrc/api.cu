@@ -196,7 +196,7 @@ void elp_destroy(elp_ctx* c) {
     for (auto p : c->d_refhot_raw) if (p) cudaFree(p);
     region_release(c->regions); region_release(c->bqsr_regions); region_release(c->known_sites);
     void* singles[] = {c->d_rg_lib, c->d_rg_cov, c->d_contig_len, c->d_ranges, c->d_err, (void*)c->d_refhot_ptrs, c->d_bq_small, c->d_qpresent, c->d_ref_len, c->d_tables,
-                       c->d_lut, c->d_clut, c->d_rowtab, c->d_cov_exists, c->d_unobs,c->d_opt_ctr, c->d_opt_hist, c->d_opt_ovf, c->d_opt_small, c->d_rg_names, c->d_rg_name_off, c->d_out_drop, c->ws.ghist, c->ws.gofs, c->ws.counters, c->ws.status};
+                       c->d_lut, c->d_clut, c->d_rowtab, c->d_cov_exists, c->d_unobs, c->d_emp, c->d_fin, c->d_qmaps, c->d_opt_ctr, c->d_opt_hist, c->d_opt_ovf, c->d_opt_small, c->d_rg_names, c->d_rg_name_off, c->d_out_drop, c->ws.ghist, c->ws.gofs, c->ws.counters, c->ws.status};
     for (void* p : singles) if (p) cudaFree(p);
     c->refid.release(); c->pos.release(); c->nref.release(); c->pnext.release(); c->tlen.release(); c->rg.release(); c->flag.release(); c->mapq.release(); c->optf.release(); c->s_optf.release();
     c->qname_off.release(); c->cigar_off.release(); c->qual_off.release(); c->seq_off.release(); c->qname.release(); c->seq.release(); c->qual.release(); c->cigar.release();
@@ -420,8 +420,8 @@ int elp_bqsr_empirical_get(elp_ctx* c, uint8_t* emp, uint64_t n) {
     if (!c || !emp) return ELP_EINVAL;
     if (!c->finalized) return c->fail(E_STATE, "elp_bqsr_empirical_get before elp_bqsr_finalize");
     if (n != c->geom.cells()) return c->fail(E_INVAL, "elp_bqsr_empirical_get: expected %zu values", c->geom.cells());
-    std::copy(c->h_emp.begin(), c->h_emp.end(), emp);
-    return ELP_OK;
+    cudaSetDevice(c->device);
+    return bqsr_empirical_copy(c, emp);
 }
 
 uint64_t elp_fetch_qual_bytes(elp_ctx* c, uint64_t first, uint64_t n) {

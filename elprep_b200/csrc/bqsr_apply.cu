@@ -390,13 +390,9 @@ int run_apply_kernel(elp_ctx* c, bool with_lut) {
     // until this call succeeds the output stream may hold a mix of recalibrated and original bytes: a fetch after a failed apply
     // materialises the original QUAL again instead of returning it
     c->qual_out_valid = false;
-    uint64_t total = 0;
-    if (n) {
-        CUDA_TRY(c, cudaMemcpyAsync(&total, c->s_out_off.p + n, 8, cudaMemcpyDeviceToHost, c->stream));
-        CUDA_TRY(c, cudaStreamSynchronize(c->stream));
-    }
-    CUDA_TRY(c, c->qual_out.reserve(total + 64, c->stream));
-    c->qual_out_total = total;
+    // the output stream holds the QUAL bytes of a subset of the stored reads, so the QUAL arena bounds it: no read-back before the launch
+    CUDA_TRY(c, c->qual_out.reserve(c->n_qual + 64, c->stream));
+    c->qual_out_total = 0;
     if (n) {
         static bool tables_set[64] = {false};
         if (!tables_set[c->device & 63]) {
@@ -429,6 +425,7 @@ int run_apply_kernel(elp_ctx* c, bool with_lut) {
             c->begin(with_lut ? "bqsr_apply" : "qual_materialize", bytes);
             bqsr_apply2_kernel<<<grid, AP2_WARPS * 32, smem, c->stream>>>(B);
             c->end(); LAUNCH_CHECK(c);
+            CUDA_TRY(c, cudaMemcpyAsync(&c->qual_out_total, c->s_out_off.p + n, 8, cudaMemcpyDeviceToHost, c->stream));   // lands at the sync below
             int rc2 = check_device_errors(c);
             if (rc2) return rc2;
             c->qual_out_valid = true;
@@ -438,6 +435,8 @@ int run_apply_kernel(elp_ctx* c, bool with_lut) {
             c->begin("qual_materialize", 2.0 * (double)c->n_qual * ((double)n / (double)c->n) + (double)n * 20);
             qual_copy_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, c->stream>>>(n, c->s_lseq.p, c->s_qual_off.p, c->s_out_off.p, c->qual.p, c->qual_out.p);
             c->end(); LAUNCH_CHECK(c);
+            CUDA_TRY(c, cudaMemcpyAsync(&c->qual_out_total, c->s_out_off.p + n, 8, cudaMemcpyDeviceToHost, c->stream));
+            CUDA_TRY(c, cudaStreamSynchronize(c->stream));
             c->qual_out_valid = true;
             return E_OK;
         }
@@ -452,6 +451,7 @@ int run_apply_kernel(elp_ctx* c, bool with_lut) {
         c->begin(with_lut ? "bqsr_apply_gmem" : "qual_materialize", bytes);
         bqsr_apply_kernel<<<(unsigned)((n + reads_per_block - 1) / reads_per_block), WARPS * 32, 0, c->stream>>>(A);
         c->end(); LAUNCH_CHECK(c);
+        CUDA_TRY(c, cudaMemcpyAsync(&c->qual_out_total, c->s_out_off.p + n, 8, cudaMemcpyDeviceToHost, c->stream));   // lands at the sync below
     }
     int rc = check_device_errors(c);
     if (rc) return rc;

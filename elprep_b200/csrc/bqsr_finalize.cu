@@ -1,73 +1,89 @@
-// bqsr_finalize.cu -- host side of BQSR between gather and apply (replaces FinalizeBQSRTables, filters/bqsr.go:677-694,
+// bqsr_finalize.cu -- BQSR between gather and apply (replaces FinalizeBQSRTables, filters/bqsr.go:677-694,
 // initializeCombinedBQSRTable :655-674, the quantizers :708-899, estimateHierarchicalBayesianQuality :901-919 as memoised
 // by ApplyBQSR :973-1000, and PrintBQSRTables, filters/print-bqsr.go:49-298).
 //
-// The tables are tiny (<= a few 10^5 integer cells), the arithmetic is IEEE double with Go's math functions
-// (gomath.hpp) and must be evaluated in the reference's operation order, so this runs on the host between two kernels.
-// Everything the apply kernel needs is folded into ONE byte look-up table indexed by
-// (read-group covariate, reported qual, cycle, context) -- exactly the memo the reference fills lazily per worker.
+// The arithmetic is IEEE double with Go's math functions (gomath.hpp) in the reference's operation order.  It runs on the
+// device, on the context's stream, with no host synchronisation between gather and apply:
+//   fin_emp       EmpiricalQuality of every table cell, one thread per cell
+//   fin_tail      one CTA: the combined per-read-group entries, the quantization map, the "unobserved QUAL" byte per covariate
+//   fin_lut       one CTA per (covariate, QUAL) row: the apply look-up table indexed by (read-group covariate, reported qual,
+//                 cycle, context) -- exactly the memo the reference fills lazily per worker
+//   fin_clut      the compact table of bqsr_apply2_kernel, copied out of the full one
+// This file is compiled with -fmad=false (csrc/Makefile): a fused multiply-add would round differently from the host and from Go.
+// The recalibration report stays host code, fed by one copy of the tables and of EmpiricalQuality made only when a report is asked for.
 // Reference non-determinism fixed here: the combined per-read-group entry accumulates in ascending-qual order
 // (the reference iterates a Go map, :657-668).
 #include <algorithm>
 #include <cfloat>
 #include <cstdio>
+#include <mutex>
 #include <string>
-#include <thread>
 #include <vector>
 #include "ctx.h"
 #include "gomath.hpp"
 
 namespace {
 
-const double kPriorCache[21] = {   // embedded data, filters/bqsr.go:569-591: log10(0.9*exp(-d^2/0.5)), last = -MaxFloat64
-    -0.045757490560675115, -0.9143464543671788, -3.5201133457866898, -7.863058164819208, -13.943180911464733, -21.760481585723266,
-    -31.314960187594806, -42.606616717079355, -55.63545117417691, -70.40146355888747, -86.90465387121104, -105.14502211114761,
-    -125.1225682786972, -146.83729237385978, -170.2891943966354, -195.47827434702398, -222.4045322250256, -251.06796803064023,
-    -281.46858176386786, -313.60637342472336, -1.7976931348623157e308};
+#define PRIOR_CACHE {   /* embedded data, filters/bqsr.go:569-591: log10(0.9*exp(-d^2/0.5)), last = -MaxFloat64 */ \
+    -0.045757490560675115, -0.9143464543671788, -3.5201133457866898, -7.863058164819208, -13.943180911464733, -21.760481585723266, \
+    -31.314960187594806, -42.606616717079355, -55.63545117417691, -70.40146355888747, -86.90465387121104, -105.14502211114761, \
+    -125.1225682786972, -146.83729237385978, -170.2891943966354, -195.47827434702398, -222.4045322250256, -251.06796803064023, \
+    -281.46858176386786, -313.60637342472336, -1.7976931348623157e308}
+#ifndef __CUDA_ARCH__
+const double kPriorCache[21] = PRIOR_CACHE;
+#endif
+__constant__ double c_prior[21] = PRIOR_CACHE;
 
-struct BinTerms {   // per-bin constants of log10BinomialProbability (:607-613): l = i/-10, m = log10(1 - 10^l)
-    double l[61], m[61];
-    BinTerms() { for (int i = 0; i < 61; i++) { l[i] = (double)i / -10.0; m[i] = (l[i] == 0.0) ? 0.0 : gomath::Log10(1.0 - gomath::Pow(10, l[i])); } }
-};
-const BinTerms& bin_terms() { static BinTerms b; return b; }
+struct BinTerms { double l[61], m[61]; };   // per-bin constants of log10BinomialProbability (:607-613): l = i/-10, m = log10(1 - 10^l)
+BinTerms make_bin_terms() {
+    BinTerms b;
+    for (int i = 0; i < 61; i++) { b.l[i] = (double)i / -10.0; b.m[i] = (b.l[i] == 0.0) ? 0.0 : gomath::Log10(1.0 - gomath::Pow(10, b.l[i])); }
+    return b;
+}
+const BinTerms& bin_terms() { static const BinTerms b = make_bin_terms(); return b; }
+__constant__ BinTerms c_bin;   // the host's BinTerms, copied once per device (ensure_fin_state): the same bits by construction
 
-inline double log10_gamma(int64_t n) { return gomath::Lgamma((double)n) * 0.4342944819032518; }   // :598-601
+GM_HD inline double log10_gamma(int64_t n) { return gomath::Lgamma((double)n) * 0.4342944819032518; }   // :598-601
 
 // calculateEmpiricalQuality (:644-649) = calculateBayesianEstimateOfEmpiricalQuality (:623-642) on the smoothed counts
 struct Entry {
     int64_t n, k; double coef;
-    Entry(int64_t obs, int64_t mis) {
+    GM_HD Entry(int64_t obs, int64_t mis) {
         n = obs + 2; k = mis + 1;
         const int64_t maxObs = 2147483647 - 1;
         if (n > maxObs) { k = (int64_t)gomath::Round((double)k * ((double)maxObs / (double)n)); n = maxObs; }
         coef = log10_gamma(n + 1) - log10_gamma(k + 1) - log10_gamma(n - k + 1);   // log10BinomialCoefficient :603-605
     }
-    uint8_t empirical(double prior) const {
-        const BinTerms& B = bin_terms();
+    GM_HD uint8_t empirical(double prior) const {
+#ifdef __CUDA_ARCH__
+        const BinTerms& B = c_bin; const double* P = c_prior;
+#else
+        const BinTerms& B = bin_terms(); const double* P = kPriorCache;
+#endif
         double best = -DBL_MAX; int bi = 0;
         for (int i = 0; i < 61; i++) {
             int d = (int)((double)i - prior); if (d < 0) d = -d; if (d > 20) d = 20;   // log10QualEmpiricalPrior :593-596
-            const double p1 = kPriorCache[d];
+            const double p1 = P[d];
             const double p2 = (B.l[i] == 0.0) ? -DBL_MAX : (coef + B.l[i] * (double)k) + B.m[i] * (double)(n - k);   // n is never 0 here (obs+2)
             const double post = p1 + p2;
             if (best < post) { best = post; bi = i; }
         }
-        return (uint8_t)std::min(bi, 93);
+        return (uint8_t)(bi < 93 ? bi : 93);
     }
 };
 
-inline double q2err(double phred) { return gomath::Pow(10, phred / -10); }
-inline double q2prob(double phred) { return 1 - gomath::Pow(10, phred / -10); }
+GM_HD inline double q2err(double phred) { return gomath::Pow(10, phred / -10); }
+GM_HD inline double q2prob(double phred) { return 1 - gomath::Pow(10, phred / -10); }
 
 struct Combined { bool exists = false; double reported = 0; int64_t obs = 0, mis = 0; uint8_t emp = 0; };
 
-struct Tables {
-    const TableGeom& g; const int64_t* t;
-    int64_t obs(int cov, int q, int col) const { return t[2 * g.idx(cov, q, col)]; }
-    int64_t mis(int cov, int q, int col) const { return t[2 * g.idx(cov, q, col) + 1]; }
+struct Tables {   // the dense tables, in host memory (report) or device memory (kernels)
+    TableGeom g; const int64_t* t;
+    GM_HD int64_t obs(int cov, int q, int col) const { return t[2 * g.idx(cov, q, col)]; }
+    GM_HD int64_t mis(int cov, int q, int col) const { return t[2 * g.idx(cov, q, col) + 1]; }
 };
 
-Combined combine(const Tables& T, int cov) {   // :655-674
+GM_HD Combined combine(const Tables& T, int cov) {   // :655-674
     Combined c;
     for (int q = 0; q < 94; q++) {
         const int64_t eo = T.obs(cov, q, 0), em = T.mis(cov, q, 0);
@@ -82,10 +98,10 @@ Combined combine(const Tables& T, int cov) {   // :655-674
     return c;
 }
 
-int err_prob_to_quality(double prob) {   // :701-706
+GM_HD int err_prob_to_quality(double prob) {   // :701-706
     if (prob == 0.0) return 93;
     int q = (int)gomath::Round(-10 * gomath::Log10(prob));
-    return std::max(std::min(q, 93), 1);
+    return q > 93 ? 93 : (q < 1 ? 1 : q);
 }
 
 std::vector<uint8_t> static_quantized(std::vector<uint8_t> quals) {   // initializeStaticQuantizedScores :710-743
@@ -106,10 +122,10 @@ std::vector<uint8_t> static_quantized(std::vector<uint8_t> quals) {   // initial
 }
 
 struct QInterval { int next; double errorRate; int64_t nobs, leafNobs, nerrors; };
-double calc_error_rate(int64_t nobs, int64_t nerr) { return nobs == 0 ? 0.0 : (double)(nerr + 1) / (double)(nobs + 1); }
+GM_HD double calc_error_rate(int64_t nobs, int64_t nerr) { return nobs == 0 ? 0.0 : (double)(nerr + 1) / (double)(nobs + 1); }
 double leaf_penalty(int k, const std::vector<QInterval>& iv, double globalErrorRate) {   // :780-786
     if (k <= 6) return 0.0;
-    return std::fabs(gomath::Log10(iv[k].errorRate) - gomath::Log10(globalErrorRate)) * (double)iv[k].leafNobs;
+    return gomath::Fabs(gomath::Log10(iv[k].errorRate) - gomath::Log10(globalErrorRate)) * (double)iv[k].leafNobs;
 }
 double merge_penalty(int i, int j, const std::vector<QInterval>& iv) {   // :795-818
     const int64_t mn = iv[i].nobs + iv[j].nobs, me = iv[i].nerrors + iv[j].nerrors;
@@ -225,40 +241,217 @@ int write_report(elp_ctx* c, const Tables& T, const std::vector<uint8_t>& emp, c
     return E_OK;
 }
 
-// run f(i) for i in [0,n) on a few host threads (the per-entry posteriors are independent)
-template <class F> void host_parallel_for(int n, F f) {
-    const int nt = std::max(1, std::min<int>({8, (int)std::thread::hardware_concurrency(), n}));
-    if (nt == 1) { for (int i = 0; i < n; i++) f(i); return; }
-    std::vector<std::thread> th;
-    for (int t = 0; t < nt; t++) th.emplace_back([=]() { for (int i = t; i < n; i += nt) f(i); });
-    for (auto& x : th) x.join();
+
+// ---- device finalize ----
+constexpr int FIN_T = 128;   // threads of the one-CTA tail kernel and of a LUT row; the tail's quantizer needs >= 94
+
+// recalibrated byte of an estimate (ApplyBQSR :996-1000): quant[clamp(round(est))], then the static map when --sqq is set.
+// qmaps: [0, 94) the quantization map, [QMAP_STAT, QMAP_STAT + 254) the static one
+constexpr int QMAP_STAT = 96, QMAP_BYTES = QMAP_STAT + 256;
+__device__ __forceinline__ uint8_t final_q(double est, const uint8_t* qmaps, int have_stat) {
+    int r = (int)gomath::Round(est); r = max(1, min(r, 93));
+    uint8_t nq = qmaps[r];
+    if (have_stat) nq = qmaps[QMAP_STAT + nq];
+    return nq;
+}
+
+// FinalizeBQSRTables: EmpiricalQuality of every existing entry with prior = its reported qual (:677-694); 0 where there is none
+__global__ void fin_emp_kernel(const int64_t* __restrict__ t, TableGeom g, uint8_t* __restrict__ emp) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= g.cells()) return;
+    const int64_t o = t[2 * i];
+    emp[i] = o > 0 ? Entry(o, t[2 * i + 1]).empirical((double)(int)((i / (size_t)g.ncols()) % 94)) : 0;
+}
+
+// mergeQuantizationIntervals' penalty of merging interval i with the next one, j (:795-818), over the leaves' constants in shared memory
+__device__ double fin_merge_penalty(int i, int j, const int* nxt, const long long* nobs, const long long* nerr, const long long* leafn, const double* leaflog) {
+    const double mer = calc_error_rate(nobs[i] + nobs[j], nerr[i] + nerr[j]);
+    if (mer == 0) return 0.0;
+    const double lg = gomath::Log10(mer);
+    double sumI = 0, sumJ = 0;
+    for (int k = i; k < j; k++) sumI += k <= 6 ? 0.0 : gomath::Fabs(leaflog[k] - lg) * (double)leafn[k];   // leaf_penalty :780-786
+    const int kend = nxt[j] >= 0 ? nxt[j] : 94;
+    for (int k = j; k < kend; k++) sumJ += k <= 6 ? 0.0 : gomath::Fabs(leaflog[k] - lg) * (double)leafn[k];
+    return sumI + sumJ;
+}
+
+// one CTA: the combined per-read-group entries (:655-674) -> fin[2 cov] = reported quality, fin[2 cov + 1] = its EmpiricalQuality minus
+// it (the read-group term dG of :959-964); the quantization map (:863-899) -> qmaps[0, 94); the byte of a QUAL without table entries
+__global__ void __launch_bounds__(FIN_T) fin_tail_kernel(const int64_t* __restrict__ t, TableGeom g, const uint8_t* __restrict__ emp, int levels, int have_stat,
+                                                         double* __restrict__ fin, uint8_t* __restrict__ qmaps, uint8_t* __restrict__ cov_exists, uint8_t* __restrict__ unobs) {
+    const Tables T{g, t};
+    const int tid = threadIdx.x;
+    for (int cv = tid; cv < g.n_cov; cv += FIN_T) {   // one covariate per thread
+        const Combined cb = combine(T, cv);
+        fin[2 * cv] = cb.reported;
+        fin[2 * cv + 1] = cb.exists ? (double)cb.emp - cb.reported : 0.0;
+        cov_exists[cv] = cb.exists ? 1 : 0;
+    }
+    __shared__ uint8_t quant[94];
+    if (levels == 0) {
+        for (int i = tid; i < 94; i += FIN_T) quant[i] = (uint8_t)i;
+    } else {
+        __shared__ long long qmap[94], nobs[94], nerr[94];
+        __shared__ double leaflog[94];
+        __shared__ int nxt[94];
+        __shared__ bool head[94];
+        __shared__ double wp[FIN_T / 32]; __shared__ int wi[FIN_T / 32];
+        __shared__ int s_min;
+        for (int i = tid; i < 94; i += FIN_T) qmap[i] = 0;
+        __syncthreads();
+        for (int j = tid; j < g.n_cov * 94; j += FIN_T) {
+            const int cv = j / 94, q = j % 94;
+            const int64_t o = T.obs(cv, q, 0);
+            if (o > 0) atomicAdd(reinterpret_cast<unsigned long long*>(&qmap[emp[g.idx(cv, q, 0)]]), (unsigned long long)o);   // integer: order free
+        }
+        __syncthreads();
+        for (int i = tid; i < 94; i += FIN_T) {
+            const double er = q2err((double)i);
+            nxt[i] = i + 1 == 94 ? -1 : i + 1; nobs[i] = qmap[i]; nerr[i] = (long long)((double)qmap[i] * er); leaflog[i] = gomath::Log10(er); head[i] = true;
+        }
+        __syncthreads();
+        // mergeMinimalPenaltyQuantizationIntervals (:820-850): every pair of neighbouring intervals is priced at once; the minimum with the
+        // lowest start wins, as the serial scan's strict '<' keeps the first
+        for (int n = 94; n > levels; n--) {
+            bool valid = tid < 94 && head[tid] && nxt[tid] >= 0;
+            double p = valid ? fin_merge_penalty(tid, nxt[tid], nxt, nobs, nerr, qmap, leaflog) : 0.0;
+            int idx = valid ? tid : 0x7fffffff;
+            for (int o = 16; o; o >>= 1) {
+                const double p2 = __shfl_down_sync(0xffffffffu, p, o); const int i2 = __shfl_down_sync(0xffffffffu, idx, o);
+                const bool v2 = i2 != 0x7fffffff;
+                if (v2 && (idx == 0x7fffffff || p2 < p || (p2 == p && i2 < idx))) { p = p2; idx = i2; }
+            }
+            if ((tid & 31) == 0) { wp[tid >> 5] = p; wi[tid >> 5] = idx; }
+            __syncthreads();
+            if (tid == 0) {
+                double bp = wp[0]; int bi = wi[0];
+                for (int w = 1; w < FIN_T / 32; w++)
+                    if (wi[w] != 0x7fffffff && (bi == 0x7fffffff || wp[w] < bp || (wp[w] == bp && wi[w] < bi))) { bp = wp[w]; bi = wi[w]; }
+                if (bi != 0x7fffffff) { const int b = nxt[bi]; nxt[bi] = nxt[b]; nobs[bi] += nobs[b]; nerr[bi] += nerr[b]; head[b] = false; }
+                s_min = bi;
+            }
+            __syncthreads();
+            if (s_min == 0x7fffffff) break;   // a single interval is left
+        }
+        if (tid == 0)
+            for (int i = 0; i >= 0;) {
+                const bool leaf = nxt[i] < 0 ? (i == 93) : (nxt[i] == i + 1);
+                const uint8_t qs = leaf ? (uint8_t)i : (uint8_t)err_prob_to_quality(calc_error_rate(nobs[i], nerr[i]));
+                const int kend = nxt[i] >= 0 ? nxt[i] : 94;
+                for (int k = i; k < kend; k++) quant[k] = qs;
+                i = nxt[i];
+            }
+    }
+    __syncthreads();
+    for (int i = tid; i < 94; i += FIN_T) qmaps[i] = quant[i];
+    __syncthreads();
+    // a QUAL value without any table entry (never observed, or above 93): only the read-group term (:901-919 with three map misses)
+    for (int cv = tid; cv < g.n_cov; cv += FIN_T) unobs[cv] = cov_exists[cv] ? final_q(0.0 + fin[2 * cv + 1] + fin[2 * cv], qmaps, have_stat) : 0;
+}
+
+// the apply look-up table (ApplyBQSR :936-1006): recalibrated QUAL for (covariate, QUAL, cycle in [-Lc, Lc], context), one CTA per
+// (covariate, QUAL) row of (2 Lc + 1) x 17 bytes; QUAL 0..5 and covariates without entries stay 0
+__global__ void __launch_bounds__(FIN_T) fin_lut_kernel(const int64_t* __restrict__ t, TableGeom g, const double* __restrict__ fin, const uint8_t* __restrict__ qmaps, int have_stat,
+                                                        const uint8_t* __restrict__ cov_exists, int Lc, uint8_t* __restrict__ lut) {
+    const Tables T{g, t};
+    const int cv = blockIdx.x / 94, q = blockIdx.x % 94, ncyc = 2 * Lc + 1, tid = threadIdx.x;
+    uint8_t* row = lut + ((size_t)cv * 94 + q) * ncyc * 17;
+    const int row_bytes = ncyc * 17;
+    if (q < 6 || !cov_exists[cv]) { for (int i = tid; i < row_bytes; i += FIN_T) row[i] = 0; return; }
+    // globalQualityScorePrior = -1 -> epsilon is always the read group's reportedQuality (:959-964)
+    const double eps = fin[2 * cv], dG = fin[2 * cv + 1];
+    const int64_t o0 = T.obs(cv, q, 0);
+    double dQ = 0;
+    if (o0 > 0) dQ = (double)Entry(o0, T.mis(cv, q, 0)).empirical(dG + eps) - dG - eps;
+    const double cp = dQ + dG + eps;
+    if (o0 <= 0) {   // QUAL never observed: no cycle/context entries either
+        const uint8_t b = final_q(cp + 0.0, qmaps, have_stat);
+        for (int i = tid; i < row_bytes; i += FIN_T) row[i] = b;
+        return;
+    }
+    __shared__ double dctx[17]; __shared__ bool hctx[17];
+    if (tid < 16) { const int col = g.col_ctx(tid); hctx[tid] = T.obs(cv, q, col) > 0; dctx[tid] = hctx[tid] ? (double)Entry(T.obs(cv, q, col), T.mis(cv, q, col)).empirical(cp) - cp : 0.0; }
+    if (tid == 16) { hctx[16] = false; dctx[16] = 0; }
+    __syncthreads();
+    for (int cy = -Lc + tid; cy <= Lc; cy += FIN_T) {
+        const int col = g.col_cycle(cy);
+        const bool hc = T.obs(cv, q, col) > 0;
+        const double dcy = hc ? (double)Entry(T.obs(cv, q, col), T.mis(cv, q, col)).empirical(cp) - cp : 0.0;
+        uint8_t* dst = row + (size_t)(cy + Lc) * 17;
+        for (int x = 0; x < 17; x++) {
+            double dC = 0;
+            if (hc) dC = dcy;
+            if (hctx[x]) dC += dctx[x];
+            dst[x] = final_q(cp + dC, qmaps, have_stat);
+        }
+    }
+}
+
+struct ClutArgs {
+    const uint8_t* lut; const uint8_t* unobs; uint8_t* clut; uint16_t* rowtab;
+    uint32_t bytes, blk, used; int Lc, S, n_slots;
+    uint8_t slot_q[88]; uint16_t rowtab_h[256];
+};
+// the compact table of bqsr_apply2_kernel (see build_compact_lut), one thread per byte
+__global__ void fin_clut_kernel(ClutArgs A) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < 256) A.rowtab[i] = A.rowtab_h[i];
+    if (i >= A.bytes) return;
+    const uint32_t ncyc = 2u * (uint32_t)A.Lc + 1u, cyb = i / A.blk, off = i % A.blk, S17 = (uint32_t)A.S * 17u;
+    uint8_t v = 0;
+    if (cyb >= 32 && cyb < 32 + ncyc && off < A.used) {
+        const uint32_t cy = cyb - 32, cv = off / S17, r = off % S17, sl = r / 17, x = r % 17;
+        v = (int)sl < A.n_slots ? A.lut[(((size_t)cv * 94 + A.slot_q[sl]) * ncyc + cy) * 17 + x] : A.unobs[cv];
+    }
+    A.clut[i] = v;
+}
+
+// BinTerms into constant memory, once per device; the device buffers of the finalize, once per context
+int ensure_fin_state(elp_ctx* c) {
+    static std::mutex mu; static bool bin_set[64] = {false};
+    {
+        std::lock_guard<std::mutex> lk(mu);
+        if (!bin_set[c->device & 63]) { CUDA_TRY(c, cudaMemcpyToSymbol(c_bin, &bin_terms(), sizeof(BinTerms))); bin_set[c->device & 63] = true; }
+    }
+    const int nc = std::max(1, c->geom.n_cov);
+    if (!c->d_emp) CUDA_TRY(c, cudaMalloc(&c->d_emp, std::max<size_t>(1, c->geom.cells())));
+    if (!c->d_fin) CUDA_TRY(c, cudaMalloc(&c->d_fin, 2 * sizeof(double) * nc));
+    if (!c->d_cov_exists) CUDA_TRY(c, cudaMalloc(&c->d_cov_exists, nc));
+    if (!c->d_unobs) CUDA_TRY(c, cudaMalloc(&c->d_unobs, nc));
+    if (!c->d_qmaps) {   // the static quantization (initializeStaticQuantizedScores) depends on --sqq only
+        CUDA_TRY(c, cudaMalloc(&c->d_qmaps, QMAP_BYTES));
+        std::vector<uint8_t> m(QMAP_BYTES, 0);
+        if (!c->sqq.empty()) { const std::vector<uint8_t> ss = static_quantized(c->sqq); std::copy(ss.begin(), ss.end(), m.begin() + QMAP_STAT); }
+        int rc = upload_small(c, c->d_qmaps, m.data(), m.size()); if (rc) return rc;
+    }
+    return E_OK;
 }
 
 }  // namespace
-
-int build_apply_lut(elp_ctx* c, int Lc);
 
 int phase_bqsr_finalize(elp_ctx* c, const char* report_path) {
     if (!c->gathered) return c->fail(E_STATE, "elp_bqsr_finalize called before elp_bqsr_gather / elp_bqsr_tables_put");
     const TableGeom& g = c->geom;
     const size_t cells = g.cells();
-    c->h_tables.resize(cells * 2);
-    CUDA_TRY(c, cudaMemcpyAsync(c->h_tables.data(), c->d_tables, cells * 2 * sizeof(int64_t), cudaMemcpyDeviceToHost, c->stream));
-    CUDA_TRY(c, cudaStreamSynchronize(c->stream));
-    Tables T{g, c->h_tables.data()};
-    // FinalizeBQSRTables: EmpiricalQuality of every existing entry with prior = its reported qual (:677-694)
-    c->h_emp.assign(cells, 0);
-    host_parallel_for(g.n_cov * 94, [&](int row) {
-        const int cv = row / 94, q = row % 94;
-        for (int col = 0; col < g.ncols(); col++) {
-            const int64_t o = T.obs(cv, q, col);
-            if (o > 0) c->h_emp[g.idx(cv, q, col)] = Entry(o, T.mis(cv, q, col)).empirical((double)q);
-        }
-    });
-    std::vector<Combined> comb(g.n_cov);
-    for (int cv = 0; cv < g.n_cov; cv++) comb[cv] = combine(T, cv);
-    if (report_path) { int rc = write_report(c, T, c->h_emp, comb, report_path); if (rc) return rc; }
-
+    { int rc = ensure_fin_state(c); if (rc) return rc; }
+    if (cells) {
+        c->begin("bqsr_fin_emp", (double)cells * 17);
+        fin_emp_kernel<<<(unsigned)((cells + 255) / 256), 256, 0, c->stream>>>(c->d_tables, g, c->d_emp);
+        c->end(); LAUNCH_CHECK(c);
+    }
+    c->begin("bqsr_fin_tail", (double)g.n_cov * 94 * 16);
+    fin_tail_kernel<<<1, FIN_T, 0, c->stream>>>(c->d_tables, g, c->d_emp, c->quantize_levels, c->sqq.empty() ? 0 : 1, c->d_fin, c->d_qmaps, c->d_cov_exists, c->d_unobs);
+    c->end(); LAUNCH_CHECK(c);
+    if (report_path) {   // the report is host text: one copy of the tables and of EmpiricalQuality
+        std::vector<int64_t> h_tables(cells * 2); std::vector<uint8_t> h_emp(cells);
+        CUDA_TRY(c, cudaMemcpyAsync(h_tables.data(), c->d_tables, cells * 2 * sizeof(int64_t), cudaMemcpyDeviceToHost, c->stream));
+        CUDA_TRY(c, cudaMemcpyAsync(h_emp.data(), c->d_emp, cells, cudaMemcpyDeviceToHost, c->stream));
+        CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+        Tables T{g, h_tables.data()};
+        std::vector<Combined> comb(g.n_cov);
+        for (int cv = 0; cv < g.n_cov; cv++) comb[cv] = combine(T, cv);
+        int rc = write_report(c, T, h_emp, comb, report_path); if (rc) return rc;
+    }
     c->finalized = true;
     // the apply look-up table covers the cycles of the reads loaded so far; elp_bqsr_apply rebuilds it if longer reads arrive
     // later (apply-only workers: tables_put -> finalize -> append -> sort -> apply)
@@ -266,69 +459,21 @@ int phase_bqsr_finalize(elp_ctx* c, const char* report_path) {
     return build_apply_lut(c, std::max(1, std::min(c->max_cycle, std::max(c->h_ranges.lseq_max, 1))));
 }
 
-// ---- the apply look-up table (ApplyBQSR :936-1006): recalibrated QUAL for (covariate, QUAL, cycle in [-Lc, Lc], context) ----
 int build_apply_lut(elp_ctx* c, int Lc) {
     if (!c->finalized) return c->fail(E_STATE, "apply look-up table requested before elp_bqsr_finalize");
     const TableGeom& g = c->geom;
-    Tables T{g, c->h_tables.data()};
-    std::vector<Combined> comb(g.n_cov);
-    for (int cv = 0; cv < g.n_cov; cv++) comb[cv] = combine(T, cv);
-    std::vector<int64_t> qmap; std::vector<uint8_t> quant;
-    quantized(T, c->h_emp, c->quantize_levels, qmap, quant);
-    std::vector<uint8_t> stat; const bool have_stat = !c->sqq.empty();
-    if (have_stat) stat = static_quantized(c->sqq);
-    const int ncyc = 2 * Lc + 1;
-    std::vector<uint8_t> lut((size_t)g.n_cov * 94 * ncyc * 17, 0);
-    std::vector<uint8_t> cov_exists(g.n_cov, 0), unobs(g.n_cov, 0);
-    std::vector<double> dGv(g.n_cov, 0.0);
-    auto final_q = [&](double est) { int r = (int)gomath::Round(est); r = std::max(1, std::min(r, 93)); uint8_t nq = quant[r]; if (have_stat) nq = stat[nq]; return nq; };
-    for (int cv = 0; cv < g.n_cov; cv++) {
-        if (!comb[cv].exists) continue;
-        cov_exists[cv] = 1;
-        // globalQualityScorePrior = -1 -> epsilon is always the read group's reportedQuality (:959-964)
-        dGv[cv] = (double)Entry(comb[cv].obs, comb[cv].mis).empirical(comb[cv].reported) - comb[cv].reported;
-        // a QUAL value without any table entry (never observed, or above 93): only the read-group term (:901-919 with three map misses)
-        unobs[cv] = final_q(0.0 + dGv[cv] + comb[cv].reported);
-    }
-    host_parallel_for(g.n_cov * 88, [&](int job) {
-        const int cv = job / 88, q = 6 + job % 88;
-        if (!comb[cv].exists) return;
-        const double eps = comb[cv].reported, dG = dGv[cv];
-        double dQ = 0;
-        if (T.obs(cv, q, 0) > 0) dQ = (double)Entry(T.obs(cv, q, 0), T.mis(cv, q, 0)).empirical(dG + eps) - dG - eps;
-        const double cp = dQ + dG + eps;
-        uint8_t* row = &lut[((size_t)cv * 94 + q) * ncyc * 17];
-        if (T.obs(cv, q, 0) <= 0) { std::memset(row, final_q(cp + 0.0), (size_t)ncyc * 17); return; }   // QUAL never observed: no cycle/context entries either
-        double dctx[17]; bool hctx[17];
-        for (int x = 0; x < 16; x++) { const int col = g.col_ctx(x); hctx[x] = T.obs(cv, q, col) > 0; dctx[x] = hctx[x] ? (double)Entry(T.obs(cv, q, col), T.mis(cv, q, col)).empirical(cp) - cp : 0.0; }
-        hctx[16] = false; dctx[16] = 0;
-        for (int cy = -Lc; cy <= Lc; cy++) {
-            const int col = g.col_cycle(cy);
-            const bool hc = T.obs(cv, q, col) > 0;
-            const double dcy = hc ? (double)Entry(T.obs(cv, q, col), T.mis(cv, q, col)).empirical(cp) - cp : 0.0;
-            uint8_t* dst = row + (size_t)(cy + Lc) * 17;
-            for (int x = 0; x < 17; x++) {
-                double dC = 0;
-                if (hc) dC = dcy;
-                if (hctx[x]) dC += dctx[x];
-                dst[x] = final_q(cp + dC);
-            }
-        }
-    });
-    if (c->lut_cap < lut.size() + 16) {
+    const size_t bytes = (size_t)g.n_cov * 94 * (2 * Lc + 1) * 17;
+    if (c->lut_cap < bytes + 16) {
         if (c->d_lut) { cudaFree(c->d_lut); c->d_lut = nullptr; }
-        CUDA_TRY(c, cudaMalloc(&c->d_lut, lut.size() + 16));
-        c->lut_cap = lut.size() + 16;
+        CUDA_TRY(c, cudaMalloc(&c->d_lut, bytes + 16));
+        c->lut_cap = bytes + 16;
     }
-    { int rcu = upload_small(c, c->d_lut, lut.data(), lut.size()); if (rcu) return rcu; }
-    if (!c->d_cov_exists) CUDA_TRY(c, cudaMalloc(&c->d_cov_exists, std::max(1, g.n_cov)));
-    { int rcu = upload_small(c, c->d_cov_exists, cov_exists.data(), g.n_cov); if (rcu) return rcu; }
-    if (!c->d_unobs) CUDA_TRY(c, cudaMalloc(&c->d_unobs, std::max(1, g.n_cov)));
-    { int rcu = upload_small(c, c->d_unobs, unobs.data(), g.n_cov); if (rcu) return rcu; }
-    c->h_unobs.swap(unobs);
-    CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+    if (g.n_cov) {
+        c->begin("bqsr_fin_lut", (double)bytes);
+        fin_lut_kernel<<<(unsigned)(g.n_cov * 94), FIN_T, 0, c->stream>>>(c->d_tables, g, c->d_fin, c->d_qmaps, c->sqq.empty() ? 0 : 1, c->d_cov_exists, Lc, c->d_lut);
+        c->end(); LAUNCH_CHECK(c);
+    }
     c->lut_maxcyc = Lc;
-    c->h_lut.swap(lut);            // kept for the compact shared-memory table (build_compact_lut)
     c->clut_Lc = 0;                // rebuilt on the next apply
     return E_OK;
 }
@@ -337,35 +482,38 @@ int build_apply_lut(elp_ctx* c, int Lc) {
 // [cycle + Lc + 32][covariate][slot][17] with 32 zero cycles of margin on both sides (lanes index up to 31 bases past a read's end) and an
 // odd number of bytes per cycle (bank spread).  When some QUAL above 93 occurs (presence bits 94..127; bit 127 stands for 128..255), one more
 // slot holds every covariate's "unobserved QUAL" byte and QUAL 94..255 map to it.  Rebuilt whenever the full table or the set of QUAL
-// values changes.
+// values changes.  The presence bits are the host copy phase_adapt (or elp_filter_target_regions) took with the range summary.
 int build_compact_lut(elp_ctx* c) {
-    uint32_t present[4] = {0, 0, 0, 0};
-    CUDA_TRY(c, cudaMemcpyAsync(present, c->d_qpresent, 16, cudaMemcpyDeviceToHost, c->stream));
-    CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+    const uint32_t* present = c->h_qpresent;
     if (c->clut_Lc == c->lut_maxcyc && memcmp(present, c->clut_present, 16) == 0) return E_OK;
     memcpy(c->clut_present, present, 16);
     c->clut_Lc = 0; c->clut_bytes = 0;
-    std::vector<int> slots;
-    for (int q = 6; q < 94; q++) if ((present[q >> 5] >> (q & 31)) & 1u) slots.push_back(q);
+    ClutArgs A{};
+    A.n_slots = 0;
+    for (int q = 6; q < 94; q++) if ((present[q >> 5] >> (q & 31)) & 1u) A.slot_q[A.n_slots++] = (uint8_t)q;
     const bool above93 = (present[2] >> 30) != 0 || present[3] != 0;   // bits 94..127
-    const int S = (int)slots.size() + (above93 ? 1 : 0), Lc = c->lut_maxcyc, ncyc = 2 * Lc + 1, n_cov = c->geom.n_cov;
-    if (S == 0 || n_cov == 0 || c->h_lut.empty()) return E_OK;
+    const int S = A.n_slots + (above93 ? 1 : 0), Lc = c->lut_maxcyc, ncyc = 2 * Lc + 1, n_cov = c->geom.n_cov;
+    if (S == 0 || n_cov == 0 || !c->d_lut) return E_OK;
     uint32_t blk = (uint32_t)(n_cov * S * 17); if (!(blk & 1)) blk++;
     const size_t bytes = ((size_t)(ncyc + 64) * blk + 15) / 16 * 16;
     if (bytes > 80 * 1024) return E_OK;                               // too large for two CTAs per SM: the global-memory kernel serves
-    std::vector<uint8_t> t(bytes, 0); std::vector<uint16_t> rowtab(256, 0);
-    for (int sl = 0; sl < (int)slots.size(); sl++) rowtab[slots[sl]] = (uint16_t)(sl * 17);
-    if (above93) for (int q = 94; q < 256; q++) rowtab[q] = (uint16_t)((S - 1) * 17);
-    for (int cy = 0; cy < ncyc; cy++) for (int cv = 0; cv < n_cov; cv++) {
-        for (int sl = 0; sl < (int)slots.size(); sl++)
-            memcpy(&t[(size_t)(cy + 32) * blk + (size_t)(cv * S + sl) * 17], &c->h_lut[(((size_t)cv * 94 + slots[sl]) * ncyc + cy) * 17], 17);
-        if (above93) memset(&t[(size_t)(cy + 32) * blk + (size_t)(cv * S + S - 1) * 17], c->h_unobs[cv], 17);
-    }
+    for (int sl = 0; sl < A.n_slots; sl++) A.rowtab_h[A.slot_q[sl]] = (uint16_t)(sl * 17);
+    if (above93) for (int q = 94; q < 256; q++) A.rowtab_h[q] = (uint16_t)((S - 1) * 17);
     if (c->clut_cap < bytes) { if (c->d_clut) cudaFree(c->d_clut); c->d_clut = nullptr; CUDA_TRY(c, cudaMalloc(&c->d_clut, bytes)); c->clut_cap = bytes; }
     if (!c->d_rowtab) CUDA_TRY(c, cudaMalloc(&c->d_rowtab, 512));
-    { int rcu = upload_small(c, c->d_clut, t.data(), bytes); if (rcu) return rcu; }
-    { int rcu = upload_small(c, c->d_rowtab, rowtab.data(), 512); if (rcu) return rcu; }
-    CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+    A.lut = c->d_lut; A.unobs = c->d_unobs; A.clut = c->d_clut; A.rowtab = c->d_rowtab;
+    A.bytes = (uint32_t)bytes; A.blk = blk; A.used = (uint32_t)(n_cov * S * 17); A.Lc = Lc; A.S = S;
+    c->begin("bqsr_fin_clut", 2.0 * (double)bytes);
+    fin_clut_kernel<<<(unsigned)((bytes + 255) / 256), 256, 0, c->stream>>>(A);
+    c->end(); LAUNCH_CHECK(c);
     c->clut_bytes = (uint32_t)bytes; c->clut_blk = blk; c->clut_S17 = (uint32_t)(S * 17); c->clut_Lc = Lc;
+    return E_OK;
+}
+
+int bqsr_empirical_copy(elp_ctx* c, uint8_t* emp) {
+    if (c->geom.cells()) {
+        CUDA_TRY(c, cudaMemcpyAsync(emp, c->d_emp, c->geom.cells(), cudaMemcpyDeviceToHost, c->stream));
+        CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+    }
     return E_OK;
 }

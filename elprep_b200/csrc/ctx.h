@@ -147,6 +147,7 @@ struct elp_ctx {
     DBuf<uint4> bq_recs, bq_segs;             // BQSR count kernel: work records of the eligible reads, segment table
     uint32_t* d_bq_small = nullptr;           // class histogram, region bases, list counters, segment counts, work-queue heads
     uint32_t* d_qpresent = nullptr;           // [4] bit q set iff QUAL value q (0..127) occurs in the arena (maintained at ingest)
+    uint32_t h_qpresent[4] = {0, 0, 0, 0};    // its host copy, taken with h_ranges (phase_adapt, elp_filter_target_regions)
 
     // ---- output order ----
     bool sorted = false;                      // columns below valid
@@ -164,8 +165,9 @@ struct elp_ctx {
     // ---- BQSR ----
     TableGeom geom;
     int64_t* d_tables = nullptr;              // dense [cells][2]
-    std::vector<int64_t> h_tables;
-    std::vector<uint8_t> h_emp;               // [cells]
+    uint8_t* d_emp = nullptr;                 // [cells] EmpiricalQuality (elp_bqsr_finalize)
+    double* d_fin = nullptr;                  // [n_cov][2] reported quality of the combined read-group entry, read-group term dG
+    uint8_t* d_qmaps = nullptr;               // quantization map [0, 94), static --sqq map at [96, 350) (bqsr_finalize.cu)
     bool gathered = false, finalized = false;
     uint64_t gather_eligible = 0;             // reads the last elp_bqsr_gather recalibrated (what the roofline line charges)
     uint8_t* d_lut = nullptr;                 // [n_cov][94][2*lut_maxcyc+1][17]
@@ -173,10 +175,8 @@ struct elp_ctx {
     size_t lut_cap = 0;
     uint8_t* d_cov_exists = nullptr;          // [n_cov]
     uint8_t* d_unobs = nullptr;               // [n_cov] recalibrated byte of a QUAL value without table entries (QUAL 94..255)
-    std::vector<uint8_t> h_unobs;
     uint8_t* d_clut = nullptr; uint16_t* d_rowtab = nullptr;   // compact apply table for the shared-memory kernel: [cycle][covariate][slot][17], QUAL -> slot offset
     uint32_t clut_bytes = 0, clut_blk = 0, clut_S17 = 0; int clut_Lc = 0; size_t clut_cap = 0; uint32_t clut_present[4] = {0, 0, 0, 0};
-    std::vector<uint8_t> h_lut;               // the full apply table [n_cov][94][2*lut_maxcyc+1][17] on the host
 
     // ---- duplication metrics (optical.cu) ----
     void* d_opt_ctr = nullptr; void* d_opt_hist = nullptr; void* d_opt_ovf = nullptr; uint32_t* d_opt_small = nullptr;
@@ -258,6 +258,7 @@ int phase_bqsr_finalize(elp_ctx* c, const char* report_path);
 int phase_bqsr_apply(elp_ctx* c);
 int build_apply_lut(elp_ctx* c, int Lc);   // bqsr_finalize.cu
 int build_compact_lut(elp_ctx* c);
+int bqsr_empirical_copy(elp_ctx* c, uint8_t* emp);   // device EmpiricalQuality -> host (synchronises)
 int upload_side_inputs(elp_ctx* c);
 int pack_reference(elp_ctx* c, int contig, const uint8_t* bases);   // bases: ref_len[contig] host bytes
 int check_device_errors(elp_ctx* c);

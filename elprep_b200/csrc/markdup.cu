@@ -461,6 +461,7 @@ int phase_adapt(elp_ctx* c) {
         c->end(); LAUNCH_CHECK(c);
     }
     CUDA_TRY(c, cudaMemcpyAsync(&c->h_ranges, c->d_ranges, sizeof(DeviceRanges), cudaMemcpyDeviceToHost, c->stream));
+    CUDA_TRY(c, cudaMemcpyAsync(c->h_qpresent, c->d_qpresent, 16, cudaMemcpyDeviceToHost, c->stream));   // the apply table's QUAL slots
     int rc = check_device_errors(c);   // synchronizes
     if (rc) return rc;
     if (c->h_ranges.n_entering == 0) { c->h_ranges.upos_min = 0; c->h_ranges.upos_max = 0; }

@@ -128,6 +128,7 @@ int phase_target_filter(elp_ctx* c, uint64_t* n_removed) {
             }
             int32_t lm = 0;
             CUDA_TRY(c, cudaMemcpyAsync(&lm, &c->d_ranges->lseq_max, 4, cudaMemcpyDeviceToHost, s));
+            CUDA_TRY(c, cudaMemcpyAsync(c->h_qpresent, c->d_qpresent, 16, cudaMemcpyDeviceToHost, s));
             CUDA_TRY(c, cudaStreamSynchronize(s));
             c->h_ranges.lseq_max = lm;
             c->n_sorted = kept;
