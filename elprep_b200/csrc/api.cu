@@ -190,6 +190,7 @@ void elp_destroy(elp_ctx* c) {
     cudaSetDevice(c->device);
     if (c->stream) cudaStreamSynchronize(c->stream);
     sam_state_release(c);
+    sites_release(c);
     sam_out_release(c);
     bgzf_release(c);
     bgzf_deflate_release(c);

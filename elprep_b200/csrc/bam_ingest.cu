@@ -402,7 +402,7 @@ int region_set(elp_ctx* c, RegionTable& t, const char* who, int32_t contig, cons
         for (uint64_t i = 0; i < n; i++) { if (m > 0 && iv[i].first <= iv[m - 1].second) { if (iv[i].second > iv[m - 1].second) iv[m - 1].second = iv[i].second; } else iv[m++] = iv[i]; }
         n = m;
     }
-    if (t.d[contig]) { cudaFree(t.d[contig]); t.d[contig] = nullptr; }
+    if (t.d[contig]) { if (t.separate(t.d[contig])) cudaFree(t.d[contig]); t.d[contig] = nullptr; }
     if (n) {
         CUDA_TRY(c, cudaMalloc(&t.d[contig], n * 8));
         CUDA_TRY(c, cudaMemcpyAsync(t.d[contig], iv.data(), n * 8, cudaMemcpyHostToDevice, c->stream));
@@ -413,7 +413,9 @@ int region_set(elp_ctx* c, RegionTable& t, const char* who, int32_t contig, cons
 }
 
 void region_release(RegionTable& t) {
-    for (auto p : t.d) if (p) cudaFree(p);
+    for (auto p : t.d) if (p && t.separate(p)) cudaFree(p);
+    if (t.block) cudaFree(t.block);
+    t.block = nullptr; t.block_pairs = 0;
     if (t.d_ptrs) cudaFree((void*)t.d_ptrs);
     if (t.d_n) cudaFree(t.d_n);
     t.d.clear(); t.n.clear(); t.d_ptrs = nullptr; t.d_n = nullptr; t.dirty = true;

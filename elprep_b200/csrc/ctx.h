@@ -41,10 +41,13 @@ struct DupCounters { int64_t ctr[7] = {0, 0, 0, 0, 0, 0, 0}; std::map<int64_t, i
 
 // per-contig interval table on the device (the ingest filter's target regions, elp_filter_target_regions' regions and the BQSR known
 // sites): per contig, the flattened, start-sorted (start, end) pairs, and the two device arrays of pointers and counts the kernels
-// index by REFID (region_set / region_upload, bam_ingest.cu)
+// index by REFID (region_set / region_upload, bam_ingest.cu).  elp_load_known_sites installs every contig's list in one allocation,
+// `block`; a d[i] inside it is not an allocation of its own (separate() is false) and is freed with the block.
 struct RegionTable {
     std::vector<int32_t*> d; std::vector<uint64_t> n;
     const int32_t** d_ptrs = nullptr; uint64_t* d_n = nullptr; bool dirty = true;
+    int32_t* block = nullptr; uint64_t block_pairs = 0;
+    bool separate(const int32_t* p) const { return !block || p < block || p >= block + 2 * block_pairs; }
 };
 
 struct KernelStat { uint64_t launches = 0; double ms = 0, alg_bytes = 0; };
@@ -92,7 +95,9 @@ struct elp_ctx {
     const uint8_t** d_refhot_ptrs = nullptr;   // [n_contigs] device array of the payload pointers
     uint64_t* d_ref_len = nullptr;
     bool side_dirty = true;
-    RegionTable known_sites;                 // elp_set_known_sites (survives elp_reset)
+    RegionTable known_sites;                 // elp_set_known_sites / elp_load_known_sites (survives elp_reset)
+    struct SitesStage* sites = nullptr;      // page-locked and device staging of elp_load_known_sites (known_sites.cu)
+    uint64_t sites_chunk = 0;                // elp_debug_set_sites_chunk: bytes per staging chunk (0: the default)
 
     // ---- reads, arrival order (SoA columns) ----
     uint64_t n = 0, n_qname = 0, n_cigar = 0, n_qual = 0, n_seq = 0;
@@ -276,6 +281,7 @@ void region_release(RegionTable& t);
 int build_output_columns(elp_ctx* c, const uint32_t* perm, uint64_t n_out, bool refilter);   // coordsort.cu: s_* columns and s_out_off of perm[0, n_out)
 int phase_target_filter(elp_ctx* c, uint64_t* n_removed);   // target_regions.cu
 void sam_state_release(elp_ctx* c);   // sam_ingest.cu
+void sites_release(elp_ctx* c);       // known_sites.cu
 void sam_out_release(elp_ctx* c);     // sam_format.cu
 void bgzf_stream_reset(elp_ctx* c);   // bgzf_inflate.cu: forget the open file (elp_reset)
 void bgzf_release(elp_ctx* c);

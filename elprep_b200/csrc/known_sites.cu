@@ -1,0 +1,548 @@
+// known_sites.cu -- --known-sites on the device: .elsites files read, parsed, sorted and flattened into the known-sites table
+// (elp_load_known_sites).
+//
+// The reference loads every file with intervals.FromElsitesFile (intervals/intervals.go:199-254), appends the intervals of each
+// chromosome (NewBaseRecalibrator, filters/bqsr.go:424-443), then sorts (ParallelSortByStart) and flattens (ParallelFlatten) each.
+//   host           checks the header and streams the rest of each file through two page-locked chunks: the upload of chunk k+1 runs
+//                  while the kernels of chunk k do; the bytes after the last '\n' of a chunk are carried into the next one
+//   sites_lines    the line finder of elp_append_sam (text_parse.cuh)
+//   sites_parse    one thread per line, a warp over 32 consecutive lines: the three fields, strconv.ParseInt, the chromosome name (each
+//                  run of equal names in a warp is looked up once: files are grouped by chromosome); then one (contig, start, end) per
+//                  @SQ line with that name, at its scanned offset
+//   sites_sort     the onesweep radix sort of contig << 32 | (start ^ 2^31), the end as payload
+//   sites_flatten  one prefix max over contig << 32 | (end ^ 2^31): interval i opens a group iff it is the first of its contig or its start
+//                  lies above every earlier end of its contig; the group heads are compacted and each group keeps the max of its ends
+// Nothing is installed before every file was read and every line accepted; the new table is one allocation (RegionTable::block).
+#include <algorithm>
+#include <cerrno>
+#include <cstdio>
+#include <cstring>
+#include <vector>
+#include "ctx.h"
+#include "text_parse.cuh"
+#include "../../include/elprep_b200.h"
+
+namespace {
+
+const char SITES_HEADER[] = "# elsites format version 1.0\n";   // intervals.ElsitesHeader (intervals/intervals.go:176)
+constexpr uint64_t SITES_HEADER_LEN = sizeof(SITES_HEADER) - 1;
+constexpr uint64_t SITES_MAX_LINE = 65536;                     // bufio.MaxScanTokenSize: a longer line stops the reference's scanner
+constexpr uint64_t SITES_CHUNK_DEFAULT = 32ull << 20;
+
+}  // namespace
+
+// page-locked and device staging, reused by every call on the context
+struct SitesStage {
+    uint64_t chunk = 0;                                          // file bytes per step; a carried partial line sits in front of them
+    uint8_t* h[2] = {nullptr, nullptr};                          // page-locked
+    uint8_t* d[2] = {nullptr, nullptr};
+    cudaEvent_t up[2] = {nullptr, nullptr};                      // the upload out of h[b] has landed in d[b] (copy stream)
+    cudaEvent_t used[2] = {nullptr, nullptr};                    // the kernels that read d[b] are done (compute stream)
+    cudaStream_t copy = nullptr;
+    unsigned long long* d_small = nullptr;                       // [0] first error (line << 8 | SitesErr), [1] unmatched lines
+    unsigned long long* h_small = nullptr;                       // page-locked: [0, 1] copies, [2] '\n' count, [3] intervals, [4] virtual line end
+    NameDict dict; bool dict_ok = false;
+};
+
+void sites_release(elp_ctx* c) {
+    SitesStage* S = c->sites;
+    if (!S) return;
+    if (S->copy) cudaStreamSynchronize(S->copy);
+    for (int b = 0; b < 2; b++) {
+        if (S->h[b]) cudaFreeHost(S->h[b]);
+        if (S->d[b]) cudaFree(S->d[b]);
+        if (S->up[b]) cudaEventDestroy(S->up[b]);
+        if (S->used[b]) cudaEventDestroy(S->used[b]);
+    }
+    if (S->copy) cudaStreamDestroy(S->copy);
+    if (S->d_small) cudaFree(S->d_small);
+    if (S->h_small) cudaFreeHost(S->h_small);
+    name_dict_release(S->dict);
+    delete S;
+    c->sites = nullptr;
+}
+
+namespace {
+
+inline unsigned nblk(uint64_t n, int t) { return (unsigned)((n + t - 1) / t); }
+template <class T> int grow(elp_ctx* c, DBuf<T>& b, size_t need, size_t keep) {
+    cudaError_t e = b.reserve(need, c->stream, keep);
+    if (e != cudaSuccess) return c->fail(e == cudaErrorMemoryAllocation ? E_NOMEM : E_CUDA, "device allocation of %zu bytes failed: %s", need * sizeof(T), cudaGetErrorString(e));
+    return E_OK;
+}
+#define TRY(x) do { int rc__ = (x); if (rc__) return rc__; } while (0)
+
+// why a line fails; the smallest (line << 8 | code) of a file is reported
+enum SitesErr : uint32_t { KS_FIELDS = 1, KS_START, KS_END, KS_LONG };
+const char* sites_err_text(uint32_t e) {
+    switch (e) {
+        case KS_FIELDS: return "invalid sites line (no chromosome before the first tab, or no second tab)";
+        case KS_START: return "start: strconv.ParseInt(s, 10, 32) fails";
+        case KS_END: return "end: strconv.ParseInt(s, 10, 32) fails";
+        case KS_LONG: return "line of 65536 bytes or more (bufio.Scanner: token too long)";
+        default: return "?";
+    }
+}
+
+// ---- sites_parse ----
+struct SitesArgs {
+    const uint8_t* text; const uint64_t* ls; uint64_t n_lines;
+    uint64_t line0;                                  // line number (header = 0) of the chunk's first line within its file
+    NameDict dict;
+    int32_t* ent; int32_t* start; int32_t* end;      // per accepted line: name entry (-1: unknown), start, end
+    uint32_t* emit;                                  // per line: intervals it contributes (one per @SQ line with its name)
+    unsigned long long* small;
+};
+
+// FromElsitesFile's loop body for one line (intervals.go:221-247), after bufio.ScanLines dropped the '\n' and one '\r' before it
+__global__ void __launch_bounds__(256) sites_parse_kernel(SitesArgs A) {
+    const unsigned lane = threadIdx.x & 31;
+    const uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const bool live = k < A.n_lines;
+    uint64_t s0 = 0, nn = 0;                         // the line's start and its name's length
+    uint32_t err = 0;
+    int64_t st = 0, en = 0;
+    if (live) {
+        s0 = A.ls[k];
+        const uint64_t raw = A.ls[k + 1] - 1 - s0;
+        const uint8_t* p = A.text + s0;
+        uint64_t n = raw;
+        if (n && p[n - 1] == '\r') n--;
+        if (raw >= SITES_MAX_LINE) err = KS_LONG;
+        else {
+            uint64_t i = 0;
+            while (i < n && p[i] != '\t') i++;
+            uint64_t j = i + 1;
+            while (j < n && p[j] != '\t') j++;
+            if (i == 0 || i >= n || j >= n) err = KS_FIELDS;
+            else if (!parse_dec(p + i + 1, j - i - 1, true, INT32_MIN, INT32_MAX, &st)) err = KS_START;
+            else if (!parse_dec(p + j + 1, n - j - 1, true, INT32_MIN, INT32_MAX, &en)) err = KS_END;
+            nn = i;
+        }
+    }
+    // the name: a line whose name equals the previous lane's takes that lane's entry; the first line of each run looks it up
+    const bool named = live && !err;
+    const uint64_t ps0 = __shfl_up_sync(FULL_MASK, s0, 1), pnn = __shfl_up_sync(FULL_MASK, nn, 1);
+    const bool pnamed = __shfl_up_sync(FULL_MASK, (int)named, 1) != 0;
+    bool lead = named;
+    if (named && lane > 0 && pnamed && pnn == nn) {
+        const uint8_t* p = A.text + s0; const uint8_t* q = A.text + ps0;
+        uint64_t j = 0;
+        while (j < nn && p[j] == q[j]) j++;
+        lead = j < nn;
+    }
+    int e = lead ? name_entry(A.dict, A.text + s0, nn) : -1;
+    const unsigned below = __ballot_sync(FULL_MASK, lead) & (0xffffffffu >> (31 - lane));
+    const int e_lead = __shfl_sync(FULL_MASK, e, below ? 31 - __clz(below) : (int)lane);
+    if (named && !lead) e = e_lead;
+    const uint32_t m = named && e >= 0 ? A.dict.all_off[e + 1] - A.dict.all_off[e] : 0;
+    if (live) {
+        A.emit[k] = m;
+        if (named) { A.ent[k] = e; A.start[k] = (int32_t)st; A.end[k] = (int32_t)en; }
+        else atomicMin(A.small, ((unsigned long long)(A.line0 + k) << 8) | err);
+    }
+    const unsigned um = __ballot_sync(FULL_MASK, named && m == 0);   // valid lines on a chromosome that is no @SQ SN ("*" included)
+    if (lane == 0 && um) atomicAdd(A.small + 1, (unsigned long long)__popc(um));
+}
+
+// the intervals of the accepted lines, at their scanned offsets: key contig << 32 | (start ^ 2^31), payload end
+__global__ void __launch_bounds__(256) sites_emit_kernel(uint64_t n, const int32_t* __restrict__ ent, const int32_t* __restrict__ start, const int32_t* __restrict__ end,
+                                                          const uint32_t* __restrict__ emit, const uint64_t* __restrict__ off, NameDict D,
+                                                          uint64_t* __restrict__ keys, uint32_t* __restrict__ vals) {
+    const uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n) return;
+    const uint32_t m = emit[k];
+    if (!m) return;
+    const uint64_t o = off[k];
+    const int32_t* ids = D.all + D.all_off[ent[k]];
+    const uint32_t lo = (uint32_t)start[k] ^ 0x80000000u, v = (uint32_t)end[k];
+    for (uint32_t j = 0; j < m; j++) { keys[o + j] = ((uint64_t)(uint32_t)ids[j] << 32) | lo; vals[o + j] = v; }
+}
+
+// ---- sites_flatten ----
+// Over the sorted intervals, v_i = contig_i << 32 | (end_i ^ 2^31).  Contigs never decrease, so the max of v over the intervals before i
+// carries contig_i exactly when i is not the first of its contig, and then its low word is the largest earlier end of the contig.
+// Flatten (intervals.go:101-117) extends the open group while start <= its end; a closed group ended below the start of the group after
+// it, so "start_i > every earlier end of the contig" is exactly "start_i > the end of the open group": i opens a group.
+constexpr int FL_T = 256, FL_ITEMS = 8, FL_TILE = FL_T * FL_ITEMS;
+
+__device__ __forceinline__ uint64_t fl_val(uint64_t key, uint32_t end) { return (key & 0xffffffff00000000ull) | (end ^ 0x80000000u); }
+
+__device__ __forceinline__ uint64_t block_max(uint64_t m, uint64_t* sh) {   // every thread gets the max over the block
+    for (int o = 16; o; o >>= 1) m = max(m, (uint64_t)__shfl_xor_sync(FULL_MASK, m, o));
+    if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = m;
+    __syncthreads();
+    m = 0;
+    for (int w = 0; w < FL_T / 32; w++) m = max(m, sh[w]);
+    return m;
+}
+
+__global__ void __launch_bounds__(FL_T) sites_tile_max_kernel(const uint64_t* __restrict__ keys, const uint32_t* __restrict__ ends, uint64_t n, uint64_t* __restrict__ tmax) {
+    __shared__ uint64_t sh[FL_T / 32];
+    const uint64_t t0 = (uint64_t)blockIdx.x * FL_TILE;
+    uint64_t m = 0;
+#pragma unroll
+    for (int j = 0; j < FL_ITEMS; j++) { const uint64_t i = t0 + (uint64_t)j * FL_T + threadIdx.x; if (i < n) m = max(m, fl_val(keys[i], ends[i])); }
+    m = block_max(m, sh);
+    if (threadIdx.x == 0) tmax[blockIdx.x] = m;
+}
+
+// tmax[t] <- the max over the tiles before t (0 for tile 0), in one CTA
+__global__ void __launch_bounds__(1024) sites_tile_scan_kernel(uint64_t* __restrict__ tmax, uint64_t tiles) {
+    __shared__ uint64_t wsum[32];
+    __shared__ uint64_t carry;
+    const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (threadIdx.x == 0) carry = 0;
+    __syncthreads();
+    for (uint64_t base = 0; base < tiles; base += 1024) {
+        const uint64_t i = base + threadIdx.x;
+        const uint64_t v = i < tiles ? tmax[i] : 0;
+        uint64_t x = v;
+        for (int o = 1; o < 32; o <<= 1) { const uint64_t y = __shfl_up_sync(FULL_MASK, x, o); if (lane >= (unsigned)o) x = max(x, y); }
+        if (lane == 31) wsum[warp] = x;
+        __syncthreads();
+        if (warp == 0) {
+            uint64_t w = wsum[lane];
+            for (int o = 1; o < 32; o <<= 1) { const uint64_t y = __shfl_up_sync(FULL_MASK, w, o); if (lane >= (unsigned)o) w = max(w, y); }
+            wsum[lane] = w;
+        }
+        __syncthreads();
+        uint64_t ex = __shfl_up_sync(FULL_MASK, x, 1);
+        if (lane == 0) ex = 0;
+        if (warp) ex = max(ex, wsum[warp - 1]);
+        const uint64_t c0 = carry, total = wsum[31];
+        __syncthreads();
+        if (i < tiles) tmax[i] = max(c0, ex);
+        if (threadIdx.x == 0) carry = max(c0, total);
+        __syncthreads();
+    }
+}
+
+// head[i] = 1 iff sorted interval i opens a group; tpre: the exclusive tile maxima of sites_tile_scan_kernel
+__global__ void __launch_bounds__(FL_T) sites_head_kernel(const uint64_t* __restrict__ keys, const uint32_t* __restrict__ ends, uint64_t n,
+                                                          const uint64_t* __restrict__ tpre, uint32_t* __restrict__ head) {
+    __shared__ uint64_t wsum[FL_T / 32];
+    const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const uint64_t i0 = (uint64_t)blockIdx.x * FL_TILE + (uint64_t)threadIdx.x * FL_ITEMS;
+    uint64_t kk[FL_ITEMS], v[FL_ITEMS], m = 0;
+#pragma unroll
+    for (int j = 0; j < FL_ITEMS; j++) {
+        const uint64_t i = i0 + j;
+        kk[j] = i < n ? keys[i] : 0;
+        v[j] = i < n ? fl_val(kk[j], ends[i]) : 0;
+        m = max(m, v[j]);
+    }
+    uint64_t x = m;   // exclusive max over the threads before this one in the tile
+    for (int o = 1; o < 32; o <<= 1) { const uint64_t y = __shfl_up_sync(FULL_MASK, x, o); if (lane >= (unsigned)o) x = max(x, y); }
+    if (lane == 31) wsum[warp] = x;
+    __syncthreads();
+    uint64_t run = __shfl_up_sync(FULL_MASK, x, 1);
+    if (lane == 0) run = 0;
+    for (unsigned w = 0; w < warp; w++) run = max(run, wsum[w]);
+    run = max(run, tpre[blockIdx.x]);
+#pragma unroll
+    for (int j = 0; j < FL_ITEMS; j++) {
+        const uint64_t i = i0 + j;
+        if (i >= n) break;
+        const int32_t s = (int32_t)((uint32_t)kk[j] ^ 0x80000000u), e = (int32_t)((uint32_t)run ^ 0x80000000u);
+        head[i] = i == 0 || (run >> 32) != (kk[j] >> 32) || s > e;
+        run = max(run, v[j]);
+    }
+}
+
+// group g = gid[i] + head[i] - 1: its head writes the start, every member raises the end (biased, so that unsigned max is signed max);
+// first[contig] = the contig's first group
+__global__ void __launch_bounds__(256) sites_compact_kernel(const uint64_t* __restrict__ keys, const uint32_t* __restrict__ ends, uint64_t n, const uint32_t* __restrict__ head,
+                                                             const uint64_t* __restrict__ gid, int32_t* __restrict__ out, uint64_t* __restrict__ first) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint64_t key = keys[i];
+    const uint32_t h = head[i];
+    const uint64_t g = gid[i] + h - 1;
+    if (h) out[2 * g] = (int32_t)((uint32_t)key ^ 0x80000000u);
+    atomicMax(reinterpret_cast<unsigned*>(out + 2 * g + 1), ends[i] ^ 0x80000000u);
+    if (i == 0 || (keys[i - 1] >> 32) != (key >> 32)) first[key >> 32] = g;
+}
+
+__global__ void __launch_bounds__(256) sites_unbias_kernel(uint64_t n_groups, int32_t* __restrict__ out) {
+    const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g < n_groups) out[2 * g + 1] = (int32_t)((uint32_t)out[2 * g + 1] ^ 0x80000000u);
+}
+
+// ---- host side ----
+struct SitesScratch {   // per call; freed on return
+    DBuf<uint32_t> cnt, emit, vals_a, vals_b, head; DBuf<uint64_t> cnt_off, ls, emit_off, keys_a, keys_b, tmax, gid, first;
+    DBuf<int32_t> ent, start, end;
+    ~SitesScratch() {
+        cnt.release(); emit.release(); vals_a.release(); vals_b.release(); head.release(); cnt_off.release(); ls.release(); emit_off.release();
+        keys_a.release(); keys_b.release(); tmax.release(); gid.release(); first.release(); ent.release(); start.release(); end.release();
+    }
+};
+
+struct Chunk { int b = 0; uint64_t m = 0; bool last = false, long_tail = false; };   // m: bytes of whole lines at the front of h[b]
+
+int stage_init(elp_ctx* c) {
+    if (!c->sites) c->sites = new SitesStage();
+    SitesStage& S = *c->sites;
+    if (!S.copy) {
+        CUDA_TRY(c, cudaStreamCreateWithFlags(&S.copy, cudaStreamNonBlocking));
+        for (int b = 0; b < 2; b++) { CUDA_TRY(c, cudaEventCreateWithFlags(&S.up[b], cudaEventDisableTiming)); CUDA_TRY(c, cudaEventCreateWithFlags(&S.used[b], cudaEventDisableTiming)); }
+    }
+    if (!S.d_small) { CUDA_TRY(c, cudaMalloc(&S.d_small, 16)); CUDA_TRY(c, cudaHostAlloc(&S.h_small, 64, cudaHostAllocDefault)); }
+    if (!S.dict_ok) { TRY(name_dict_upload(c, S.dict)); S.dict_ok = true; }
+    const uint64_t want = c->sites_chunk ? c->sites_chunk : SITES_CHUNK_DEFAULT;
+    if (S.chunk != want) {
+        CUDA_TRY(c, cudaStreamSynchronize(S.copy));
+        for (int b = 0; b < 2; b++) {
+            if (S.h[b]) cudaFreeHost(S.h[b]);
+            if (S.d[b]) cudaFree(S.d[b]);
+            S.h[b] = S.d[b] = nullptr;
+        }
+        S.chunk = 0;
+        const uint64_t cap = want + SITES_MAX_LINE, dcap = (cap + SAM_CHUNK - 1) / SAM_CHUNK * SAM_CHUNK + SAM_CHUNK;
+        for (int b = 0; b < 2; b++) {
+            if (cudaHostAlloc(&S.h[b], cap, cudaHostAllocDefault) != cudaSuccess || cudaMalloc(&S.d[b], dcap) != cudaSuccess) {
+                cudaGetLastError();
+                return c->fail(E_NOMEM, "elp_load_known_sites: staging allocation of 2 x %llu bytes failed", (unsigned long long)cap);
+            }
+        }
+        S.chunk = want;
+    }
+    return E_OK;
+}
+
+// the carried bytes and the next chunk of the file into h[b]
+int read_fill(elp_ctx* c, SitesStage& S, FILE* f, const char* path, std::vector<uint8_t>& carry, int b, Chunk* ch) {
+    CUDA_TRY(c, cudaEventSynchronize(S.up[b]));   // the last upload out of h[b] has read it
+    uint8_t* h = S.h[b];
+    const uint64_t nc = carry.size();
+    if (nc) memcpy(h, carry.data(), nc);
+    const size_t got = fread(h + nc, 1, S.chunk, f);
+    if (got < S.chunk && ferror(f)) return c->fail(E_INVAL, "elp_load_known_sites: cannot read %s: %s", path, strerror(errno));
+    const uint64_t n = nc + got;
+    ch->b = b; ch->last = got < S.chunk;
+    if (ch->last) ch->m = n;   // the last line may lack its '\n'
+    else {
+        const void* q = got ? memrchr(h + nc, '\n', got) : nullptr;
+        ch->m = q ? (uint64_t)(static_cast<const uint8_t*>(q) - h) + 1 : 0;
+    }
+    carry.assign(h + ch->m, h + n);
+    ch->long_tail = !ch->last && carry.size() >= SITES_MAX_LINE;
+    return E_OK;
+}
+
+int upload(elp_ctx* c, SitesStage& S, const Chunk& ch) {
+    if (!ch.m) return E_OK;
+    const uint64_t padded = (ch.m + SAM_CHUNK - 1) / SAM_CHUNK * SAM_CHUNK + SAM_CHUNK;
+    CUDA_TRY(c, cudaStreamWaitEvent(S.copy, S.used[ch.b], 0));
+    CUDA_TRY(c, cudaMemcpyAsync(S.d[ch.b], S.h[ch.b], ch.m, cudaMemcpyHostToDevice, S.copy));
+    CUDA_TRY(c, cudaMemsetAsync(S.d[ch.b] + ch.m, 0, padded - ch.m, S.copy));
+    CUDA_TRY(c, cudaEventRecord(S.up[ch.b], S.copy));
+    return E_OK;
+}
+
+// '\n' count of the chunk into h_small[2] (read after the next synchronisation)
+int count_lines(elp_ctx* c, SitesStage& S, SitesScratch& X, const Chunk& ch) {
+    const uint64_t n_chunks = (ch.m + SAM_CHUNK - 1) / SAM_CHUNK;
+    TRY(grow(c, X.cnt, n_chunks + 8, 0)); TRY(grow(c, X.cnt_off, n_chunks + 2, 0));
+    CUDA_TRY(c, cudaStreamWaitEvent(c->stream, S.up[ch.b], 0));
+    c->begin("sites_lines", (double)ch.m);
+    sam_count_kernel<<<nblk(n_chunks, 256), 256, 0, c->stream>>>(S.d[ch.b], n_chunks, X.cnt.p);
+    c->end(); LAUNCH_CHECK(c);
+    TRY(exclusive_scan_u32_to_u64(c, X.cnt.p, X.cnt_off.p, n_chunks));
+    CUDA_TRY(c, cudaMemcpyAsync(S.h_small + 2, X.cnt_off.p + n_chunks, 8, cudaMemcpyDeviceToHost, c->stream));
+    return E_OK;
+}
+
+// the chunk's lines: line starts, parse and the scan of the interval counts are enqueued; *n_lines is the chunk's line count
+int parse_launch(elp_ctx* c, SitesStage& S, SitesScratch& X, const Chunk& ch, uint64_t line0, uint64_t* n_lines) {
+    cudaStream_t s = c->stream;
+    CUDA_TRY(c, cudaStreamSynchronize(s));
+    const uint64_t n_nl = S.h_small[2], n_chunks = (ch.m + SAM_CHUNK - 1) / SAM_CHUNK;
+    const bool open_end = S.h[ch.b][ch.m - 1] != '\n';
+    const uint64_t nl = n_nl + (open_end ? 1 : 0);
+    TRY(grow(c, X.ls, nl + 2, 0)); TRY(grow(c, X.ent, nl + 8, 0)); TRY(grow(c, X.start, nl + 8, 0)); TRY(grow(c, X.end, nl + 8, 0));
+    TRY(grow(c, X.emit, nl + 8, 0)); TRY(grow(c, X.emit_off, nl + 2, 0));
+    CUDA_TRY(c, cudaMemsetAsync(X.ls.p, 0, 8, s));
+    c->begin("sites_lines", (double)ch.m + 8.0 * (double)n_nl);
+    sam_lines_kernel<<<nblk(n_chunks, 256), 256, 0, s>>>(S.d[ch.b], n_chunks, X.cnt_off.p, X.ls.p);
+    c->end(); LAUNCH_CHECK(c);
+    if (open_end) { S.h_small[4] = ch.m + 1; CUDA_TRY(c, cudaMemcpyAsync(X.ls.p + nl, S.h_small + 4, 8, cudaMemcpyHostToDevice, s)); }   // a virtual '\n' past the text
+    SitesArgs A{};
+    A.text = S.d[ch.b]; A.ls = X.ls.p; A.n_lines = nl; A.line0 = line0; A.dict = S.dict;
+    A.ent = X.ent.p; A.start = X.start.p; A.end = X.end.p; A.emit = X.emit.p; A.small = S.d_small;
+    c->begin("sites_parse", (double)ch.m + 8.0 * (double)(nl + 1) + 16.0 * (double)nl);
+    sites_parse_kernel<<<nblk(nl, 256), 256, 0, s>>>(A);
+    c->end(); LAUNCH_CHECK(c);
+    TRY(exclusive_scan_u32_to_u64(c, X.emit.p, X.emit_off.p, nl));
+    CUDA_TRY(c, cudaMemcpyAsync(S.h_small, S.d_small, 16, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(c, cudaMemcpyAsync(S.h_small + 3, X.emit_off.p + nl, 8, cudaMemcpyDeviceToHost, s));
+    *n_lines = nl;
+    return E_OK;
+}
+
+// the parse's verdict, then the chunk's intervals appended at keys_a / vals_a + *total
+int parse_finish(elp_ctx* c, SitesStage& S, SitesScratch& X, const Chunk& ch, int file, const char* path, uint64_t nl, uint64_t* total) {
+    cudaStream_t s = c->stream;
+    CUDA_TRY(c, cudaStreamSynchronize(s));
+    if (S.h_small[0] != ~0ull)
+        return c->fail(E_SITES, "elp_load_known_sites: %s (file %d), line %llu (0-based, header = line 0): %s", path, file, (unsigned long long)(S.h_small[0] >> 8),
+                       sites_err_text((uint32_t)(S.h_small[0] & 0xff)));
+    const uint64_t add = S.h_small[3], t0 = *total;
+    if (t0 + add >= (1ull << 30)) return c->fail(E_LIMIT, "elp_load_known_sites: 2^30 or more intervals in total (the limit of the device sort)");
+    if (t0 + add + 4 > X.keys_a.cap) { const size_t want = std::max<size_t>(t0 + add + 4, 2 * X.keys_a.cap); TRY(grow(c, X.keys_a, want, t0)); TRY(grow(c, X.vals_a, want, t0)); }
+    c->begin("sites_parse", 24.0 * (double)nl + 12.0 * (double)add);
+    sites_emit_kernel<<<nblk(nl, 256), 256, 0, s>>>(nl, X.ent.p, X.start.p, X.end.p, X.emit.p, X.emit_off.p, S.dict, X.keys_a.p + t0, X.vals_a.p + t0);
+    c->end(); LAUNCH_CHECK(c);
+    CUDA_TRY(c, cudaEventRecord(S.used[ch.b], s));
+    *total = t0 + add;
+    return E_OK;
+}
+
+// one file: the header on the host, then every line through the device, appended behind *total
+int load_file(elp_ctx* c, SitesStage& S, SitesScratch& X, int file, const char* path, uint64_t* total) {
+    FILE* f = fopen(path, "rb");
+    if (!f) return c->fail(E_INVAL, "elp_load_known_sites: cannot open %s: %s", path, strerror(errno));
+    struct Closer { FILE* f; ~Closer() { fclose(f); } } closer{f};
+    char hd[SITES_HEADER_LEN];   // bufio.Reader.ReadString('\n') must return exactly ElsitesHeader (intervals.go:204-210)
+    const size_t got = fread(hd, 1, SITES_HEADER_LEN, f);
+    if (got < SITES_HEADER_LEN && ferror(f)) return c->fail(E_INVAL, "elp_load_known_sites: cannot read %s: %s", path, strerror(errno));
+    if (got < SITES_HEADER_LEN || memcmp(hd, SITES_HEADER, SITES_HEADER_LEN) != 0)
+        return c->fail(E_SITES, "elp_load_known_sites: %s (file %d), line 0 (0-based, header = line 0): not a .elsites file - the first line is not \"# elsites format version 1.0\"", path, file);
+    std::vector<uint8_t> carry;
+    uint64_t line0 = 1;
+    Chunk cur;
+    TRY(read_fill(c, S, f, path, carry, 0, &cur));
+    TRY(upload(c, S, cur));
+    for (;;) {
+        uint64_t nl = 0;
+        if (cur.m) { TRY(count_lines(c, S, X, cur)); TRY(parse_launch(c, S, X, cur, line0, &nl)); }
+        const bool more = !cur.last && !cur.long_tail;
+        Chunk nxt;
+        if (more) { TRY(read_fill(c, S, f, path, carry, cur.b ^ 1, &nxt)); TRY(upload(c, S, nxt)); }   // overlaps the kernels of cur
+        if (cur.m) TRY(parse_finish(c, S, X, cur, file, path, nl, total));
+        line0 += nl;
+        if (cur.long_tail) return c->fail(E_SITES, "elp_load_known_sites: %s (file %d), line %llu (0-based, header = line 0): %s", path, file, (unsigned long long)line0, sites_err_text(KS_LONG));
+        if (!more) return E_OK;
+        cur = nxt;
+    }
+}
+
+// sorted intervals -> flattened groups in one allocation (*block, *n_groups pairs); first[contig] = its first group or ~0
+int flatten(elp_ctx* c, SitesScratch& X, const uint64_t* keys, const uint32_t* ends, uint64_t n, int32_t** block, uint64_t* n_groups, std::vector<uint64_t>& first) {
+    cudaStream_t s = c->stream;
+    const int nc = c->n_contigs;
+    const uint64_t tiles = (n + FL_TILE - 1) / FL_TILE;
+    TRY(grow(c, X.tmax, tiles + 1, 0)); TRY(grow(c, X.head, n + 4, 0)); TRY(grow(c, X.gid, n + 2, 0)); TRY(grow(c, X.first, nc + 1, 0));
+    c->begin("sites_flatten", 12.0 * (double)n + 8.0 * (double)tiles);
+    sites_tile_max_kernel<<<(unsigned)tiles, FL_T, 0, s>>>(keys, ends, n, X.tmax.p);
+    c->end(); LAUNCH_CHECK(c);
+    c->begin("sites_flatten", 16.0 * (double)tiles);
+    sites_tile_scan_kernel<<<1, 1024, 0, s>>>(X.tmax.p, tiles);
+    c->end(); LAUNCH_CHECK(c);
+    c->begin("sites_flatten", 16.0 * (double)n + 8.0 * (double)tiles);
+    sites_head_kernel<<<(unsigned)tiles, FL_T, 0, s>>>(keys, ends, n, X.tmax.p, X.head.p);
+    c->end(); LAUNCH_CHECK(c);
+    TRY(exclusive_scan_u32_to_u64(c, X.head.p, X.gid.p, n));
+    uint64_t G = 0;
+    CUDA_TRY(c, cudaMemcpyAsync(&G, X.gid.p + n, 8, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(c, cudaStreamSynchronize(s));
+    int32_t* out = nullptr;
+    cudaError_t e = cudaMalloc(&out, G * 8);
+    if (e != cudaSuccess) { cudaGetLastError(); return c->fail(e == cudaErrorMemoryAllocation ? E_NOMEM : E_CUDA, "device allocation of %llu bytes failed", (unsigned long long)(G * 8)); }
+    int rc = E_OK;
+    auto step = [&](cudaError_t x) { if (rc == E_OK && x != cudaSuccess) rc = c->fail(E_CUDA, "elp_load_known_sites: %s", cudaGetErrorString(x)); };
+    step(cudaMemsetAsync(out, 0, G * 8, s));
+    step(cudaMemsetAsync(X.first.p, 0xff, (size_t)nc * 8, s));
+    c->begin("sites_flatten", 24.0 * (double)n + 8.0 * (double)G);
+    sites_compact_kernel<<<nblk(n, 256), 256, 0, s>>>(keys, ends, n, X.head.p, X.gid.p, out, X.first.p);
+    c->end(); step(cudaGetLastError());
+    c->begin("sites_flatten", 8.0 * (double)G);
+    sites_unbias_kernel<<<nblk(G, 256), 256, 0, s>>>(G, out);
+    c->end(); step(cudaGetLastError());
+    first.assign(nc, ~0ull);
+    if (nc) step(cudaMemcpyAsync(first.data(), X.first.p, (size_t)nc * 8, cudaMemcpyDeviceToHost, s));
+    step(cudaStreamSynchronize(s));
+    if (rc) { cudaFree(out); return rc; }
+    *block = out; *n_groups = G;
+    return E_OK;
+}
+
+}  // namespace
+
+extern "C" int elp_load_known_sites(elp_ctx* c, const char* const* paths, int32_t n_paths, uint64_t* n_unmatched) {
+    if (!c) return ELP_EINVAL;
+    cudaSetDevice(c->device);
+    if (n_paths < 0 || (n_paths && !paths)) return c->fail(E_INVAL, "elp_load_known_sites: %d paths at %p", n_paths, (const void*)paths);
+    for (int i = 0; i < n_paths; i++) if (!paths[i]) return c->fail(E_INVAL, "elp_load_known_sites: path %d is null", i);
+    if (c->n_contigs > 0 && !c->has_contig_names)
+        return c->fail(E_INVAL, "elp_load_known_sites: the context was created without elp_config.contig_names, so chromosome names cannot be resolved");
+    const int nc = c->n_contigs;
+    int32_t* block = nullptr; uint64_t G = 0, unmatched = 0;
+    std::vector<uint64_t> first(nc, ~0ull);
+    if (n_paths) {
+        TRY(stage_init(c));
+        SitesStage& S = *c->sites;
+        struct Drain { cudaStream_t s; ~Drain() { cudaStreamSynchronize(s); } } drain{S.copy};   // no upload outlives the call
+        SitesScratch X;
+        CUDA_TRY(c, cudaMemsetAsync(S.d_small, 0xff, 8, c->stream));
+        CUDA_TRY(c, cudaMemsetAsync(S.d_small + 1, 0, 8, c->stream));
+        uint64_t total = 0;
+        for (int i = 0; i < n_paths; i++) TRY(load_file(c, S, X, i, paths[i], &total));
+        CUDA_TRY(c, cudaMemcpyAsync(S.h_small + 1, S.d_small + 1, 8, cudaMemcpyDeviceToHost, c->stream));
+        CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+        unmatched = S.h_small[1];
+        if (total) {
+            TRY(grow(c, X.keys_b, total + 4, 0)); TRY(grow(c, X.vals_b, total + 4, 0));
+            int bits = 32;
+            for (uint32_t v = (uint32_t)nc; v; v >>= 1) bits++;
+            // sites_sort spans the radix passes (which also report under radix_*_sites); it is recorded once the sort is enqueued
+            cudaEvent_t ea = nullptr;
+            if (c->profile) { ea = c->get_event(); cudaEventRecord(ea, c->stream); }
+            bool in_b = false;
+            TRY(radix_sort_u64(c, X.keys_a.p, X.keys_b.p, X.vals_a.p, X.vals_b.p, total, bits, &in_b, "sites"));
+            if (c->profile) {
+                PendingEvent pe; pe.name = "sites_sort"; pe.a = ea; pe.b = c->get_event();
+                pe.alg_bytes = (double)rs::make_plan(bits).n_passes * 2.0 * 12.0 * (double)total;
+                cudaEventRecord(pe.b, c->stream);
+                c->pending.push_back(pe);
+            }
+            TRY(flatten(c, X, in_b ? X.keys_b.p : X.keys_a.p, in_b ? X.vals_b.p : X.vals_a.p, total, &block, &G, first));
+        }
+    }
+    // install: every contig's list is replaced (contigs appear in increasing order, so a contig's groups end at the next one's first)
+    RegionTable& t = c->known_sites;
+    for (auto p : t.d) if (p && t.separate(p)) cudaFree(p);
+    if (t.block) cudaFree(t.block);
+    t.d.assign(nc, nullptr); t.n.assign(nc, 0);
+    t.block = block; t.block_pairs = G;
+    uint64_t next = G;
+    for (int i = nc - 1; i >= 0; i--)
+        if (first[i] != ~0ull) { t.d[i] = block + 2 * first[i]; t.n[i] = next - first[i]; next = first[i]; }
+    t.dirty = true;
+    if (n_unmatched) *n_unmatched = unmatched;
+    return ELP_OK;
+}
+
+extern "C" int64_t elp_known_sites_get(elp_ctx* c, int32_t contig, int32_t* se, uint64_t cap) {
+    if (!c) return -1;
+    cudaSetDevice(c->device);
+    if (contig < 0 || contig >= c->n_contigs) { c->fail(E_INVAL, "elp_known_sites_get: contig %d out of range", contig); return -1; }
+    const RegionTable& t = c->known_sites;
+    const uint64_t n = (int)t.d.size() == c->n_contigs ? t.n[contig] : 0;
+    const uint64_t k = std::min(n, cap);
+    if (se && k) {
+        if (cudaMemcpyAsync(se, t.d[contig], k * 8, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) {
+            c->fail(E_CUDA, "elp_known_sites_get: %s", cudaGetErrorString(cudaGetLastError()));
+            return -1;
+        }
+    }
+    return (int64_t)n;
+}
+
+extern "C" int elp_debug_set_sites_chunk(elp_ctx* c, uint64_t bytes) {
+    if (!c) return ELP_EINVAL;
+    if (bytes > (1ull << 32)) return c->fail(E_INVAL, "elp_debug_set_sites_chunk: %llu bytes (at most 2^32)", (unsigned long long)bytes);
+    c->sites_chunk = bytes;   // the staging is reallocated by the next load
+    return ELP_OK;
+}

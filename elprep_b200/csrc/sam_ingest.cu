@@ -13,8 +13,8 @@
 #include <cmath>
 #include <cstdlib>
 #include <locale.h>
-#include <map>
 #include "ctx.h"
+#include "text_parse.cuh"
 #include "../../include/elprep_b200.h"
 
 struct SlowF { uint64_t text_off, out_off; uint32_t len, line; };   // one float value host-rounded: text, position in bam_raw, line
@@ -23,7 +23,7 @@ struct SamState {
     DBuf<uint8_t> text; DBuf<uint32_t> cnt, len; DBuf<uint64_t> cnt_off, ls;
     DBuf<SlowF> slow; DBuf<uint64_t> patch_off; DBuf<uint32_t> patch_bits;
     DBuf<uint8_t> lost;                       // per line: 1 if its RNAME / RNEXT text is lost in the record (see parse_line)
-    uint8_t* d_names = nullptr; uint32_t* d_name_off = nullptr; int32_t* d_name_id = nullptr; int n_names = 0;
+    NameDict dict;                            // RNAME / RNEXT dictionary (text_parse.cuh)
     unsigned long long* d_small = nullptr;   // [0] first error (line << 8 | SamErr), [1] floats handed to the host, [2] lines with a lost name
     uint64_t h_last = 0;                      // source of the virtual line end of a final line without '\n'
 };
@@ -33,8 +33,8 @@ void sam_state_release(elp_ctx* c) {
     if (!S) return;
     S->text.release(); S->cnt.release(); S->len.release(); S->cnt_off.release(); S->ls.release();
     S->slow.release(); S->patch_off.release(); S->patch_bits.release(); S->lost.release();
-    void* singles[] = {S->d_names, S->d_name_off, S->d_name_id, S->d_small};
-    for (void* p : singles) if (p) cudaFree(p);
+    name_dict_release(S->dict);
+    if (S->d_small) cudaFree(S->d_small);
     delete S;
     c->sam = nullptr;
 }
@@ -48,8 +48,6 @@ template <class T> int grow(elp_ctx* c, DBuf<T>& b, size_t need, size_t keep) {
     return E_OK;
 }
 #define TRY(x) do { int rc__ = (x); if (rc__) return rc__; } while (0)
-
-constexpr int SAM_CHUNK = 64;   // text bytes per thread of the line finder
 
 // which field of the line failed; the smallest (line << 8 | code) of a call is reported
 enum SamErr : uint32_t {
@@ -84,39 +82,10 @@ const char* sam_err_text(uint32_t e) {
     }
 }
 
-// ---- line finder ----
-__device__ __forceinline__ uint32_t nl_mask(uint32_t w) { return __vcmpeq4(w, 0x0a0a0a0au); }   // 0xff in every '\n' byte
-
-__global__ void __launch_bounds__(256) sam_count_kernel(const uint8_t* __restrict__ t, uint64_t n_chunks, uint32_t* __restrict__ cnt) {
-    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n_chunks) return;
-    const uint4* q = reinterpret_cast<const uint4*>(t + i * SAM_CHUNK);
-    uint32_t k = 0;
-#pragma unroll
-    for (int j = 0; j < SAM_CHUNK / 16; j++) { const uint4 v = q[j]; k += __popc(nl_mask(v.x)) + __popc(nl_mask(v.y)) + __popc(nl_mask(v.z)) + __popc(nl_mask(v.w)); }
-    cnt[i] = k >> 3;
-}
-// ls[j + 1] = the byte after the j-th '\n'
-__global__ void __launch_bounds__(256) sam_lines_kernel(const uint8_t* __restrict__ t, uint64_t n_chunks, const uint64_t* __restrict__ off, uint64_t* __restrict__ ls) {
-    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n_chunks) return;
-    const uint4* q = reinterpret_cast<const uint4*>(t + i * SAM_CHUNK);
-    uint64_t o = off[i] + 1;
-#pragma unroll
-    for (int j = 0; j < SAM_CHUNK / 16; j++) {
-        const uint4 v = q[j];
-        const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-        for (int h = 0; h < 4; h++)
-            for (uint32_t m = nl_mask(w[h]) & 0x01010101u; m; m &= m - 1)
-                ls[o++] = i * SAM_CHUNK + 16 * j + 4 * h + ((__ffs(m) - 1) >> 3) + 1;
-    }
-}
-
 // ---- the line parser ----
 struct SamArgs {
     const uint8_t* text; const uint64_t* ls; uint64_t n_lines;
-    const uint8_t* names; const uint32_t* name_off; const int32_t* name_id; int n_names;   // "*" and @SQ SN, sorted, with their refid
+    NameDict dict;             // "*" and @SQ SN, sorted, with their refid
     uint32_t* len;             // measure: BAM record length per line
     uint8_t* lost;             // measure: 1 if the record loses the line's RNAME / RNEXT text
     const uint64_t* rec_off;   // emit: record offsets in out
@@ -132,23 +101,6 @@ __device__ __forceinline__ uint64_t next_tab(const uint8_t* p, uint64_t from, ui
         if (m) return b + __ffs(m) - 1;
     }
     return n;
-}
-
-// strconv.ParseInt (sgn) / ParseUint (!sgn), base 10, accepted only inside [lo, hi] (every range used here lies in [-2^31, 2^32-1])
-__device__ bool parse_dec(const uint8_t* p, uint64_t n, bool sgn, int64_t lo, int64_t hi, int64_t* v) {
-    uint64_t i = 0; bool neg = false;
-    if (sgn && n && (p[0] == '+' || p[0] == '-')) { neg = p[0] == '-'; i = 1; }
-    if (i >= n) return false;
-    uint64_t m = 0;
-    for (; i < n; i++) {
-        const uint32_t d = (uint32_t)p[i] - '0';
-        if (d > 9) return false;
-        if (m < (1ull << 40)) m = m * 10 + d;   // saturates far above any accepted range
-    }
-    const int64_t x = neg ? -(int64_t)m : (int64_t)m;
-    if (x < lo || x > hi) return false;
-    *v = x;
-    return true;
 }
 
 __device__ __forceinline__ bool ieq(const uint8_t* p, const char* s, int n) { for (int i = 0; i < n; i++) if ((p[i] | 0x20) != (uint8_t)s[i]) return false; return true; }
@@ -193,22 +145,6 @@ __device__ int parse_f32(const uint8_t* p, uint64_t n, uint32_t* bits) {
     f = e10 >= 0 ? __fmul_rn(f, pw) : __fdiv_rn(f, pw);
     *bits = __float_as_uint(neg ? -f : f);
     return 1;
-}
-
-// dictTable of formatBamAlignment / AddREFID: "*" -> -1, @SQ SN -> index (the last of equal names wins), anything else -> -1
-__device__ int32_t refid_of(const SamArgs& A, const uint8_t* s, uint64_t n) {
-    int lo = 0, hi = A.n_names - 1;
-    while (lo <= hi) {
-        const int mid = (lo + hi) >> 1;
-        const uint8_t* q = A.names + A.name_off[mid];
-        const uint64_t qn = A.name_off[mid + 1] - A.name_off[mid];
-        int cmp = 0;
-        for (uint64_t j = 0; j < qn && j < n && !cmp; j++) cmp = (int)q[j] - (int)s[j];
-        if (!cmp) cmp = qn < n ? -1 : (qn > n ? 1 : 0);
-        if (!cmp) return A.name_id[mid];
-        if (cmp < 0) lo = mid + 1; else hi = mid - 1;
-    }
-    return -1;
 }
 
 __device__ __forceinline__ int cigar_code(uint8_t ch) {   // "MmIiDdNnSsHhPpXx=" -> BAM op (sam/sam-types.go:661-670)
@@ -324,9 +260,9 @@ template <bool W> __device__ int parse_line(const SamArgs& A, uint64_t k, const 
     if (!parse_dec(p + e[3] + 1, e[4] - e[3] - 1, false, 0, 255, &mapq)) return SE_MAPQ;
     if (!parse_dec(p + e[6] + 1, e[7] - e[6] - 1, true, INT32_MIN, INT32_MAX, &pnext)) return SE_PNEXT;
     if (!parse_dec(p + e[7] + 1, e[8] - e[7] - 1, true, INT32_MIN, INT32_MAX, &tlen)) return SE_TLEN;
-    const int32_t refid = refid_of(A, p + e[1] + 1, e[2] - e[1] - 1);
+    const int32_t refid = refid_of(A.dict, p + e[1] + 1, e[2] - e[1] - 1);
     const bool rnext_eq = e[6] - e[5] - 1 == 1 && p[e[5] + 1] == '=';
-    const int32_t nref = rnext_eq ? refid : refid_of(A, p + e[5] + 1, e[6] - e[5] - 1);
+    const int32_t nref = rnext_eq ? refid : refid_of(A.dict, p + e[5] + 1, e[6] - e[5] - 1);
     // names the record cannot give back to elp_fetch_sam: an RNAME that is neither "*" nor an @SQ name, likewise an RNEXT other than
     // "=", and RNEXT "=" with an RNAME that resolves to -1 ("*" included; the reference's SAM -> SAM text keeps the '=')
     const bool rname_star = e[2] - e[1] - 1 == 1 && p[e[1] + 1] == '*', rnext_star = e[6] - e[5] - 1 == 1 && p[e[5] + 1] == '*';
@@ -450,23 +386,12 @@ __global__ void __launch_bounds__(256) sam_fpatch_kernel(uint64_t n, const uint6
     if (i < n) for (int b = 0; b < 4; b++) out[off[i] + b] = (uint8_t)(bits[i] >> (8 * b));
 }
 
-// the RNAME / RNEXT dictionary, uploaded once per context
+// the RNAME / RNEXT dictionary and the error words, uploaded once per context
 int sam_tables(elp_ctx* c) {
     if (c->sam && c->sam->d_small) return E_OK;
     if (!c->sam) c->sam = new SamState();
     SamState& S = *c->sam;
-    std::map<std::string, int32_t> dict;
-    dict["*"] = -1;
-    for (int i = 0; i < c->n_contigs; i++) dict[c->contig_names[i]] = i;
-    std::vector<uint8_t> names; std::vector<uint32_t> off(1, 0); std::vector<int32_t> id;
-    for (auto& kv : dict) { names.insert(names.end(), kv.first.begin(), kv.first.end()); off.push_back((uint32_t)names.size()); id.push_back(kv.second); }
-    CUDA_TRY(c, cudaMalloc(&S.d_names, std::max<size_t>(names.size(), 1)));
-    CUDA_TRY(c, cudaMalloc(&S.d_name_off, off.size() * 4));
-    CUDA_TRY(c, cudaMalloc(&S.d_name_id, id.size() * 4));
-    CUDA_TRY(c, cudaMemcpy(S.d_names, names.data(), names.size(), cudaMemcpyHostToDevice));
-    CUDA_TRY(c, cudaMemcpy(S.d_name_off, off.data(), off.size() * 4, cudaMemcpyHostToDevice));
-    CUDA_TRY(c, cudaMemcpy(S.d_name_id, id.data(), id.size() * 4, cudaMemcpyHostToDevice));
-    S.n_names = (int)id.size();
+    TRY(name_dict_upload(c, S.dict));
     CUDA_TRY(c, cudaMalloc(&S.d_small, 24));
     return E_OK;
 }
@@ -520,7 +445,7 @@ extern "C" int elp_append_sam(elp_ctx* c, const char* text, uint64_t n_bytes) {
     // measure: validate every line and size its record
     SamArgs A{};
     A.text = S.text.p; A.ls = S.ls.p; A.n_lines = nl;
-    A.names = S.d_names; A.name_off = S.d_name_off; A.name_id = S.d_name_id; A.n_names = S.n_names;
+    A.dict = S.dict;
     A.len = S.len.p; A.lost = S.lost.p; A.rec_off = c->bam_off.p; A.small = S.d_small;
     CUDA_TRY(c, cudaMemsetAsync(S.d_small, 0xff, 8, s)); CUDA_TRY(c, cudaMemsetAsync(S.d_small + 1, 0, 16, s));
     c->begin("sam_measure", (double)n_bytes);

@@ -3,6 +3,7 @@ method is one C call; errors surface as ``ElprepError`` carrying the reference's
 from __future__ import annotations
 
 import ctypes as C
+import os
 
 import numpy as np
 
@@ -75,6 +76,27 @@ class Context:
     def set_known_sites(self, contig, start_end, already_flat=True):
         se = np.ascontiguousarray(start_end, dtype=np.int32).reshape(-1)
         self._ck(self.L.elp_set_known_sites(self.h, contig, _vp(se) if se.size else None, se.size // 2, int(already_flat)))
+
+    def load_known_sites(self, paths):
+        """--known-sites: .elsites files parsed, sorted and flattened on the device into every contig's list -> lines on chromosomes
+        that are no @SQ SN"""
+        arr = _cstrs([os.fspath(p) for p in paths])
+        nu = C.c_uint64()
+        self._ck(self.L.elp_load_known_sites(self.h, arr, len(paths), C.byref(nu)))
+        return int(nu.value)
+
+    def known_sites(self, contig):
+        """one contig's known sites as the gather uses them -> (k, 2) int32"""
+        k = self.L.elp_known_sites_get(self.h, contig, None, 0)
+        if k < 0:
+            raise ElprepError(-1, (self.L.elp_last_error(self.h) or b"").decode())
+        out = np.zeros((k, 2), np.int32)
+        if k and self.L.elp_known_sites_get(self.h, contig, _vp(out), k) != k:
+            raise ElprepError(-1, (self.L.elp_last_error(self.h) or b"").decode())
+        return out
+
+    def debug_set_sites_chunk(self, nbytes):
+        self._ck(self.L.elp_debug_set_sites_chunk(self.h, nbytes))
 
     # ---- phases ----
     def reserve(self, n_reads, n_bases, n_cigar, n_qname):

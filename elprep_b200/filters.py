@@ -29,6 +29,8 @@ exactly where the reference sorts (``sam/filter-pipeline.go:113-117``).  Failure
 """
 from __future__ import annotations
 
+import os
+
 import numpy as np
 
 from . import device, sam
@@ -330,23 +332,32 @@ class BaseRecalibrator:
     """filters.BaseRecalibrator (filters/bqsr.go:417-443): known sites + reference."""
 
     def __init__(self, known_sites, reference):
-        self.known_sites, self.reference = known_sites, reference   # per contig: (k,2) int32 intervals; uint8 bases
+        self.known_sites, self.reference = known_sites, reference   # per contig: (k,2) int32 intervals, or .elsites paths; uint8 bases
+
+    def _sites_are_files(self):
+        ks = self.known_sites
+        return bool(ks) and all(isinstance(p, (str, bytes, os.PathLike)) for p in ks)
 
     def Recalibrate(self, reads, maxCycle):
         """(*BaseRecalibrator).Recalibrate (filters/bqsr.go:467-551) -> *BaseRecalibratorTables"""
         ctx = reads.ctx
         if ctx.max_cycle != maxCycle:
             raise ValueError("maxCycle differs from the context's --max-cycle")
+        files = self._sites_are_files()
+        if files:
+            ctx.load_known_sites(list(self.known_sites))
         for ci in range(len(reads.Header.SQ)):
             ctx.set_reference(ci, self.reference[ci])
-            ctx.set_known_sites(ci, self.known_sites[ci] if self.known_sites else np.zeros((0, 2), np.int32), already_flat=False)
+            if not files:
+                ctx.set_known_sites(ci, self.known_sites[ci] if self.known_sites else np.zeros((0, 2), np.int32), already_flat=False)
         ctx.bqsr_gather()
         return BaseRecalibratorTables(reads)
 
 
 def NewBaseRecalibrator(knownSites, referenceFasta):
     """filters.NewBaseRecalibrator (filters/bqsr.go:424-443). knownSites: per-contig interval arrays (sorted+flattened
-    inside, as intervals.ParallelSortByStart/ParallelFlatten do); referenceFasta: per-contig base arrays (fasta.Seq)."""
+    inside, as intervals.ParallelSortByStart/ParallelFlatten do), or a list of .elsites paths like the reference's []string
+    (loaded on the device by Context.load_known_sites); referenceFasta: per-contig base arrays (fasta.Seq)."""
     return BaseRecalibrator(knownSites, referenceFasta)
 
 

@@ -386,6 +386,23 @@ func (d *DeviceSam) SetKnownSites(contig int, startEnd []int32) {
 	check(d.ctx, C.elp_set_known_sites(d.ctx, C.int32_t(contig), p, C.uint64_t(len(startEnd)/2), 0))
 }
 
+// LoadKnownSites: --known-sites as the reference takes it (cmd/filter.go:459,530-538), a list of .elsites files, parsed, sorted and
+// flattened on the device into every contig's list.  Returns the lines whose chromosome is no @SQ SN.
+func (d *DeviceSam) LoadKnownSites(paths []string) uint64 {
+	cs := make([]*C.char, len(paths)+1)
+	for i, p := range paths {
+		cs[i] = C.CString(p)
+	}
+	defer func() {
+		for _, c := range cs[:len(paths)] {
+			C.free(unsafe.Pointer(c))
+		}
+	}()
+	var unmatched C.uint64_t
+	check(d.ctx, C.elp_load_known_sites(d.ctx, (**C.char)(unsafe.Pointer(&cs[0])), C.int32_t(len(paths)), &unmatched))
+	return uint64(unmatched)
+}
+
 // Recalibrate: (*BaseRecalibrator).Recalibrate (bqsr.go:467-551).  The tables stay on the device.
 // --target-regions: RemoveNonOverlappingReads(bedRegions) over the marked reads, before Recalibrate (cmd/filter.go:171-180, 288-296).
 // SetTargetRegions takes one contig's BED Start / End pairs (sorted and flattened inside); FilterTargetRegions returns the reads dropped.

@@ -38,6 +38,7 @@ extern "C" {
 #define ELP_EBAM (-18)       /* malformed BAM alignment record, or an RG:Z value that is not an @RG ID */
 #define ELP_EBGZF (-19)      /* malformed BGZF block (header, BC subfield, CRC32 or ISIZE), utils/bgzf/bgzf-files.go:95-127 */
 #define ELP_ESAM (-20)       /* malformed SAM alignment line; elp_last_error names the line (0-based, within the call) and the field */
+#define ELP_ESITES (-21)     /* malformed .elsites file; elp_last_error names the file (index in paths), the line (0-based, header = line 0) and the reason */
 
 /* sam.SortingOrder (sam/sam-types.go:40-58) */
 #define ELP_SO_KEEP 0
@@ -111,6 +112,32 @@ int elp_reset(elp_ctx *ctx);
  * of NewBaseRecalibrator (filters/bqsr.go:424-443). start/end pairs; flattened inside unless already_flat. ---- */
 int elp_set_reference(elp_ctx *ctx, int32_t contig, const uint8_t *bases, uint64_t n);
 int elp_set_known_sites(elp_ctx *ctx, int32_t contig, const int32_t *start_end_pairs, uint64_t n_intervals, int already_flat);
+/* --known-sites a.elsites,b.elsites (cmd/filter.go:459,530-538): NewBaseRecalibrator's loop over the files (filters/bqsr.go:424-443)
+ * with intervals.FromElsitesFile (intervals/intervals.go:199-254), then ParallelSortByStart + ParallelFlatten per contig, all on the
+ * device.  Replaces the known-sites list of EVERY contig (a contig without sites gets an empty list); n_paths == 0 clears them all.
+ *  - Header: each file starts with exactly "# elsites format version 1.0\n" (ReadString('\n'), intervals.go:204-210); a "\r\n" header,
+ *    a missing header and an empty file are ELP_ESITES at line 0.
+ *  - Lines follow bufio.ScanLines: they end at '\n', one '\r' before it is dropped, the last line may lack its '\n'; an empty segment
+ *    after the last '\n' is no line.  A line is CHROM '\t' START '\t' END (intervals.go:221-247): CHROM is everything before the first
+ *    tab (empty, or no tab at all, is invalid, and so is a missing second tab; an empty line is invalid); START and END go through
+ *    strconv.ParseInt(s, 10, 32) (an optional sign, decimal digits, inside int32; "+5", "-0" and "007" are accepted).  A line of 65536
+ *    bytes or more (before its '\n') is ELP_ESITES: bufio.Scanner's default token limit stops the reference's scanner there (the pargo
+ *    scanner is not part of the reference tree; this assumes it keeps bufio's default buffer).  Lines on unknown chromosomes are
+ *    validated as well.  Any rejected line fails the whole call; the smallest (file, line) is reported.
+ *  - CHROM resolves against elp_config.contig_names byte for byte; a context with @SQ lines created without names is ELP_EINVAL.  A line
+ *    whose CHROM is "*" or no @SQ SN counts in *n_unmatched (may be NULL; the reference keeps such intervals but never looks them up).
+ *    When several @SQ lines share one SN, each of those contigs gets the line's interval (the gather looks sites up by RNAME, bqsr.go:496).
+ *  - Each contig's list equals what elp_set_known_sites(already_flat = 0) makes of the same intervals: a stable sort by start, then the
+ *    serial Flatten (also where ParallelFlatten would panic, see DESIGN.md).
+ *  - A missing or unreadable file is ELP_EINVAL (the message names the path); 2^30 or more intervals in total are ELP_ELIMIT.
+ *  - Atomic: on any error the previous table is unchanged.  The table survives elp_reset; elp_set_known_sites afterwards replaces one
+ *    contig's list, and the two calls mix in either order. */
+int elp_load_known_sites(elp_ctx *ctx, const char *const *paths, int32_t n_paths, uint64_t *n_unmatched);
+/* one contig's known sites as the gather uses them: writes up to cap (start, end) pairs and returns the number of pairs (-1 on error);
+ * start_end_pairs may be NULL to ask for the count */
+int64_t elp_known_sites_get(elp_ctx *ctx, int32_t contig, int32_t *start_end_pairs, uint64_t cap);
+/* tests: bytes of the page-locked staging chunks the files are streamed through (0: the default, 32 MiB) */
+int elp_debug_set_sites_chunk(elp_ctx *ctx, uint64_t bytes);
 
 /* ---- phase 1: (*sam.Sam).AddNodes receiving batches (sam/filter-pipeline.go:108-128) ---- */
 int elp_append_batch(elp_ctx *ctx, const elp_batch *batch);

@@ -154,6 +154,15 @@ class DeviceSam {
 
     void SetReference(int contig, const std::string& bases) { check(elp_set_reference(ctx_, contig, reinterpret_cast<const uint8_t*>(bases.data()), bases.size())); }
     void SetKnownSites(int contig, const std::vector<int32_t>& startEnd) { check(elp_set_known_sites(ctx_, contig, startEnd.empty() ? nullptr : startEnd.data(), startEnd.size() / 2, 0)); }
+    // --known-sites a.elsites,b.elsites: every file parsed, sorted and flattened on the device into every contig's list; returns the
+    // lines whose chromosome is no @SQ SN
+    uint64_t LoadKnownSites(const std::vector<std::string>& paths) {
+        std::vector<const char*> p;
+        for (const auto& s : paths) p.push_back(s.c_str());
+        uint64_t unmatched = 0;
+        check(elp_load_known_sites(ctx_, p.empty() ? nullptr : p.data(), (int32_t)p.size(), &unmatched));
+        return unmatched;
+    }
     // `--target-regions`: RemoveNonOverlappingReads(bedRegions) after marking, before Recalibrate (cmd/filter.go:171-180, 288-296); one
     // contig's BED Start / End pairs per call, sorted and flattened inside.  FilterTargetRegions returns the number of reads dropped.
     void SetTargetRegions(int contig, const std::vector<int32_t>& startEnd) { check(elp_set_bqsr_target_regions(ctx_, contig, startEnd.empty() ? nullptr : startEnd.data(), startEnd.size() / 2, 0)); }
