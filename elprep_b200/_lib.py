@@ -12,7 +12,7 @@ SO_PATH = os.environ.get("ELPREP_B200_LIB", os.path.join(_HERE, "lib", "libelpre
 
 SO_KEEP, SO_UNKNOWN, SO_UNSORTED, SO_QUERYNAME, SO_COORDINATE = 0, 1, 2, 3, 4
 MARKDUP, MARKDUP_OPTICAL = 1, 2
-EINVAL, ELIMIT, ESTATE, EBAM, EBGZF, ESAM, ESITES = -1, -15, -16, -18, -19, -20, -21
+EINVAL, EREFEND, ELIMIT, ESTATE, EBAM, EBGZF, ESAM, ESITES, EFASTA = -1, -14, -15, -16, -18, -19, -20, -21, -22
 FILTER_UNMAPPED, FILTER_UNMAPPED_STRICT, FILTER_NON_EXACT, FILTER_DUPLICATES, FILTER_NON_EXACT_STRICT, FILTER_TARGET_REGIONS = 1, 2, 4, 8, 16, 32
 FILTER_CLEAR_DUPLICATE_FLAG = 64
 OUT_REMOVE_DUPLICATES, OUT_REMOVE_OPTIONAL_READS, OUT_KEEP_FIELDS = 1, 2, 4
@@ -51,7 +51,8 @@ EXPORTS = ["elp_create", "elp_destroy", "elp_last_error", "elp_reserve", "elp_re
            "elp_print_duplicates_metrics",
            "elp_bgzf_inflate_bound", "elp_bgzf_inflate", "elp_bgzf_deflate_bound", "elp_bgzf_deflate", "elp_bam_header_size",
            "elp_append_bgzf", "elp_append_bgzf_end", "elp_debug_inflate", "elp_fetch_bgzf", "elp_debug_deflate",
-           "elp_load_known_sites", "elp_known_sites_get", "elp_debug_set_sites_chunk"]
+           "elp_load_known_sites", "elp_known_sites_get", "elp_debug_set_sites_chunk",
+           "elp_load_reference", "elp_reference_get", "elp_debug_set_reference_chunk"]
 
 _lib = None
 
@@ -89,6 +90,10 @@ def load():
     L.elp_known_sites_get.restype = C.c_int64
     L.elp_known_sites_get.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_uint64]
     L.elp_debug_set_sites_chunk.argtypes = [C.c_void_p, C.c_uint64]
+    L.elp_load_reference.argtypes = [C.c_void_p, C.c_char_p, C.POINTER(C.c_uint64), C.POINTER(C.c_int32)]
+    L.elp_reference_get.restype = C.c_int64
+    L.elp_reference_get.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_uint64]
+    L.elp_debug_set_reference_chunk.argtypes = [C.c_void_p, C.c_uint64]
     L.elp_append_batch.argtypes = [C.c_void_p, C.POINTER(ElpBatch)]
     for f in ("elp_bqsr_tables_write_elrecal", "elp_bqsr_tables_add_elrecal", "elp_optical_write_gob", "elp_optical_add_gob"):
         getattr(L, f).argtypes = [C.c_void_p, C.c_char_p]

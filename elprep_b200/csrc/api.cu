@@ -194,7 +194,8 @@ void elp_destroy(elp_ctx* c) {
     sam_out_release(c);
     bgzf_release(c);
     bgzf_deflate_release(c);
-    for (auto p : c->d_refhot_raw) if (p) cudaFree(p);
+    for (auto p : c->d_refhot_raw) if (p && c->refhot_separate(p)) cudaFree(p);
+    if (c->refhot_block) cudaFree(c->refhot_block);
     region_release(c->regions); region_release(c->bqsr_regions); region_release(c->known_sites);
     void* singles[] = {c->d_rg_lib, c->d_rg_cov, c->d_contig_len, c->d_ranges, c->d_err, (void*)c->d_refhot_ptrs, c->d_bq_small, c->d_qpresent, c->d_ref_len, c->d_tables,
                        c->d_lut, c->d_clut, c->d_rowtab, c->d_cov_exists, c->d_unobs, c->d_emp, c->d_fin, c->d_qmaps, c->d_opt_ctr, c->d_opt_hist, c->d_opt_ovf, c->d_opt_small, c->d_rg_names, c->d_rg_name_off, c->d_out_drop, c->ws.ghist, c->ws.gofs, c->ws.counters, c->ws.status};

@@ -230,6 +230,11 @@ static int inflate_blocks(elp_ctx* c, const char* who, const std::vector<std::pa
     return E_OK;
 }
 
+int bgzf_inflate_run(elp_ctx* c, const char* who, const uint8_t* in, uint64_t n_in, const std::vector<BgzfBlock>& blocks, uint64_t total, uint8_t* out) {
+    TRY(bgzf_state(c));
+    return inflate_blocks(c, who, {{in, n_in}}, blocks, total, out);
+}
+
 // the reference list of a complete header at bam_raw[0, hdr) against elp_config: n_ref, every l_ref and (when given) every name
 static int check_header(elp_ctx* c, uint64_t ref_at, uint64_t hdr) {
     std::vector<uint8_t> h(hdr - ref_at);

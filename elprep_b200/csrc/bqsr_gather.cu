@@ -19,6 +19,7 @@
 #include "ctx.h"
 #include "bqsr_simd.cuh"
 #include "bqsr_lane.cuh"
+#include "refhot.cuh"
 
 namespace {
 
@@ -777,9 +778,10 @@ __global__ void derive_q_kernel(TableGeom geom, long long* tables) {
 // (windows of reads at the start of a contig and the shifted window of an insertion start before base 0), 64 behind (the aligned
 // window loads past the last base). The n host bases pass through a temporary device buffer that is freed before the return; the copy
 // goes on the context's stream, since a pageable cudaMemcpy may return before its DMA has landed and the stream does not wait for it.
+// A contig that elp_load_reference installed lives inside refhot_block: its old buffer is not freed here.
 int pack_reference(elp_ctx* c, int contig, const uint8_t* bases) {
     const uint64_t n = c->ref_len[contig], n_out = (n + 1) / 2;
-    if (c->d_refhot_raw[contig]) { cudaFree(c->d_refhot_raw[contig]); c->d_refhot_raw[contig] = nullptr; }
+    if (c->d_refhot_raw[contig]) { if (c->refhot_separate(c->d_refhot_raw[contig])) cudaFree(c->d_refhot_raw[contig]); c->d_refhot_raw[contig] = nullptr; }
     CUDA_TRY(c, cudaMalloc(&c->d_refhot_raw[contig], n_out + REFHOT_PAD + 64));
     CUDA_TRY(c, cudaMemsetAsync(c->d_refhot_raw[contig], 0, n_out + REFHOT_PAD + 64, c->stream));
     uint8_t* d_bases = nullptr;

@@ -92,6 +92,9 @@ struct elp_ctx {
     // ---- reference genome + known sites (device) ----
     std::vector<uint64_t> ref_len;
     std::vector<uint8_t*> d_refhot_raw;   // per contig: the reference as one-hot nibbles (bqsr_gather.cu pack_reference), payload at +REFHOT_PAD
+    uint8_t* refhot_block = nullptr; uint64_t refhot_block_bytes = 0;   // elp_load_reference installs every contig in this one allocation
+    bool refhot_separate(const uint8_t* p) const { return !refhot_block || p < refhot_block || p >= refhot_block + refhot_block_bytes; }
+    uint64_t ref_chunk = 0;                  // elp_debug_set_reference_chunk: bytes per staging chunk of elp_load_reference (0: the default)
     const uint8_t** d_refhot_ptrs = nullptr;   // [n_contigs] device array of the payload pointers
     uint64_t* d_ref_len = nullptr;
     bool side_dirty = true;
@@ -285,5 +288,7 @@ void sites_release(elp_ctx* c);       // known_sites.cu
 void sam_out_release(elp_ctx* c);     // sam_format.cu
 void bgzf_stream_reset(elp_ctx* c);   // bgzf_inflate.cu: forget the open file (elp_reset)
 void bgzf_release(elp_ctx* c);
+struct BgzfBlock;
+int bgzf_inflate_run(elp_ctx* c, const char* who, const uint8_t* in, uint64_t n_in, const std::vector<BgzfBlock>& blocks, uint64_t total, uint8_t* out);   // bgzf_inflate.cu: whole blocks -> out
 int bgzf_deflate_run(elp_ctx* c, const uint8_t* in, uint64_t n, int write_eof, uint8_t* out, uint64_t* out_n);   // bgzf_deflate.cu: in[0, n) on the device -> BGZF at out
 void bgzf_deflate_release(elp_ctx* c);

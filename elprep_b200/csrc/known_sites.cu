@@ -20,6 +20,7 @@
 #include <vector>
 #include "ctx.h"
 #include "text_parse.cuh"
+#include "file_stage.cuh"
 #include "../../include/elprep_b200.h"
 
 namespace {
@@ -33,12 +34,7 @@ constexpr uint64_t SITES_CHUNK_DEFAULT = 32ull << 20;
 
 // page-locked and device staging, reused by every call on the context
 struct SitesStage {
-    uint64_t chunk = 0;                                          // file bytes per step; a carried partial line sits in front of them
-    uint8_t* h[2] = {nullptr, nullptr};                          // page-locked
-    uint8_t* d[2] = {nullptr, nullptr};
-    cudaEvent_t up[2] = {nullptr, nullptr};                      // the upload out of h[b] has landed in d[b] (copy stream)
-    cudaEvent_t used[2] = {nullptr, nullptr};                    // the kernels that read d[b] are done (compute stream)
-    cudaStream_t copy = nullptr;
+    FileStage f;                                                 // the two chunks (file_stage.cuh); a carried partial line sits in front of the file bytes
     unsigned long long* d_small = nullptr;                       // [0] first error (line << 8 | SitesErr), [1] unmatched lines
     unsigned long long* h_small = nullptr;                       // page-locked: [0, 1] copies, [2] '\n' count, [3] intervals, [4] virtual line end
     NameDict dict; bool dict_ok = false;
@@ -47,14 +43,7 @@ struct SitesStage {
 void sites_release(elp_ctx* c) {
     SitesStage* S = c->sites;
     if (!S) return;
-    if (S->copy) cudaStreamSynchronize(S->copy);
-    for (int b = 0; b < 2; b++) {
-        if (S->h[b]) cudaFreeHost(S->h[b]);
-        if (S->d[b]) cudaFree(S->d[b]);
-        if (S->up[b]) cudaEventDestroy(S->up[b]);
-        if (S->used[b]) cudaEventDestroy(S->used[b]);
-    }
-    if (S->copy) cudaStreamDestroy(S->copy);
+    stage_release(S->f);
     if (S->d_small) cudaFree(S->d_small);
     if (S->h_small) cudaFreeHost(S->h_small);
     name_dict_release(S->dict);
@@ -279,75 +268,25 @@ struct SitesScratch {   // per call; freed on return
     }
 };
 
-struct Chunk { int b = 0; uint64_t m = 0; bool last = false, long_tail = false; };   // m: bytes of whole lines at the front of h[b]
-
-int stage_init(elp_ctx* c) {
+int sites_stage_init(elp_ctx* c) {
     if (!c->sites) c->sites = new SitesStage();
     SitesStage& S = *c->sites;
-    if (!S.copy) {
-        CUDA_TRY(c, cudaStreamCreateWithFlags(&S.copy, cudaStreamNonBlocking));
-        for (int b = 0; b < 2; b++) { CUDA_TRY(c, cudaEventCreateWithFlags(&S.up[b], cudaEventDisableTiming)); CUDA_TRY(c, cudaEventCreateWithFlags(&S.used[b], cudaEventDisableTiming)); }
-    }
+    const uint64_t want = c->sites_chunk ? c->sites_chunk : SITES_CHUNK_DEFAULT, cap = want + SITES_MAX_LINE;
+    TRY(stage_init(c, S.f, want, cap, stage_padded(cap), "elp_load_known_sites"));
     if (!S.d_small) { CUDA_TRY(c, cudaMalloc(&S.d_small, 16)); CUDA_TRY(c, cudaHostAlloc(&S.h_small, 64, cudaHostAllocDefault)); }
     if (!S.dict_ok) { TRY(name_dict_upload(c, S.dict)); S.dict_ok = true; }
-    const uint64_t want = c->sites_chunk ? c->sites_chunk : SITES_CHUNK_DEFAULT;
-    if (S.chunk != want) {
-        CUDA_TRY(c, cudaStreamSynchronize(S.copy));
-        for (int b = 0; b < 2; b++) {
-            if (S.h[b]) cudaFreeHost(S.h[b]);
-            if (S.d[b]) cudaFree(S.d[b]);
-            S.h[b] = S.d[b] = nullptr;
-        }
-        S.chunk = 0;
-        const uint64_t cap = want + SITES_MAX_LINE, dcap = (cap + SAM_CHUNK - 1) / SAM_CHUNK * SAM_CHUNK + SAM_CHUNK;
-        for (int b = 0; b < 2; b++) {
-            if (cudaHostAlloc(&S.h[b], cap, cudaHostAllocDefault) != cudaSuccess || cudaMalloc(&S.d[b], dcap) != cudaSuccess) {
-                cudaGetLastError();
-                return c->fail(E_NOMEM, "elp_load_known_sites: staging allocation of 2 x %llu bytes failed", (unsigned long long)cap);
-            }
-        }
-        S.chunk = want;
-    }
     return E_OK;
 }
 
-// the carried bytes and the next chunk of the file into h[b]
-int read_fill(elp_ctx* c, SitesStage& S, FILE* f, const char* path, std::vector<uint8_t>& carry, int b, Chunk* ch) {
-    CUDA_TRY(c, cudaEventSynchronize(S.up[b]));   // the last upload out of h[b] has read it
-    uint8_t* h = S.h[b];
-    const uint64_t nc = carry.size();
-    if (nc) memcpy(h, carry.data(), nc);
-    const size_t got = fread(h + nc, 1, S.chunk, f);
-    if (got < S.chunk && ferror(f)) return c->fail(E_INVAL, "elp_load_known_sites: cannot read %s: %s", path, strerror(errno));
-    const uint64_t n = nc + got;
-    ch->b = b; ch->last = got < S.chunk;
-    if (ch->last) ch->m = n;   // the last line may lack its '\n'
-    else {
-        const void* q = got ? memrchr(h + nc, '\n', got) : nullptr;
-        ch->m = q ? (uint64_t)(static_cast<const uint8_t*>(q) - h) + 1 : 0;
-    }
-    carry.assign(h + ch->m, h + n);
-    ch->long_tail = !ch->last && carry.size() >= SITES_MAX_LINE;
-    return E_OK;
-}
-
-int upload(elp_ctx* c, SitesStage& S, const Chunk& ch) {
-    if (!ch.m) return E_OK;
-    const uint64_t padded = (ch.m + SAM_CHUNK - 1) / SAM_CHUNK * SAM_CHUNK + SAM_CHUNK;
-    CUDA_TRY(c, cudaStreamWaitEvent(S.copy, S.used[ch.b], 0));
-    CUDA_TRY(c, cudaMemcpyAsync(S.d[ch.b], S.h[ch.b], ch.m, cudaMemcpyHostToDevice, S.copy));
-    CUDA_TRY(c, cudaMemsetAsync(S.d[ch.b] + ch.m, 0, padded - ch.m, S.copy));
-    CUDA_TRY(c, cudaEventRecord(S.up[ch.b], S.copy));
-    return E_OK;
-}
+int upload(elp_ctx* c, SitesStage& S, const LineChunk& ch) { return stage_upload(c, S.f, ch.b, ch.m, 0); }
 
 // '\n' count of the chunk into h_small[2] (read after the next synchronisation)
-int count_lines(elp_ctx* c, SitesStage& S, SitesScratch& X, const Chunk& ch) {
+int count_lines(elp_ctx* c, SitesStage& S, SitesScratch& X, const LineChunk& ch) {
     const uint64_t n_chunks = (ch.m + SAM_CHUNK - 1) / SAM_CHUNK;
     TRY(grow(c, X.cnt, n_chunks + 8, 0)); TRY(grow(c, X.cnt_off, n_chunks + 2, 0));
-    CUDA_TRY(c, cudaStreamWaitEvent(c->stream, S.up[ch.b], 0));
+    CUDA_TRY(c, cudaStreamWaitEvent(c->stream, S.f.up[ch.b], 0));
     c->begin("sites_lines", (double)ch.m);
-    sam_count_kernel<<<nblk(n_chunks, 256), 256, 0, c->stream>>>(S.d[ch.b], n_chunks, X.cnt.p);
+    sam_count_kernel<<<nblk(n_chunks, 256), 256, 0, c->stream>>>(S.f.d[ch.b], n_chunks, X.cnt.p);
     c->end(); LAUNCH_CHECK(c);
     TRY(exclusive_scan_u32_to_u64(c, X.cnt.p, X.cnt_off.p, n_chunks));
     CUDA_TRY(c, cudaMemcpyAsync(S.h_small + 2, X.cnt_off.p + n_chunks, 8, cudaMemcpyDeviceToHost, c->stream));
@@ -355,21 +294,21 @@ int count_lines(elp_ctx* c, SitesStage& S, SitesScratch& X, const Chunk& ch) {
 }
 
 // the chunk's lines: line starts, parse and the scan of the interval counts are enqueued; *n_lines is the chunk's line count
-int parse_launch(elp_ctx* c, SitesStage& S, SitesScratch& X, const Chunk& ch, uint64_t line0, uint64_t* n_lines) {
+int parse_launch(elp_ctx* c, SitesStage& S, SitesScratch& X, const LineChunk& ch, uint64_t line0, uint64_t* n_lines) {
     cudaStream_t s = c->stream;
     CUDA_TRY(c, cudaStreamSynchronize(s));
     const uint64_t n_nl = S.h_small[2], n_chunks = (ch.m + SAM_CHUNK - 1) / SAM_CHUNK;
-    const bool open_end = S.h[ch.b][ch.m - 1] != '\n';
+    const bool open_end = S.f.h[ch.b][ch.m - 1] != '\n';
     const uint64_t nl = n_nl + (open_end ? 1 : 0);
     TRY(grow(c, X.ls, nl + 2, 0)); TRY(grow(c, X.ent, nl + 8, 0)); TRY(grow(c, X.start, nl + 8, 0)); TRY(grow(c, X.end, nl + 8, 0));
     TRY(grow(c, X.emit, nl + 8, 0)); TRY(grow(c, X.emit_off, nl + 2, 0));
     CUDA_TRY(c, cudaMemsetAsync(X.ls.p, 0, 8, s));
     c->begin("sites_lines", (double)ch.m + 8.0 * (double)n_nl);
-    sam_lines_kernel<<<nblk(n_chunks, 256), 256, 0, s>>>(S.d[ch.b], n_chunks, X.cnt_off.p, X.ls.p);
+    sam_lines_kernel<<<nblk(n_chunks, 256), 256, 0, s>>>(S.f.d[ch.b], n_chunks, X.cnt_off.p, X.ls.p);
     c->end(); LAUNCH_CHECK(c);
     if (open_end) { S.h_small[4] = ch.m + 1; CUDA_TRY(c, cudaMemcpyAsync(X.ls.p + nl, S.h_small + 4, 8, cudaMemcpyHostToDevice, s)); }   // a virtual '\n' past the text
     SitesArgs A{};
-    A.text = S.d[ch.b]; A.ls = X.ls.p; A.n_lines = nl; A.line0 = line0; A.dict = S.dict;
+    A.text = S.f.d[ch.b]; A.ls = X.ls.p; A.n_lines = nl; A.line0 = line0; A.dict = S.dict;
     A.ent = X.ent.p; A.start = X.start.p; A.end = X.end.p; A.emit = X.emit.p; A.small = S.d_small;
     c->begin("sites_parse", (double)ch.m + 8.0 * (double)(nl + 1) + 16.0 * (double)nl);
     sites_parse_kernel<<<nblk(nl, 256), 256, 0, s>>>(A);
@@ -382,7 +321,7 @@ int parse_launch(elp_ctx* c, SitesStage& S, SitesScratch& X, const Chunk& ch, ui
 }
 
 // the parse's verdict, then the chunk's intervals appended at keys_a / vals_a + *total
-int parse_finish(elp_ctx* c, SitesStage& S, SitesScratch& X, const Chunk& ch, int file, const char* path, uint64_t nl, uint64_t* total) {
+int parse_finish(elp_ctx* c, SitesStage& S, SitesScratch& X, const LineChunk& ch, int file, const char* path, uint64_t nl, uint64_t* total) {
     cudaStream_t s = c->stream;
     CUDA_TRY(c, cudaStreamSynchronize(s));
     if (S.h_small[0] != ~0ull)
@@ -394,7 +333,7 @@ int parse_finish(elp_ctx* c, SitesStage& S, SitesScratch& X, const Chunk& ch, in
     c->begin("sites_parse", 24.0 * (double)nl + 12.0 * (double)add);
     sites_emit_kernel<<<nblk(nl, 256), 256, 0, s>>>(nl, X.ent.p, X.start.p, X.end.p, X.emit.p, X.emit_off.p, S.dict, X.keys_a.p + t0, X.vals_a.p + t0);
     c->end(); LAUNCH_CHECK(c);
-    CUDA_TRY(c, cudaEventRecord(S.used[ch.b], s));
+    CUDA_TRY(c, cudaEventRecord(S.f.used[ch.b], s));
     *total = t0 + add;
     return E_OK;
 }
@@ -411,15 +350,15 @@ int load_file(elp_ctx* c, SitesStage& S, SitesScratch& X, int file, const char* 
         return c->fail(E_SITES, "elp_load_known_sites: %s (file %d), line 0 (0-based, header = line 0): not a .elsites file - the first line is not \"# elsites format version 1.0\"", path, file);
     std::vector<uint8_t> carry;
     uint64_t line0 = 1;
-    Chunk cur;
-    TRY(read_fill(c, S, f, path, carry, 0, &cur));
+    LineChunk cur;
+    TRY(stage_read_lines(c, S.f, f, path, "elp_load_known_sites", SITES_MAX_LINE, carry, 0, &cur));
     TRY(upload(c, S, cur));
     for (;;) {
         uint64_t nl = 0;
         if (cur.m) { TRY(count_lines(c, S, X, cur)); TRY(parse_launch(c, S, X, cur, line0, &nl)); }
         const bool more = !cur.last && !cur.long_tail;
-        Chunk nxt;
-        if (more) { TRY(read_fill(c, S, f, path, carry, cur.b ^ 1, &nxt)); TRY(upload(c, S, nxt)); }   // overlaps the kernels of cur
+        LineChunk nxt;
+        if (more) { TRY(stage_read_lines(c, S.f, f, path, "elp_load_known_sites", SITES_MAX_LINE, carry, cur.b ^ 1, &nxt)); TRY(upload(c, S, nxt)); }   // overlaps the kernels of cur
         if (cur.m) TRY(parse_finish(c, S, X, cur, file, path, nl, total));
         line0 += nl;
         if (cur.long_tail) return c->fail(E_SITES, "elp_load_known_sites: %s (file %d), line %llu (0-based, header = line 0): %s", path, file, (unsigned long long)line0, sites_err_text(KS_LONG));
@@ -481,9 +420,9 @@ extern "C" int elp_load_known_sites(elp_ctx* c, const char* const* paths, int32_
     int32_t* block = nullptr; uint64_t G = 0, unmatched = 0;
     std::vector<uint64_t> first(nc, ~0ull);
     if (n_paths) {
-        TRY(stage_init(c));
+        TRY(sites_stage_init(c));
         SitesStage& S = *c->sites;
-        struct Drain { cudaStream_t s; ~Drain() { cudaStreamSynchronize(s); } } drain{S.copy};   // no upload outlives the call
+        struct Drain { cudaStream_t s; ~Drain() { cudaStreamSynchronize(s); } } drain{S.f.copy};   // no upload outlives the call
         SitesScratch X;
         CUDA_TRY(c, cudaMemsetAsync(S.d_small, 0xff, 8, c->stream));
         CUDA_TRY(c, cudaMemsetAsync(S.d_small + 1, 0, 8, c->stream));

@@ -98,6 +98,26 @@ class Context:
     def debug_set_sites_chunk(self, nbytes):
         self._ck(self.L.elp_debug_set_sites_chunk(self.h, nbytes))
 
+    def load_reference(self, path):
+        """--reference: an .elfasta or a FASTA file (plain or BGZF) read and packed on the device into every contig's reference ->
+        (sequences whose name is no @SQ SN, contigs left without a sequence)"""
+        nu, nm = C.c_uint64(), C.c_int32()
+        self._ck(self.L.elp_load_reference(self.h, os.fsencode(path), C.byref(nu), C.byref(nm)))
+        return int(nu.value), int(nm.value)
+
+    def reference(self, contig):
+        """one contig's reference as the gather reads it -> (length in bases, uint8 one-hot nibbles, (length + 1) // 2 bytes)"""
+        n = self.L.elp_reference_get(self.h, contig, None, 0)
+        if n < 0:
+            raise ElprepError(-1, (self.L.elp_last_error(self.h) or b"").decode())
+        out = np.zeros((n + 1) // 2, np.uint8)
+        if out.size and self.L.elp_reference_get(self.h, contig, _vp(out), out.size) != n:
+            raise ElprepError(-1, (self.L.elp_last_error(self.h) or b"").decode())
+        return int(n), out
+
+    def debug_set_reference_chunk(self, nbytes):
+        self._ck(self.L.elp_debug_set_reference_chunk(self.h, nbytes))
+
     # ---- phases ----
     def reserve(self, n_reads, n_bases, n_cigar, n_qname):
         self._ck(self.L.elp_reserve(self.h, n_reads, n_bases, n_cigar, n_qname))

@@ -332,7 +332,7 @@ class BaseRecalibrator:
     """filters.BaseRecalibrator (filters/bqsr.go:417-443): known sites + reference."""
 
     def __init__(self, known_sites, reference):
-        self.known_sites, self.reference = known_sites, reference   # per contig: (k,2) int32 intervals, or .elsites paths; uint8 bases
+        self.known_sites, self.reference = known_sites, reference   # per contig: (k,2) int32 intervals, or .elsites paths; uint8 bases, or a path
 
     def _sites_are_files(self):
         ks = self.known_sites
@@ -346,8 +346,12 @@ class BaseRecalibrator:
         files = self._sites_are_files()
         if files:
             ctx.load_known_sites(list(self.known_sites))
+        ref_file = isinstance(self.reference, (str, bytes, os.PathLike))
+        if ref_file:
+            ctx.load_reference(self.reference)
         for ci in range(len(reads.Header.SQ)):
-            ctx.set_reference(ci, self.reference[ci])
+            if not ref_file:
+                ctx.set_reference(ci, self.reference[ci])
             if not files:
                 ctx.set_known_sites(ci, self.known_sites[ci] if self.known_sites else np.zeros((0, 2), np.int32), already_flat=False)
         ctx.bqsr_gather()
@@ -357,7 +361,8 @@ class BaseRecalibrator:
 def NewBaseRecalibrator(knownSites, referenceFasta):
     """filters.NewBaseRecalibrator (filters/bqsr.go:424-443). knownSites: per-contig interval arrays (sorted+flattened
     inside, as intervals.ParallelSortByStart/ParallelFlatten do), or a list of .elsites paths like the reference's []string
-    (loaded on the device by Context.load_known_sites); referenceFasta: per-contig base arrays (fasta.Seq)."""
+    (loaded on the device by Context.load_known_sites); referenceFasta: per-contig base arrays (fasta.Seq), or the path of an .elfasta or
+    FASTA file (plain or BGZF) like the reference's --reference (loaded on the device by Context.load_reference)."""
     return BaseRecalibrator(knownSites, referenceFasta)
 
 

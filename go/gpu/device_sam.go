@@ -403,6 +403,18 @@ func (d *DeviceSam) LoadKnownSites(paths []string) uint64 {
 	return uint64(unmatched)
 }
 
+// LoadReference: --reference as the reference takes it (an .elfasta, fasta.OpenElfasta), or the FASTA file itself, plain or
+// BGZF-compressed (fasta.ParseFasta), read and packed on the device into every contig's reference.  Returns the sequences whose name is
+// no @SQ SN and the contigs left without a sequence.
+func (d *DeviceSam) LoadReference(path string) (uint64, int32) {
+	cp := C.CString(path)
+	defer C.free(unsafe.Pointer(cp))
+	var unmatched C.uint64_t
+	var missing C.int32_t
+	check(d.ctx, C.elp_load_reference(d.ctx, cp, &unmatched, &missing))
+	return uint64(unmatched), int32(missing)
+}
+
 // Recalibrate: (*BaseRecalibrator).Recalibrate (bqsr.go:467-551).  The tables stay on the device.
 // --target-regions: RemoveNonOverlappingReads(bedRegions) over the marked reads, before Recalibrate (cmd/filter.go:171-180, 288-296).
 // SetTargetRegions takes one contig's BED Start / End pairs (sorted and flattened inside); FilterTargetRegions returns the reads dropped.

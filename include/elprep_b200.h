@@ -39,6 +39,7 @@ extern "C" {
 #define ELP_EBGZF (-19)      /* malformed BGZF block (header, BC subfield, CRC32 or ISIZE), utils/bgzf/bgzf-files.go:95-127 */
 #define ELP_ESAM (-20)       /* malformed SAM alignment line; elp_last_error names the line (0-based, within the call) and the field */
 #define ELP_ESITES (-21)     /* malformed .elsites file; elp_last_error names the file (index in paths), the line (0-based, header = line 0) and the reason */
+#define ELP_EFASTA (-22)     /* malformed reference file: elp_last_error names the file, the line (FASTA, 1-based) or byte offset (.elfasta), and the reason */
 
 /* sam.SortingOrder (sam/sam-types.go:40-58) */
 #define ELP_SO_KEEP 0
@@ -138,6 +139,31 @@ int elp_load_known_sites(elp_ctx *ctx, const char *const *paths, int32_t n_paths
 int64_t elp_known_sites_get(elp_ctx *ctx, int32_t contig, int32_t *start_end_pairs, uint64_t cap);
 /* tests: bytes of the page-locked staging chunks the files are streamed through (0: the default, 32 MiB) */
 int elp_debug_set_sites_chunk(elp_ctx *ctx, uint64_t bytes);
+/* --reference (cmd/filter.go): the one-hot reference of EVERY contig from one file, read and packed on the device.  The format is decided
+ * from the content: the first four bytes 31 FA 57 A1 (ElfastaMagic) make an .elfasta (fasta.OpenElfasta, fasta/fasta-files.go:286-336);
+ * a first byte 0x1f makes a BGZF-compressed FASTA, anything else is FASTA text (fasta.ParseFasta(path, nil, false, false) as
+ * `elprep fasta-to-elfasta` calls it, fasta-files.go:159-229).
+ *  - Contig k afterwards holds what elp_set_reference(k, Seq(SN_k)) gives.  When several @SQ lines share an SN, each gets the sequence.
+ *    A contig whose SN has no sequence in the file has none, like a contig never set: a recalibrated read on it is ELP_EREFEND.
+ *  - FASTA: lines as bufio.ScanLines splits them (a line of 65536 bytes or more is refused); empty lines before the first header are
+ *    skipped and the first other line must start with '>'; after empty lines only a header or the end of the file may follow; a header's
+ *    name is its first run of bytes in '!'..'~' after the '>' (contigFromHeader); every other line is appended verbatim; the last of equal
+ *    names wins.  An empty file, or one of empty lines only, is refused.  Refusals are ELP_EFASTA naming the 1-based line.
+ *  - BGZF: the rules of elp_append_bgzf / elp_append_bgzf_end (BC subfield, CRC32, ISIZE, the EOF marker block at the end); a violation
+ *    is ELP_EBGZF naming the file offset; a plain (non-BGZF) gzip file is refused there.
+ *  - .elfasta: the offset table (name '\t' then two binary.Varint fields of 10 bytes: offset and size) up to an entry that starts with
+ *    '\n'; the last of equal names wins; a table that runs past the end of the file, a field binary.Varint rejects, or a sequence outside
+ *    the file is ELP_EFASTA naming the byte offset.  Only the sequences of names that are an @SQ SN are read.
+ *  - *n_unmatched (may be NULL): the file's sequences whose name is no SN; *n_missing (may be NULL): the contigs left without a sequence.
+ *  - A context with @SQ lines created without names is ELP_EINVAL; so is a missing or unreadable file (the message names the path).
+ *  - Atomic: on any error the previous references are unchanged.  They survive elp_reset; elp_set_reference afterwards replaces one
+ *    contig, and the two calls mix in either order. */
+int elp_load_reference(elp_ctx *ctx, const char *path, uint64_t *n_unmatched, int32_t *n_missing);
+/* one contig's reference as the gather reads it: returns its length in bases (-1 on error) and copies its (len + 1) / 2 one-hot nibble
+ * bytes (low nibble first: A 1, C 2, G 4, T 8, anything else 0) when nibbles is not NULL and cap allows */
+int64_t elp_reference_get(elp_ctx *ctx, int32_t contig, uint8_t *nibbles, uint64_t cap);
+/* tests: bytes of the page-locked staging chunks the reference file is streamed through (0: the default, 32 MiB) */
+int elp_debug_set_reference_chunk(elp_ctx *ctx, uint64_t bytes);
 
 /* ---- phase 1: (*sam.Sam).AddNodes receiving batches (sam/filter-pipeline.go:108-128) ---- */
 int elp_append_batch(elp_ctx *ctx, const elp_batch *batch);

@@ -22,6 +22,7 @@
 #include <stdexcept>
 #include <string>
 #include <unordered_map>
+#include <utility>
 #include <vector>
 
 #include "elprep_b200.h"
@@ -162,6 +163,13 @@ class DeviceSam {
         uint64_t unmatched = 0;
         check(elp_load_known_sites(ctx_, p.empty() ? nullptr : p.data(), (int32_t)p.size(), &unmatched));
         return unmatched;
+    }
+    // --reference: an .elfasta or a FASTA file (plain or BGZF), read and packed on the device into every contig's reference; returns
+    // (sequences whose name is no @SQ SN, contigs left without a sequence)
+    std::pair<uint64_t, int32_t> LoadReference(const std::string& path) {
+        uint64_t unmatched = 0; int32_t missing = 0;
+        check(elp_load_reference(ctx_, path.c_str(), &unmatched, &missing));
+        return {unmatched, missing};
     }
     // `--target-regions`: RemoveNonOverlappingReads(bedRegions) after marking, before Recalibrate (cmd/filter.go:171-180, 288-296); one
     // contig's BED Start / End pairs per call, sorted and flattened inside.  FilterTargetRegions returns the number of reads dropped.
