@@ -52,7 +52,7 @@ EXPORTS = ["elp_create", "elp_destroy", "elp_last_error", "elp_reserve", "elp_re
            "elp_bgzf_inflate_bound", "elp_bgzf_inflate", "elp_bgzf_deflate_bound", "elp_bgzf_deflate", "elp_bam_header_size",
            "elp_append_bgzf", "elp_append_bgzf_end", "elp_debug_inflate", "elp_fetch_bgzf", "elp_debug_deflate",
            "elp_load_known_sites", "elp_known_sites_get", "elp_debug_set_sites_chunk",
-           "elp_load_reference", "elp_reference_get", "elp_debug_set_reference_chunk"]
+           "elp_load_reference", "elp_reference_get", "elp_debug_set_reference_chunk", "elp_debug_live_allocations"]
 
 _lib = None
 
@@ -94,6 +94,8 @@ def load():
     L.elp_reference_get.restype = C.c_int64
     L.elp_reference_get.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_uint64]
     L.elp_debug_set_reference_chunk.argtypes = [C.c_void_p, C.c_uint64]
+    L.elp_debug_live_allocations.restype = C.c_int64
+    L.elp_debug_live_allocations.argtypes = []
     L.elp_append_batch.argtypes = [C.c_void_p, C.POINTER(ElpBatch)]
     for f in ("elp_bqsr_tables_write_elrecal", "elp_bqsr_tables_add_elrecal", "elp_optical_write_gob", "elp_optical_add_gob"):
         getattr(L, f).argtypes = [C.c_void_p, C.c_char_p]

@@ -14,8 +14,6 @@ namespace {
 
 thread_local std::string g_create_error;
 
-inline unsigned nblk(uint64_t n, int t) { return (unsigned)((n + t - 1) / t); }
-
 __global__ void __launch_bounds__(256) rebase_kernel(uint64_t n, const uint64_t* __restrict__ rel, uint64_t base, uint64_t* __restrict__ out) {
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) out[i] = rel[i] + base;
@@ -66,14 +64,9 @@ __global__ void __launch_bounds__(256) qual_presence_kernel(const uint8_t* __res
     }
 }
 
-template <class T> int grow(elp_ctx* c, DBuf<T>& b, size_t need, size_t keep) {
-    cudaError_t e = b.reserve(need, c->stream, keep);
-    if (e != cudaSuccess) return c->fail(e == cudaErrorMemoryAllocation ? E_NOMEM : E_CUDA, "device allocation of %zu bytes failed: %s", need * sizeof(T), cudaGetErrorString(e));
-    return E_OK;
-}
-#define TRY(x) do { int rc__ = (x); if (rc__) return rc__; } while (0)
-
 }  // namespace
+
+std::atomic<int64_t> g_live_allocations{0};
 
 // Small host->device uploads INSIDE the phases (value ranges, look-up tables, ...) do not go through the copy engine: it serves its queue in
 // order, so behind the multi-gigabyte upload of another context of a pipelined caller they would wait for all of it.  The bytes are staged in
@@ -87,9 +80,9 @@ int upload_small(elp_ctx* c, void* dst, const void* src, size_t bytes) {
     constexpr size_t CAP = 8u << 20;
     if (!bytes) return E_OK;
     if (bytes > CAP || (reinterpret_cast<uintptr_t>(dst) & 15)) { CUDA_TRY(c, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, c->stream)); return E_OK; }
-    if (!c->h_stage) CUDA_TRY(c, cudaHostAlloc(&c->h_stage, CAP, cudaHostAllocPortable | cudaHostAllocMapped));
+    CUDA_TRY(c, c->h_stage.fit(CAP, cudaHostAllocPortable | cudaHostAllocMapped));
     if (c->stage_off + bytes > CAP) { CUDA_TRY(c, cudaStreamSynchronize(c->stream)); c->stage_off = 0; }
-    uint8_t* st = reinterpret_cast<uint8_t*>(c->h_stage) + c->stage_off;
+    uint8_t* st = c->h_stage.p + c->stage_off;
     memcpy(st, src, bytes);
     void* dev_src = st;
     CUDA_TRY(c, cudaHostGetDevicePointer(&dev_src, st, 0));
@@ -104,23 +97,18 @@ int qual_presence_update(elp_ctx* c, uint64_t first_byte, uint64_t n_bytes) {
     if (!n_bytes) return E_OK;
     const unsigned grid = (unsigned)std::min<uint64_t>((n_bytes / 16 + 255) / 256 + 1, 132 * 16);
     c->launches++;
-    qual_presence_kernel<<<grid, 256, 0, c->stream>>>(c->qual.p + first_byte, n_bytes, c->d_qpresent);
+    qual_presence_kernel<<<grid, 256, 0, c->stream>>>(c->qual.p + first_byte, n_bytes, c->d_qpresent.p);
     LAUNCH_CHECK(c);
     return E_OK;
 }
 
-int upload_side_inputs(elp_ctx* c) {
-    if (!c->side_dirty) return E_OK;
-    const int nc = c->n_contigs;
-    std::vector<const uint8_t*> hp(nc);
-    for (int i = 0; i < nc; i++) hp[i] = c->d_refhot_raw[i] ? c->d_refhot_raw[i] + REFHOT_PAD : nullptr;
-    if (nc) {
-        CUDA_TRY(c, cudaMemcpyAsync(c->d_refhot_ptrs, hp.data(), nc * sizeof(void*), cudaMemcpyHostToDevice, c->stream));
-        CUDA_TRY(c, cudaMemcpyAsync(c->d_ref_len, c->ref_len.data(), nc * 8, cudaMemcpyHostToDevice, c->stream));
-        CUDA_TRY(c, cudaStreamSynchronize(c->stream));
-    }
-    c->side_dirty = false;
-    return E_OK;
+elp_ctx::~elp_ctx() {
+    for (auto& pe : pending) { cudaEventDestroy(pe.a); cudaEventDestroy(pe.b); }
+    for (auto e : event_pool) cudaEventDestroy(e);
+    if (timer_a) { cudaEventDestroy(timer_a); cudaEventDestroy(timer_b); }
+    if (copy_in) { cudaStreamDestroy(copy_in); cudaEventDestroy(ev_in); cudaEventDestroy(ev_staged); }
+    if (copy_out) { cudaStreamDestroy(copy_out); cudaEventDestroy(ev_out); }
+    if (stream) cudaStreamDestroy(stream);
 }
 
 extern "C" {
@@ -167,19 +155,19 @@ int elp_create(const elp_config* cfg, elp_ctx** out) {
     c->optical_pixel_distance = cfg->optical_pixel_distance > 0 ? cfg->optical_pixel_distance : 100;
     c->geom.n_cov = (int)c->cov_names.size(); c->geom.max_cycle = c->max_cycle;
     const int nc = std::max(1, c->n_contigs), nr = std::max(1, c->n_rg);
-    bool ok = cudaMalloc(&c->d_rg_lib, nr * 4) == cudaSuccess && cudaMalloc(&c->d_rg_cov, nr * 4) == cudaSuccess && cudaMalloc(&c->d_contig_len, nc * 4) == cudaSuccess &&
-              cudaMalloc(&c->d_ranges, sizeof(DeviceRanges)) == cudaSuccess && cudaMalloc(&c->d_err, 4) == cudaSuccess &&
-              cudaMalloc(&c->d_refhot_ptrs, nc * sizeof(void*)) == cudaSuccess &&
-              cudaMalloc(&c->d_bq_small, 512 * 4) == cudaSuccess && cudaMalloc(&c->d_qpresent, 16) == cudaSuccess && cudaMalloc(&c->d_ref_len, nc * 8) == cudaSuccess &&
-              cudaMalloc(&c->d_tables, std::max<size_t>(16, c->geom.cells() * 2 * sizeof(int64_t))) == cudaSuccess;
+    const size_t n_tables = std::max<size_t>(2, c->geom.cells() * 2);
+    const bool ok = c->d_rg_lib.fit(nr) == cudaSuccess && c->d_rg_cov.fit(nr) == cudaSuccess && c->d_contig_len.fit(nc) == cudaSuccess && c->d_ranges.fit(1) == cudaSuccess &&
+                    c->d_err.fit(1) == cudaSuccess && c->d_bq_small.fit(512) == cudaSuccess && c->d_qpresent.fit(4) == cudaSuccess && c->d_tables.fit(n_tables) == cudaSuccess &&
+                    c->d_rowtab.fit(256) == cudaSuccess;
     if (!ok) { c->err = "device allocation failed in elp_create"; return bail(ELP_ENOMEM); }
-    if (c->n_rg) { cudaMemcpy(c->d_rg_lib, c->rg_lib.data(), c->n_rg * 4, cudaMemcpyHostToDevice); cudaMemcpy(c->d_rg_cov, c->rg_cov.data(), c->n_rg * 4, cudaMemcpyHostToDevice); }
-    if (c->n_contigs) cudaMemcpy(c->d_contig_len, c->contig_len.data(), c->n_contigs * 4, cudaMemcpyHostToDevice);
-    cudaMemset(c->d_err, 0, 4);
-    cudaMemset(c->d_qpresent, 0, 16);
+    if (c->n_rg) { cudaMemcpy(c->d_rg_lib.p, c->rg_lib.data(), c->n_rg * 4, cudaMemcpyHostToDevice); cudaMemcpy(c->d_rg_cov.p, c->rg_cov.data(), c->n_rg * 4, cudaMemcpyHostToDevice); }
+    if (c->n_contigs) cudaMemcpy(c->d_contig_len.p, c->contig_len.data(), c->n_contigs * 4, cudaMemcpyHostToDevice);
+    cudaMemset(c->d_err.p, 0, 4);
+    cudaMemset(c->d_qpresent.p, 0, 16);
     c->n_qual = c->n_seq = ARENA_FRONT_PAD;
-    cudaMemset(c->d_tables, 0, std::max<size_t>(16, c->geom.cells() * 2 * sizeof(int64_t)));
-    c->d_refhot_raw.assign(c->n_contigs, nullptr); c->ref_len.assign(c->n_contigs, 0);
+    cudaMemset(c->d_tables.p, 0, n_tables * sizeof(int64_t));
+    cudaMemset(c->d_rowtab.p, 0, 256 * sizeof(uint16_t));
+    c->ref.resize(c->n_contigs); c->known_sites.resize(c->n_contigs); c->regions.resize(c->n_contigs); c->bqsr_regions.resize(c->n_contigs);
     if ((e = cudaGetLastError()) != cudaSuccess) { c->err = std::string("elp_create: ") + cudaGetErrorString(e); return bail(ELP_ECUDA); }
     *out = c;
     return ELP_OK;
@@ -189,35 +177,11 @@ void elp_destroy(elp_ctx* c) {
     if (!c) return;
     cudaSetDevice(c->device);
     if (c->stream) cudaStreamSynchronize(c->stream);
-    sam_state_release(c);
-    sites_release(c);
-    sam_out_release(c);
-    bgzf_release(c);
-    bgzf_deflate_release(c);
-    for (auto p : c->d_refhot_raw) if (p && c->refhot_separate(p)) cudaFree(p);
-    if (c->refhot_block) cudaFree(c->refhot_block);
-    region_release(c->regions); region_release(c->bqsr_regions); region_release(c->known_sites);
-    void* singles[] = {c->d_rg_lib, c->d_rg_cov, c->d_contig_len, c->d_ranges, c->d_err, (void*)c->d_refhot_ptrs, c->d_bq_small, c->d_qpresent, c->d_ref_len, c->d_tables,
-                       c->d_lut, c->d_clut, c->d_rowtab, c->d_cov_exists, c->d_unobs, c->d_emp, c->d_fin, c->d_qmaps, c->d_opt_ctr, c->d_opt_hist, c->d_opt_ovf, c->d_opt_small, c->d_rg_names, c->d_rg_name_off, c->d_out_drop, c->ws.ghist, c->ws.gofs, c->ws.counters, c->ws.status};
-    for (void* p : singles) if (p) cudaFree(p);
-    c->refid.release(); c->pos.release(); c->nref.release(); c->pnext.release(); c->tlen.release(); c->rg.release(); c->flag.release(); c->mapq.release(); c->optf.release(); c->s_optf.release();
-    c->qname_off.release(); c->cigar_off.release(); c->qual_off.release(); c->seq_off.release(); c->qname.release(); c->seq.release(); c->qual.release(); c->cigar.release();
-    c->bam_raw.release(); c->bam_off.release(); c->bam_all.release(); c->bam_all_off.release(); c->bam_start.release(); c->out_sel.release(); c->lseq_stage.release(); c->off_stage.release(); c->upos.release(); c->score.release(); c->qhash.release(); c->keys_a.release(); c->keys_b.release();
-    c->bq_recs.release(); c->bq_segs.release(); c->vals_a.release(); c->vals_b.release(); c->mate.release(); c->pair_a.release(); c->pair_b.release(); c->pair_score.release(); c->tie_bits.release(); c->scan_tmp.release(); c->scan_blk.release(); c->bytes_tmp.release();
-    c->perm.release(); c->s_refid.release(); c->s_pos.release(); c->s_nref.release(); c->s_pnext.release(); c->s_tlen.release(); c->s_rg.release(); c->s_lseq.release();
-    c->s_flag.release(); c->s_mapq.release(); c->s_qual_off.release(); c->s_seq_off.release(); c->s_cigar_off.release(); c->s_out_off.release(); c->s_ncigar.release(); c->qual_out.release();
-    for (auto& pe : c->pending) { cudaEventDestroy(pe.a); cudaEventDestroy(pe.b); }
-    for (auto e : c->event_pool) cudaEventDestroy(e);
-    if (c->timer_a) { cudaEventDestroy(c->timer_a); cudaEventDestroy(c->timer_b); }
     elp_comm_destroy(c);
-    if (c->d_owner) cudaFree(c->d_owner);
-    c->sp_sendbuf.release(); c->sp_recvbuf.release(); c->sp_sent_idx.release();
-    if (c->h_stage) cudaFreeHost(c->h_stage);
-    if (c->copy_in) { cudaStreamDestroy(c->copy_in); cudaEventDestroy(c->ev_in); cudaEventDestroy(c->ev_staged); }
-    if (c->copy_out) { cudaStreamDestroy(c->copy_out); cudaEventDestroy(c->ev_out); }
-    if (c->stream) cudaStreamDestroy(c->stream);
     delete c;
 }
+
+int64_t elp_debug_live_allocations(void) { return g_live_allocations.load(); }
 
 int elp_reset(elp_ctx* c) {
     if (!c) return ELP_EINVAL;
@@ -226,12 +190,12 @@ int elp_reset(elp_ctx* c) {
     if (c->copy_out) CUDA_TRY(c, cudaStreamSynchronize(c->copy_out));
     CUDA_TRY(c, cudaStreamSynchronize(c->stream));
     c->n = c->n_sorted = c->n_qname = c->n_cigar = 0; c->n_qual = c->n_seq = ARENA_FRONT_PAD; c->n_bam = c->bam_reads = 0; c->n_filtered = 0; c->n_cleaned = 0; c->n_sam_lost_names = 0;
-    CUDA_TRY(c, cudaMemsetAsync(c->d_qpresent, 0, 16, c->stream));
+    CUDA_TRY(c, cudaMemsetAsync(c->d_qpresent.p, 0, 16, c->stream));
     c->adapted = c->sorted = c->qual_out_valid = c->gathered = c->finalized = c->opt_valid = false;
     c->out_sel_valid = false; c->n_out = 0;   // (the output filter setting itself stays)
     c->launches = 0;
     bgzf_stream_reset(c);
-    CUDA_TRY(c, cudaMemsetAsync(c->d_err, 0, 4, c->stream));
+    CUDA_TRY(c, cudaMemsetAsync(c->d_err.p, 0, 4, c->stream));
     return ELP_OK;
 }
 
@@ -252,8 +216,7 @@ int elp_set_reference(elp_ctx* c, int32_t contig, const uint8_t* bases, uint64_t
     if (!c) return ELP_EINVAL;
     cudaSetDevice(c->device);
     if (contig < 0 || contig >= c->n_contigs) return c->fail(E_INVAL, "elp_set_reference: contig %d out of range", contig);
-    c->ref_len[contig] = n; c->side_dirty = true;
-    return pack_reference(c, contig, bases);
+    return pack_reference(c, contig, bases, n);
 }
 
 int elp_set_known_sites(elp_ctx* c, int32_t contig, const int32_t* se, uint64_t n_intervals, int already_flat) {
@@ -397,7 +360,7 @@ int elp_bqsr_tables_get(elp_ctx* c, int64_t* dense, uint64_t n) {
     if (!c || !dense) return ELP_EINVAL;
     cudaSetDevice(c->device);
     if (n != elp_bqsr_tables_len(c)) return c->fail(E_INVAL, "elp_bqsr_tables_get: expected %llu values", (unsigned long long)elp_bqsr_tables_len(c));
-    CUDA_TRY(c, cudaMemcpyAsync(dense, c->d_tables, n * 8, cudaMemcpyDeviceToHost, c->stream));
+    CUDA_TRY(c, cudaMemcpyAsync(dense, c->d_tables.p, n * 8, cudaMemcpyDeviceToHost, c->stream));
     CUDA_TRY(c, cudaStreamSynchronize(c->stream));
     return ELP_OK;
 }
@@ -405,7 +368,7 @@ int elp_bqsr_tables_put(elp_ctx* c, const int64_t* dense, uint64_t n) {
     if (!c || !dense) return ELP_EINVAL;
     cudaSetDevice(c->device);
     if (n != elp_bqsr_tables_len(c)) return c->fail(E_INVAL, "elp_bqsr_tables_put: expected %llu values", (unsigned long long)elp_bqsr_tables_len(c));
-    CUDA_TRY(c, cudaMemcpyAsync(c->d_tables, dense, n * 8, cudaMemcpyHostToDevice, c->stream));
+    CUDA_TRY(c, cudaMemcpyAsync(c->d_tables.p, dense, n * 8, cudaMemcpyHostToDevice, c->stream));
     CUDA_TRY(c, cudaStreamSynchronize(c->stream));
     c->gathered = true; c->finalized = false;
     return ELP_OK;
@@ -414,7 +377,7 @@ int elp_bqsr_tables_device(elp_ctx* c, void** p, uint64_t* n) {
     if (!c || !p || !n) return ELP_EINVAL;
     cudaSetDevice(c->device);
     CUDA_TRY(c, cudaStreamSynchronize(c->stream));
-    *p = c->d_tables; *n = elp_bqsr_tables_len(c);
+    *p = c->d_tables.p; *n = elp_bqsr_tables_len(c);
     c->finalized = false;
     return ELP_OK;
 }

@@ -20,8 +20,6 @@
 
 namespace {
 
-inline unsigned nblk(uint64_t n, int t) { return (unsigned)((n + t - 1) / t); }
-
 __device__ __forceinline__ uint32_t rd32(const uint8_t* p) { return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24); }
 __device__ __forceinline__ uint32_t rd16(const uint8_t* p) { return (uint32_t)p[0] | ((uint32_t)p[1] << 8); }
 
@@ -362,37 +360,13 @@ __global__ void __launch_bounds__(256) bam_out_fields_emit_kernel(uint64_t n, ui
     }
 }
 
-template <class T> int grow(elp_ctx* c, DBuf<T>& b, size_t need, size_t keep) {
-    cudaError_t e = b.reserve(need, c->stream, keep);
-    if (e != cudaSuccess) return c->fail(e == cudaErrorMemoryAllocation ? E_NOMEM : E_CUDA, "device allocation of %zu bytes failed: %s", need * sizeof(T), cudaGetErrorString(e));
-    return E_OK;
-}
-#define TRY(x) do { int rc__ = (x); if (rc__) return rc__; } while (0)
-
 }  // namespace
 
 // ---- region tables (RegionTable, ctx.h): the ingest filter's, the one of elp_filter_target_regions and the BQSR known sites ----
-// Uploads go on the context's stream and are waited for: a pageable cudaMemcpy may return before its DMA has landed, and the
-// (non-blocking) stream of the kernels that read the table does not wait for it.
-int region_upload(elp_ctx* c, RegionTable& t) {
-    if (!t.dirty && t.d_ptrs) return E_OK;
-    const int nc = std::max(1, c->n_contigs);
-    if ((int)t.d.size() != c->n_contigs) { t.d.assign(c->n_contigs, nullptr); t.n.assign(c->n_contigs, 0); }
-    if (!t.d_ptrs) { CUDA_TRY(c, cudaMalloc(&t.d_ptrs, nc * sizeof(void*))); CUDA_TRY(c, cudaMalloc(&t.d_n, nc * 8)); }
-    if (c->n_contigs) {
-        CUDA_TRY(c, cudaMemcpyAsync(t.d_ptrs, t.d.data(), c->n_contigs * sizeof(void*), cudaMemcpyHostToDevice, c->stream));
-        CUDA_TRY(c, cudaMemcpyAsync(t.d_n, t.n.data(), c->n_contigs * 8, cudaMemcpyHostToDevice, c->stream));
-        CUDA_TRY(c, cudaStreamSynchronize(c->stream));
-    }
-    t.dirty = false;
-    return E_OK;
-}
-
 // one contig's regions: sorted by start and flattened unless already_flat (intervals.ParallelSortByStart + ParallelFlatten, intervals/intervals.go:88-117)
 int region_set(elp_ctx* c, RegionTable& t, const char* who, int32_t contig, const int32_t* se, uint64_t n_intervals, int already_flat) {
     if (contig < 0 || contig >= c->n_contigs) return c->fail(E_INVAL, "%s: contig %d out of range", who, contig);
     if (n_intervals && !se) return c->fail(E_INVAL, "%s: null interval array", who);
-    if ((int)t.d.size() != c->n_contigs) { t.d.assign(c->n_contigs, nullptr); t.n.assign(c->n_contigs, 0); }
     std::vector<std::pair<int32_t, int32_t>> iv(n_intervals);
     for (uint64_t i = 0; i < n_intervals; i++) iv[i] = {se[2 * i], se[2 * i + 1]};
     uint64_t n = n_intervals;
@@ -402,23 +376,15 @@ int region_set(elp_ctx* c, RegionTable& t, const char* who, int32_t contig, cons
         for (uint64_t i = 0; i < n; i++) { if (m > 0 && iv[i].first <= iv[m - 1].second) { if (iv[i].second > iv[m - 1].second) iv[m - 1].second = iv[i].second; } else iv[m++] = iv[i]; }
         n = m;
     }
-    if (t.d[contig]) { if (t.separate(t.d[contig])) cudaFree(t.d[contig]); t.d[contig] = nullptr; }
+    t.clear(contig);
     if (n) {
-        CUDA_TRY(c, cudaMalloc(&t.d[contig], n * 8));
-        CUDA_TRY(c, cudaMemcpyAsync(t.d[contig], iv.data(), n * 8, cudaMemcpyHostToDevice, c->stream));
+        DBuf<int32_t>& own = t.own[contig];
+        CUDA_TRY(c, own.fit(2 * n));
+        CUDA_TRY(c, cudaMemcpyAsync(own.p, iv.data(), n * 8, cudaMemcpyHostToDevice, c->stream));
         CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+        t.d[contig] = own.p; t.n[contig] = n;
     }
-    t.n[contig] = n; t.dirty = true;
     return ELP_OK;
-}
-
-void region_release(RegionTable& t) {
-    for (auto p : t.d) if (p && t.separate(p)) cudaFree(p);
-    if (t.block) cudaFree(t.block);
-    t.block = nullptr; t.block_pairs = 0;
-    if (t.d_ptrs) cudaFree((void*)t.d_ptrs);
-    if (t.d_n) cudaFree(t.d_n);
-    t.d.clear(); t.n.clear(); t.d_ptrs = nullptr; t.d_n = nullptr; t.dirty = true;
 }
 
 extern "C" int elp_append_bam(elp_ctx* c, const uint8_t* records, uint64_t n_bytes, const uint64_t* record_off, uint64_t n_records) {
@@ -462,20 +428,20 @@ int bam_ingest_core(elp_ctx* c, uint64_t n_bytes, uint64_t nrec) {
     TRY(grow(c, c->bam_start, nrec + 2, 0));
     const uint64_t* d_start = c->bam_off.p;                   // without filters: record i is read n0 + i
     // @RG ID strings for the RG:Z match
-    if (!c->d_rg_names && c->n_rg) {
+    if (!c->d_rg_names.p && c->n_rg) {
         std::vector<uint8_t> names; std::vector<uint32_t> off(1, 0);
         for (auto& id : c->rg_ids) { names.insert(names.end(), id.begin(), id.end()); off.push_back((uint32_t)names.size()); }
-        CUDA_TRY(c, cudaMalloc(&c->d_rg_names, std::max<size_t>(names.size(), 1)));
-        CUDA_TRY(c, cudaMalloc(&c->d_rg_name_off, off.size() * 4));
-        CUDA_TRY(c, cudaMemcpy(c->d_rg_names, names.data(), names.size(), cudaMemcpyHostToDevice));
-        CUDA_TRY(c, cudaMemcpy(c->d_rg_name_off, off.data(), off.size() * 4, cudaMemcpyHostToDevice));
+        CUDA_TRY(c, c->d_rg_names.fit(std::max<size_t>(names.size(), 1)));
+        CUDA_TRY(c, c->d_rg_name_off.fit(off.size()));
+        CUDA_TRY(c, cudaMemcpy(c->d_rg_names.p, names.data(), names.size(), cudaMemcpyHostToDevice));
+        CUDA_TRY(c, cudaMemcpy(c->d_rg_name_off.p, off.data(), off.size() * 4, cudaMemcpyHostToDevice));
     }
     if (c->filter_mask || c->filter_min_mapq > 0) {
         TRY(grow(c, c->scan_tmp, nrec + 8, 0)); TRY(grow(c, c->off_stage, nrec + 2, 0));
         c->begin("bam_keep", (double)nrec * 48);
-        if (c->filter_mask & ELP_FILTER_TARGET_REGIONS) { int rcr = region_upload(c, c->regions); if (rcr) return rcr; }
-        bam_keep_kernel<<<nblk(nrec, 256), 256, 0, s>>>(nrec, c->bam_raw.p, c->bam_off.p, n_bytes, c->filter_mask, c->filter_min_mapq, c->regions.d_ptrs, c->regions.d_n, c->n_contigs,
-                                                        RgNames{c->d_rg_names, c->d_rg_name_off, c->n_rg}, c->scan_tmp.p, c->d_err);
+        if (c->filter_mask & ELP_FILTER_TARGET_REGIONS) TRY(table_upload(c, c->regions));
+        bam_keep_kernel<<<nblk(nrec, 256), 256, 0, s>>>(nrec, c->bam_raw.p, c->bam_off.p, n_bytes, c->filter_mask, c->filter_min_mapq, c->regions.d_ptrs.p, c->regions.d_n.p, c->n_contigs,
+                                                        RgNames{c->d_rg_names.p, c->d_rg_name_off.p, c->n_rg}, c->scan_tmp.p, c->d_err.p);
         c->end(); LAUNCH_CHECK(c);
         TRY(exclusive_scan_u32_to_u64(c, c->scan_tmp.p, c->off_stage.p, nrec));
         bam_compact_kernel<<<nblk(nrec, 256), 256, 0, s>>>(nrec, c->scan_tmp.p, c->off_stage.p, c->bam_off.p, c->bam_start.p); c->launches++;
@@ -497,7 +463,7 @@ int bam_ingest_core(elp_ctx* c, uint64_t n_bytes, uint64_t nrec) {
     A.n = bn; A.n0 = n0; A.raw = c->bam_raw.p; A.start = d_start; A.n_bytes = n_bytes; A.chained = d_start == c->bam_off.p; A.clear_dup = c->clear_dup;
     A.refid = c->refid.p; A.pos = c->pos.p; A.nref = c->nref.p; A.pnext = c->pnext.p; A.tlen = c->tlen.p; A.rg = c->rg.p; A.flag = c->flag.p; A.mapq = c->mapq.p; A.optf = c->optf.p;
     A.len_qname = c->scan_tmp.p; A.len_cigar = c->scan_tmp.p + (bn + 4); A.len_seq = c->scan_tmp.p + 2 * (bn + 4); A.len_qual = c->scan_tmp.p + 3 * (bn + 4);
-    A.rg_names = c->d_rg_names; A.rg_name_off = c->d_rg_name_off; A.n_rg = c->n_rg; A.n_contigs = c->n_contigs; A.err = c->d_err;
+    A.rg_names = c->d_rg_names.p; A.rg_name_off = c->d_rg_name_off.p; A.n_rg = c->n_rg; A.n_contigs = c->n_contigs; A.err = c->d_err.p;
     c->begin("bam_fixed", (double)bn * 36 + (double)n_bytes * 0.2);
     bam_fixed_kernel<<<nblk(bn, 256), 256, 0, s>>>(A);
     c->end(); LAUNCH_CHECK(c);
@@ -579,7 +545,7 @@ static int bam_out_prepare(elp_ctx* c, uint64_t first, uint64_t n, uint64_t* tot
     TRY(grow(c, c->scan_tmp, n + 8, 0)); TRY(grow(c, c->off_stage, n + 2, 0));
     if (c->out_fields) {
         c->begin("bam_out_fields_measure", (double)c->n_bam * (double)n / (double)std::max<uint64_t>(c->n, 1) + 4.0 * (double)n);
-        bam_out_fields_measure_kernel<<<nblk(n * 32, 256), 256, 0, c->stream>>>(n, first, *sel, c->perm.p, c->bam_all_off.p, c->bam_all.p, c->d_out_drop, c->scan_tmp.p);
+        bam_out_fields_measure_kernel<<<nblk(n * 32, 256), 256, 0, c->stream>>>(n, first, *sel, c->perm.p, c->bam_all_off.p, c->bam_all.p, c->d_out_drop.p, c->scan_tmp.p);
         c->end();
     } else {
         bam_out_len_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(n, first, *sel, c->perm.p, c->bam_all_off.p, c->bam_all.p, c->scan_tmp.p); c->launches++;
@@ -595,7 +561,7 @@ static int bam_out_prepare(elp_ctx* c, uint64_t first, uint64_t n, uint64_t* tot
 static int bam_out_format(elp_ctx* c, uint64_t first, uint64_t n, const uint32_t* sel, uint64_t total, uint8_t* dst) {
     if (c->out_fields) {
         c->begin("bam_out_fields_emit", (double)c->n_bam * (double)n / (double)std::max<uint64_t>(c->n, 1) + (double)total);
-        bam_out_fields_emit_kernel<<<nblk(n * 32, 256), 256, 0, c->stream>>>(n, first, sel, c->perm.p, c->bam_all_off.p, c->bam_all.p, c->d_out_drop, c->off_stage.p, dst,
+        bam_out_fields_emit_kernel<<<nblk(n * 32, 256), 256, 0, c->stream>>>(n, first, sel, c->perm.p, c->bam_all_off.p, c->bam_all.p, c->d_out_drop.p, c->off_stage.p, dst,
                                                                              c->s_flag.p, c->s_mapq.p, c->s_out_off.p, c->qual_out_valid ? c->qual_out.p : nullptr);
     } else {
         c->begin("bam_format", 2.0 * (double)total);
@@ -682,8 +648,8 @@ extern "C" int elp_set_output_filter(elp_ctx* c, uint32_t mask, const char* cons
     bool any = false;
     for (uint32_t w : drop) any |= w != 0;
     if (any) {
-        if (!c->d_out_drop) CUDA_TRY(c, cudaMalloc(&c->d_out_drop, 2048 * 4));
-        CUDA_TRY(c, cudaMemcpyAsync(c->d_out_drop, drop.data(), 2048 * 4, cudaMemcpyHostToDevice, c->stream));
+        CUDA_TRY(c, c->d_out_drop.fit(2048));
+        CUDA_TRY(c, cudaMemcpyAsync(c->d_out_drop.p, drop.data(), 2048 * 4, cudaMemcpyHostToDevice, c->stream));
         CUDA_TRY(c, cudaStreamSynchronize(c->stream));   // (drop is pageable host memory)
     }
     c->out_mask = mask & ~(uint32_t)ELP_OUT_KEEP_FIELDS; c->out_fields = any; c->out_sel_valid = false;

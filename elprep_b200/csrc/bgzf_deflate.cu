@@ -27,8 +27,6 @@ static_assert(dfl::stored_bytes((uint32_t)BLK_IN) <= SLOT, "a block's stream fit
 const uint8_t EOF_MARKER[28] = {0x1f, 0x8b, 0x08, 0x04, 0, 0, 0, 0, 0x00, 0xff, 0x06, 0x00, 0x42, 0x43, 0x02, 0x00, 0x1b, 0x00, 0x03, 0x00, 0, 0, 0, 0, 0, 0, 0, 0};
 __constant__ uint8_t BGZF_HEADER[16] = {0x1f, 0x8b, 0x08, 0x04, 0, 0, 0, 0, 0x00, 0xff, 0x06, 0x00, 0x42, 0x43, 0x02, 0x00};   // bgzf-files.go:336-340, BSIZE follows
 
-inline unsigned nblk(uint64_t n, int t) { return (unsigned)((n + t - 1) / t); }
-
 // the chain team: one warp, lanes grouped by hash with __match_any_sync
 struct ChainWarp {
     static constexpr unsigned size = 32;
@@ -88,13 +86,6 @@ __global__ void __launch_bounds__(256) bgzf_compact_kernel(const uint8_t* __rest
     }
 }
 
-template <class T> int grow(elp_ctx* c, DBuf<T>& b, size_t need) {
-    cudaError_t e = b.reserve(need, c->stream, 0);
-    if (e != cudaSuccess) return c->fail(e == cudaErrorMemoryAllocation ? E_NOMEM : E_CUDA, "device allocation of %zu bytes failed: %s", need * sizeof(T), cudaGetErrorString(e));
-    return E_OK;
-}
-#define TRY(x) do { int rc__ = (x); if (rc__) return rc__; } while (0)
-
 }  // namespace
 
 // device scratch of the writer: bounded by ROUND, whatever the bytes of a call (DESIGN.md §3d)
@@ -103,28 +94,24 @@ struct DeflateState {
     DBuf<uint16_t> prev;
     DBuf<uint32_t> match, bsize[2], crc[2];
     DBuf<uint64_t> off[2];
-    uint64_t* h_total = nullptr;               // page-locked: the bytes of the last two rounds
+    HBuf<uint64_t> h_total;                    // the bytes of the last two rounds
     cudaStream_t down = nullptr;
     cudaEvent_t done[2] = {nullptr, nullptr};
     X2n x2n;
+    ~DeflateState() {
+        for (int k = 0; k < 2; k++) if (done[k]) cudaEventDestroy(done[k]);
+        if (down) cudaStreamDestroy(down);
+    }
 };
 
-void bgzf_deflate_release(elp_ctx* c) {
-    if (!c->bgzf_out) return;
-    DeflateState& D = *c->bgzf_out;
-    D.in.release(); D.slots.release(); D.prev.release(); D.match.release();
-    for (int k = 0; k < 2; k++) { D.rout[k].release(); D.bsize[k].release(); D.crc[k].release(); D.off[k].release(); if (D.done[k]) cudaEventDestroy(D.done[k]); }
-    if (D.h_total) cudaFreeHost(D.h_total);
-    if (D.down) cudaStreamDestroy(D.down);
-    delete c->bgzf_out; c->bgzf_out = nullptr;
-}
+void free_state(DeflateState* D) { delete D; }
 
 static int deflate_state(elp_ctx* c) {
     if (c->bgzf_out) return E_OK;
-    c->bgzf_out = new DeflateState();
+    c->bgzf_out.reset(new DeflateState());
     DeflateState& D = *c->bgzf_out;
     dfl::x2n_table(D.x2n.v);
-    CUDA_TRY(c, cudaHostAlloc(&D.h_total, 2 * sizeof(uint64_t), cudaHostAllocDefault));
+    CUDA_TRY(c, D.h_total.fit(2));
     CUDA_TRY(c, cudaStreamCreateWithFlags(&D.down, cudaStreamNonBlocking));
     for (int k = 0; k < 2; k++) CUDA_TRY(c, cudaEventCreateWithFlags(&D.done[k], cudaEventDisableTiming));
     CUDA_TRY(c, cudaFuncSetAttribute(bgzf_deflate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(dfl::EncShared)));
@@ -148,7 +135,7 @@ int bgzf_deflate_run(elp_ctx* c, const uint8_t* in, uint64_t n, int write_eof, u
     size_t pend_ev[2] = {0, 0};                          // (its bgzf_deflate and bgzf_compact entries among the pending timing events)
     auto download = [&](int k) -> int {                  // wait for round k, copy its bytes out
         CUDA_TRY(c, cudaEventSynchronize(D.done[k]));
-        const uint64_t bytes = D.h_total[k];
+        const uint64_t bytes = D.h_total.p[k];
         if (c->profile) { c->pending[pend_ev[0]].alg_bytes += (double)bytes; c->pending[pend_ev[1]].alg_bytes += 2.0 * (double)bytes; }
         CUDA_TRY(c, cudaMemcpyAsync(out + w, D.rout[k].p, bytes, cudaMemcpyDeviceToHost, D.down));
         CUDA_TRY(c, cudaStreamSynchronize(D.down));
@@ -170,7 +157,7 @@ int bgzf_deflate_run(elp_ctx* c, const uint8_t* in, uint64_t n, int write_eof, u
         c->begin("bgzf_compact", 0);                             // (2 x the output bytes, once known)
         bgzf_compact_kernel<<<(unsigned)m, 256, 0, s>>>(D.slots.p, D.bsize[k].p, D.off[k].p, D.crc[k].p, n, b0, D.rout[k].p);
         c->end(); LAUNCH_CHECK(c);
-        CUDA_TRY(c, cudaMemcpyAsync(&D.h_total[k], D.off[k].p + m, 8, cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(c, cudaMemcpyAsync(&D.h_total.p[k], D.off[k].p + m, 8, cudaMemcpyDeviceToHost, s));
         CUDA_TRY(c, cudaEventRecord(D.done[k], s));
         if (pend >= 0) TRY(download(pend));              // (the previous round downloads while this one computes)
         pend = k; pend_ev[0] = ev; pend_ev[1] = ev_compact;

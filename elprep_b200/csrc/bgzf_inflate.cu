@@ -25,7 +25,6 @@
 
 namespace {
 
-inline unsigned nblk(uint64_t n, int t) { return (unsigned)((n + t - 1) / t); }
 __device__ __forceinline__ uint32_t drd32(const uint8_t* p) { return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24); }
 __device__ __forceinline__ uint32_t drd16(const uint8_t* p) { return (uint32_t)p[0] | ((uint32_t)p[1] << 8); }
 
@@ -157,13 +156,6 @@ __global__ void __launch_bounds__(256) bam_frame_emit_kernel(Frame F, const uint
 }
 __global__ void set_u64_kernel(uint64_t* p, uint64_t v) { *p = v; }
 
-template <class T> int grow(elp_ctx* c, DBuf<T>& b, size_t need, size_t keep) {
-    cudaError_t e = b.reserve(need, c->stream, keep);
-    if (e != cudaSuccess) return c->fail(e == cudaErrorMemoryAllocation ? E_NOMEM : E_CUDA, "device allocation of %zu bytes failed: %s", need * sizeof(T), cudaGetErrorString(e));
-    return E_OK;
-}
-#define TRY(x) do { int rc__ = (x); if (rc__) return rc__; } while (0)
-
 }  // namespace
 
 struct BgzfStream {
@@ -174,7 +166,7 @@ struct BgzfStream {
     DBuf<BlockDesc> tab;
     DBuf<uint32_t> status, seg_cnt;
     DBuf<uint64_t> seg;                      // framing: guess and exit of every segment, two generations
-    uint64_t* d_small = nullptr;             // [4] header walk result
+    DBuf<uint64_t> d_small;                  // [4] header walk result
     X2n x2n;
 };
 
@@ -185,19 +177,13 @@ void bgzf_stream_reset(elp_ctx* c) {
     S.carry.clear(); S.poisoned = S.header_done = S.last_eof = false; S.tail = 0;
 }
 
-void bgzf_release(elp_ctx* c) {
-    if (!c->bgzf) return;
-    BgzfStream& S = *c->bgzf;
-    S.in.release(); S.spare.release(); S.dbg_out.release(); S.tab.release(); S.status.release(); S.seg_cnt.release(); S.seg.release();
-    if (S.d_small) cudaFree(S.d_small);
-    delete c->bgzf; c->bgzf = nullptr;
-}
+void free_state(BgzfStream* S) { delete S; }
 
 static int bgzf_state(elp_ctx* c) {
     if (c->bgzf) return E_OK;
-    c->bgzf = new BgzfStream();
+    c->bgzf.reset(new BgzfStream());
     dfl::x2n_table(c->bgzf->x2n.v);
-    CUDA_TRY(c, cudaMalloc(&c->bgzf->d_small, 4 * 8));
+    CUDA_TRY(c, c->bgzf->d_small.fit(4));
     return E_OK;
 }
 
@@ -266,7 +252,7 @@ static int frame_records(elp_ctx* c, uint64_t n, uint64_t* nrec, uint64_t* used)
     TRY(grow(c, S.seg, 4 * nseg + 4, 0)); TRY(grow(c, S.seg_cnt, nseg + 8, 0)); TRY(grow(c, c->off_stage, nseg + 2, 0));
     const Frame F{c->bam_raw.p, n, nseg, c->n_contigs};
     uint64_t *g0 = S.seg.p, *x0 = g0 + nseg, *g1 = x0 + nseg, *x1 = g1 + nseg;   // generation 0 and 1: guesses, then exits
-    uint32_t* changed = reinterpret_cast<uint32_t*>(S.d_small);
+    uint32_t* changed = reinterpret_cast<uint32_t*>(S.d_small.p);
     c->begin("bam_frame", (double)n);
     bam_frame_guess_kernel<<<nblk(nseg, 256), 256, 0, s>>>(F, g0, x0);
     c->end(); LAUNCH_CHECK(c);
@@ -342,9 +328,9 @@ static int append_bgzf(elp_ctx* c, const uint8_t* data, uint64_t n) {
     if (!S.header_done) {
         uint64_t r[3] = {0, 0, 0};
         c->begin("bam_header", (double)avail);
-        bam_header_walk_kernel<<<1, 32, 0, c->stream>>>(c->bam_raw.p, avail, S.d_small);
+        bam_header_walk_kernel<<<1, 32, 0, c->stream>>>(c->bam_raw.p, avail, S.d_small.p);
         c->end(); LAUNCH_CHECK(c);
-        CUDA_TRY(c, cudaMemcpyAsync(r, S.d_small, 24, cudaMemcpyDeviceToHost, c->stream));
+        CUDA_TRY(c, cudaMemcpyAsync(r, S.d_small.p, 24, cudaMemcpyDeviceToHost, c->stream));
         CUDA_TRY(c, cudaStreamSynchronize(c->stream));
         if (r[0] == 2) return c->fail(E_BAM, "elp_append_bgzf: not a BAM file (magic or header lengths)");
         if (r[0] == 1) return E_OK;                                // the header continues in a later call

@@ -403,20 +403,18 @@ int run_apply_kernel(elp_ctx* c, bool with_lut) {
         }
         ApplyArgs A{};
         A.n = n; A.flag = c->s_flag.p; A.rg = c->s_rg.p; A.lseq = c->s_lseq.p; A.qual_off = c->s_qual_off.p; A.seq_off = c->s_seq_off.p; A.out_off = c->s_out_off.p;
-        A.seq = c->seq.p; A.qual = c->qual.p; A.out = c->qual_out.p; A.rg_cov = c->d_rg_cov; A.n_rg = c->n_rg; A.cov_exists = c->d_cov_exists;
-        A.lut = with_lut ? c->d_lut : nullptr; A.lut_maxcyc = c->lut_maxcyc; A.max_cycle = c->max_cycle; A.unobs = c->d_unobs; A.err = c->d_err;
+        A.seq = c->seq.p; A.qual = c->qual.p; A.out = c->qual_out.p; A.rg_cov = c->d_rg_cov.p; A.n_rg = c->n_rg; A.cov_exists = c->d_cov_exists.p;
+        A.lut = with_lut ? c->d_lut.p : nullptr; A.lut_maxcyc = c->lut_maxcyc; A.max_cycle = c->max_cycle; A.unobs = c->d_unobs.p; A.err = c->d_err.p;
         const double bytes = (double)n * (2 + 4 + 4 + 8 + 8 + 8) + ((double)c->n_seq + 2.0 * (double)c->n_qual) * ((double)n / (double)c->n);
         // second-generation kernel: whenever the compact table fits shared memory and every cycle is inside it
         const char* force = getenv("ELPREP_B200_APPLY");
-        const bool want_v2 = !(force && std::string(force) == "v1") && (!with_lut || (c->d_clut && c->clut_bytes && c->clut_Lc == c->lut_maxcyc && c->h_ranges.lseq_max <= c->clut_Lc)) && c->h_ranges.lseq_max <= 1024;
+        const bool want_v2 = !(force && std::string(force) == "v1") && (!with_lut || (c->d_clut.p && c->clut_bytes && c->clut_Lc == c->lut_maxcyc && c->h_ranges.lseq_max <= c->clut_Lc)) && c->h_ranges.lseq_max <= 1024;
         if (want_v2) {
             Apply2Args B{};
             B.n = n; B.flag = c->s_flag.p; B.rg = c->s_rg.p; B.lseq = c->s_lseq.p; B.qual_off = c->s_qual_off.p; B.seq_off = c->s_seq_off.p; B.out_off = c->s_out_off.p;
-            B.seq = c->seq.p; B.qual = c->qual.p; B.out = c->qual_out.p; B.rg_cov = c->d_rg_cov; B.n_rg = c->n_rg; B.cov_exists = c->d_cov_exists;
-            B.clut = with_lut ? c->d_clut : nullptr; B.clut_bytes = with_lut ? c->clut_bytes : 0; B.blk = c->clut_blk; B.Lc = (uint32_t)c->clut_Lc; B.rowtab = c->d_rowtab; B.S17 = c->clut_S17;
-            B.lpr = std::min(32, std::max(1, (c->h_ranges.lseq_max + 31) / 32)); B.rpw = 32 / B.lpr; B.err = c->d_err;
-            if (!c->d_rowtab) { CUDA_TRY(c, cudaMalloc(&c->d_rowtab, 512)); CUDA_TRY(c, cudaMemsetAsync(c->d_rowtab, 0, 512, c->stream)); }
-            B.rowtab = c->d_rowtab;
+            B.seq = c->seq.p; B.qual = c->qual.p; B.out = c->qual_out.p; B.rg_cov = c->d_rg_cov.p; B.n_rg = c->n_rg; B.cov_exists = c->d_cov_exists.p;
+            B.clut = with_lut ? c->d_clut.p : nullptr; B.clut_bytes = with_lut ? c->clut_bytes : 0; B.blk = c->clut_blk; B.Lc = (uint32_t)c->clut_Lc; B.rowtab = c->d_rowtab.p; B.S17 = c->clut_S17;
+            B.lpr = std::min(32, std::max(1, (c->h_ranges.lseq_max + 31) / 32)); B.rpw = 32 / B.lpr; B.err = c->d_err.p;
             int sms = 132; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device);
             const size_t smem = ((size_t)B.clut_bytes + 15) / 16 * 16 + (size_t)AP2_WARPS * (B.rpw * B.lpr * 32 + 32) + 16;
             CUDA_TRY(c, cudaFuncSetAttribute(bqsr_apply2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

@@ -414,15 +414,15 @@ int ensure_fin_state(elp_ctx* c) {
         if (!bin_set[c->device & 63]) { CUDA_TRY(c, cudaMemcpyToSymbol(c_bin, &bin_terms(), sizeof(BinTerms))); bin_set[c->device & 63] = true; }
     }
     const int nc = std::max(1, c->geom.n_cov);
-    if (!c->d_emp) CUDA_TRY(c, cudaMalloc(&c->d_emp, std::max<size_t>(1, c->geom.cells())));
-    if (!c->d_fin) CUDA_TRY(c, cudaMalloc(&c->d_fin, 2 * sizeof(double) * nc));
-    if (!c->d_cov_exists) CUDA_TRY(c, cudaMalloc(&c->d_cov_exists, nc));
-    if (!c->d_unobs) CUDA_TRY(c, cudaMalloc(&c->d_unobs, nc));
-    if (!c->d_qmaps) {   // the static quantization (initializeStaticQuantizedScores) depends on --sqq only
-        CUDA_TRY(c, cudaMalloc(&c->d_qmaps, QMAP_BYTES));
+    CUDA_TRY(c, c->d_emp.fit(std::max<size_t>(1, c->geom.cells())));
+    CUDA_TRY(c, c->d_fin.fit(2 * (size_t)nc));
+    CUDA_TRY(c, c->d_cov_exists.fit(nc));
+    CUDA_TRY(c, c->d_unobs.fit(nc));
+    if (!c->d_qmaps.p) {   // the static quantization (initializeStaticQuantizedScores) depends on --sqq only
+        CUDA_TRY(c, c->d_qmaps.fit(QMAP_BYTES));
         std::vector<uint8_t> m(QMAP_BYTES, 0);
         if (!c->sqq.empty()) { const std::vector<uint8_t> ss = static_quantized(c->sqq); std::copy(ss.begin(), ss.end(), m.begin() + QMAP_STAT); }
-        int rc = upload_small(c, c->d_qmaps, m.data(), m.size()); if (rc) return rc;
+        int rc = upload_small(c, c->d_qmaps.p, m.data(), m.size()); if (rc) return rc;
     }
     return E_OK;
 }
@@ -436,16 +436,16 @@ int phase_bqsr_finalize(elp_ctx* c, const char* report_path) {
     { int rc = ensure_fin_state(c); if (rc) return rc; }
     if (cells) {
         c->begin("bqsr_fin_emp", (double)cells * 17);
-        fin_emp_kernel<<<(unsigned)((cells + 255) / 256), 256, 0, c->stream>>>(c->d_tables, g, c->d_emp);
+        fin_emp_kernel<<<(unsigned)((cells + 255) / 256), 256, 0, c->stream>>>(c->d_tables.p, g, c->d_emp.p);
         c->end(); LAUNCH_CHECK(c);
     }
     c->begin("bqsr_fin_tail", (double)g.n_cov * 94 * 16);
-    fin_tail_kernel<<<1, FIN_T, 0, c->stream>>>(c->d_tables, g, c->d_emp, c->quantize_levels, c->sqq.empty() ? 0 : 1, c->d_fin, c->d_qmaps, c->d_cov_exists, c->d_unobs);
+    fin_tail_kernel<<<1, FIN_T, 0, c->stream>>>(c->d_tables.p, g, c->d_emp.p, c->quantize_levels, c->sqq.empty() ? 0 : 1, c->d_fin.p, c->d_qmaps.p, c->d_cov_exists.p, c->d_unobs.p);
     c->end(); LAUNCH_CHECK(c);
     if (report_path) {   // the report is host text: one copy of the tables and of EmpiricalQuality
         std::vector<int64_t> h_tables(cells * 2); std::vector<uint8_t> h_emp(cells);
-        CUDA_TRY(c, cudaMemcpyAsync(h_tables.data(), c->d_tables, cells * 2 * sizeof(int64_t), cudaMemcpyDeviceToHost, c->stream));
-        CUDA_TRY(c, cudaMemcpyAsync(h_emp.data(), c->d_emp, cells, cudaMemcpyDeviceToHost, c->stream));
+        CUDA_TRY(c, cudaMemcpyAsync(h_tables.data(), c->d_tables.p, cells * 2 * sizeof(int64_t), cudaMemcpyDeviceToHost, c->stream));
+        CUDA_TRY(c, cudaMemcpyAsync(h_emp.data(), c->d_emp.p, cells, cudaMemcpyDeviceToHost, c->stream));
         CUDA_TRY(c, cudaStreamSynchronize(c->stream));
         Tables T{g, h_tables.data()};
         std::vector<Combined> comb(g.n_cov);
@@ -463,14 +463,10 @@ int build_apply_lut(elp_ctx* c, int Lc) {
     if (!c->finalized) return c->fail(E_STATE, "apply look-up table requested before elp_bqsr_finalize");
     const TableGeom& g = c->geom;
     const size_t bytes = (size_t)g.n_cov * 94 * (2 * Lc + 1) * 17;
-    if (c->lut_cap < bytes + 16) {
-        if (c->d_lut) { cudaFree(c->d_lut); c->d_lut = nullptr; }
-        CUDA_TRY(c, cudaMalloc(&c->d_lut, bytes + 16));
-        c->lut_cap = bytes + 16;
-    }
+    CUDA_TRY(c, c->d_lut.fit(bytes + 16));
     if (g.n_cov) {
         c->begin("bqsr_fin_lut", (double)bytes);
-        fin_lut_kernel<<<(unsigned)(g.n_cov * 94), FIN_T, 0, c->stream>>>(c->d_tables, g, c->d_fin, c->d_qmaps, c->sqq.empty() ? 0 : 1, c->d_cov_exists, Lc, c->d_lut);
+        fin_lut_kernel<<<(unsigned)(g.n_cov * 94), FIN_T, 0, c->stream>>>(c->d_tables.p, g, c->d_fin.p, c->d_qmaps.p, c->sqq.empty() ? 0 : 1, c->d_cov_exists.p, Lc, c->d_lut.p);
         c->end(); LAUNCH_CHECK(c);
     }
     c->lut_maxcyc = Lc;
@@ -493,15 +489,14 @@ int build_compact_lut(elp_ctx* c) {
     for (int q = 6; q < 94; q++) if ((present[q >> 5] >> (q & 31)) & 1u) A.slot_q[A.n_slots++] = (uint8_t)q;
     const bool above93 = (present[2] >> 30) != 0 || present[3] != 0;   // bits 94..127
     const int S = A.n_slots + (above93 ? 1 : 0), Lc = c->lut_maxcyc, ncyc = 2 * Lc + 1, n_cov = c->geom.n_cov;
-    if (S == 0 || n_cov == 0 || !c->d_lut) return E_OK;
+    if (S == 0 || n_cov == 0 || !c->d_lut.p) return E_OK;
     uint32_t blk = (uint32_t)(n_cov * S * 17); if (!(blk & 1)) blk++;
     const size_t bytes = ((size_t)(ncyc + 64) * blk + 15) / 16 * 16;
     if (bytes > 80 * 1024) return E_OK;                               // too large for two CTAs per SM: the global-memory kernel serves
     for (int sl = 0; sl < A.n_slots; sl++) A.rowtab_h[A.slot_q[sl]] = (uint16_t)(sl * 17);
     if (above93) for (int q = 94; q < 256; q++) A.rowtab_h[q] = (uint16_t)((S - 1) * 17);
-    if (c->clut_cap < bytes) { if (c->d_clut) cudaFree(c->d_clut); c->d_clut = nullptr; CUDA_TRY(c, cudaMalloc(&c->d_clut, bytes)); c->clut_cap = bytes; }
-    if (!c->d_rowtab) CUDA_TRY(c, cudaMalloc(&c->d_rowtab, 512));
-    A.lut = c->d_lut; A.unobs = c->d_unobs; A.clut = c->d_clut; A.rowtab = c->d_rowtab;
+    CUDA_TRY(c, c->d_clut.fit(bytes));
+    A.lut = c->d_lut.p; A.unobs = c->d_unobs.p; A.clut = c->d_clut.p; A.rowtab = c->d_rowtab.p;
     A.bytes = (uint32_t)bytes; A.blk = blk; A.used = (uint32_t)(n_cov * S * 17); A.Lc = Lc; A.S = S;
     c->begin("bqsr_fin_clut", 2.0 * (double)bytes);
     fin_clut_kernel<<<(unsigned)((bytes + 255) / 256), 256, 0, c->stream>>>(A);
@@ -512,7 +507,7 @@ int build_compact_lut(elp_ctx* c) {
 
 int bqsr_empirical_copy(elp_ctx* c, uint8_t* emp) {
     if (c->geom.cells()) {
-        CUDA_TRY(c, cudaMemcpyAsync(emp, c->d_emp, c->geom.cells(), cudaMemcpyDeviceToHost, c->stream));
+        CUDA_TRY(c, cudaMemcpyAsync(emp, c->d_emp.p, c->geom.cells(), cudaMemcpyDeviceToHost, c->stream));
         CUDA_TRY(c, cudaStreamSynchronize(c->stream));
     }
     return E_OK;

@@ -778,22 +778,23 @@ __global__ void derive_q_kernel(TableGeom geom, long long* tables) {
 // (windows of reads at the start of a contig and the shifted window of an insertion start before base 0), 64 behind (the aligned
 // window loads past the last base). The n host bases pass through a temporary device buffer that is freed before the return; the copy
 // goes on the context's stream, since a pageable cudaMemcpy may return before its DMA has landed and the stream does not wait for it.
-// A contig that elp_load_reference installed lives inside refhot_block: its old buffer is not freed here.
-int pack_reference(elp_ctx* c, int contig, const uint8_t* bases) {
-    const uint64_t n = c->ref_len[contig], n_out = (n + 1) / 2;
-    if (c->d_refhot_raw[contig]) { if (c->refhot_separate(c->d_refhot_raw[contig])) cudaFree(c->d_refhot_raw[contig]); c->d_refhot_raw[contig] = nullptr; }
-    CUDA_TRY(c, cudaMalloc(&c->d_refhot_raw[contig], n_out + REFHOT_PAD + 64));
-    CUDA_TRY(c, cudaMemsetAsync(c->d_refhot_raw[contig], 0, n_out + REFHOT_PAD + 64, c->stream));
-    uint8_t* d_bases = nullptr;
-    cudaError_t e = n ? cudaMalloc(&d_bases, n) : cudaSuccess;
-    if (e == cudaSuccess && n) e = cudaMemcpyAsync(d_bases, bases, n, cudaMemcpyHostToDevice, c->stream);
+int pack_reference(elp_ctx* c, int contig, const uint8_t* bases, uint64_t n) {
+    const uint64_t n_out = (n + 1) / 2;
+    ContigTable<uint8_t>& t = c->ref;
+    t.clear(contig);
+    DBuf<uint8_t>& own = t.own[contig];
+    CUDA_TRY(c, own.fit(n_out + REFHOT_PAD + 64));
+    CUDA_TRY(c, cudaMemsetAsync(own.p, 0, n_out + REFHOT_PAD + 64, c->stream));
+    t.d[contig] = own.p + REFHOT_PAD; t.n[contig] = n;
+    DBuf<uint8_t> d_bases;
+    cudaError_t e = d_bases.fit(n);
+    if (e == cudaSuccess && n) e = cudaMemcpyAsync(d_bases.p, bases, n, cudaMemcpyHostToDevice, c->stream);
     if (e == cudaSuccess && n) {
         c->launches++;
-        ref_pack_hot_kernel<<<(unsigned)((n_out + 255) / 256), 256, 0, c->stream>>>(d_bases, n, c->d_refhot_raw[contig] + REFHOT_PAD, n_out);
+        ref_pack_hot_kernel<<<(unsigned)((n_out + 255) / 256), 256, 0, c->stream>>>(d_bases.p, n, own.p + REFHOT_PAD, n_out);
         e = cudaGetLastError();
     }
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    if (d_bases) cudaFree(d_bases);
     CUDA_TRY(c, e);
     return E_OK;
 }
@@ -938,25 +939,25 @@ template <int S> int launch_count(elp_ctx* c, CountArgs K, bool indel, unsigned 
 
 int phase_bqsr_gather(elp_ctx* c) {
     if (!c->sorted) return c->fail(E_STATE, "elp_bqsr_gather called before elp_sort_markdup");
-    int rc = upload_side_inputs(c);
-    if (!rc) rc = region_upload(c, c->known_sites);
-    if (rc) return rc;
+    TRY(table_upload(c, c->ref));
+    TRY(table_upload(c, c->known_sites));
+    int rc = E_OK;
     const size_t cells = c->geom.cells();
-    CUDA_TRY(c, cudaMemsetAsync(c->d_tables, 0, cells * 2 * sizeof(int64_t), c->stream));
+    CUDA_TRY(c, cudaMemsetAsync(c->d_tables.p, 0, cells * 2 * sizeof(int64_t), c->stream));
     const uint64_t n = c->n_sorted;                       // the output order: every read, or those elp_filter_target_regions kept
     c->gather_eligible = 0;
     if (n) {
         GatherArgs A{};
         A.n = n; A.refid = c->s_refid.p; A.pos = c->s_pos.p; A.nref = c->s_nref.p; A.pnext = c->s_pnext.p; A.tlen = c->s_tlen.p; A.rg = c->s_rg.p; A.lseq = c->s_lseq.p;
         A.flag = c->s_flag.p; A.mapq = c->s_mapq.p; A.optf = c->s_optf.p; A.qual_off = c->s_qual_off.p; A.seq_off = c->s_seq_off.p; A.cigar_off = c->s_cigar_off.p; A.ncigar = c->s_ncigar.p;
-        A.cigar = c->cigar.p; A.seq = c->seq.p; A.qual = c->qual.p; A.rg_cov = c->d_rg_cov; A.n_rg = c->n_rg; A.contig_len = c->d_contig_len; A.n_contigs = c->n_contigs;
-        A.refhot = c->d_refhot_ptrs; A.ref_len = c->d_ref_len; A.sites = c->known_sites.d_ptrs; A.n_sites = c->known_sites.d_n;
-        A.geom = c->geom; A.tables = reinterpret_cast<unsigned long long*>(c->d_tables); A.err = c->d_err;
-        uint64_t ref_bytes = 0; for (auto l : c->ref_len) ref_bytes += l;
+        A.cigar = c->cigar.p; A.seq = c->seq.p; A.qual = c->qual.p; A.rg_cov = c->d_rg_cov.p; A.n_rg = c->n_rg; A.contig_len = c->d_contig_len.p; A.n_contigs = c->n_contigs;
+        A.refhot = c->ref.d_ptrs.p; A.ref_len = c->ref.d_n.p; A.sites = c->known_sites.d_ptrs.p; A.n_sites = c->known_sites.d_n.p;
+        A.geom = c->geom; A.tables = reinterpret_cast<unsigned long long*>(c->d_tables.p); A.err = c->d_err.p;
+        uint64_t ref_bytes = 0; for (auto l : c->ref.n) ref_bytes += l;
         // SURVEY.md 8d: N_eligible * (19 + 4 + 4 c + L/2 + L) + genome bytes once; per-read averages of the arenas stand in for c and L
         const double per_read = 23.0 + ((double)c->n_cigar * 4 + (double)(c->n_seq - ARENA_FRONT_PAD) + (double)(c->n_qual - ARENA_FRONT_PAD)) / (double)c->n;
         uint32_t present[4] = {0, 0, 0, 0};
-        CUDA_TRY(c, cudaMemcpyAsync(present, c->d_qpresent, 16, cudaMemcpyDeviceToHost, c->stream));
+        CUDA_TRY(c, cudaMemcpyAsync(present, c->d_qpresent.p, 16, cudaMemcpyDeviceToHost, c->stream));
         CUDA_TRY(c, cudaStreamSynchronize(c->stream));
         const FastPlan F = plan_fast(c, present);
         if (!F.ok) {
@@ -969,7 +970,7 @@ int phase_bqsr_gather(elp_ctx* c) {
             const int lpr = std::min(32, std::max(1, (c->h_ranges.lseq_max + 31) / 32)), rpw = 32 / lpr;
             int sms = 132; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device);
             // small device words: [0,64) class histogram | [64,129) region bases | [136,265) list counters | [272,274) segment counts | [276,278) queue heads
-            uint32_t* sm = c->d_bq_small;
+            uint32_t* sm = c->d_bq_small.p;
             uint32_t *d_hist = sm, *d_region = sm + 64, *d_keycnt = sm + 136, *d_nseg = sm + 272, *d_next = sm + 276;
             CUDA_TRY(c, cudaMemsetAsync(sm, 0, 512 * 4, c->stream));
             const uint64_t seg_cap = n / ((uint64_t)SEG_PASSES * rpw) + 2 * MAX_CLS + 16;
@@ -989,7 +990,7 @@ int phase_bqsr_gather(elp_ctx* c) {
             seg_build_kernel<<<1, 128, 0, c->stream>>>(n_cls, rpw, d_region, d_keycnt, segs0, segs1, d_nseg);
             c->launches++; LAUNCH_CHECK(c);
             CountArgs K{};
-            K.qual = c->qual.p; K.seq = c->seq.p; K.refhot = c->d_refhot_ptrs; K.recs = c->bq_recs.p; K.tables = A.tables; K.geom = c->geom;
+            K.qual = c->qual.p; K.seq = c->seq.p; K.refhot = c->ref.d_ptrs.p; K.recs = c->bq_recs.p; K.tables = A.tables; K.geom = c->geom;
             K.lpr = lpr; K.rpw = rpw; K.rec_bytes = 32u * (uint32_t)rpw; K.n_cls = n_cls; K.sh = F.sh; K.lut_lo = F.lut_lo; K.lut_hi = F.lut_hi;
             for (int s = 0; s < 4; s++) K.slot_q[s] = F.slot_q[s];
             const unsigned grid = (unsigned)sms * CNT_MINB;
@@ -1019,7 +1020,7 @@ int phase_bqsr_gather(elp_ctx* c) {
         }
     }
     c->begin("bqsr_g_derive_q", 0);
-    derive_q_kernel<<<c->geom.n_cov * 94, 256, 0, c->stream>>>(c->geom, reinterpret_cast<long long*>(c->d_tables));
+    derive_q_kernel<<<c->geom.n_cov * 94, 256, 0, c->stream>>>(c->geom, reinterpret_cast<long long*>(c->d_tables.p));
     c->end(); LAUNCH_CHECK(c);
     rc = check_device_errors(c);
     if (rc) return rc;

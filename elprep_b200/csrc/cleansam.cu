@@ -8,7 +8,6 @@
 
 namespace {
 
-inline unsigned nblk(uint64_t n, int t) { return (unsigned)((n + t - 1) / t); }
 __device__ __forceinline__ int cons_read(uint32_t o) { return o == 0 || o == 1 || o == 4 || o == 7 || o == 8; }
 __device__ __forceinline__ int cons_ref(uint32_t o) { return o == 0 || o == 2 || o == 3 || o == 7 || o == 8; }
 // int32 addition as Go does it: wraps (`pos += endPos` doubles pos, so a long CIGAR overflows it)
@@ -84,7 +83,7 @@ extern "C" int elp_clean_sam(elp_ctx* c, uint64_t* n_rewritten) {
     uint32_t* d_changed = c->scan_tmp.p + n + 4;
     CUDA_TRY(c, cudaMemsetAsync(d_changed, 0, 4, s));
     c->begin("clean_sam_count", (double)n * 19 + (double)c->n_cigar * 4);
-    clean_count_kernel<<<nblk(n, 256), 256, 0, s>>>(n, c->flag.p, c->mapq.p, c->refid.p, c->pos.p, c->cigar_off.p, c->cigar.p, c->d_contig_len, c->n_contigs, c->scan_tmp.p, d_changed, c->d_err);
+    clean_count_kernel<<<nblk(n, 256), 256, 0, s>>>(n, c->flag.p, c->mapq.p, c->refid.p, c->pos.p, c->cigar_off.p, c->cigar.p, c->d_contig_len.p, c->n_contigs, c->scan_tmp.p, d_changed, c->d_err.p);
     c->end(); LAUNCH_CHECK(c);
     uint32_t changed = 0;
     CUDA_TRY(c, cudaMemcpyAsync(&changed, d_changed, 4, cudaMemcpyDeviceToHost, s));
@@ -96,18 +95,16 @@ extern "C" int elp_clean_sam(elp_ctx* c, uint64_t* n_rewritten) {
     DBuf<uint64_t> new_off; DBuf<uint32_t> new_cigar;
     CUDA_TRY(c, new_off.reserve(n + 2, s));
     rc = exclusive_scan_u32_to_u64(c, c->scan_tmp.p, new_off.p, n);
-    if (rc) { new_off.release(); return rc; }
+    if (rc) return rc;
     uint64_t total = 0;
     CUDA_TRY(c, cudaMemcpyAsync(&total, new_off.p + n, 8, cudaMemcpyDeviceToHost, s));
     CUDA_TRY(c, cudaStreamSynchronize(s));
     CUDA_TRY(c, new_cigar.reserve(std::max<uint64_t>(total + 16, c->cigar.cap), s));
     c->begin("clean_sam_write", (double)n * 26 + (double)c->n_cigar * 8);
-    clean_write_kernel<<<nblk(n, 256), 256, 0, s>>>(n, c->flag.p, c->refid.p, c->pos.p, c->cigar_off.p, c->cigar.p, c->d_contig_len, c->n_contigs, new_off.p, new_cigar.p, c->d_err);
+    clean_write_kernel<<<nblk(n, 256), 256, 0, s>>>(n, c->flag.p, c->refid.p, c->pos.p, c->cigar_off.p, c->cigar.p, c->d_contig_len.p, c->n_contigs, new_off.p, new_cigar.p, c->d_err.p);
     c->end(); LAUNCH_CHECK(c);
     CUDA_TRY(c, cudaStreamSynchronize(s));
-    std::swap(c->cigar.p, new_cigar.p); std::swap(c->cigar.cap, new_cigar.cap);
-    std::swap(c->cigar_off.p, new_off.p); std::swap(c->cigar_off.cap, new_off.cap);
-    new_cigar.release(); new_off.release();
+    std::swap(c->cigar, new_cigar); std::swap(c->cigar_off, new_off);
     c->n_cigar = total; c->n_cleaned += changed; c->adapted = false;
     return ELP_OK;
 }

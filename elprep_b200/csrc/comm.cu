@@ -54,7 +54,6 @@ NcclApi* nccl_api(std::string* err) {
 }
 #define NCCL_TRY(c, api, call) do { ncclResult_t r__ = (call); if (r__ != ncclSuccess) return (c)->fail(E_CUDA, "NCCL error at %s:%d: %s", __FILE__, __LINE__, (api)->GetErrorString(r__)); } while (0)
 
-inline unsigned nblk(uint64_t n, int t) { return (unsigned)((n + t - 1) / t); }
 constexpr int SP_REC = 128, SP_NAME = 92;   // bytes per spread record / of its QNAME
 
 // destination rank of a read's spread record, or -1: true pair entering duplicate marking (mark-duplicates.go:182-184, 436) whose mate maps to a
@@ -190,7 +189,7 @@ int comm_allreduce_ranges(elp_ctx* c, int local_rc) {
 // ships the visiting mates to the owners of their pairs and appends what arrives as ghost reads n .. n + n_ghost - 1
 int spread_exchange_begin(elp_ctx* c) {
     c->n_ghost = 0; c->sp_sent_total = 0;
-    if (!c->comm || c->world < 2 || !c->d_owner) return E_OK;
+    if (!c->comm || c->world < 2 || !c->d_owner.p) return E_OK;
     NcclApi* N = nccl_api(&c->err); if (!N) return E_CUDA;
     const uint64_t n = c->n; const int W = c->world; cudaStream_t s = c->stream;
     // per rank, W + 2 words are gathered: the records to every rank, the reads among them with a QNAME too long for a record, and the
@@ -199,7 +198,7 @@ int spread_exchange_begin(elp_ctx* c) {
     CUDA_TRY(c, c->scan_tmp.reserve(P * (W + 1) + 2 * W + 16, s));
     uint32_t* d_cnt = c->scan_tmp.p; uint32_t* d_all = d_cnt + P; uint32_t* d_base = d_all + P * W; uint32_t* d_cur = d_base + W;
     CUDA_TRY(c, cudaMemsetAsync(d_cnt, 0, (P * (W + 1) + 2 * W) * 4, s));
-    if (n) { c->begin("spread_count", (double)n * 10); spread_count_kernel<<<nblk(n, 256), 256, W * 4, s>>>(n, c->flag.p, c->refid.p, c->nref.p, c->qname_off.p, c->d_owner, c->n_contigs, c->rank, W, d_cnt); c->end(); LAUNCH_CHECK(c); }
+    if (n) { c->begin("spread_count", (double)n * 10); spread_count_kernel<<<nblk(n, 256), 256, W * 4, s>>>(n, c->flag.p, c->refid.p, c->nref.p, c->qname_off.p, c->d_owner.p, c->n_contigs, c->rank, W, d_cnt); c->end(); LAUNCH_CHECK(c); }
     NCCL_TRY(c, N, N->AllGather(d_cnt, d_all, P, ncclUint32, (ncclComm_t)c->comm, s));
     std::vector<uint32_t> all(P * W);
     CUDA_TRY(c, cudaMemcpyAsync(all.data(), d_all, all.size() * 4, cudaMemcpyDeviceToHost, s));
@@ -233,7 +232,7 @@ int spread_exchange_begin(elp_ctx* c) {
             { int rcu = upload_small(c, d_base, base.data(), (size_t)W * 4); if (rcu) return rcu; }
             FillArgs A{};
             A.n = n; A.flag = c->flag.p; A.refid = c->refid.p; A.nref = c->nref.p; A.rg = c->rg.p; A.upos = c->upos.p; A.score = c->score.p; A.qhash = c->qhash.p; A.qname_off = c->qname_off.p; A.qname = c->qname.p;
-            A.owner = c->d_owner; A.n_contigs = c->n_contigs; A.me = c->rank; A.base = d_base; A.cursor = d_cur; A.recs = c->sp_sendbuf.p; A.sent_idx = c->sp_sent_idx.p; A.err = c->d_err;
+            A.owner = c->d_owner.p; A.n_contigs = c->n_contigs; A.me = c->rank; A.base = d_base; A.cursor = d_cur; A.recs = c->sp_sendbuf.p; A.sent_idx = c->sp_sent_idx.p; A.err = c->d_err.p;
             c->begin("spread_fill", (double)n * 10 + (double)tot_send * 200); spread_fill_kernel<<<nblk(n, 256), 256, 0, s>>>(A); c->end(); LAUNCH_CHECK(c);
         }
         return E_OK;
@@ -271,7 +270,7 @@ int spread_exchange_begin(elp_ctx* c) {
 
 // returns the 0x400 bits of the ghosts to the ranks the reads live on
 int spread_exchange_end(elp_ctx* c) {
-    if (!c->comm || c->world < 2 || !c->d_owner) return E_OK;
+    if (!c->comm || c->world < 2 || !c->d_owner.p) return E_OK;
     NcclApi* N = nccl_api(&c->err); if (!N) return E_CUDA;
     const int W = c->world; cudaStream_t s = c->stream;
     const uint64_t g = c->n_ghost, m = c->sp_sent_total;
@@ -327,8 +326,8 @@ int elp_comm_set_partition(elp_ctx* c, const int32_t* contig_owner) {
     if (!c || !contig_owner) return ELP_EINVAL;
     cudaSetDevice(c->device);
     for (int i = 0; i < c->n_contigs; i++) if (contig_owner[i] < 0 || contig_owner[i] >= std::max(1, c->world)) return c->fail(E_INVAL, "elp_comm_set_partition: owner %d of contig %d is not a rank", contig_owner[i], i);
-    if (!c->d_owner) CUDA_TRY(c, cudaMalloc(&c->d_owner, std::max(1, c->n_contigs) * 4));
-    CUDA_TRY(c, cudaMemcpy(c->d_owner, contig_owner, (size_t)c->n_contigs * 4, cudaMemcpyHostToDevice));
+    CUDA_TRY(c, c->d_owner.fit(std::max(1, c->n_contigs)));
+    CUDA_TRY(c, cudaMemcpy(c->d_owner.p, contig_owner, (size_t)c->n_contigs * 4, cudaMemcpyHostToDevice));
     return ELP_OK;
 }
 
@@ -339,7 +338,7 @@ int elp_bqsr_tables_allreduce(elp_ctx* c) {
     if (!c->gathered) return c->fail(E_STATE, "elp_bqsr_tables_allreduce before elp_bqsr_gather");
     NcclApi* N = nccl_api(&c->err); if (!N) return ELP_ECUDA;
     c->begin("nccl_allreduce_tables", (double)c->geom.cells() * 16);
-    ncclResult_t r = N->AllReduce(c->d_tables, c->d_tables, c->geom.cells() * 2, ncclInt64, ncclSum, (ncclComm_t)c->comm, c->stream);
+    ncclResult_t r = N->AllReduce(c->d_tables.p, c->d_tables.p, c->geom.cells() * 2, ncclInt64, ncclSum, (ncclComm_t)c->comm, c->stream);
     c->end();
     if (r != ncclSuccess) return c->fail(E_CUDA, "ncclAllReduce: %s", N->GetErrorString(r));
     c->finalized = false;

@@ -18,8 +18,6 @@ constexpr int SHORT_RUN = 32;
 constexpr int QC0 = 4;          // chunk id of the last (least significant) QNAME chunk
 constexpr int FLAG_SLICE = 64;  // chunks tie_long_flag_kernel reduces per round through shared memory
 
-inline unsigned nblk(uint64_t n, int t) { return (unsigned)((n + t - 1) / t); }
-
 struct CoordLayout { int bP, bR; int n_contigs; int key_bits; };
 
 CoordLayout coord_layout(const elp_ctx* c) {   // after phase_adapt (pos_max)

@@ -1,34 +1,66 @@
 // ctx.h -- the device context behind the C ABI (include/elprep_b200.h).
 #pragma once
 #include <cuda_runtime.h>
+#include <algorithm>
+#include <atomic>
 #include <cstdarg>
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
 #include <map>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <vector>
 #include "common.cuh"
 #include "radix_sort.cuh"
 
-// simple growable device buffer
-template <class T> struct DBuf {
+// Owners of device and page-locked host memory.  Every allocation has exactly one owner, which frees it when it is destroyed; owners
+// move but never copy.  Kernels take the raw pointer (.p), or a trivially copyable argument struct built from raw pointers, never an
+// owner.  g_live_allocations counts the allocations all owners of the process hold (elp_debug_live_allocations).
+extern std::atomic<int64_t> g_live_allocations;
+
+template <class T, bool PINNED> struct Owned {
     T* p = nullptr;
     size_t cap = 0;   // elements
-    cudaError_t reserve(size_t n, cudaStream_t s, size_t keep = 0) {   // keeps the first `keep` elements
+    Owned() = default;
+    Owned(Owned&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+    Owned& operator=(Owned&& o) noexcept {
+        if (this != &o) { release(); p = o.p; cap = o.cap; o.p = nullptr; o.cap = 0; }
+        return *this;
+    }
+    ~Owned() { release(); }
+    // exactly n elements (the fixed buffers); reallocates, without keeping the contents, only when n exceeds the capacity
+    cudaError_t fit(size_t n, unsigned host_flags = cudaHostAllocDefault) {
         if (n <= cap) return cudaSuccess;
-        size_t ncap = n + n / 8 + 64;
+        release();
         T* q = nullptr;
-        cudaError_t e = cudaMalloc(&q, ncap * sizeof(T));
+        const cudaError_t e = PINNED ? cudaHostAlloc(&q, n * sizeof(T), host_flags) : cudaMalloc(&q, n * sizeof(T));
         if (e != cudaSuccess) return e;
-        if (p && keep) { e = cudaMemcpyAsync(q, p, keep * sizeof(T), cudaMemcpyDeviceToDevice, s); if (e != cudaSuccess) return e; }
-        if (p) { cudaStreamSynchronize(s); cudaFree(p); }
-        p = q; cap = ncap;
+        p = q; cap = n; g_live_allocations++;
         return cudaSuccess;
     }
-    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
+    void release() {
+        if (p) { if (PINNED) cudaFreeHost(p); else cudaFree(p); g_live_allocations--; }
+        p = nullptr; cap = 0;
+    }
 };
+
+// growable device buffer
+template <class T> struct DBuf : Owned<T, false> {
+    // at least n elements, with room to grow; keeps the first `keep` elements
+    cudaError_t reserve(size_t n, cudaStream_t s, size_t keep = 0) {
+        if (n <= this->cap) return cudaSuccess;
+        DBuf q;
+        cudaError_t e = q.fit(n + n / 8 + 64);
+        if (e != cudaSuccess) return e;
+        if (this->p && keep) { e = cudaMemcpyAsync(q.p, this->p, keep * sizeof(T), cudaMemcpyDeviceToDevice, s); if (e != cudaSuccess) return e; }
+        if (this->p) cudaStreamSynchronize(s);
+        Owned<T, false>::operator=(std::move(q));
+        return cudaSuccess;
+    }
+};
+template <class T> using HBuf = Owned<T, true>;   // page-locked host memory (cudaHostAlloc)
 
 // duplication metrics of one library (filters.DuplicatesCtr, mark-optical-duplicates.go:95-110): the seven counters in the
 // reference's field order and the three count histograms (all, non-optical, optical)
@@ -39,16 +71,55 @@ struct DupCounters { int64_t ctr[7] = {0, 0, 0, 0, 0, 0, 0}; std::map<int64_t, i
 #define OPT_HBINS 1024
 #define OPT_OVF_CAP (1 << 16)
 
-// per-contig interval table on the device (the ingest filter's target regions, elp_filter_target_regions' regions and the BQSR known
-// sites): per contig, the flattened, start-sorted (start, end) pairs, and the two device arrays of pointers and counts the kernels
-// index by REFID (region_set / region_upload, bam_ingest.cu).  elp_load_known_sites installs every contig's list in one allocation,
-// `block`; a d[i] inside it is not an allocation of its own (separate() is false) and is freed with the block.
-struct RegionTable {
-    std::vector<int32_t*> d; std::vector<uint64_t> n;
-    const int32_t** d_ptrs = nullptr; uint64_t* d_n = nullptr; bool dirty = true;
-    int32_t* block = nullptr; uint64_t block_pairs = 0;
-    bool separate(const int32_t* p) const { return !block || p < block || p >= block + 2 * block_pairs; }
+// Per-contig table on the device, indexed by REFID: the interval tables (RegionTable: per contig the flattened, start-sorted (start, end)
+// pairs, n counts pairs) and the reference (per contig the one-hot nibbles, d at the payload, n counts bases).  d[i] is the view of contig
+// i (null: nothing).  It points into own[i], the buffer elp_set_* made for that contig, or into `block`, the one allocation the last
+// elp_load_* filled for every contig; the block lives until the next load or the context's end, whatever elp_set_* replaced since.
+// The kernels read the views through d_ptrs and d_n, uploaded when dirty (table_upload).
+template <class T> struct ContigTable {
+    std::vector<T*> d; std::vector<uint64_t> n;
+    std::vector<DBuf<T>> own;
+    DBuf<T> block;
+    DBuf<const T*> d_ptrs; DBuf<uint64_t> d_n;
+    bool dirty = true;
+    void resize(int nc) { d.assign(nc, nullptr); n.assign(nc, 0); own.clear(); own.resize(nc); dirty = true; }
+    // contig i loses its view and its own buffer (elp_set_* then allocates own[i] and points d[i] into it)
+    void clear(int i) { own[i].release(); d[i] = nullptr; n[i] = 0; dirty = true; }
+    // every contig replaced by the views into b (elp_load_*)
+    void install(DBuf<T>&& b, std::vector<T*>&& views, std::vector<uint64_t>&& counts) {
+        block = std::move(b); own.clear(); own.resize(views.size());
+        d = std::move(views); n = std::move(counts); dirty = true;
+    }
 };
+using RegionTable = ContigTable<int32_t>;
+
+// "*" and every @SQ SN, sorted bytewise.  id: the refid of dictTable / AddREFID ("*" -> -1, an @SQ SN -> its index, the last of equal
+// names wins).  all[all_off[e], all_off[e + 1]): every @SQ index with entry e's name, in header order ("*" has none).  The view the
+// kernels take (text_parse.cuh name_entry, refid_of).
+struct NameDict {
+    uint8_t* names = nullptr; uint32_t* off = nullptr; int32_t* id = nullptr;
+    uint32_t* all_off = nullptr; int32_t* all = nullptr;
+    int n = 0;
+};
+// its owner: one per context, uploaded on first use (name_dict_upload, text_parse.cuh) by elp_append_sam and elp_load_known_sites
+struct NameDictBufs {
+    DBuf<uint8_t> names; DBuf<uint32_t> off; DBuf<int32_t> id; DBuf<uint32_t> all_off; DBuf<int32_t> all;
+    int n = 0;   // entries; 0 until uploaded
+    NameDict view() const { return NameDict{names.p, off.p, id.p, all_off.p, all.p, n}; }
+};
+
+// the radix sort's device workspace (sort.cu)
+struct SortWorkspace {
+    DBuf<uint32_t> ghist, gofs;   // [MAX_PASSES][RADIX]
+    DBuf<uint32_t> counters;      // [MAX_PASSES]
+    DBuf<uint32_t> status;        // [passes][tiles][RADIX]
+};
+
+// State of a module that the context owns through a StatePtr; each module defines free_state for its type, where the type is complete.
+struct SamState; struct SamOutState; struct BgzfStream; struct DeflateState; struct SitesStage;
+void free_state(SamState* p); void free_state(SamOutState* p); void free_state(BgzfStream* p); void free_state(DeflateState* p); void free_state(SitesStage* p);
+struct FreeState { template <class T> void operator()(T* p) const { free_state(p); } };
+template <class T> using StatePtr = std::unique_ptr<T, FreeState>;
 
 struct KernelStat { uint64_t launches = 0; double ms = 0, alg_bytes = 0; };
 struct PendingEvent { std::string name; cudaEvent_t a, b; double alg_bytes; };
@@ -68,7 +139,7 @@ struct elp_ctx {
     cudaStream_t stream = nullptr;
     cudaStream_t copy_in = nullptr, copy_out = nullptr;   // upload / download streams of the asynchronous append / fetch
     cudaEvent_t ev_in = nullptr, ev_staged = nullptr, ev_out = nullptr;
-    void* h_stage = nullptr; size_t stage_off = 0;        // page-locked staging of upload_small
+    HBuf<uint8_t> h_stage; size_t stage_off = 0;         // page-locked staging of upload_small
     std::string err;
     std::mutex append_mu;
     bool profile = false;
@@ -85,21 +156,16 @@ struct elp_ctx {
     int max_cycle = 500, quantize_levels = 0, optical_pixel_distance = 100;
     std::vector<uint8_t> sqq;
     std::string prefix = "GATK";
-    int32_t* d_rg_lib = nullptr;     // [n_rg]
-    int32_t* d_rg_cov = nullptr;     // [n_rg]
-    int32_t* d_contig_len = nullptr; // [n_contigs]
+    DBuf<int32_t> d_rg_lib;          // [n_rg]
+    DBuf<int32_t> d_rg_cov;          // [n_rg]
+    DBuf<int32_t> d_contig_len;      // [n_contigs]
 
     // ---- reference genome + known sites (device) ----
-    std::vector<uint64_t> ref_len;
-    std::vector<uint8_t*> d_refhot_raw;   // per contig: the reference as one-hot nibbles (bqsr_gather.cu pack_reference), payload at +REFHOT_PAD
-    uint8_t* refhot_block = nullptr; uint64_t refhot_block_bytes = 0;   // elp_load_reference installs every contig in this one allocation
-    bool refhot_separate(const uint8_t* p) const { return !refhot_block || p < refhot_block || p >= refhot_block + refhot_block_bytes; }
+    ContigTable<uint8_t> ref;                // elp_set_reference / elp_load_reference: one-hot nibbles (bqsr_gather.cu pack_reference), REFHOT_PAD
+                                             // bytes in front of each view and 64 behind; n: the contig's bases
     uint64_t ref_chunk = 0;                  // elp_debug_set_reference_chunk: bytes per staging chunk of elp_load_reference (0: the default)
-    const uint8_t** d_refhot_ptrs = nullptr;   // [n_contigs] device array of the payload pointers
-    uint64_t* d_ref_len = nullptr;
-    bool side_dirty = true;
     RegionTable known_sites;                 // elp_set_known_sites / elp_load_known_sites (survives elp_reset)
-    struct SitesStage* sites = nullptr;      // page-locked and device staging of elp_load_known_sites (known_sites.cu)
+    StatePtr<SitesStage> sites;              // page-locked and device staging of elp_load_known_sites (known_sites.cu)
     uint64_t sites_chunk = 0;                // elp_debug_set_sites_chunk: bytes per staging chunk (0: the default)
 
     // ---- reads, arrival order (SoA columns) ----
@@ -118,43 +184,44 @@ struct elp_ctx {
     bool clear_dup = false;                   // elp_set_ingest_filter ELP_FILTER_CLEAR_DUPLICATE_FLAG: 0x400 cleared in the FLAG column at ingest
     // write-phase filters of elp_fetch_bam / elp_fetch_sam (elp_set_output_filter; survive elp_reset)
     uint32_t out_mask = 0;                    // record bits (ELP_OUT_REMOVE_DUPLICATES, ELP_OUT_REMOVE_OPTIONAL_READS)
-    uint32_t* d_out_drop = nullptr; bool out_fields = false;   // 65 536-bit tag table (bit set: the field is dropped); out_fields: some bit is set
+    DBuf<uint32_t> d_out_drop; bool out_fields = false;        // 65 536-bit tag table (bit set: the field is dropped); out_fields: some bit is set
     DBuf<uint32_t> out_sel; uint64_t n_out = 0; bool out_sel_valid = false;   // output positions of the records that pass, built on first use
     RegionTable regions;                     // --filter-non-overlapping-reads: the ingest filter ELP_FILTER_TARGET_REGIONS (elp_set_target_regions)
     RegionTable bqsr_regions;                // --target-regions: elp_filter_target_regions after marking (elp_set_bqsr_target_regions); both survive elp_reset
     uint64_t n_cleaned = 0;                  // reads whose CIGAR elp_clean_sam rewrote
     bool has_contig_names = false;           // elp_config.contig_names was given (elp_append_sam resolves RNAME / RNEXT against it)
-    struct SamState* sam = nullptr;          // device tables and staging of elp_append_sam (sam_ingest.cu)
+    StatePtr<SamState> sam;                  // device staging of elp_append_sam (sam_ingest.cu)
+    NameDictBufs names;                      // RNAME / RNEXT and known-sites chromosome dictionary
     uint64_t n_sam_lost_names = 0;           // reads of elp_append_sam whose RNAME / RNEXT text the stored record cannot reproduce (elp_fetch_sam refuses)
-    struct SamOutState* sam_out = nullptr;   // @SQ names and float staging of elp_fetch_sam (sam_format.cu)
-    struct BgzfStream* bgzf = nullptr;       // carried bytes and device staging of elp_append_bgzf / elp_debug_inflate (bgzf_inflate.cu)
-    struct DeflateState* bgzf_out = nullptr;  // device scratch of elp_fetch_bgzf / elp_debug_deflate (bgzf_deflate.cu)
+    StatePtr<SamOutState> sam_out;           // @SQ names and float staging of elp_fetch_sam (sam_format.cu)
+    StatePtr<BgzfStream> bgzf;               // carried bytes and device staging of elp_append_bgzf / elp_debug_inflate (bgzf_inflate.cu)
+    StatePtr<DeflateState> bgzf_out;         // device scratch of elp_fetch_bgzf / elp_debug_deflate (bgzf_deflate.cu)
     bool bgzf_open = false;                  // a BGZF file is open (elp_append_bgzf until elp_append_bgzf_end or elp_reset): the other appends
                                              // and elp_sort_markdup refuse, as the file's records are not all in yet
-    uint8_t* d_rg_names = nullptr; uint32_t* d_rg_name_off = nullptr; std::vector<std::string> rg_ids;   // @RG IDs for the RG:Z match
+    DBuf<uint8_t> d_rg_names; DBuf<uint32_t> d_rg_name_off; std::vector<std::string> rg_ids;   // @RG IDs for the RG:Z match
     DBuf<int32_t> lseq_stage;       // staging for l_seq of the batch being appended
     DBuf<uint64_t> off_stage;       // staging for batch-relative offsets
 
     // ---- per-read temps (arrival order) ----
     DBuf<int32_t> upos, score;
     DBuf<uint64_t> qhash;
-    DeviceRanges* d_ranges = nullptr;
+    DBuf<DeviceRanges> d_ranges;
     DeviceRanges h_ranges{};
-    uint32_t* d_err = nullptr;       // device error word
+    DBuf<uint32_t> d_err;            // device error word
     bool adapted = false;
 
     // ---- sort scratch ----
     DBuf<uint64_t> keys_a, keys_b;           // u64 keys, or u128 keys as pairs (2 words per key)
     DBuf<uint32_t> vals_a, vals_b;
-    rs::Workspace ws;
+    SortWorkspace ws;
     DBuf<uint32_t> mate;                      // [n] mate index or 0xffffffff
     DBuf<uint32_t> pair_a, pair_b, scan_tmp, scan_blk;
     DBuf<int32_t> pair_score;                 // [npairs] summed phred score of both mates of a pair (duplicate marking)
     DBuf<uint64_t> tie_bits;                  // [2][chunks] OR and AND of each chunk key over the long tie runs (coordinate sort)
     DBuf<uint8_t> bytes_tmp;
     DBuf<uint4> bq_recs, bq_segs;             // BQSR count kernel: work records of the eligible reads, segment table
-    uint32_t* d_bq_small = nullptr;           // class histogram, region bases, list counters, segment counts, work-queue heads
-    uint32_t* d_qpresent = nullptr;           // [4] bit q set iff QUAL value q (0..127) occurs in the arena (maintained at ingest)
+    DBuf<uint32_t> d_bq_small;                // class histogram, region bases, list counters, segment counts, work-queue heads
+    DBuf<uint32_t> d_qpresent;                // [4] bit q set iff QUAL value q (0..127) occurs in the arena (maintained at ingest)
     uint32_t h_qpresent[4] = {0, 0, 0, 0};    // its host copy, taken with h_ranges (phase_adapt, elp_filter_target_regions)
 
     // ---- output order ----
@@ -172,29 +239,28 @@ struct elp_ctx {
 
     // ---- BQSR ----
     TableGeom geom;
-    int64_t* d_tables = nullptr;              // dense [cells][2]
-    uint8_t* d_emp = nullptr;                 // [cells] EmpiricalQuality (elp_bqsr_finalize)
-    double* d_fin = nullptr;                  // [n_cov][2] reported quality of the combined read-group entry, read-group term dG
-    uint8_t* d_qmaps = nullptr;               // quantization map [0, 94), static --sqq map at [96, 350) (bqsr_finalize.cu)
+    DBuf<int64_t> d_tables;                   // dense [cells][2]
+    DBuf<uint8_t> d_emp;                      // [cells] EmpiricalQuality (elp_bqsr_finalize)
+    DBuf<double> d_fin;                       // [n_cov][2] reported quality of the combined read-group entry, read-group term dG
+    DBuf<uint8_t> d_qmaps;                    // quantization map [0, 94), static --sqq map at [96, 350) (bqsr_finalize.cu)
     bool gathered = false, finalized = false;
     uint64_t gather_eligible = 0;             // reads the last elp_bqsr_gather recalibrated (what the roofline line charges)
-    uint8_t* d_lut = nullptr;                 // [n_cov][94][2*lut_maxcyc+1][17]
+    DBuf<uint8_t> d_lut;                      // [n_cov][94][2*lut_maxcyc+1][17]
     int lut_maxcyc = 0;
-    size_t lut_cap = 0;
-    uint8_t* d_cov_exists = nullptr;          // [n_cov]
-    uint8_t* d_unobs = nullptr;               // [n_cov] recalibrated byte of a QUAL value without table entries (QUAL 94..255)
-    uint8_t* d_clut = nullptr; uint16_t* d_rowtab = nullptr;   // compact apply table for the shared-memory kernel: [cycle][covariate][slot][17], QUAL -> slot offset
-    uint32_t clut_bytes = 0, clut_blk = 0, clut_S17 = 0; int clut_Lc = 0; size_t clut_cap = 0; uint32_t clut_present[4] = {0, 0, 0, 0};
+    DBuf<uint8_t> d_cov_exists;               // [n_cov]
+    DBuf<uint8_t> d_unobs;                    // [n_cov] recalibrated byte of a QUAL value without table entries (QUAL 94..255)
+    DBuf<uint8_t> d_clut; DBuf<uint16_t> d_rowtab;   // compact apply table for the shared-memory kernel: [cycle][covariate][slot][17], QUAL -> slot offset
+    uint32_t clut_bytes = 0, clut_blk = 0, clut_S17 = 0; int clut_Lc = 0; uint32_t clut_present[4] = {0, 0, 0, 0};
 
     // ---- duplication metrics (optical.cu) ----
-    void* d_opt_ctr = nullptr; void* d_opt_hist = nullptr; void* d_opt_ovf = nullptr; uint32_t* d_opt_small = nullptr;
+    DBuf<unsigned long long> d_opt_ctr, d_opt_hist, d_opt_ovf; DBuf<uint32_t> d_opt_small;
     std::vector<DupCounters> opt;             // [n_lib + 1], slot 0 = "Unknown Library"
     bool opt_valid = false;
 
     // ---- several GPUs (comm.cu) ----
     void* comm = nullptr;                     // ncclComm_t
     int rank = 0, world = 1;
-    int32_t* d_owner = nullptr;               // [n_contigs] rank owning each contig
+    DBuf<int32_t> d_owner;                    // [n_contigs] rank owning each contig
     uint64_t n_ghost = 0, sp_sent_total = 0;  // visiting mates appended behind the local reads during duplicate marking; records this rank sent
     std::vector<uint32_t> sp_send, sp_recv;   // records to / from every rank
     DBuf<uint4> sp_sendbuf, sp_recvbuf; DBuf<uint32_t> sp_sent_idx;
@@ -206,6 +272,8 @@ struct elp_ctx {
     std::vector<PendingEvent> pending;
     std::vector<cudaEvent_t> event_pool;
     cudaEvent_t timer_a = nullptr, timer_b = nullptr;
+
+    ~elp_ctx();   // api.cu: the streams and events; the owners free the memory
 
     int fail(int code, const char* fmt, ...) {
         char buf[1024];
@@ -249,6 +317,30 @@ struct elp_ctx {
     } while (0)
 
 #define LAUNCH_CHECK(ctx) CUDA_TRY(ctx, cudaGetLastError())
+#define TRY(x) do { int rc__ = (x); if (rc__) return rc__; } while (0)
+
+inline unsigned nblk(uint64_t n, int t) { return (unsigned)((n + t - 1) / t); }
+
+template <class T> int grow(elp_ctx* c, DBuf<T>& b, size_t need, size_t keep = 0) {
+    cudaError_t e = b.reserve(need, c->stream, keep);
+    if (e != cudaSuccess) return c->fail(e == cudaErrorMemoryAllocation ? E_NOMEM : E_CUDA, "device allocation of %zu bytes failed: %s", need * sizeof(T), cudaGetErrorString(e));
+    return E_OK;
+}
+
+// the views and counts of a per-contig table -> d_ptrs / d_n.  Uploads go on the context's stream and are waited for: a pageable cudaMemcpy
+// may return before its DMA has landed, and the (non-blocking) stream of the kernels that read the table does not wait for it.
+template <class T> int table_upload(elp_ctx* c, ContigTable<T>& t) {
+    if (!t.dirty) return E_OK;
+    const size_t nc = std::max(1, c->n_contigs);
+    CUDA_TRY(c, t.d_ptrs.fit(nc)); CUDA_TRY(c, t.d_n.fit(nc));
+    if (c->n_contigs) {
+        CUDA_TRY(c, cudaMemcpyAsync(t.d_ptrs.p, t.d.data(), c->n_contigs * sizeof(void*), cudaMemcpyHostToDevice, c->stream));
+        CUDA_TRY(c, cudaMemcpyAsync(t.d_n.p, t.n.data(), c->n_contigs * 8, cudaMemcpyHostToDevice, c->stream));
+        CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+    }
+    t.dirty = false;
+    return E_OK;
+}
 
 // ---- internal phase entry points (implemented in the .cu files) ----
 // stable sort by key bits [lo_bit, lo_bit + key_bits); the bits below lo_bit do not take part in the order
@@ -267,8 +359,7 @@ int phase_bqsr_apply(elp_ctx* c);
 int build_apply_lut(elp_ctx* c, int Lc);   // bqsr_finalize.cu
 int build_compact_lut(elp_ctx* c);
 int bqsr_empirical_copy(elp_ctx* c, uint8_t* emp);   // device EmpiricalQuality -> host (synchronises)
-int upload_side_inputs(elp_ctx* c);
-int pack_reference(elp_ctx* c, int contig, const uint8_t* bases);   // bases: ref_len[contig] host bytes
+int pack_reference(elp_ctx* c, int contig, const uint8_t* bases, uint64_t n);   // bases: n host bytes
 int check_device_errors(elp_ctx* c);
 int upload_small(elp_ctx* c, void* dst, const void* src, size_t bytes);   // api.cu: host -> device without the copy engine
 int comm_allreduce_ranges(elp_ctx* c, int local_rc);   // comm.cu: returns local_rc, or a peer's error code
@@ -279,16 +370,9 @@ int qual_presence_update(elp_ctx* c, uint64_t first_byte, uint64_t n_bytes);   /
 int bam_ingest_core(elp_ctx* c, uint64_t n_bytes, uint64_t nrec);   // bam_ingest.cu: records staged in bam_raw / bam_off -> reads (elp_append_bam, elp_append_sam)
 int out_select(elp_ctx* c, const uint32_t** sel, uint64_t* n_out);   // bam_ingest.cu: the record filters' selection (sel null and n_out = n_sorted without record bits)
 int region_set(elp_ctx* c, RegionTable& t, const char* who, int32_t contig, const int32_t* se, uint64_t n_intervals, int already_flat);   // bam_ingest.cu
-int region_upload(elp_ctx* c, RegionTable& t);
-void region_release(RegionTable& t);
 int build_output_columns(elp_ctx* c, const uint32_t* perm, uint64_t n_out, bool refilter);   // coordsort.cu: s_* columns and s_out_off of perm[0, n_out)
 int phase_target_filter(elp_ctx* c, uint64_t* n_removed);   // target_regions.cu
-void sam_state_release(elp_ctx* c);   // sam_ingest.cu
-void sites_release(elp_ctx* c);       // known_sites.cu
-void sam_out_release(elp_ctx* c);     // sam_format.cu
 void bgzf_stream_reset(elp_ctx* c);   // bgzf_inflate.cu: forget the open file (elp_reset)
-void bgzf_release(elp_ctx* c);
 struct BgzfBlock;
 int bgzf_inflate_run(elp_ctx* c, const char* who, const uint8_t* in, uint64_t n_in, const std::vector<BgzfBlock>& blocks, uint64_t total, uint8_t* out);   // bgzf_inflate.cu: whole blocks -> out
 int bgzf_deflate_run(elp_ctx* c, const uint8_t* in, uint64_t n, int write_eof, uint8_t* out, uint64_t* out_n);   // bgzf_deflate.cu: in[0, n) on the device -> BGZF at out
-void bgzf_deflate_release(elp_ctx* c);

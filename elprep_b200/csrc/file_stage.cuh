@@ -13,29 +13,24 @@
 
 struct FileStage {
     uint64_t chunk = 0, hcap = 0, dcap = 0;                      // file bytes per step; capacities of h[b] and d[b]
-    uint8_t* h[2] = {nullptr, nullptr};                          // page-locked
-    uint8_t* d[2] = {nullptr, nullptr};
+    HBuf<uint8_t> h[2];
+    DBuf<uint8_t> d[2];
     cudaEvent_t up[2] = {nullptr, nullptr};                      // the upload out of h[b] has landed in d[b] (copy stream)
     cudaEvent_t used[2] = {nullptr, nullptr};                    // the kernels that read d[b] are done (compute stream)
     cudaStream_t copy = nullptr;
+    FileStage() = default;
+    FileStage(const FileStage&) = delete;
+    ~FileStage() {   // the chunks are freed after the last upload out of them
+        if (copy) cudaStreamSynchronize(copy);
+        for (int b = 0; b < 2; b++) { if (up[b]) cudaEventDestroy(up[b]); if (used[b]) cudaEventDestroy(used[b]); }
+        if (copy) cudaStreamDestroy(copy);
+    }
 };
 
 // a chunk of whole lines at the front of h[b]: m bytes; last: the file ends with it; long_tail: the carried line is already too long
 struct LineChunk { int b = 0; uint64_t m = 0; bool last = false, long_tail = false; };
 
 namespace {
-
-inline void stage_release(FileStage& S) {
-    if (S.copy) cudaStreamSynchronize(S.copy);
-    for (int b = 0; b < 2; b++) {
-        if (S.h[b]) cudaFreeHost(S.h[b]);
-        if (S.d[b]) cudaFree(S.d[b]);
-        if (S.up[b]) cudaEventDestroy(S.up[b]);
-        if (S.used[b]) cudaEventDestroy(S.used[b]);
-    }
-    if (S.copy) cudaStreamDestroy(S.copy);
-    S = FileStage();
-}
 
 // the stream, the events, and both chunks of hcap host and dcap device bytes (kept when the sizes are unchanged)
 inline int stage_init(elp_ctx* c, FileStage& S, uint64_t chunk, uint64_t hcap, uint64_t dcap, const char* who) {
@@ -45,14 +40,10 @@ inline int stage_init(elp_ctx* c, FileStage& S, uint64_t chunk, uint64_t hcap, u
     }
     if (S.chunk == chunk && S.hcap == hcap && S.dcap == dcap) return E_OK;
     CUDA_TRY(c, cudaStreamSynchronize(S.copy));
-    for (int b = 0; b < 2; b++) {
-        if (S.h[b]) cudaFreeHost(S.h[b]);
-        if (S.d[b]) cudaFree(S.d[b]);
-        S.h[b] = S.d[b] = nullptr;
-    }
+    for (int b = 0; b < 2; b++) { S.h[b].release(); S.d[b].release(); }
     S.chunk = S.hcap = S.dcap = 0;
     for (int b = 0; b < 2; b++) {
-        if (cudaHostAlloc(&S.h[b], hcap, cudaHostAllocDefault) != cudaSuccess || cudaMalloc(&S.d[b], dcap) != cudaSuccess) {
+        if (S.h[b].fit(hcap) != cudaSuccess || S.d[b].fit(dcap) != cudaSuccess) {
             cudaGetLastError();
             return c->fail(E_NOMEM, "%s: staging allocation of 2 x %llu bytes failed", who, (unsigned long long)hcap);
         }
@@ -75,8 +66,8 @@ inline int stage_upload(elp_ctx* c, FileStage& S, int b, uint64_t n, uint64_t at
     if (!n) return E_OK;
     const uint64_t padded = stage_padded(at + n);
     CUDA_TRY(c, cudaStreamWaitEvent(S.copy, S.used[b], 0));
-    CUDA_TRY(c, cudaMemcpyAsync(S.d[b] + at, S.h[b], n, cudaMemcpyHostToDevice, S.copy));
-    CUDA_TRY(c, cudaMemsetAsync(S.d[b] + at + n, 0, padded - at - n, S.copy));
+    CUDA_TRY(c, cudaMemcpyAsync(S.d[b].p + at, S.h[b].p, n, cudaMemcpyHostToDevice, S.copy));
+    CUDA_TRY(c, cudaMemsetAsync(S.d[b].p + at + n, 0, padded - at - n, S.copy));
     CUDA_TRY(c, cudaEventRecord(S.up[b], S.copy));
     return E_OK;
 }
@@ -84,7 +75,7 @@ inline int stage_upload(elp_ctx* c, FileStage& S, int b, uint64_t n, uint64_t at
 // the carried bytes and the next chunk of the file into h[b]; lines of max_line bytes or more cannot be carried
 inline int stage_read_lines(elp_ctx* c, FileStage& S, FILE* f, const char* path, const char* who, uint64_t max_line, std::vector<uint8_t>& carry, int b, LineChunk* ch) {
     if (const int rc = stage_wait_host(c, S, b)) return rc;
-    uint8_t* h = S.h[b];
+    uint8_t* h = S.h[b].p;
     const uint64_t nc = carry.size();
     if (nc) memcpy(h, carry.data(), nc);
     const size_t got = fread(h + nc, 1, S.chunk, f);

@@ -178,7 +178,7 @@ extern "C" {
 int elp_bqsr_tables_clear(elp_ctx* c) {
     if (!c) return ELP_EINVAL;
     cudaSetDevice(c->device);
-    CUDA_TRY(c, cudaMemsetAsync(c->d_tables, 0, c->geom.cells() * 2 * sizeof(int64_t), c->stream));
+    CUDA_TRY(c, cudaMemsetAsync(c->d_tables.p, 0, c->geom.cells() * 2 * sizeof(int64_t), c->stream));
     CUDA_TRY(c, cudaStreamSynchronize(c->stream));
     c->gathered = true; c->finalized = false;
     return ELP_OK;
@@ -190,7 +190,7 @@ int elp_bqsr_tables_write_elrecal(elp_ctx* c, const char* path) {
     if (!c->gathered) return c->fail(E_STATE, "elp_bqsr_tables_write_elrecal before elp_bqsr_gather / elp_bqsr_tables_put");
     const TableGeom& g = c->geom;
     std::vector<int64_t> t(g.cells() * 2);
-    CUDA_TRY(c, cudaMemcpyAsync(t.data(), c->d_tables, t.size() * 8, cudaMemcpyDeviceToHost, c->stream));
+    CUDA_TRY(c, cudaMemcpyAsync(t.data(), c->d_tables.p, t.size() * 8, cudaMemcpyDeviceToHost, c->stream));
     CUDA_TRY(c, cudaStreamSynchronize(c->stream));
     // type ids of a fresh Go process: BaseRecalibratorTables 64, bqsrTableKey 65, bqsrEntry 66, bqsrTable 67 (a map gets its id after its key and element)
     std::string out = def_struct(64, "BaseRecalibratorTables", {{"QualityScores", 67}, {"Cycles", 67}, {"Contexts", 67}});
@@ -229,7 +229,7 @@ int elp_bqsr_tables_add_elrecal(elp_ctx* c, const char* path) {
     if (!v || d.bad || v->kind != 3) return c->fail(E_INVAL, "%s: not a gob stream of filters.BaseRecalibratorTables", path);
     const TableGeom& g = c->geom;
     std::vector<int64_t> t(g.cells() * 2);
-    CUDA_TRY(c, cudaMemcpyAsync(t.data(), c->d_tables, t.size() * 8, cudaMemcpyDeviceToHost, c->stream));
+    CUDA_TRY(c, cudaMemcpyAsync(t.data(), c->d_tables.p, t.size() * 8, cudaMemcpyDeviceToHost, c->stream));
     CUDA_TRY(c, cudaStreamSynchronize(c->stream));
     const char* names[3] = {"QualityScores", "Cycles", "Contexts"};
     for (int table = 0; table < 3; table++) {
@@ -252,7 +252,7 @@ int elp_bqsr_tables_add_elrecal(elp_ctx* c, const char* path) {
             t[2 * g.idx(cv, (int)q, col) + 1] += geti(*kv.second, "Mismatches");
         }
     }
-    CUDA_TRY(c, cudaMemcpyAsync(c->d_tables, t.data(), t.size() * 8, cudaMemcpyHostToDevice, c->stream));
+    CUDA_TRY(c, cudaMemcpyAsync(c->d_tables.p, t.data(), t.size() * 8, cudaMemcpyHostToDevice, c->stream));
     CUDA_TRY(c, cudaStreamSynchronize(c->stream));
     c->gathered = true; c->finalized = false;
     return ELP_OK;

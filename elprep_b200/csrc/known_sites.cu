@@ -12,7 +12,7 @@
 //   sites_sort     the onesweep radix sort of contig << 32 | (start ^ 2^31), the end as payload
 //   sites_flatten  one prefix max over contig << 32 | (end ^ 2^31): interval i opens a group iff it is the first of its contig or its start
 //                  lies above every earlier end of its contig; the group heads are compacted and each group keeps the max of its ends
-// Nothing is installed before every file was read and every line accepted; the new table is one allocation (RegionTable::block).
+// Nothing is installed before every file was read and every line accepted; the new table is one allocation (ContigTable::block).
 #include <algorithm>
 #include <cerrno>
 #include <cstdio>
@@ -35,31 +35,13 @@ constexpr uint64_t SITES_CHUNK_DEFAULT = 32ull << 20;
 // page-locked and device staging, reused by every call on the context
 struct SitesStage {
     FileStage f;                                                 // the two chunks (file_stage.cuh); a carried partial line sits in front of the file bytes
-    unsigned long long* d_small = nullptr;                       // [0] first error (line << 8 | SitesErr), [1] unmatched lines
-    unsigned long long* h_small = nullptr;                       // page-locked: [0, 1] copies, [2] '\n' count, [3] intervals, [4] virtual line end
-    NameDict dict; bool dict_ok = false;
+    DBuf<unsigned long long> d_small;                            // [0] first error (line << 8 | SitesErr), [1] unmatched lines
+    HBuf<unsigned long long> h_small;                            // [0, 1] copies, [2] '\n' count, [3] intervals, [4] virtual line end
 };
 
-void sites_release(elp_ctx* c) {
-    SitesStage* S = c->sites;
-    if (!S) return;
-    stage_release(S->f);
-    if (S->d_small) cudaFree(S->d_small);
-    if (S->h_small) cudaFreeHost(S->h_small);
-    name_dict_release(S->dict);
-    delete S;
-    c->sites = nullptr;
-}
+void free_state(SitesStage* S) { delete S; }
 
 namespace {
-
-inline unsigned nblk(uint64_t n, int t) { return (unsigned)((n + t - 1) / t); }
-template <class T> int grow(elp_ctx* c, DBuf<T>& b, size_t need, size_t keep) {
-    cudaError_t e = b.reserve(need, c->stream, keep);
-    if (e != cudaSuccess) return c->fail(e == cudaErrorMemoryAllocation ? E_NOMEM : E_CUDA, "device allocation of %zu bytes failed: %s", need * sizeof(T), cudaGetErrorString(e));
-    return E_OK;
-}
-#define TRY(x) do { int rc__ = (x); if (rc__) return rc__; } while (0)
 
 // why a line fails; the smallest (line << 8 | code) of a file is reported
 enum SitesErr : uint32_t { KS_FIELDS = 1, KS_START, KS_END, KS_LONG };
@@ -262,20 +244,15 @@ __global__ void __launch_bounds__(256) sites_unbias_kernel(uint64_t n_groups, in
 struct SitesScratch {   // per call; freed on return
     DBuf<uint32_t> cnt, emit, vals_a, vals_b, head; DBuf<uint64_t> cnt_off, ls, emit_off, keys_a, keys_b, tmax, gid, first;
     DBuf<int32_t> ent, start, end;
-    ~SitesScratch() {
-        cnt.release(); emit.release(); vals_a.release(); vals_b.release(); head.release(); cnt_off.release(); ls.release(); emit_off.release();
-        keys_a.release(); keys_b.release(); tmax.release(); gid.release(); first.release(); ent.release(); start.release(); end.release();
-    }
 };
 
 int sites_stage_init(elp_ctx* c) {
-    if (!c->sites) c->sites = new SitesStage();
+    if (!c->sites) c->sites.reset(new SitesStage());
     SitesStage& S = *c->sites;
     const uint64_t want = c->sites_chunk ? c->sites_chunk : SITES_CHUNK_DEFAULT, cap = want + SITES_MAX_LINE;
     TRY(stage_init(c, S.f, want, cap, stage_padded(cap), "elp_load_known_sites"));
-    if (!S.d_small) { CUDA_TRY(c, cudaMalloc(&S.d_small, 16)); CUDA_TRY(c, cudaHostAlloc(&S.h_small, 64, cudaHostAllocDefault)); }
-    if (!S.dict_ok) { TRY(name_dict_upload(c, S.dict)); S.dict_ok = true; }
-    return E_OK;
+    CUDA_TRY(c, S.d_small.fit(2)); CUDA_TRY(c, S.h_small.fit(8));
+    return name_dict_upload(c);
 }
 
 int upload(elp_ctx* c, SitesStage& S, const LineChunk& ch) { return stage_upload(c, S.f, ch.b, ch.m, 0); }
@@ -286,10 +263,10 @@ int count_lines(elp_ctx* c, SitesStage& S, SitesScratch& X, const LineChunk& ch)
     TRY(grow(c, X.cnt, n_chunks + 8, 0)); TRY(grow(c, X.cnt_off, n_chunks + 2, 0));
     CUDA_TRY(c, cudaStreamWaitEvent(c->stream, S.f.up[ch.b], 0));
     c->begin("sites_lines", (double)ch.m);
-    sam_count_kernel<<<nblk(n_chunks, 256), 256, 0, c->stream>>>(S.f.d[ch.b], n_chunks, X.cnt.p);
+    sam_count_kernel<<<nblk(n_chunks, 256), 256, 0, c->stream>>>(S.f.d[ch.b].p, n_chunks, X.cnt.p);
     c->end(); LAUNCH_CHECK(c);
     TRY(exclusive_scan_u32_to_u64(c, X.cnt.p, X.cnt_off.p, n_chunks));
-    CUDA_TRY(c, cudaMemcpyAsync(S.h_small + 2, X.cnt_off.p + n_chunks, 8, cudaMemcpyDeviceToHost, c->stream));
+    CUDA_TRY(c, cudaMemcpyAsync(S.h_small.p + 2, X.cnt_off.p + n_chunks, 8, cudaMemcpyDeviceToHost, c->stream));
     return E_OK;
 }
 
@@ -297,25 +274,25 @@ int count_lines(elp_ctx* c, SitesStage& S, SitesScratch& X, const LineChunk& ch)
 int parse_launch(elp_ctx* c, SitesStage& S, SitesScratch& X, const LineChunk& ch, uint64_t line0, uint64_t* n_lines) {
     cudaStream_t s = c->stream;
     CUDA_TRY(c, cudaStreamSynchronize(s));
-    const uint64_t n_nl = S.h_small[2], n_chunks = (ch.m + SAM_CHUNK - 1) / SAM_CHUNK;
-    const bool open_end = S.f.h[ch.b][ch.m - 1] != '\n';
+    const uint64_t n_nl = S.h_small.p[2], n_chunks = (ch.m + SAM_CHUNK - 1) / SAM_CHUNK;
+    const bool open_end = S.f.h[ch.b].p[ch.m - 1] != '\n';
     const uint64_t nl = n_nl + (open_end ? 1 : 0);
     TRY(grow(c, X.ls, nl + 2, 0)); TRY(grow(c, X.ent, nl + 8, 0)); TRY(grow(c, X.start, nl + 8, 0)); TRY(grow(c, X.end, nl + 8, 0));
     TRY(grow(c, X.emit, nl + 8, 0)); TRY(grow(c, X.emit_off, nl + 2, 0));
     CUDA_TRY(c, cudaMemsetAsync(X.ls.p, 0, 8, s));
     c->begin("sites_lines", (double)ch.m + 8.0 * (double)n_nl);
-    sam_lines_kernel<<<nblk(n_chunks, 256), 256, 0, s>>>(S.f.d[ch.b], n_chunks, X.cnt_off.p, X.ls.p);
+    sam_lines_kernel<<<nblk(n_chunks, 256), 256, 0, s>>>(S.f.d[ch.b].p, n_chunks, X.cnt_off.p, X.ls.p);
     c->end(); LAUNCH_CHECK(c);
-    if (open_end) { S.h_small[4] = ch.m + 1; CUDA_TRY(c, cudaMemcpyAsync(X.ls.p + nl, S.h_small + 4, 8, cudaMemcpyHostToDevice, s)); }   // a virtual '\n' past the text
+    if (open_end) { S.h_small.p[4] = ch.m + 1; CUDA_TRY(c, cudaMemcpyAsync(X.ls.p + nl, S.h_small.p + 4, 8, cudaMemcpyHostToDevice, s)); }   // a virtual '\n' past the text
     SitesArgs A{};
-    A.text = S.f.d[ch.b]; A.ls = X.ls.p; A.n_lines = nl; A.line0 = line0; A.dict = S.dict;
-    A.ent = X.ent.p; A.start = X.start.p; A.end = X.end.p; A.emit = X.emit.p; A.small = S.d_small;
+    A.text = S.f.d[ch.b].p; A.ls = X.ls.p; A.n_lines = nl; A.line0 = line0; A.dict = c->names.view();
+    A.ent = X.ent.p; A.start = X.start.p; A.end = X.end.p; A.emit = X.emit.p; A.small = S.d_small.p;
     c->begin("sites_parse", (double)ch.m + 8.0 * (double)(nl + 1) + 16.0 * (double)nl);
     sites_parse_kernel<<<nblk(nl, 256), 256, 0, s>>>(A);
     c->end(); LAUNCH_CHECK(c);
     TRY(exclusive_scan_u32_to_u64(c, X.emit.p, X.emit_off.p, nl));
-    CUDA_TRY(c, cudaMemcpyAsync(S.h_small, S.d_small, 16, cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(c, cudaMemcpyAsync(S.h_small + 3, X.emit_off.p + nl, 8, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(c, cudaMemcpyAsync(S.h_small.p, S.d_small.p, 16, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(c, cudaMemcpyAsync(S.h_small.p + 3, X.emit_off.p + nl, 8, cudaMemcpyDeviceToHost, s));
     *n_lines = nl;
     return E_OK;
 }
@@ -324,14 +301,14 @@ int parse_launch(elp_ctx* c, SitesStage& S, SitesScratch& X, const LineChunk& ch
 int parse_finish(elp_ctx* c, SitesStage& S, SitesScratch& X, const LineChunk& ch, int file, const char* path, uint64_t nl, uint64_t* total) {
     cudaStream_t s = c->stream;
     CUDA_TRY(c, cudaStreamSynchronize(s));
-    if (S.h_small[0] != ~0ull)
-        return c->fail(E_SITES, "elp_load_known_sites: %s (file %d), line %llu (0-based, header = line 0): %s", path, file, (unsigned long long)(S.h_small[0] >> 8),
-                       sites_err_text((uint32_t)(S.h_small[0] & 0xff)));
-    const uint64_t add = S.h_small[3], t0 = *total;
+    if (S.h_small.p[0] != ~0ull)
+        return c->fail(E_SITES, "elp_load_known_sites: %s (file %d), line %llu (0-based, header = line 0): %s", path, file, (unsigned long long)(S.h_small.p[0] >> 8),
+                       sites_err_text((uint32_t)(S.h_small.p[0] & 0xff)));
+    const uint64_t add = S.h_small.p[3], t0 = *total;
     if (t0 + add >= (1ull << 30)) return c->fail(E_LIMIT, "elp_load_known_sites: 2^30 or more intervals in total (the limit of the device sort)");
     if (t0 + add + 4 > X.keys_a.cap) { const size_t want = std::max<size_t>(t0 + add + 4, 2 * X.keys_a.cap); TRY(grow(c, X.keys_a, want, t0)); TRY(grow(c, X.vals_a, want, t0)); }
     c->begin("sites_parse", 24.0 * (double)nl + 12.0 * (double)add);
-    sites_emit_kernel<<<nblk(nl, 256), 256, 0, s>>>(nl, X.ent.p, X.start.p, X.end.p, X.emit.p, X.emit_off.p, S.dict, X.keys_a.p + t0, X.vals_a.p + t0);
+    sites_emit_kernel<<<nblk(nl, 256), 256, 0, s>>>(nl, X.ent.p, X.start.p, X.end.p, X.emit.p, X.emit_off.p, c->names.view(), X.keys_a.p + t0, X.vals_a.p + t0);
     c->end(); LAUNCH_CHECK(c);
     CUDA_TRY(c, cudaEventRecord(S.f.used[ch.b], s));
     *total = t0 + add;
@@ -368,7 +345,7 @@ int load_file(elp_ctx* c, SitesStage& S, SitesScratch& X, int file, const char* 
 }
 
 // sorted intervals -> flattened groups in one allocation (*block, *n_groups pairs); first[contig] = its first group or ~0
-int flatten(elp_ctx* c, SitesScratch& X, const uint64_t* keys, const uint32_t* ends, uint64_t n, int32_t** block, uint64_t* n_groups, std::vector<uint64_t>& first) {
+int flatten(elp_ctx* c, SitesScratch& X, const uint64_t* keys, const uint32_t* ends, uint64_t n, DBuf<int32_t>* block, uint64_t* n_groups, std::vector<uint64_t>& first) {
     cudaStream_t s = c->stream;
     const int nc = c->n_contigs;
     const uint64_t tiles = (n + FL_TILE - 1) / FL_TILE;
@@ -386,24 +363,24 @@ int flatten(elp_ctx* c, SitesScratch& X, const uint64_t* keys, const uint32_t* e
     uint64_t G = 0;
     CUDA_TRY(c, cudaMemcpyAsync(&G, X.gid.p + n, 8, cudaMemcpyDeviceToHost, s));
     CUDA_TRY(c, cudaStreamSynchronize(s));
-    int32_t* out = nullptr;
-    cudaError_t e = cudaMalloc(&out, G * 8);
+    DBuf<int32_t> out;
+    cudaError_t e = out.fit(2 * G);
     if (e != cudaSuccess) { cudaGetLastError(); return c->fail(e == cudaErrorMemoryAllocation ? E_NOMEM : E_CUDA, "device allocation of %llu bytes failed", (unsigned long long)(G * 8)); }
     int rc = E_OK;
     auto step = [&](cudaError_t x) { if (rc == E_OK && x != cudaSuccess) rc = c->fail(E_CUDA, "elp_load_known_sites: %s", cudaGetErrorString(x)); };
-    step(cudaMemsetAsync(out, 0, G * 8, s));
+    step(cudaMemsetAsync(out.p, 0, G * 8, s));
     step(cudaMemsetAsync(X.first.p, 0xff, (size_t)nc * 8, s));
     c->begin("sites_flatten", 24.0 * (double)n + 8.0 * (double)G);
-    sites_compact_kernel<<<nblk(n, 256), 256, 0, s>>>(keys, ends, n, X.head.p, X.gid.p, out, X.first.p);
+    sites_compact_kernel<<<nblk(n, 256), 256, 0, s>>>(keys, ends, n, X.head.p, X.gid.p, out.p, X.first.p);
     c->end(); step(cudaGetLastError());
     c->begin("sites_flatten", 8.0 * (double)G);
-    sites_unbias_kernel<<<nblk(G, 256), 256, 0, s>>>(G, out);
+    sites_unbias_kernel<<<nblk(G, 256), 256, 0, s>>>(G, out.p);
     c->end(); step(cudaGetLastError());
     first.assign(nc, ~0ull);
     if (nc) step(cudaMemcpyAsync(first.data(), X.first.p, (size_t)nc * 8, cudaMemcpyDeviceToHost, s));
     step(cudaStreamSynchronize(s));
-    if (rc) { cudaFree(out); return rc; }
-    *block = out; *n_groups = G;
+    if (rc) return rc;
+    *block = std::move(out); *n_groups = G;
     return E_OK;
 }
 
@@ -417,20 +394,20 @@ extern "C" int elp_load_known_sites(elp_ctx* c, const char* const* paths, int32_
     if (c->n_contigs > 0 && !c->has_contig_names)
         return c->fail(E_INVAL, "elp_load_known_sites: the context was created without elp_config.contig_names, so chromosome names cannot be resolved");
     const int nc = c->n_contigs;
-    int32_t* block = nullptr; uint64_t G = 0, unmatched = 0;
+    DBuf<int32_t> block; uint64_t G = 0, unmatched = 0;
     std::vector<uint64_t> first(nc, ~0ull);
     if (n_paths) {
         TRY(sites_stage_init(c));
         SitesStage& S = *c->sites;
         struct Drain { cudaStream_t s; ~Drain() { cudaStreamSynchronize(s); } } drain{S.f.copy};   // no upload outlives the call
         SitesScratch X;
-        CUDA_TRY(c, cudaMemsetAsync(S.d_small, 0xff, 8, c->stream));
-        CUDA_TRY(c, cudaMemsetAsync(S.d_small + 1, 0, 8, c->stream));
+        CUDA_TRY(c, cudaMemsetAsync(S.d_small.p, 0xff, 8, c->stream));
+        CUDA_TRY(c, cudaMemsetAsync(S.d_small.p + 1, 0, 8, c->stream));
         uint64_t total = 0;
         for (int i = 0; i < n_paths; i++) TRY(load_file(c, S, X, i, paths[i], &total));
-        CUDA_TRY(c, cudaMemcpyAsync(S.h_small + 1, S.d_small + 1, 8, cudaMemcpyDeviceToHost, c->stream));
+        CUDA_TRY(c, cudaMemcpyAsync(S.h_small.p + 1, S.d_small.p + 1, 8, cudaMemcpyDeviceToHost, c->stream));
         CUDA_TRY(c, cudaStreamSynchronize(c->stream));
-        unmatched = S.h_small[1];
+        unmatched = S.h_small.p[1];
         if (total) {
             TRY(grow(c, X.keys_b, total + 4, 0)); TRY(grow(c, X.vals_b, total + 4, 0));
             int bits = 32;
@@ -450,15 +427,11 @@ extern "C" int elp_load_known_sites(elp_ctx* c, const char* const* paths, int32_
         }
     }
     // install: every contig's list is replaced (contigs appear in increasing order, so a contig's groups end at the next one's first)
-    RegionTable& t = c->known_sites;
-    for (auto p : t.d) if (p && t.separate(p)) cudaFree(p);
-    if (t.block) cudaFree(t.block);
-    t.d.assign(nc, nullptr); t.n.assign(nc, 0);
-    t.block = block; t.block_pairs = G;
+    std::vector<int32_t*> d(nc, nullptr); std::vector<uint64_t> cnt(nc, 0);
     uint64_t next = G;
     for (int i = nc - 1; i >= 0; i--)
-        if (first[i] != ~0ull) { t.d[i] = block + 2 * first[i]; t.n[i] = next - first[i]; next = first[i]; }
-    t.dirty = true;
+        if (first[i] != ~0ull) { d[i] = block.p + 2 * first[i]; cnt[i] = next - first[i]; next = first[i]; }
+    c->known_sites.install(std::move(block), std::move(d), std::move(cnt));
     if (n_unmatched) *n_unmatched = unmatched;
     return ELP_OK;
 }
@@ -468,7 +441,7 @@ extern "C" int64_t elp_known_sites_get(elp_ctx* c, int32_t contig, int32_t* se, 
     cudaSetDevice(c->device);
     if (contig < 0 || contig >= c->n_contigs) { c->fail(E_INVAL, "elp_known_sites_get: contig %d out of range", contig); return -1; }
     const RegionTable& t = c->known_sites;
-    const uint64_t n = (int)t.d.size() == c->n_contigs ? t.n[contig] : 0;
+    const uint64_t n = t.n[contig];
     const uint64_t k = std::min(n, cap);
     if (se && k) {
         if (cudaMemcpyAsync(se, t.d[contig], k * 8, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) {

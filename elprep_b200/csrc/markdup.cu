@@ -405,16 +405,14 @@ __global__ void __launch_bounds__(256) pair_mark_kernel(uint64_t m, const uint64
         if (t != win) { const uint32_t p = vals[t]; atomic_or_u16(flag, pair_a[p], F_DUPLICATE); atomic_or_u16(flag, pair_b[p], F_DUPLICATE); }
 }
 
-inline unsigned nblk(uint64_t n, int t) { return (unsigned)((n + t - 1) / t); }
-
 }  // namespace
 
 int check_device_errors(elp_ctx* c) {
     uint32_t e = 0;
-    CUDA_TRY(c, cudaMemcpyAsync(&e, c->d_err, 4, cudaMemcpyDeviceToHost, c->stream));
+    CUDA_TRY(c, cudaMemcpyAsync(&e, c->d_err.p, 4, cudaMemcpyDeviceToHost, c->stream));
     CUDA_TRY(c, cudaStreamSynchronize(c->stream));
     if (!e) return E_OK;
-    CUDA_TRY(c, cudaMemsetAsync(c->d_err, 0, 4, c->stream));
+    CUDA_TRY(c, cudaMemsetAsync(c->d_err.p, 0, 4, c->stream));
     if (e & DERR_QUAL) return c->fail(E_QUAL, "Invalid QUAL character in a read entering duplicate marking");
     if (e & DERR_NORG) return c->fail(E_NORG, "Error: BQSR requires input with read groups. An alignment has no read group. Please fix input, e.g. rerun with the --replace-read-group option.");
     if (e & DERR_CYCLE) return c->fail(E_CYCLE, "cycle value exceeds maximum cycle value");
@@ -440,13 +438,13 @@ int phase_adapt(elp_ctx* c) {
     CUDA_TRY(c, c->score.reserve(n + 1, c->stream));
     CUDA_TRY(c, c->qhash.reserve(n + 1, c->stream));
     DeviceRanges init{}; init.pos_max = 0; init.upos_min = INT_MAX; init.upos_max = INT_MIN; init.score_max = 0; init.lseq_max = 0;
-    { int rcu = upload_small(c, c->d_ranges, &init, sizeof init); if (rcu) return rcu; }
+    { int rcu = upload_small(c, c->d_ranges.p, &init, sizeof init); if (rcu) return rcu; }
     if (n) {
         int sms = 132; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device);
         AdaptArgs A{};
-        A.n = n; A.flag = c->flag.p; A.pos = c->pos.p; A.rg = c->rg.p; A.rg_lib = c->d_rg_lib; A.n_rg = c->n_rg; A.cigar_off = c->cigar_off.p; A.cigar = c->cigar.p;
+        A.n = n; A.flag = c->flag.p; A.pos = c->pos.p; A.rg = c->rg.p; A.rg_lib = c->d_rg_lib.p; A.n_rg = c->n_rg; A.cigar_off = c->cigar_off.p; A.cigar = c->cigar.p;
         A.qual_off = c->qual_off.p; A.qual = c->qual.p; A.qname_off = c->qname_off.p; A.qname = c->qname.p; A.upos = c->upos.p; A.score = c->score.p; A.qhash = c->qhash.p;
-        A.ranges = c->d_ranges; A.err = c->d_err;
+        A.ranges = c->d_ranges.p; A.err = c->d_err.p;
         // reads per tile: as many as fit the ring slot on average (256 reads of 150 bases; fewer for longer reads)
         const double avg_q = (double)(c->n_qual - ARENA_FRONT_PAD) / (double)n + 1, avg_n = (double)c->n_qname / (double)n + 1, avg_c = 4.0 * (double)c->n_cigar / (double)n + 1;
         int rpt = (int)std::min({(double)AD_T, 0.94 * AD_QCAP / avg_q, 0.94 * AD_NCAP / avg_n, 0.94 * AD_CCAP / avg_c});
@@ -460,8 +458,8 @@ int phase_adapt(elp_ctx* c) {
         adapt_kernel<<<grid, AD_T, smem, c->stream>>>(A);
         c->end(); LAUNCH_CHECK(c);
     }
-    CUDA_TRY(c, cudaMemcpyAsync(&c->h_ranges, c->d_ranges, sizeof(DeviceRanges), cudaMemcpyDeviceToHost, c->stream));
-    CUDA_TRY(c, cudaMemcpyAsync(c->h_qpresent, c->d_qpresent, 16, cudaMemcpyDeviceToHost, c->stream));   // the apply table's QUAL slots
+    CUDA_TRY(c, cudaMemcpyAsync(&c->h_ranges, c->d_ranges.p, sizeof(DeviceRanges), cudaMemcpyDeviceToHost, c->stream));
+    CUDA_TRY(c, cudaMemcpyAsync(c->h_qpresent, c->d_qpresent.p, 16, cudaMemcpyDeviceToHost, c->stream));   // the apply table's QUAL slots
     int rc = check_device_errors(c);   // synchronizes
     if (rc) return rc;
     if (c->h_ranges.n_entering == 0) { c->h_ranges.upos_min = 0; c->h_ranges.upos_max = 0; }
@@ -483,7 +481,7 @@ static int mark_pairs(elp_ctx* c, bool optical, uint64_t nt, uint64_t n_true_pai
     if (rc) return rc;
     const uint64_t m = n_true_pairs;
     c->begin("join", (double)m * 12);
-    join_kernel<<<nblk(m, 256), 256, 0, c->stream>>>(m, in_b ? c->keys_b.p : c->keys_a.p, in_b ? c->vals_b.p : c->vals_a.p, c->rg.p, c->d_rg_lib, c->n_rg, c->qname_off.p, c->qname.p, c->mate.p);
+    join_kernel<<<nblk(m, 256), 256, 0, c->stream>>>(m, in_b ? c->keys_b.p : c->keys_a.p, in_b ? c->vals_b.p : c->vals_a.p, c->rg.p, c->d_rg_lib.p, c->n_rg, c->qname_off.p, c->qname.p, c->mate.p);
     c->end(); LAUNCH_CHECK(c);
     // deterministic pair list, ordered by the arrival of the later mate
     CUDA_TRY(c, c->scan_tmp.reserve(nt + 4, c->stream));
@@ -507,7 +505,7 @@ static int mark_pairs(elp_ctx* c, bool optical, uint64_t nt, uint64_t n_true_pai
         CUDA_TRY(c, c->bytes_tmp.reserve((size_t)npairs * 8 * words + 64, c->stream));
         uint64_t* kb2 = reinterpret_cast<uint64_t*>(c->bytes_tmp.p);
         c->begin("pair_keys", (double)nt * 12 + (double)npairs * (2 * 18 + 8 * words + 16));
-        pair_keys_kernel<<<nblk(nt, 256), 256, 0, c->stream>>>(nt, c->mate.p, slot, c->flag.p, c->refid.p, c->rg.p, c->d_rg_lib, c->n_rg, c->upos.p, c->score.p, L,
+        pair_keys_kernel<<<nblk(nt, 256), 256, 0, c->stream>>>(nt, c->mate.p, slot, c->flag.p, c->refid.p, c->rg.p, c->d_rg_lib.p, c->n_rg, c->upos.p, c->score.p, L,
                                                               c->keys_a.p, c->vals_a.p, c->pair_a.p, c->pair_b.p, c->pair_score.p);
         c->end(); LAUNCH_CHECK(c);
         rc = words == 1 ? radix_sort_u64(c, c->keys_a.p, kb2, c->vals_a.p, c->vals_b.p, npairs, L.key_bits, &in_b, "u64")
@@ -556,7 +554,7 @@ int phase_markdup(elp_ctx* c, bool optical) {
                 L.key_bits = L.bS + 2 + L.bU + L.bR + L.bL;
                 if (L.key_bits > 64) return c->fail(E_LIMIT, "fragment signature needs %d bits (>64): too many contigs/libraries for the packed key", L.key_bits);
                 c->begin("frag_keys", (double)n * (2 + 4 + 4 + 4 + 4 + 8 + 4));
-                frag_keys_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(n, c->flag.p, c->refid.p, c->rg.p, c->d_rg_lib, c->n_rg, c->upos.p, c->score.p, L, c->keys_a.p, c->vals_a.p);
+                frag_keys_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(n, c->flag.p, c->refid.p, c->rg.p, c->d_rg_lib.p, c->n_rg, c->upos.p, c->score.p, L, c->keys_a.p, c->vals_a.p);
                 c->end(); LAUNCH_CHECK(c);
                 // only the group (bits from bS + 1 up) needs to be contiguous: frag_mark_kernel finds the winner from the low bits
                 bool in_b = false;

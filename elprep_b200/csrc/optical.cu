@@ -263,22 +263,16 @@ __global__ void __launch_bounds__(256) opt_big_groups_kernel(MemberArgs M, OptAc
     }
 }
 
-inline unsigned nblk(uint64_t n, int t) { return (unsigned)((n + t - 1) / t); }
-
 }  // namespace
 
 // ---------------------------------------------------------------- host side
 static int opt_alloc(elp_ctx* c) {
     const size_t slots = (size_t)c->n_lib + 1;
-    if (!c->d_opt_ctr) {
-        CUDA_TRY(c, cudaMalloc(&c->d_opt_ctr, slots * OPT_NCTR * 8));
-        CUDA_TRY(c, cudaMalloc(&c->d_opt_hist, slots * 3 * OPT_HBINS * 8));
-        CUDA_TRY(c, cudaMalloc(&c->d_opt_ovf, (size_t)OPT_OVF_CAP * 16));
-        CUDA_TRY(c, cudaMalloc(&c->d_opt_small, 16));
-    }
-    CUDA_TRY(c, cudaMemsetAsync(c->d_opt_ctr, 0, slots * OPT_NCTR * 8, c->stream));
-    CUDA_TRY(c, cudaMemsetAsync(c->d_opt_hist, 0, slots * 3 * OPT_HBINS * 8, c->stream));
-    CUDA_TRY(c, cudaMemsetAsync(c->d_opt_small, 0, 16, c->stream));
+    CUDA_TRY(c, c->d_opt_ctr.fit(slots * OPT_NCTR)); CUDA_TRY(c, c->d_opt_hist.fit(slots * 3 * OPT_HBINS));
+    CUDA_TRY(c, c->d_opt_ovf.fit((size_t)OPT_OVF_CAP * 2)); CUDA_TRY(c, c->d_opt_small.fit(4));
+    CUDA_TRY(c, cudaMemsetAsync(c->d_opt_ctr.p, 0, slots * OPT_NCTR * 8, c->stream));
+    CUDA_TRY(c, cudaMemsetAsync(c->d_opt_hist.p, 0, slots * 3 * OPT_HBINS * 8, c->stream));
+    CUDA_TRY(c, cudaMemsetAsync(c->d_opt_small.p, 0, 16, c->stream));
     return E_OK;
 }
 
@@ -289,12 +283,12 @@ int phase_optical(elp_ctx* c, uint64_t npairs, const uint64_t* sorted_keys, cons
     const uint64_t n = c->n;
     const size_t slots = (size_t)c->n_lib + 1;
     OptAcc A{};
-    A.ctr = reinterpret_cast<unsigned long long*>(c->d_opt_ctr); A.hist = reinterpret_cast<unsigned long long*>(c->d_opt_hist);
-    A.ovf = reinterpret_cast<unsigned long long*>(c->d_opt_ovf); A.ovf_n = c->d_opt_small; A.ovf_cap = OPT_OVF_CAP;
-    A.big_n = c->d_opt_small + 1;
+    A.ctr = c->d_opt_ctr.p; A.hist = c->d_opt_hist.p;
+    A.ovf = c->d_opt_ovf.p; A.ovf_n = c->d_opt_small.p; A.ovf_cap = OPT_OVF_CAP;
+    A.big_n = c->d_opt_small.p + 1;
     if (n) {
         c->begin("opt_read_counters", (double)n * 6);
-        opt_read_counters_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(n, c->flag.p, c->rg.p, c->d_rg_lib, c->n_rg, A.ctr);
+        opt_read_counters_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(n, c->flag.p, c->rg.p, c->d_rg_lib.p, c->n_rg, A.ctr);
         c->end(); LAUNCH_CHECK(c);
     }
     uint32_t small[4] = {0, 0, 0, 0};
@@ -303,7 +297,7 @@ int phase_optical(elp_ctx* c, uint64_t npairs, const uint64_t* sorted_keys, cons
         uint32_t* base = reinterpret_cast<uint32_t*>(c->keys_b.p);
         MemberArgs M{};
         M.npairs = npairs; M.keys = sorted_keys; M.vals = sorted_vals; M.key_words = key_words; M.pair_a = c->pair_a.p; M.pair_b = c->pair_b.p;
-        M.flag = c->flag.p; M.rg = c->rg.p; M.rg_lib = c->d_rg_lib; M.n_rg = c->n_rg; M.qname_off = c->qname_off.p; M.qname = c->qname.p;
+        M.flag = c->flag.p; M.rg = c->rg.p; M.rg_lib = c->d_rg_lib.p; M.n_rg = c->n_rg; M.qname_off = c->qname_off.p; M.qname = c->qname.p;
         M.m_t = reinterpret_cast<int32_t*>(base); M.m_x = reinterpret_cast<int32_t*>(base + npairs); M.m_y = reinterpret_cast<int32_t*>(base + 2 * npairs);
         M.m_info = base + 3 * npairs;
         uint32_t* par = base + 4 * npairs;
@@ -312,14 +306,14 @@ int phase_optical(elp_ctx* c, uint64_t npairs, const uint64_t* sorted_keys, cons
         opt_members_kernel<<<nblk(npairs, 256), 256, 0, c->stream>>>(M, A);
         c->end(); LAUNCH_CHECK(c);
         c->begin("opt_small_groups", (double)npairs * 16);
-        opt_small_groups_kernel<<<nblk(npairs, 256), 256, 0, c->stream>>>(M, A, c->optical_pixel_distance, c->d_err);
+        opt_small_groups_kernel<<<nblk(npairs, 256), 256, 0, c->stream>>>(M, A, c->optical_pixel_distance, c->d_err.p);
         c->end(); LAUNCH_CHECK(c);
-        CUDA_TRY(c, cudaMemcpyAsync(small, c->d_opt_small, 16, cudaMemcpyDeviceToHost, c->stream));
+        CUDA_TRY(c, cudaMemcpyAsync(small, c->d_opt_small.p, 16, cudaMemcpyDeviceToHost, c->stream));
         CUDA_TRY(c, cudaStreamSynchronize(c->stream));
         if (small[1] > A.big_cap) return c->fail(E_CUDA, "optical: long-run queue overflow (%u > %u)", small[1], A.big_cap);
         if (small[1]) {
             c->begin("opt_big_groups", (double)small[1] * 33 * 16);
-            opt_big_groups_kernel<<<small[1], 256, 0, c->stream>>>(M, A, c->optical_pixel_distance, par, c->d_err);
+            opt_big_groups_kernel<<<small[1], 256, 0, c->stream>>>(M, A, c->optical_pixel_distance, par, c->d_err.p);
             c->end(); LAUNCH_CHECK(c);
         }
     }
@@ -327,13 +321,13 @@ int phase_optical(elp_ctx* c, uint64_t npairs, const uint64_t* sorted_keys, cons
     if (rc) return rc;
     // bring the accumulators back
     std::vector<unsigned long long> h_ctr(slots * OPT_NCTR), h_hist(slots * 3 * OPT_HBINS);
-    CUDA_TRY(c, cudaMemcpyAsync(h_ctr.data(), c->d_opt_ctr, h_ctr.size() * 8, cudaMemcpyDeviceToHost, c->stream));
-    CUDA_TRY(c, cudaMemcpyAsync(h_hist.data(), c->d_opt_hist, h_hist.size() * 8, cudaMemcpyDeviceToHost, c->stream));
-    CUDA_TRY(c, cudaMemcpyAsync(small, c->d_opt_small, 16, cudaMemcpyDeviceToHost, c->stream));
+    CUDA_TRY(c, cudaMemcpyAsync(h_ctr.data(), c->d_opt_ctr.p, h_ctr.size() * 8, cudaMemcpyDeviceToHost, c->stream));
+    CUDA_TRY(c, cudaMemcpyAsync(h_hist.data(), c->d_opt_hist.p, h_hist.size() * 8, cudaMemcpyDeviceToHost, c->stream));
+    CUDA_TRY(c, cudaMemcpyAsync(small, c->d_opt_small.p, 16, cudaMemcpyDeviceToHost, c->stream));
     CUDA_TRY(c, cudaStreamSynchronize(c->stream));
     if (small[0] > OPT_OVF_CAP) return c->fail(E_LIMIT, "optical: more than %d histogram keys above %d", OPT_OVF_CAP, OPT_HBINS);
     std::vector<unsigned long long> h_ovf(2 * (size_t)small[0]);
-    if (small[0]) { CUDA_TRY(c, cudaMemcpyAsync(h_ovf.data(), c->d_opt_ovf, h_ovf.size() * 8, cudaMemcpyDeviceToHost, c->stream)); CUDA_TRY(c, cudaStreamSynchronize(c->stream)); }
+    if (small[0]) { CUDA_TRY(c, cudaMemcpyAsync(h_ovf.data(), c->d_opt_ovf.p, h_ovf.size() * 8, cudaMemcpyDeviceToHost, c->stream)); CUDA_TRY(c, cudaStreamSynchronize(c->stream)); }
     c->opt.assign(slots, DupCounters{});
     for (size_t s = 0; s < slots; s++) {
         DupCounters& d = c->opt[s];

@@ -281,14 +281,6 @@ __global__ void __launch_bounds__(THREADS, MIN_CTAS) rs_onesweep_kernel(const K*
 }
 
 // ---------------------------------------------------------------- host driver
-struct Workspace {
-    uint32_t* ghist = nullptr;      // [MAX_PASSES][RADIX]
-    uint32_t* gofs = nullptr;       // [MAX_PASSES][RADIX]
-    uint32_t* counters = nullptr;   // [MAX_PASSES]
-    uint32_t* status = nullptr;     // [passes][tiles][RADIX]
-    size_t status_bytes = 0;
-};
-
 template <class K> struct Cfg;
 // 384 x 16 keys per tile, 2 CTAs per SM: on an H100 (tools/sort_roofline.py) this beat 256 x 12 at 4 CTAs (the look-back
 // wait dominated), 256 x 24 at 2, and 384 x 24 / 384 x 30 / 512 x 16 at 1 CTA per SM (ranking latency with 12-16 warps per SM)

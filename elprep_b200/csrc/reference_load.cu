@@ -18,7 +18,7 @@
 //   ref_pack        after the last chunk, the sequence of each name that is an @SQ SN, from the raw buffer through ref_pack_hot_kernel
 // .elfasta follows OpenElfasta (fasta-files.go:286-336): the offset table is read and checked on the host; only the byte ranges of names
 // that are an @SQ SN are read, through the same chunks, and ref_pack_span_kernel packs each chunk at its base offset in the contig.
-// Nothing is installed before the whole file was accepted; the new references are one allocation (elp_ctx::refhot_block).
+// Nothing is installed before the whole file was accepted; the new references are one allocation (ContigTable::block of elp_ctx::ref).
 #include <algorithm>
 #include <cerrno>
 #include <cstdio>
@@ -43,13 +43,6 @@ constexpr uint64_t BGZF_MAX_BLOCK = 65536;
 const uint8_t ELFASTA_MAGIC[4] = {0x31, 0xFA, 0x57, 0xA1};
 constexpr int VARINT_FIELD = 10;                 // binary.MaxVarintLen64
 
-inline unsigned nblk(uint64_t n, int t) { return (unsigned)((n + t - 1) / t); }
-template <class T> int grow(elp_ctx* c, DBuf<T>& b, size_t need, size_t keep) {
-    cudaError_t e = b.reserve(need, c->stream, keep);
-    if (e != cudaSuccess) return c->fail(e == cudaErrorMemoryAllocation ? E_NOMEM : E_CUDA, "device allocation of %zu bytes failed: %s", need * sizeof(T), cudaGetErrorString(e));
-    return E_OK;
-}
-#define TRY(x) do { int rc__ = (x); if (rc__) return rc__; } while (0)
 
 // why a FASTA file is refused; the smallest (line << 8 | code) is reported (1-based lines)
 enum FaErr : uint32_t { FA_FIRST = 1, FA_LONG, FA_EMPTY };
@@ -140,20 +133,12 @@ __global__ void __launch_bounds__(256) fasta_scatter_kernel(FaScatter A) {
 
 // ---- host side ----
 struct RefScratch {   // per call; freed on return
-    FileStage S;
     DBuf<uint32_t> cnt, seqlen, hdr, namelen, namest;
     DBuf<uint64_t> cnt_off, ls, seq_off, hdr_off, name_off, hdr_line, hdr_raw, hdr_name;
     DBuf<uint8_t> raw, names, tb[2];
-    unsigned long long* d_w = nullptr;
-    unsigned long long* h_w = nullptr;   // page-locked: [0, 8) readbacks, [8, 16) uploads
-    ~RefScratch() {
-        stage_release(S);
-        cnt.release(); seqlen.release(); hdr.release(); namelen.release(); namest.release(); cnt_off.release(); ls.release(); seq_off.release();
-        hdr_off.release(); name_off.release(); hdr_line.release(); hdr_raw.release(); hdr_name.release(); raw.release(); names.release();
-        tb[0].release(); tb[1].release();
-        if (d_w) cudaFree(d_w);
-        if (h_w) cudaFreeHost(h_w);
-    }
+    DBuf<unsigned long long> d_w;
+    HBuf<unsigned long long> h_w;   // [0, 8) readbacks, [8, 16) uploads
+    FileStage S;                    // last: destroyed first, so its uploads have landed before the buffers above are freed
 };
 
 struct Seq { std::string name; uint64_t line, raw, len; };   // one header of the file and its sequence in the raw buffer
@@ -172,7 +157,7 @@ struct FaState {      // carried from chunk to chunk
 template <class F>
 int fasta_chunk(elp_ctx* c, RefScratch& X, FaState& St, uint8_t* buf, uint64_t nnew, bool last, const char* path, cudaEvent_t release_prev, F&& overlap) {
     cudaStream_t s = c->stream;
-    unsigned long long* hw = X.h_w;
+    unsigned long long* hw = X.h_w.p;
     const uint64_t nc = St.carry_n, a = (FA_FRONT - nc) & ~(uint64_t)(SAM_CHUNK - 1), front = FA_FRONT - nc - a, end = FA_FRONT + nnew - a;
     uint8_t* t = buf + a;
     if (nc) CUDA_TRY(c, cudaMemcpyAsync(buf + FA_FRONT - nc, St.carry, nc, cudaMemcpyDeviceToDevice, s));
@@ -207,8 +192,8 @@ int fasta_chunk(elp_ctx* c, RefScratch& X, FaState& St, uint8_t* buf, uint64_t n
         TRY(grow(c, X.seq_off, nl + 2, 0)); TRY(grow(c, X.hdr_off, nl + 2, 0)); TRY(grow(c, X.name_off, nl + 2, 0));
         FaArgs A{};
         A.t = t; A.ls = X.ls.p; A.n_lines = nl; A.line0 = St.line0;
-        A.prev_in = X.d_w + W_PREV + St.prev; A.prev_out = X.d_w + W_PREV + (St.prev ^ 1);
-        A.seqlen = X.seqlen.p; A.hdr = X.hdr.p; A.namelen = X.namelen.p; A.namest = X.namest.p; A.w = X.d_w;
+        A.prev_in = X.d_w.p + W_PREV + St.prev; A.prev_out = X.d_w.p + W_PREV + (St.prev ^ 1);
+        A.seqlen = X.seqlen.p; A.hdr = X.hdr.p; A.namelen = X.namelen.p; A.namest = X.namest.p; A.w = X.d_w.p;
         c->begin("fasta_classify", (double)(m - front) + 8.0 * (double)(nl + 1) + 16.0 * (double)nl);
         fasta_classify_kernel<<<nblk(nl, 256), 256, 0, s>>>(A);
         c->end(); LAUNCH_CHECK(c);
@@ -218,7 +203,7 @@ int fasta_chunk(elp_ctx* c, RefScratch& X, FaState& St, uint8_t* buf, uint64_t n
         CUDA_TRY(c, cudaMemcpyAsync(hw + 2, X.seq_off.p + nl, 8, cudaMemcpyDeviceToHost, s));
         CUDA_TRY(c, cudaMemcpyAsync(hw + 3, X.hdr_off.p + nl, 8, cudaMemcpyDeviceToHost, s));
         CUDA_TRY(c, cudaMemcpyAsync(hw + 4, X.name_off.p + nl, 8, cudaMemcpyDeviceToHost, s));
-        CUDA_TRY(c, cudaMemcpyAsync(hw + 5, X.d_w, 16, cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(c, cudaMemcpyAsync(hw + 5, X.d_w.p, 16, cudaMemcpyDeviceToHost, s));
         CUDA_TRY(c, cudaStreamSynchronize(s));
         St.prev ^= 1;
         St.first = hw[6];
@@ -261,7 +246,7 @@ int load_fasta_plain(elp_ctx* c, RefScratch& X, FaState& St, FILE* f, const char
     TRY(grow(c, X.raw, size + 64, 0));   // the sequence bytes are at most the file's bytes
     auto fill = [&](int b, uint64_t* got, bool* last) -> int {
         TRY(stage_wait_host(c, S, b));
-        *got = fread(S.h[b], 1, chunk, f);
+        *got = fread(S.h[b].p, 1, chunk, f);
         if (*got < chunk && ferror(f)) return read_fail(c, path);
         *last = *got < chunk;
         return stage_upload(c, S, b, *got, FA_FRONT);
@@ -271,8 +256,8 @@ int load_fasta_plain(elp_ctx* c, RefScratch& X, FaState& St, FILE* f, const char
     for (;;) {
         uint64_t got2 = 0; bool last2 = true;
         CUDA_TRY(c, cudaStreamWaitEvent(c->stream, S.up[b], 0));
-        if (!got) CUDA_TRY(c, cudaMemsetAsync(S.d[b] + FA_FRONT, 0, SAM_CHUNK, c->stream));
-        TRY(fasta_chunk(c, X, St, S.d[b], got, last, path, S.used[b ^ 1], [&]() { return last ? E_OK : fill(b ^ 1, &got2, &last2); }));
+        if (!got) CUDA_TRY(c, cudaMemsetAsync(S.d[b].p + FA_FRONT, 0, SAM_CHUNK, c->stream));
+        TRY(fasta_chunk(c, X, St, S.d[b].p, got, last, path, S.used[b ^ 1], [&]() { return last ? E_OK : fill(b ^ 1, &got2, &last2); }));
         if (last) break;
         b ^= 1; got = got2; last = last2;   // (fasta_chunk of the next chunk records used[b ^ 1] behind its copy of the carried line)
     }
@@ -289,7 +274,7 @@ int load_fasta_bgzf(elp_ctx* c, RefScratch& X, FaState& St, FILE* f, const char*
     bool eof_block = false;
     int b = 0;
     for (;;) {
-        uint8_t* h = S.h[0];
+        uint8_t* h = S.h[0].p;
         const uint64_t nc = cz.size();
         if (nc) memcpy(h, cz.data(), nc);
         const size_t got = fread(h + nc, 1, chunk, f);
@@ -390,9 +375,8 @@ int elfasta_table(elp_ctx* c, FILE* f, const char* path, uint64_t size, std::map
 
 // the new references: one zeroed allocation, a region per distinct matched name (shared by the @SQ lines with that SN)
 struct Install {
-    uint8_t* block = nullptr; uint64_t bytes = 0;
-    std::vector<uint8_t*> raw; std::vector<uint64_t> len;   // per contig: the region (nullptr: no sequence) and its length
-    ~Install() { if (block) cudaFree(block); }
+    DBuf<uint8_t> block; uint64_t bytes = 0;
+    std::vector<uint8_t*> ref; std::vector<uint64_t> len;   // per contig: the payload of its region (nullptr: no sequence) and its length
 };
 inline uint64_t region_bytes(uint64_t n) { return (n + 1) / 2 + REFHOT_PAD + 64; }
 
@@ -413,18 +397,18 @@ int plan_install(elp_ctx* c, const std::map<std::string, uint64_t>& lens, bool f
         I.bytes += region_bytes(kv.second);
     }
     if (I.bytes) {
-        cudaError_t e = cudaMalloc(&I.block, I.bytes);
+        cudaError_t e = I.block.fit(I.bytes);
         if (e != cudaSuccess) { cudaGetLastError(); return c->fail(e == cudaErrorMemoryAllocation ? E_NOMEM : E_CUDA, "elp_load_reference: device allocation of %llu bytes failed", (unsigned long long)I.bytes); }
-        CUDA_TRY(c, cudaMemsetAsync(I.block, 0, I.bytes, c->stream));
+        CUDA_TRY(c, cudaMemsetAsync(I.block.p, 0, I.bytes, c->stream));
     }
-    I.raw.assign(nc, nullptr); I.len.assign(nc, 0);
+    I.ref.assign(nc, nullptr); I.len.assign(nc, 0);
     int32_t miss = 0;
     for (int i = 0; i < nc; i++) {
         auto it = at.find(c->contig_names[i]);
         if (it == at.end()) { miss++; continue; }
-        I.raw[i] = I.block + it->second; I.len[i] = lens.at(it->first);
+        I.ref[i] = I.block.p + it->second + REFHOT_PAD; I.len[i] = lens.at(it->first);
     }
-    for (auto& kv : at) region[kv.first] = I.block + kv.second + REFHOT_PAD;
+    for (auto& kv : at) region[kv.first] = I.block.p + kv.second + REFHOT_PAD;
     *n_unmatched = um; *n_missing = miss;
     return E_OK;
 }
@@ -476,12 +460,12 @@ int load_elfasta(elp_ctx* c, RefScratch& X, FILE* f, const char* path, uint64_t 
         const Piece& p = pieces[i];
         const int b = (int)(i & 1);
         TRY(stage_wait_host(c, S, b));   // (the host reads piece i + 1 while piece i uploads and packs)
-        if (fseeko(f, (off_t)p.off, SEEK_SET) != 0 || fread(S.h[b], 1, p.len, f) != p.len) return read_fail(c, path);
+        if (fseeko(f, (off_t)p.off, SEEK_SET) != 0 || fread(S.h[b].p, 1, p.len, f) != p.len) return read_fail(c, path);
         TRY(stage_upload(c, S, b, p.len, 0));
         CUDA_TRY(c, cudaStreamWaitEvent(s, S.up[b], 0));
         const uint64_t n_out = (p.b0 + p.len + 1) / 2 - p.b0 / 2;
         c->begin("ref_pack", 1.5 * (double)p.len);
-        ref_pack_span_kernel<<<nblk(n_out, 256), 256, 0, s>>>(S.d[b], p.len, p.b0, p.out);
+        ref_pack_span_kernel<<<nblk(n_out, 256), 256, 0, s>>>(S.d[b].p, p.len, p.b0, p.out);
         c->end(); LAUNCH_CHECK(c);
         CUDA_TRY(c, cudaEventRecord(S.used[b], s));
     }
@@ -508,20 +492,15 @@ extern "C" int elp_load_reference(elp_ctx* c, const char* path, uint64_t* n_unma
     if (got < 4 && ferror(f)) return read_fail(c, path);
     if (fseeko(f, 0, SEEK_SET) != 0) return read_fail(c, path);
     RefScratch X;
-    CUDA_TRY(c, cudaMalloc(&X.d_w, W_N * 8));
-    CUDA_TRY(c, cudaHostAlloc(&X.h_w, 16 * 8, cudaHostAllocDefault));
+    CUDA_TRY(c, X.d_w.fit(W_N));
+    CUDA_TRY(c, X.h_w.fit(16));
     const unsigned long long w0[W_N] = {~0ull, ~0ull, 1, 0};   // the file start counts as an empty line before line 1
-    CUDA_TRY(c, cudaMemcpy(X.d_w, w0, sizeof w0, cudaMemcpyHostToDevice));
+    CUDA_TRY(c, cudaMemcpy(X.d_w.p, w0, sizeof w0, cudaMemcpyHostToDevice));
     Install I;
     uint64_t um = 0; int32_t miss = 0;
     if (got == 4 && memcmp(magic, ELFASTA_MAGIC, 4) == 0) TRY(load_elfasta(c, X, f, path, size, chunk, I, &um, &miss));
     else TRY(load_fasta(c, X, f, path, got > 0 && magic[0] == 0x1f, size, chunk, I, &um, &miss));
-    // install: every contig's reference is replaced
-    for (auto p : c->d_refhot_raw) if (p && c->refhot_separate(p)) cudaFree(p);
-    if (c->refhot_block) cudaFree(c->refhot_block);
-    c->refhot_block = I.block; c->refhot_block_bytes = I.bytes; I.block = nullptr;
-    for (int i = 0; i < c->n_contigs; i++) { c->d_refhot_raw[i] = I.raw[i]; c->ref_len[i] = I.len[i]; }
-    c->side_dirty = true;
+    c->ref.install(std::move(I.block), std::move(I.ref), std::move(I.len));   // every contig's reference is replaced
     if (n_unmatched) *n_unmatched = um;
     if (n_missing) *n_missing = miss;
     return ELP_OK;
@@ -531,10 +510,10 @@ extern "C" int64_t elp_reference_get(elp_ctx* c, int32_t contig, uint8_t* nibble
     if (!c) return -1;
     cudaSetDevice(c->device);
     if (contig < 0 || contig >= c->n_contigs) { c->fail(E_INVAL, "elp_reference_get: contig %d out of range", contig); return -1; }
-    const uint64_t n = c->ref_len[contig], k = (n + 1) / 2;
-    const uint8_t* p = c->d_refhot_raw[contig];
+    const uint64_t n = c->ref.n[contig], k = (n + 1) / 2;
+    const uint8_t* p = c->ref.d[contig];
     if (nibbles && p && k && cap >= k) {
-        if (cudaMemcpyAsync(nibbles, p + REFHOT_PAD, k, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) {
+        if (cudaMemcpyAsync(nibbles, p, k, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) {
             c->fail(E_CUDA, "elp_reference_get: %s", cudaGetErrorString(cudaGetLastError()));
             return -1;
         }

@@ -20,30 +20,14 @@
 #include "../../include/elprep_b200.h"
 
 struct SamOutState {
-    uint8_t* d_names = nullptr; uint32_t* d_name_off = nullptr; int32_t* d_canon = nullptr;   // @SQ names, and per contig the first index with its name
-    DBuf<uint32_t> nf, fbits; DBuf<uint64_t> fbase, foff; DBuf<uint8_t> ftext;               // float values: count per line, slots, texts
-    unsigned long long* d_small = nullptr;                                                   // [0] error bits, [1] float values
+    DBuf<uint8_t> d_names; DBuf<uint32_t> d_name_off; DBuf<int32_t> d_canon;   // @SQ names, and per contig the first index with its name
+    DBuf<uint32_t> nf, fbits; DBuf<uint64_t> fbase, foff; DBuf<uint8_t> ftext;  // float values: count per line, slots, texts
+    DBuf<unsigned long long> d_small;                                           // [0] error bits, [1] float values
 };
 
-void sam_out_release(elp_ctx* c) {
-    SamOutState* S = c->sam_out;
-    if (!S) return;
-    S->nf.release(); S->fbits.release(); S->fbase.release(); S->foff.release(); S->ftext.release();
-    void* singles[] = {S->d_names, S->d_name_off, S->d_canon, S->d_small};
-    for (void* p : singles) if (p) cudaFree(p);
-    delete S;
-    c->sam_out = nullptr;
-}
+void free_state(SamOutState* S) { delete S; }
 
 namespace {
-
-inline unsigned nblk(uint64_t n, int t) { return (unsigned)((n + t - 1) / t); }
-template <class T> int grow(elp_ctx* c, DBuf<T>& b, size_t need, size_t keep) {
-    cudaError_t e = b.reserve(need, c->stream, keep);
-    if (e != cudaSuccess) return c->fail(e == cudaErrorMemoryAllocation ? E_NOMEM : E_CUDA, "device allocation of %zu bytes failed: %s", need * sizeof(T), cudaGetErrorString(e));
-    return E_OK;
-}
-#define TRY(x) do { int rc__ = (x); if (rc__) return rc__; } while (0)
 
 enum { FM_MEASURE = 0, FM_LIST = 1, FM_EMIT = 2 };
 enum : unsigned long long { FE_CIGAR_OP = 1, FE_LINE_LIMIT = 2 };
@@ -292,8 +276,8 @@ __global__ void __launch_bounds__(256) sam_out_flen_kernel(uint64_t n, const uin
 // @SQ names and their canon (first index with the same name), uploaded once per context
 int sam_out_tables(elp_ctx* c) {
     if (c->sam_out) return E_OK;
-    SamOutState* S = new SamOutState();
-    c->sam_out = S;
+    c->sam_out.reset(new SamOutState());
+    SamOutState* S = c->sam_out.get();
     std::vector<uint8_t> names; std::vector<uint32_t> off(1, 0); std::vector<int32_t> canon(c->n_contigs + 1, -1);
     std::map<std::string, int32_t> first;
     for (int i = 0; i < c->n_contigs; i++) {
@@ -303,13 +287,13 @@ int sam_out_tables(elp_ctx* c) {
     }
     auto star = first.find("*");
     if (star != first.end()) canon[c->n_contigs] = star->second;
-    CUDA_TRY(c, cudaMalloc(&S->d_names, std::max<size_t>(names.size(), 1)));
-    CUDA_TRY(c, cudaMalloc(&S->d_name_off, off.size() * 4));
-    CUDA_TRY(c, cudaMalloc(&S->d_canon, canon.size() * 4));
-    CUDA_TRY(c, cudaMalloc(&S->d_small, 16));
-    CUDA_TRY(c, cudaMemcpy(S->d_names, names.data(), names.size(), cudaMemcpyHostToDevice));
-    CUDA_TRY(c, cudaMemcpy(S->d_name_off, off.data(), off.size() * 4, cudaMemcpyHostToDevice));
-    CUDA_TRY(c, cudaMemcpy(S->d_canon, canon.data(), canon.size() * 4, cudaMemcpyHostToDevice));
+    CUDA_TRY(c, S->d_names.fit(std::max<size_t>(names.size(), 1)));
+    CUDA_TRY(c, S->d_name_off.fit(off.size()));
+    CUDA_TRY(c, S->d_canon.fit(canon.size()));
+    CUDA_TRY(c, S->d_small.fit(2));
+    CUDA_TRY(c, cudaMemcpy(S->d_names.p, names.data(), names.size(), cudaMemcpyHostToDevice));
+    CUDA_TRY(c, cudaMemcpy(S->d_name_off.p, off.data(), off.size() * 4, cudaMemcpyHostToDevice));
+    CUDA_TRY(c, cudaMemcpy(S->d_canon.p, canon.data(), canon.size() * 4, cudaMemcpyHostToDevice));
     return E_OK;
 }
 
@@ -336,17 +320,17 @@ int sam_out_prepare(elp_ctx* c, uint64_t first, uint64_t n, const uint32_t* sel,
     cudaStream_t s = c->stream;
     TRY(grow(c, c->scan_tmp, n + 8, 0)); TRY(grow(c, c->off_stage, n + 2, 0)); TRY(grow(c, S.nf, n + 8, 0));
     FmtArgs A{};
-    A.n = n; A.first = first; A.sel = sel; A.drop = c->out_fields ? c->d_out_drop : nullptr; A.perm = c->perm.p; A.all_start = c->bam_all_off.p; A.all = c->bam_all.p;
+    A.n = n; A.first = first; A.sel = sel; A.drop = c->out_fields ? c->d_out_drop.p : nullptr; A.perm = c->perm.p; A.all_start = c->bam_all_off.p; A.all = c->bam_all.p;
     A.flag = c->s_flag.p; A.mapq = c->s_mapq.p; A.qoff = c->s_out_off.p; A.qual = c->qual_out_valid ? c->qual_out.p : nullptr;
-    A.names = S.d_names; A.name_off = S.d_name_off; A.canon = S.d_canon; A.n_contigs = c->n_contigs;
-    A.len = c->scan_tmp.p; A.nf = S.nf.p; A.small = S.d_small;
-    CUDA_TRY(c, cudaMemsetAsync(S.d_small, 0, 16, s));
+    A.names = S.d_names.p; A.name_off = S.d_name_off.p; A.canon = S.d_canon.p; A.n_contigs = c->n_contigs;
+    A.len = c->scan_tmp.p; A.nf = S.nf.p; A.small = S.d_small.p;
+    CUDA_TRY(c, cudaMemsetAsync(S.d_small.p, 0, 16, s));
     c->begin("sam_out_measure", (double)c->n_bam * (double)n / (double)std::max<uint64_t>(c->n, 1));
     sam_out_kernel<FM_MEASURE><<<nblk(n * 32, 256), 256, 0, s>>>(A);
     c->end(); LAUNCH_CHECK(c);
     TRY(exclusive_scan_u32_to_u64(c, c->scan_tmp.p, c->off_stage.p, n));
     unsigned long long small[2];
-    CUDA_TRY(c, cudaMemcpyAsync(small, S.d_small, 16, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(c, cudaMemcpyAsync(small, S.d_small.p, 16, cudaMemcpyDeviceToHost, s));
     CUDA_TRY(c, cudaMemcpyAsync(total, c->off_stage.p + n, 8, cudaMemcpyDeviceToHost, s));
     CUDA_TRY(c, cudaStreamSynchronize(s));
     if (small[0] & FE_CIGAR_OP) return c->fail(E_BAM, "elp_fetch_sam: a CIGAR operation code above 8 (cigarOps of the reference has 9 entries, sam/bam-files.go:356-362)");

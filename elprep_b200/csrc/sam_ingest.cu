@@ -23,31 +23,13 @@ struct SamState {
     DBuf<uint8_t> text; DBuf<uint32_t> cnt, len; DBuf<uint64_t> cnt_off, ls;
     DBuf<SlowF> slow; DBuf<uint64_t> patch_off; DBuf<uint32_t> patch_bits;
     DBuf<uint8_t> lost;                       // per line: 1 if its RNAME / RNEXT text is lost in the record (see parse_line)
-    NameDict dict;                            // RNAME / RNEXT dictionary (text_parse.cuh)
-    unsigned long long* d_small = nullptr;   // [0] first error (line << 8 | SamErr), [1] floats handed to the host, [2] lines with a lost name
+    DBuf<unsigned long long> d_small;         // [0] first error (line << 8 | SamErr), [1] floats handed to the host, [2] lines with a lost name
     uint64_t h_last = 0;                      // source of the virtual line end of a final line without '\n'
 };
 
-void sam_state_release(elp_ctx* c) {
-    SamState* S = c->sam;
-    if (!S) return;
-    S->text.release(); S->cnt.release(); S->len.release(); S->cnt_off.release(); S->ls.release();
-    S->slow.release(); S->patch_off.release(); S->patch_bits.release(); S->lost.release();
-    name_dict_release(S->dict);
-    if (S->d_small) cudaFree(S->d_small);
-    delete S;
-    c->sam = nullptr;
-}
+void free_state(SamState* S) { delete S; }
 
 namespace {
-
-inline unsigned nblk(uint64_t n, int t) { return (unsigned)((n + t - 1) / t); }
-template <class T> int grow(elp_ctx* c, DBuf<T>& b, size_t need, size_t keep) {
-    cudaError_t e = b.reserve(need, c->stream, keep);
-    if (e != cudaSuccess) return c->fail(e == cudaErrorMemoryAllocation ? E_NOMEM : E_CUDA, "device allocation of %zu bytes failed: %s", need * sizeof(T), cudaGetErrorString(e));
-    return E_OK;
-}
-#define TRY(x) do { int rc__ = (x); if (rc__) return rc__; } while (0)
 
 // which field of the line failed; the smallest (line << 8 | code) of a call is reported
 enum SamErr : uint32_t {
@@ -388,12 +370,9 @@ __global__ void __launch_bounds__(256) sam_fpatch_kernel(uint64_t n, const uint6
 
 // the RNAME / RNEXT dictionary and the error words, uploaded once per context
 int sam_tables(elp_ctx* c) {
-    if (c->sam && c->sam->d_small) return E_OK;
-    if (!c->sam) c->sam = new SamState();
-    SamState& S = *c->sam;
-    TRY(name_dict_upload(c, S.dict));
-    CUDA_TRY(c, cudaMalloc(&S.d_small, 24));
-    return E_OK;
+    if (!c->sam) c->sam.reset(new SamState());
+    CUDA_TRY(c, c->sam->d_small.fit(3));
+    return name_dict_upload(c);
 }
 
 // strconv.ParseFloat(s, 32) for a decimal the device already checked: strtof rounds correctly; only overflow is an error in Go
@@ -445,15 +424,15 @@ extern "C" int elp_append_sam(elp_ctx* c, const char* text, uint64_t n_bytes) {
     // measure: validate every line and size its record
     SamArgs A{};
     A.text = S.text.p; A.ls = S.ls.p; A.n_lines = nl;
-    A.dict = S.dict;
-    A.len = S.len.p; A.lost = S.lost.p; A.rec_off = c->bam_off.p; A.small = S.d_small;
-    CUDA_TRY(c, cudaMemsetAsync(S.d_small, 0xff, 8, s)); CUDA_TRY(c, cudaMemsetAsync(S.d_small + 1, 0, 16, s));
+    A.dict = c->names.view();
+    A.len = S.len.p; A.lost = S.lost.p; A.rec_off = c->bam_off.p; A.small = S.d_small.p;
+    CUDA_TRY(c, cudaMemsetAsync(S.d_small.p, 0xff, 8, s)); CUDA_TRY(c, cudaMemsetAsync(S.d_small.p + 1, 0, 16, s));
     c->begin("sam_measure", (double)n_bytes);
     sam_line_kernel<false><<<nblk(nl * 32, 256), 256, 0, s>>>(A);
     c->end(); LAUNCH_CHECK(c);
     TRY(exclusive_scan_u32_to_u64(c, S.len.p, c->bam_off.p, nl));
     unsigned long long small[3]; uint64_t total = 0;
-    CUDA_TRY(c, cudaMemcpyAsync(small, S.d_small, 24, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(c, cudaMemcpyAsync(small, S.d_small.p, 24, cudaMemcpyDeviceToHost, s));
     CUDA_TRY(c, cudaMemcpyAsync(&total, c->bam_off.p + nl, 8, cudaMemcpyDeviceToHost, s));
     CUDA_TRY(c, cudaStreamSynchronize(s));
     if (small[0] != ~0ull) {
@@ -464,7 +443,7 @@ extern "C" int elp_append_sam(elp_ctx* c, const char* text, uint64_t n_bytes) {
     // emit: the same parser writes every record at its offset
     TRY(grow(c, c->bam_raw, total + 64, 0)); TRY(grow(c, S.slow, n_slow + 1, 0));
     A.out = c->bam_raw.p; A.slow = S.slow.p;
-    CUDA_TRY(c, cudaMemsetAsync(S.d_small + 1, 0, 8, s));
+    CUDA_TRY(c, cudaMemsetAsync(S.d_small.p + 1, 0, 8, s));
     c->begin("sam_emit", (double)n_bytes + (double)total);
     sam_line_kernel<true><<<nblk(nl * 32, 256), 256, 0, s>>>(A);
     c->end(); LAUNCH_CHECK(c);
@@ -492,9 +471,9 @@ extern "C" int elp_append_sam(elp_ctx* c, const char* text, uint64_t n_bytes) {
     uint64_t lost = small[2];
     if (lost && (c->filter_mask || c->filter_min_mapq > 0)) {   // count only the lines the filters kept (bam_start: their record starts)
         const uint64_t nk = c->n - n0;
-        CUDA_TRY(c, cudaMemsetAsync(S.d_small + 2, 0, 8, s));
-        if (nk) { sam_lost_kept_kernel<<<nblk(nk, 256), 256, 0, s>>>(nk, c->bam_start.p, c->bam_off.p, nl, S.lost.p, S.d_small + 2); c->launches++; LAUNCH_CHECK(c); }
-        CUDA_TRY(c, cudaMemcpyAsync(&lost, S.d_small + 2, 8, cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(c, cudaMemsetAsync(S.d_small.p + 2, 0, 8, s));
+        if (nk) { sam_lost_kept_kernel<<<nblk(nk, 256), 256, 0, s>>>(nk, c->bam_start.p, c->bam_off.p, nl, S.lost.p, S.d_small.p + 2); c->launches++; LAUNCH_CHECK(c); }
+        CUDA_TRY(c, cudaMemcpyAsync(&lost, S.d_small.p + 2, 8, cudaMemcpyDeviceToHost, s));
         CUDA_TRY(c, cudaStreamSynchronize(s));
     }
     c->n_sam_lost_names += lost;

@@ -11,23 +11,18 @@ int radix_sort_impl(elp_ctx* c, K* ka, K* kb, uint32_t* va, uint32_t* vb, uint64
     if (n >= (1ull << 30)) return c->fail(E_LIMIT, "radix sort: %llu keys exceed the 2^30 limit of the look-back status words", (unsigned long long)n);
     if (lo_bit < 0 || lo_bit + key_bits > (int)(8 * sizeof(K))) return c->fail(E_INVAL, "radix sort: bits [%d, %d) outside the key", lo_bit, lo_bit + key_bits);
     Plan plan = make_plan(key_bits, lo_bit);
-    Workspace& ws = c->ws;
-    if (!ws.ghist) {
-        CUDA_TRY(c, cudaMalloc(&ws.ghist, MAX_PASSES * RADIX * 4));
-        CUDA_TRY(c, cudaMalloc(&ws.gofs, MAX_PASSES * RADIX * 4));
-        CUDA_TRY(c, cudaMalloc(&ws.counters, MAX_PASSES * 4));
-    }
+    SortWorkspace& ws = c->ws;
+    CUDA_TRY(c, ws.ghist.fit(MAX_PASSES * RADIX)); CUDA_TRY(c, ws.gofs.fit(MAX_PASSES * RADIX)); CUDA_TRY(c, ws.counters.fit(MAX_PASSES));
     const size_t tile = tile_size<K>();
     const uint64_t tiles = (n + tile - 1) / tile;
-    const size_t need = (size_t)plan.n_passes * tiles * RADIX * 4;
-    if (need > ws.status_bytes) {
-        if (ws.status) { cudaStreamSynchronize(c->stream); cudaFree(ws.status); }
-        ws.status_bytes = need + need / 4;
-        CUDA_TRY(c, cudaMalloc(&ws.status, ws.status_bytes));
+    const size_t need = (size_t)plan.n_passes * tiles * RADIX;   // status words
+    if (need > ws.status.cap) {
+        if (ws.status.p) cudaStreamSynchronize(c->stream);
+        CUDA_TRY(c, ws.status.fit(need + need / 4));
     }
-    CUDA_TRY(c, cudaMemsetAsync(ws.ghist, 0, MAX_PASSES * RADIX * 4, c->stream));
-    CUDA_TRY(c, cudaMemsetAsync(ws.counters, 0, MAX_PASSES * 4, c->stream));
-    CUDA_TRY(c, cudaMemsetAsync(ws.status, 0, need, c->stream));
+    CUDA_TRY(c, cudaMemsetAsync(ws.ghist.p, 0, MAX_PASSES * RADIX * 4, c->stream));
+    CUDA_TRY(c, cudaMemsetAsync(ws.counters.p, 0, MAX_PASSES * 4, c->stream));
+    CUDA_TRY(c, cudaMemsetAsync(ws.status.p, 0, need * 4, c->stream));
 
     int dev_sms = 132;
     cudaDeviceGetAttribute(&dev_sms, cudaDevAttrMultiProcessorCount, c->device);
@@ -37,11 +32,11 @@ int radix_sort_impl(elp_ctx* c, K* ka, K* kb, uint32_t* va, uint32_t* vb, uint64
         int grid = (int)std::min<uint64_t>(want, (uint64_t)dev_sms * 4);
         if (grid < 1) grid = 1;
         c->begin(nm.c_str(), (double)n * sizeof(K));
-        rs_hist_kernel<K><<<grid, 512, 0, c->stream>>>(ka, n, plan, ws.ghist);
+        rs_hist_kernel<K><<<grid, 512, 0, c->stream>>>(ka, n, plan, ws.ghist.p);
         c->end();
         LAUNCH_CHECK(c);
         c->begin("radix_scan", 0);
-        rs_scan_kernel<<<plan.n_passes, RADIX, 0, c->stream>>>(ws.ghist, ws.gofs);
+        rs_scan_kernel<<<plan.n_passes, RADIX, 0, c->stream>>>(ws.ghist.p, ws.gofs.p);
         c->end();
         LAUNCH_CHECK(c);
     }
@@ -53,8 +48,8 @@ int radix_sort_impl(elp_ctx* c, K* ka, K* kb, uint32_t* va, uint32_t* vb, uint64
     K* in = ka; K* out = kb; uint32_t* vin = va; uint32_t* vout = vb;
     for (int p = 0; p < plan.n_passes; p++) {
         c->begin(nm.c_str(), (double)n * 2.0 * (sizeof(K) + 4));
-        kern<<<(unsigned)tiles, Cfg<K>::THREADS, smem, c->stream>>>(in, out, vin, vout, n, plan.shift[p], plan.bits[p], ws.gofs + p * RADIX,
-                                                                   ws.status + (size_t)p * tiles * RADIX, ws.counters + p);
+        kern<<<(unsigned)tiles, Cfg<K>::THREADS, smem, c->stream>>>(in, out, vin, vout, n, plan.shift[p], plan.bits[p], ws.gofs.p + p * RADIX,
+                                                                   ws.status.p + (size_t)p * tiles * RADIX, ws.counters.p + p);
         c->end();
         LAUNCH_CHECK(c);
         std::swap(in, out); std::swap(vin, vout);

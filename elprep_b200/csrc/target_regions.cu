@@ -16,8 +16,6 @@
 
 namespace {
 
-inline unsigned nblk(uint64_t n, int t) { return (unsigned)((n + t - 1) / t); }
-
 // alnStart = POS; alnEnd = End() for a mapped read whose CIGAR has read bases, else POS (:318-324).  The sums are Go's int32 sums: they wrap.
 __global__ void __launch_bounds__(256) target_keep_kernel(uint64_t n, const int32_t* __restrict__ refid, const int32_t* __restrict__ pos, const uint16_t* __restrict__ flag,
                                                            const uint64_t* __restrict__ cigar_off, const uint32_t* __restrict__ ncigar, const uint32_t* __restrict__ cigar,
@@ -76,13 +74,6 @@ __global__ void __launch_bounds__(256) target_summary_kernel(uint64_t n, const i
     }
 }
 
-template <class T> int grow(elp_ctx* c, DBuf<T>& b, size_t need) {
-    cudaError_t e = b.reserve(need, c->stream);
-    if (e != cudaSuccess) return c->fail(e == cudaErrorMemoryAllocation ? E_NOMEM : E_CUDA, "device allocation of %zu bytes failed: %s", need * sizeof(T), cudaGetErrorString(e));
-    return E_OK;
-}
-#define TRY(x) do { int rc__ = (x); if (rc__) return rc__; } while (0)
-
 }  // namespace
 
 int phase_target_filter(elp_ctx* c, uint64_t* n_removed) {
@@ -92,15 +83,15 @@ int phase_target_filter(elp_ctx* c, uint64_t* n_removed) {
     uint64_t kept = n;
     if (n) {
         cudaStream_t s = c->stream;
-        TRY(region_upload(c, c->bqsr_regions));
+        TRY(table_upload(c, c->bqsr_regions));
         TRY(grow(c, c->scan_tmp, n + 8));
         // the kept count lives in the BQSR gather's small words (cleared by the gather before its own use)
-        unsigned long long* d_kept = reinterpret_cast<unsigned long long*>(c->d_bq_small);
+        unsigned long long* d_kept = reinterpret_cast<unsigned long long*>(c->d_bq_small.p);
         CUDA_TRY(c, cudaMemsetAsync(d_kept, 0, 8, s));
         const double cigar_bytes = 4.0 * (double)c->n_cigar * (double)n / (double)std::max<uint64_t>(c->n, 1);
         c->begin("target_keep", (double)n * (4 + 4 + 2 + 8 + 4 + 4) + cigar_bytes);
         target_keep_kernel<<<nblk(n, 256), 256, 0, s>>>(n, c->s_refid.p, c->s_pos.p, c->s_flag.p, c->s_cigar_off.p, c->s_ncigar.p, c->cigar.p,
-                                                         c->bqsr_regions.d_ptrs, c->bqsr_regions.d_n, c->n_contigs, c->scan_tmp.p, d_kept);
+                                                         c->bqsr_regions.d_ptrs.p, c->bqsr_regions.d_n.p, c->n_contigs, c->scan_tmp.p, d_kept);
         c->end(); LAUNCH_CHECK(c);
         unsigned long long hk = 0;
         CUDA_TRY(c, cudaMemcpyAsync(&hk, d_kept, 8, cudaMemcpyDeviceToHost, s));
@@ -116,19 +107,19 @@ int phase_target_filter(elp_ctx* c, uint64_t* n_removed) {
             TRY(build_output_columns(c, c->perm.p, kept, true));
             // whole-context summaries the BQSR phases choose kernels and table sizes by, now over the kept reads: lseq_max (h_ranges, which
             // phase_adapt keeps while `adapted` holds: no read can be appended after the sort) and the QUAL presence bitmap
-            CUDA_TRY(c, cudaMemsetAsync(c->d_qpresent, 0, 16, s));
-            CUDA_TRY(c, cudaMemsetAsync(&c->d_ranges->lseq_max, 0, 4, s));
+            CUDA_TRY(c, cudaMemsetAsync(c->d_qpresent.p, 0, 16, s));
+            CUDA_TRY(c, cudaMemsetAsync(&c->d_ranges.p->lseq_max, 0, 4, s));
             if (kept) {
                 int sms = 132; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device);
                 const double qual_bytes = (double)(c->n_qual - ARENA_FRONT_PAD) * (double)kept / (double)std::max<uint64_t>(c->n, 1);
                 c->begin("target_summary", (double)kept * (4 + 8) + qual_bytes);
                 target_summary_kernel<<<(unsigned)std::min<uint64_t>(nblk(kept * 32, 256), (uint64_t)sms * 16), 256, 0, s>>>(kept, c->s_lseq.p, c->s_qual_off.p, c->qual.p,
-                                                                                                                      c->d_qpresent, &c->d_ranges->lseq_max);
+                                                                                                                      c->d_qpresent.p, &c->d_ranges.p->lseq_max);
                 c->end(); LAUNCH_CHECK(c);
             }
             int32_t lm = 0;
-            CUDA_TRY(c, cudaMemcpyAsync(&lm, &c->d_ranges->lseq_max, 4, cudaMemcpyDeviceToHost, s));
-            CUDA_TRY(c, cudaMemcpyAsync(c->h_qpresent, c->d_qpresent, 16, cudaMemcpyDeviceToHost, s));
+            CUDA_TRY(c, cudaMemcpyAsync(&lm, &c->d_ranges.p->lseq_max, 4, cudaMemcpyDeviceToHost, s));
+            CUDA_TRY(c, cudaMemcpyAsync(c->h_qpresent, c->d_qpresent.p, 16, cudaMemcpyDeviceToHost, s));
             CUDA_TRY(c, cudaStreamSynchronize(s));
             c->h_ranges.lseq_max = lm;
             c->n_sorted = kept;

@@ -2,22 +2,14 @@
 // (known_sites.cu).
 //   sam_count_kernel / sam_lines_kernel   the line finder: '\n' count per 64-byte chunk, exclusive scan (host), line starts
 //   parse_dec                             strconv.ParseInt / ParseUint, base 10
-//   NameDict, name_entry, refid_of        "*" and the @SQ SN names on the device, and their upload (name_dict_upload)
+//   name_entry, refid_of                  lookups in the context's dictionary of "*" and the @SQ SN names (NameDict, ctx.h), and its
+//                                         upload (name_dict_upload)
 #pragma once
 #include <algorithm>
 #include <map>
 #include <string>
 #include <vector>
 #include "ctx.h"
-
-// ---- reference names ----
-// "*" and every @SQ SN, sorted bytewise.  id: the refid of dictTable / AddREFID ("*" -> -1, an @SQ SN -> its index, the last of equal
-// names wins).  all[all_off[e], all_off[e + 1]): every @SQ index with entry e's name, in header order ("*" has none).
-struct NameDict {
-    uint8_t* names = nullptr; uint32_t* off = nullptr; int32_t* id = nullptr;
-    uint32_t* all_off = nullptr; int32_t* all = nullptr;
-    int n = 0;
-};
 
 namespace {
 
@@ -90,15 +82,10 @@ __device__ __forceinline__ int32_t refid_of(const NameDict& D, const uint8_t* s,
     return e < 0 ? -1 : D.id[e];
 }
 
-void name_dict_release(NameDict& D) {
-    void* p[] = {D.names, D.off, D.id, D.all_off, D.all};
-    for (void* q : p) if (q) cudaFree(q);
-    D = NameDict();
-}
-
-// the dictionary of the context's elp_config.contig_names, uploaded with blocking copies
-int name_dict_upload(elp_ctx* c, NameDict& D) {
-    name_dict_release(D);
+// the dictionary of the context's elp_config.contig_names (c->names), uploaded with blocking copies on first use
+int name_dict_upload(elp_ctx* c) {
+    NameDictBufs& D = c->names;
+    if (D.n) return E_OK;
     std::map<std::string, std::vector<int32_t>> dict;
     dict["*"];
     for (int i = 0; i < c->n_contigs; i++) dict[c->contig_names[i]].push_back(i);
@@ -109,16 +96,16 @@ int name_dict_upload(elp_ctx* c, NameDict& D) {
         if (kv.first != "*") all.insert(all.end(), kv.second.begin(), kv.second.end());
         all_off.push_back((uint32_t)all.size());
     }
-    CUDA_TRY(c, cudaMalloc(&D.names, std::max<size_t>(names.size(), 1)));
-    CUDA_TRY(c, cudaMalloc(&D.off, off.size() * 4));
-    CUDA_TRY(c, cudaMalloc(&D.id, id.size() * 4));
-    CUDA_TRY(c, cudaMalloc(&D.all_off, all_off.size() * 4));
-    CUDA_TRY(c, cudaMalloc(&D.all, std::max<size_t>(all.size(), 1) * 4));
-    CUDA_TRY(c, cudaMemcpy(D.names, names.data(), names.size(), cudaMemcpyHostToDevice));
-    CUDA_TRY(c, cudaMemcpy(D.off, off.data(), off.size() * 4, cudaMemcpyHostToDevice));
-    CUDA_TRY(c, cudaMemcpy(D.id, id.data(), id.size() * 4, cudaMemcpyHostToDevice));
-    CUDA_TRY(c, cudaMemcpy(D.all_off, all_off.data(), all_off.size() * 4, cudaMemcpyHostToDevice));
-    if (!all.empty()) CUDA_TRY(c, cudaMemcpy(D.all, all.data(), all.size() * 4, cudaMemcpyHostToDevice));
+    CUDA_TRY(c, D.names.fit(std::max<size_t>(names.size(), 1)));
+    CUDA_TRY(c, D.off.fit(off.size()));
+    CUDA_TRY(c, D.id.fit(id.size()));
+    CUDA_TRY(c, D.all_off.fit(all_off.size()));
+    CUDA_TRY(c, D.all.fit(std::max<size_t>(all.size(), 1)));
+    CUDA_TRY(c, cudaMemcpy(D.names.p, names.data(), names.size(), cudaMemcpyHostToDevice));
+    CUDA_TRY(c, cudaMemcpy(D.off.p, off.data(), off.size() * 4, cudaMemcpyHostToDevice));
+    CUDA_TRY(c, cudaMemcpy(D.id.p, id.data(), id.size() * 4, cudaMemcpyHostToDevice));
+    CUDA_TRY(c, cudaMemcpy(D.all_off.p, all_off.data(), all_off.size() * 4, cudaMemcpyHostToDevice));
+    if (!all.empty()) CUDA_TRY(c, cudaMemcpy(D.all.p, all.data(), all.size() * 4, cudaMemcpyHostToDevice));
     D.n = (int)id.size();
     return E_OK;
 }

@@ -28,6 +28,11 @@ def _cstrs(items):
     return arr
 
 
+def live_allocations():
+    """Device and page-locked allocations the library holds, over every context of the process."""
+    return int(_lib.load().elp_debug_live_allocations())
+
+
 class Context:
     """One device context = one (*sam.Sam) being filled, sorted, duplicate-marked and recalibrated."""
 

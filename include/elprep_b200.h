@@ -104,6 +104,9 @@ typedef struct {
 int elp_create(const elp_config *cfg, elp_ctx **out);
 void elp_destroy(elp_ctx *ctx);
 const char *elp_last_error(const elp_ctx *ctx);          /* ctx may be NULL: error of the last failed elp_create */
+/* tests: device and page-locked allocations that the library holds, over every context of the process (back to its earlier value
+ * once every context created since has been destroyed) */
+int64_t elp_debug_live_allocations(void);
 /* optional capacity hint so that appends never reallocate */
 int elp_reserve(elp_ctx *ctx, uint64_t n_reads, uint64_t n_bases, uint64_t n_cigar_ops, uint64_t n_qname_bytes);
 /* forget all reads/tables but keep device allocations, reference and known sites (bench steps) */
