@@ -12,7 +12,7 @@ SO_PATH = os.environ.get("ELPREP_B200_LIB", os.path.join(_HERE, "lib", "libelpre
 
 SO_KEEP, SO_UNKNOWN, SO_UNSORTED, SO_QUERYNAME, SO_COORDINATE = 0, 1, 2, 3, 4
 MARKDUP, MARKDUP_OPTICAL = 1, 2
-EINVAL, EREFEND, ELIMIT, ESTATE, EBAM, EBGZF, ESAM, ESITES, EFASTA = -1, -14, -15, -16, -18, -19, -20, -21, -22
+EINVAL, EREFEND, ELIMIT, ESTATE, EBAM, EBGZF, ESAM, ESITES, EFASTA, EVCF = -1, -14, -15, -16, -18, -19, -20, -21, -22, -23
 FILTER_UNMAPPED, FILTER_UNMAPPED_STRICT, FILTER_NON_EXACT, FILTER_DUPLICATES, FILTER_NON_EXACT_STRICT, FILTER_TARGET_REGIONS = 1, 2, 4, 8, 16, 32
 FILTER_CLEAR_DUPLICATE_FLAG = 64
 OUT_REMOVE_DUPLICATES, OUT_REMOVE_OPTIONAL_READS, OUT_KEEP_FIELDS = 1, 2, 4

@@ -26,6 +26,7 @@
 #define E_SAM (-20)
 #define E_SITES (-21)
 #define E_FASTA (-22)
+#define E_VCF (-23)
 #define E_STATE (-16)
 
 // device-side error word bits (one u32 in global memory, OR-ed by kernels, read by the host after the phase)

@@ -12,15 +12,25 @@
 //   sites_sort     the onesweep radix sort of contig << 32 | (start ^ 2^31), the end as payload
 //   sites_flatten  one prefix max over contig << 32 | (end ^ 2^31): interval i opens a group iff it is the first of its contig or its start
 //                  lies above every earlier end of its contig; the group heads are compacted and each group keeps the max of its ends
+// A VCF in the list (plain or BGZF, see vcf.cuh) gives the intervals of intervals.FromVcfFile (intervals/intervals.go:306-338):
+//   host           the header, parsed as ParseHeader does (BGZF: its leading blocks inflated with zlib); then the data lines go through
+//                  the two chunks as reference_load.cu streams FASTA (plain text uploaded, BGZF blocks inflated by bgzf_inflate), the
+//                  partial line at a chunk's end carried on the device
+//   sites_lines    the same line finder
+//   vcf_parse      a warp per 32 lines (vcf.cuh) into the arrays sites_parse fills; sites_sort, sites_flatten and the install follow as
+//                  for .elsites lines, over the intervals of every file in list order
 // Nothing is installed before every file was read and every line accepted; the new table is one allocation (ContigTable::block).
 #include <algorithm>
 #include <cerrno>
 #include <cstdio>
 #include <cstring>
 #include <vector>
+#include <zlib.h>
 #include "ctx.h"
 #include "text_parse.cuh"
 #include "file_stage.cuh"
+#include "bgzf_scan.hpp"
+#include "vcf.cuh"
 #include "../../include/elprep_b200.h"
 
 namespace {
@@ -29,14 +39,18 @@ const char SITES_HEADER[] = "# elsites format version 1.0\n";   // intervals.Els
 constexpr uint64_t SITES_HEADER_LEN = sizeof(SITES_HEADER) - 1;
 constexpr uint64_t SITES_MAX_LINE = 65536;                     // bufio.MaxScanTokenSize: a longer line stops the reference's scanner
 constexpr uint64_t SITES_CHUNK_DEFAULT = 32ull << 20;
+constexpr uint64_t VCF_FRONT = VCF_MAX_LINE;                   // device bytes ahead of a VCF chunk's text: room for the carried partial line
+constexpr uint64_t BGZF_MAX_BLOCK = 65536;
 
 }  // namespace
 
 // page-locked and device staging, reused by every call on the context
 struct SitesStage {
     FileStage f;                                                 // the two chunks (file_stage.cuh); a carried partial line sits in front of the file bytes
-    DBuf<unsigned long long> d_small;                            // [0] first error (line << 8 | SitesErr), [1] unmatched lines
-    HBuf<unsigned long long> h_small;                            // [0, 1] copies, [2] '\n' count, [3] intervals, [4] virtual line end
+    FileStage v;                                                 // the chunks of VCF files: VCF_FRONT device bytes ahead of each chunk's text
+    DBuf<uint8_t> tb[2];                                         // inflated BGZF VCF text, VCF_FRONT bytes in
+    DBuf<unsigned long long> d_small;                            // [0] first error (line << 8 | SitesErr or VcfErr), [1] unmatched lines, [2] QUAL band count
+    HBuf<unsigned long long> h_small;                            // [0, 1] copies, [2] '\n' count, [3] intervals, [4] virtual line end, [5, 8) VCF words
 };
 
 void free_state(SitesStage* S) { delete S; }
@@ -244,6 +258,8 @@ __global__ void __launch_bounds__(256) sites_unbias_kernel(uint64_t n_groups, in
 struct SitesScratch {   // per call; freed on return
     DBuf<uint32_t> cnt, emit, vals_a, vals_b, head; DBuf<uint64_t> cnt_off, ls, emit_off, keys_a, keys_b, tmax, gid, first;
     DBuf<int32_t> ent, start, end;
+    DBuf<uint64_t> band_line, band_at;                           // VCF: QUAL values next to the overflow bound
+    DBuf<uint8_t> inames, itype; DBuf<uint32_t> ioff; DBuf<int32_t> inum;   // VCF: the declared INFO IDs
 };
 
 int sites_stage_init(elp_ctx* c) {
@@ -251,7 +267,7 @@ int sites_stage_init(elp_ctx* c) {
     SitesStage& S = *c->sites;
     const uint64_t want = c->sites_chunk ? c->sites_chunk : SITES_CHUNK_DEFAULT, cap = want + SITES_MAX_LINE;
     TRY(stage_init(c, S.f, want, cap, stage_padded(cap), "elp_load_known_sites"));
-    CUDA_TRY(c, S.d_small.fit(2)); CUDA_TRY(c, S.h_small.fit(8));
+    CUDA_TRY(c, S.d_small.fit(4)); CUDA_TRY(c, S.h_small.fit(16));
     return name_dict_upload(c);
 }
 
@@ -315,7 +331,291 @@ int parse_finish(elp_ctx* c, SitesStage& S, SitesScratch& X, const LineChunk& ch
     return E_OK;
 }
 
-// one file: the header on the host, then every line through the device, appended behind *total
+// ---- VCF files ----
+int vcf_fail(elp_ctx* c, const char* path, int file, uint64_t line, const char* why) {
+    return c->fail(E_VCF, "elp_load_known_sites: %s (file %d), line %llu (1-based, header lines counted): %s", path, file, (unsigned long long)line, why);
+}
+int read_fail(elp_ctx* c, const char* path) { return c->fail(E_INVAL, "elp_load_known_sites: cannot read %s: %s", path, strerror(errno)); }
+
+struct VcfState {     // carried from chunk to chunk
+    uint64_t line0 = 1;                                      // the 1-based number of the next chunk's first line
+    const uint8_t* carry = nullptr; uint64_t carry_n = 0;    // the partial line at the end of the last chunk (device)
+};
+
+// the QUAL values in the band next to the overflow bound, decided with strtod: the smallest chunk line whose value overflows, or ~0
+int vcf_band(elp_ctx* c, SitesScratch& X, const uint8_t* t, uint64_t n_band, uint64_t* bad) {
+    std::vector<uint64_t> ln(n_band), at(n_band);
+    CUDA_TRY(c, cudaMemcpy(ln.data(), X.band_line.p, n_band * 8, cudaMemcpyDeviceToHost));
+    CUDA_TRY(c, cudaMemcpy(at.data(), X.band_at.p, n_band * 8, cudaMemcpyDeviceToHost));
+    std::vector<uint64_t> order(n_band);
+    for (uint64_t i = 0; i < n_band; i++) order[i] = i;
+    std::sort(order.begin(), order.end(), [&](uint64_t a, uint64_t b) { return ln[a] < ln[b]; });
+    std::vector<uint8_t> q;
+    *bad = ~0ull;
+    for (uint64_t i : order) {
+        q.resize(at[i] & 0xffff);
+        CUDA_TRY(c, cudaMemcpy(q.data(), t + (at[i] >> 16), q.size(), cudaMemcpyDeviceToHost));
+        if (go_float_overflows(q.data(), q.size())) { *bad = ln[i]; return E_OK; }
+    }
+    return E_OK;
+}
+
+// one chunk of VCF text: nnew bytes at buf + VCF_FRONT (zero bytes behind them), of which the first `skip` still belong to the header,
+// behind the carried partial line; its intervals are appended at keys_a / vals_a + *total.  `overlap` runs on the host while the line
+// count runs.
+template <class F>
+int vcf_chunk(elp_ctx* c, SitesStage& S, SitesScratch& X, VcfState& St, const VcfInfoTab& info, uint8_t* buf, uint64_t skip, uint64_t nnew, bool last,
+              int file, const char* path, cudaEvent_t release_prev, uint64_t* total, F&& overlap) {
+    cudaStream_t s = c->stream;
+    unsigned long long* hw = S.h_small.p;
+    const uint64_t nc = St.carry_n, a = (VCF_FRONT - nc) & ~(uint64_t)(SAM_CHUNK - 1), front = VCF_FRONT - nc + skip - a, end = VCF_FRONT + nnew - a;
+    uint8_t* t = buf + a;
+    if (nc) CUDA_TRY(c, cudaMemcpyAsync(buf + VCF_FRONT - nc, St.carry, nc, cudaMemcpyDeviceToDevice, s));
+    if (VCF_FRONT - nc - a) CUDA_TRY(c, cudaMemsetAsync(t, 0, VCF_FRONT - nc - a, s));   // (no '\n' in front of the first line)
+    if (skip) CUDA_TRY(c, cudaMemsetAsync(buf + VCF_FRONT, 0, skip, s));                  // (nor in the header's bytes)
+    if (release_prev) CUDA_TRY(c, cudaEventRecord(release_prev, s));
+    St.carry = nullptr; St.carry_n = 0;
+    if (end == front) return overlap();
+    const uint64_t n_chunks = (end + SAM_CHUNK - 1) / SAM_CHUNK;
+    TRY(grow(c, X.cnt, n_chunks + 8, 0)); TRY(grow(c, X.cnt_off, n_chunks + 2, 0));
+    c->begin("sites_lines", (double)(end - front));
+    sam_count_kernel<<<nblk(n_chunks, 256), 256, 0, s>>>(t, n_chunks, X.cnt.p);
+    c->end(); LAUNCH_CHECK(c);
+    TRY(exclusive_scan_u32_to_u64(c, X.cnt.p, X.cnt_off.p, n_chunks));
+    CUDA_TRY(c, cudaMemcpyAsync(hw + 2, X.cnt_off.p + n_chunks, 8, cudaMemcpyDeviceToHost, s));
+    TRY(overlap());
+    CUDA_TRY(c, cudaStreamSynchronize(s));
+    const uint64_t n_nl = hw[2];
+    TRY(grow(c, X.ls, n_nl + 2, 0));
+    hw[7] = front;
+    CUDA_TRY(c, cudaMemcpyAsync(X.ls.p, hw + 7, 8, cudaMemcpyHostToDevice, s));
+    c->begin("sites_lines", (double)(end - front) + 8.0 * (double)n_nl);
+    sam_lines_kernel<<<nblk(n_chunks, 256), 256, 0, s>>>(t, n_chunks, X.cnt_off.p, X.ls.p);
+    c->end(); LAUNCH_CHECK(c);
+    CUDA_TRY(c, cudaMemcpyAsync(hw + 6, X.ls.p + n_nl, 8, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(c, cudaStreamSynchronize(s));
+    const uint64_t m = hw[6];   // the end of the whole lines
+    uint64_t nl = n_nl;
+    if (last && m < end) { hw[4] = end + 1; nl++; CUDA_TRY(c, cudaMemcpyAsync(X.ls.p + nl, hw + 4, 8, cudaMemcpyHostToDevice, s)); }   // a virtual '\n'
+    if (!last) { St.carry = t + m; St.carry_n = end - m; }
+    if (nl) {
+        TRY(grow(c, X.ent, nl + 8, 0)); TRY(grow(c, X.start, nl + 8, 0)); TRY(grow(c, X.end, nl + 8, 0)); TRY(grow(c, X.emit, nl + 8, 0));
+        TRY(grow(c, X.emit_off, nl + 2, 0)); TRY(grow(c, X.band_line, nl + 1, 0)); TRY(grow(c, X.band_at, nl + 1, 0));
+        CUDA_TRY(c, cudaMemsetAsync(S.d_small.p + 2, 0, 8, s));
+        VcfArgs A{};
+        A.t = t; A.ls = X.ls.p; A.n_lines = nl; A.line0 = St.line0; A.dict = c->names.view(); A.info = info;
+        A.ent = X.ent.p; A.start = X.start.p; A.end = X.end.p; A.emit = X.emit.p; A.small = S.d_small.p;
+        A.band_line = X.band_line.p; A.band_at = X.band_at.p; A.n_band = S.d_small.p + 2;
+        const uint64_t groups = (nl + 31) / 32;
+        const unsigned grid = (unsigned)std::min<uint64_t>((groups + VP_T / 32 - 1) / (VP_T / 32), 132 * 16);
+        c->begin("vcf_parse", (double)(std::max(m, end) - front) + 8.0 * (double)(nl + 1) + 16.0 * (double)nl);
+        vcf_parse_kernel<<<grid, VP_T, 0, s>>>(A);
+        c->end(); LAUNCH_CHECK(c);
+        TRY(exclusive_scan_u32_to_u64(c, X.emit.p, X.emit_off.p, nl));
+        CUDA_TRY(c, cudaMemcpyAsync(hw + 8, S.d_small.p, 24, cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(c, cudaMemcpyAsync(hw + 3, X.emit_off.p + nl, 8, cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(c, cudaStreamSynchronize(s));
+        unsigned long long err = hw[8];
+        if (hw[10]) {
+            uint64_t bad = ~0ull;
+            TRY(vcf_band(c, X, t, hw[10], &bad));
+            if (bad != ~0ull && St.line0 + bad <= (err >> 8)) err = ((St.line0 + bad) << 8) | VL_QUAL_RANGE;   // QUAL precedes FILTER and INFO
+        }
+        if (err != ~0ull) return vcf_fail(c, path, file, err >> 8, vcf_err_text((uint32_t)(err & 0xff)));
+        const uint64_t add = hw[3], t0 = *total;
+        if (t0 + add >= (1ull << 30)) return c->fail(E_LIMIT, "elp_load_known_sites: 2^30 or more intervals in total (the limit of the device sort)");
+        if (t0 + add + 4 > X.keys_a.cap) { const size_t want = std::max<size_t>(t0 + add + 4, 2 * X.keys_a.cap); TRY(grow(c, X.keys_a, want, t0)); TRY(grow(c, X.vals_a, want, t0)); }
+        c->begin("sites_parse", 24.0 * (double)nl + 12.0 * (double)add);
+        sites_emit_kernel<<<nblk(nl, 256), 256, 0, s>>>(nl, X.ent.p, X.start.p, X.end.p, X.emit.p, X.emit_off.p, c->names.view(), X.keys_a.p + t0, X.vals_a.p + t0);
+        c->end(); LAUNCH_CHECK(c);
+        *total = t0 + add;
+        St.line0 += nl;
+    }
+    if (St.carry_n >= VCF_MAX_LINE) return vcf_fail(c, path, file, St.line0, vcf_err_text(VL_LONG));
+    return E_OK;
+}
+
+// the leading BGZF blocks of a file, inflated on the host one at a time for the header (HReader's byte source)
+struct BgzfHead {
+    elp_ctx* c; FILE* f; const char* path;
+    std::vector<uint8_t> cz; uint64_t cz_at = 0, out = 0;   // compressed bytes not yet inflated, their file offset; bytes inflated
+    std::vector<BgzfBlock> blocks;                          // in_off: file offset, out_off, isize
+    int operator()(std::vector<uint8_t>& buf) {
+        for (;;) {
+            std::vector<BgzfBlock> bl; uint64_t tot = 0, used = 0;
+            if (scan_blocks(cz.data(), cz.size(), bl, &tot, &used, 1))
+                return c->fail(E_BGZF, "elp_load_known_sites: %s, file offset %llu: malformed BGZF block header (gzip magic, FEXTRA, BC subfield, block size or ISIZE)", path, (unsigned long long)cz_at);
+            if (!bl.empty()) {
+                BgzfBlock b = bl[0];
+                const size_t o = buf.size();
+                buf.resize(o + b.isize);
+                bool ok = true;
+                if (b.isize) {
+                    z_stream zs; memset(&zs, 0, sizeof zs);
+                    ok = inflateInit2(&zs, -15) == Z_OK;
+                    if (ok) {
+                        zs.next_in = cz.data() + b.cdata_off; zs.avail_in = (uInt)b.cdata_len; zs.next_out = buf.data() + o; zs.avail_out = b.isize;
+                        ok = inflate(&zs, Z_FINISH) == Z_STREAM_END && zs.total_out == b.isize;
+                        inflateEnd(&zs);
+                    }
+                }
+                if (!ok || (uint32_t)crc32(crc32(0L, Z_NULL, 0), buf.data() + o, b.isize) != b.crc)
+                    return c->fail(E_BGZF, "elp_load_known_sites: %s, BGZF block at file offset %llu: bad DEFLATE data or CRC32", path, (unsigned long long)cz_at);
+                b.in_off = cz_at; b.out_off = out;
+                blocks.push_back(b);
+                out += b.isize;
+                cz.erase(cz.begin(), cz.begin() + used); cz_at += used;
+                if (b.isize) return 1;
+                continue;
+            }
+            uint8_t tmp[1 << 16];
+            const size_t got = fread(tmp, 1, sizeof tmp, f);
+            if (!got) {
+                if (ferror(f)) return read_fail(c, path);
+                if (!cz.empty()) return c->fail(E_BGZF, "elp_load_known_sites: %s, file offset %llu: the file ends inside a BGZF block", path, (unsigned long long)cz_at);
+                return 0;
+            }
+            cz.insert(cz.end(), tmp, tmp + got);
+        }
+    }
+};
+
+struct PlainHead {
+    elp_ctx* c; FILE* f; const char* path;
+    int operator()(std::vector<uint8_t>& buf) {
+        const size_t o = buf.size();
+        buf.resize(o + (1 << 16));
+        const size_t got = fread(buf.data() + o, 1, 1 << 16, f);
+        buf.resize(o + got);
+        if (!got && ferror(f)) return read_fail(c, path);
+        return got ? 1 : 0;
+    }
+};
+
+// the declared INFO IDs to the device (the first of equal IDs, as SmallMap.Get finds it)
+int vcf_info_upload(elp_ctx* c, SitesScratch& X, const VcfHeader& h, VcfInfoTab* T) {
+    std::vector<uint8_t> names, type; std::vector<uint32_t> off(1, 0); std::vector<int32_t> num;
+    std::vector<std::string> seen;
+    for (const VcfInfo& fi : h.infos) {
+        if (std::find(seen.begin(), seen.end(), fi.id) != seen.end()) continue;
+        seen.push_back(fi.id);
+        names.insert(names.end(), fi.id.begin(), fi.id.end()); off.push_back((uint32_t)names.size()); type.push_back(fi.type); num.push_back(fi.number);
+    }
+    TRY(grow(c, X.inames, names.size() + 1, 0)); TRY(grow(c, X.ioff, off.size(), 0)); TRY(grow(c, X.itype, type.size() + 1, 0)); TRY(grow(c, X.inum, num.size() + 1, 0));
+    if (!names.empty()) CUDA_TRY(c, cudaMemcpy(X.inames.p, names.data(), names.size(), cudaMemcpyHostToDevice));
+    CUDA_TRY(c, cudaMemcpy(X.ioff.p, off.data(), off.size() * 4, cudaMemcpyHostToDevice));
+    if (!type.empty()) CUDA_TRY(c, cudaMemcpy(X.itype.p, type.data(), type.size(), cudaMemcpyHostToDevice));
+    if (!num.empty()) CUDA_TRY(c, cudaMemcpy(X.inum.p, num.data(), num.size() * 4, cudaMemcpyHostToDevice));
+    *T = VcfInfoTab{X.inames.p, X.ioff.p, X.itype.p, X.inum.p, (int)type.size()};
+    return E_OK;
+}
+
+// plain VCF text after the header: chunk k+1 is read and uploaded while the line count of chunk k runs
+int vcf_plain(elp_ctx* c, SitesStage& S, SitesScratch& X, VcfState& St, const VcfInfoTab& info, FILE* f, int file, const char* path, uint64_t* total) {
+    FileStage& V = S.v;
+    const uint64_t chunk = V.chunk;
+    auto fill = [&](int b, uint64_t* got, bool* last) -> int {
+        TRY(stage_wait_host(c, V, b));
+        *got = fread(V.h[b].p, 1, chunk, f);
+        if (*got < chunk && ferror(f)) return read_fail(c, path);
+        *last = *got < chunk;
+        return stage_upload(c, V, b, *got, VCF_FRONT);
+    };
+    int b = 0; uint64_t got = 0; bool last = false;
+    TRY(fill(b, &got, &last));
+    for (;;) {
+        uint64_t got2 = 0; bool last2 = true;
+        CUDA_TRY(c, cudaStreamWaitEvent(c->stream, V.up[b], 0));
+        if (!got) CUDA_TRY(c, cudaMemsetAsync(V.d[b].p + VCF_FRONT, 0, SAM_CHUNK, c->stream));
+        TRY(vcf_chunk(c, S, X, St, info, V.d[b].p, 0, got, last, file, path, V.used[b ^ 1], total, [&]() { return last ? E_OK : fill(b ^ 1, &got2, &last2); }));
+        if (last) break;
+        b ^= 1; got = got2; last = last2;   // (vcf_chunk of the next chunk records used[b ^ 1] behind its copy of the carried line)
+    }
+    return E_OK;
+}
+
+// BGZF VCF from file offset `at` (a block start), the first `skip` inflated bytes being header: the whole blocks of each chunk inflated
+// on the device, an incomplete last block carried to the next chunk on the host (as reference_load.cu reads BGZF FASTA)
+int vcf_bgzf(elp_ctx* c, SitesStage& S, SitesScratch& X, VcfState& St, const VcfInfoTab& info, FILE* f, int file, const char* path, uint64_t at, uint64_t skip, uint64_t* total) {
+    FileStage& V = S.v;
+    const uint64_t chunk = V.chunk;
+    std::vector<uint8_t> cz;
+    std::vector<BgzfBlock> blocks;
+    bool eof_block = false;
+    int b = 0;
+    for (;;) {
+        uint8_t* h = V.h[0].p;
+        const uint64_t nc = cz.size();
+        if (nc) memcpy(h, cz.data(), nc);
+        const size_t got = fread(h + nc, 1, chunk, f);
+        if (got < chunk && ferror(f)) return read_fail(c, path);
+        const bool last = got < chunk;
+        const uint64_t n = nc + got;
+        uint64_t tot = 0, used = 0;
+        blocks.clear();
+        if (scan_blocks(h, n, blocks, &tot, &used)) {
+            const uint64_t bad = blocks.empty() ? 0 : blocks.back().cdata_off + blocks.back().cdata_len + BGZF_TRL;
+            return c->fail(E_BGZF, "elp_load_known_sites: %s, file offset %llu: malformed BGZF block header (gzip magic, FEXTRA, BC subfield, block size or ISIZE)", path,
+                           (unsigned long long)(at + bad));
+        }
+        if (last && used < n)
+            return c->fail(E_BGZF, "elp_load_known_sites: %s, file offset %llu: the file ends inside a BGZF block (%llu bytes left)", path, (unsigned long long)(at + used),
+                           (unsigned long long)(n - used));
+        if (!blocks.empty()) {
+            const BgzfBlock& lb = blocks.back();
+            eof_block = lb.cdata_len == 2 && h[lb.cdata_off] == 3 && h[lb.cdata_off + 1] == 0 && lb.crc == 0 && lb.isize == 0;   // bgzf-files.go:111-115
+        }
+        if (last && !eof_block) return c->fail(E_BGZF, "elp_load_known_sites: %s, file offset %llu: invalid BGZF file: does not end in proper EOF marker", path, (unsigned long long)(at + used));
+        if (!blocks.empty() || last) {
+            TRY(grow(c, S.tb[b], VCF_FRONT + stage_padded(tot), 0));
+            if (!blocks.empty()) {
+                char who[1200];
+                snprintf(who, sizeof who, "elp_load_known_sites: %s, BGZF blocks from file offset %llu", path, (unsigned long long)at);
+                TRY(bgzf_inflate_run(c, who, h, used, blocks, tot, S.tb[b].p + VCF_FRONT));
+            }
+            CUDA_TRY(c, cudaMemsetAsync(S.tb[b].p + VCF_FRONT + tot, 0, stage_padded(tot) - tot, c->stream));
+            TRY(vcf_chunk(c, S, X, St, info, S.tb[b].p, std::min(skip, tot), tot, last, file, path, nullptr, total, []() { return E_OK; }));
+            skip = 0;
+            b ^= 1;
+        }
+        cz.assign(h + used, h + n);
+        at += used;
+        if (last) return E_OK;
+    }
+}
+
+// one VCF file: the header on the host, then every data line through the device, appended behind *total
+int load_vcf(elp_ctx* c, SitesStage& S, SitesScratch& X, int file, const char* path, FILE* f, bool bgzf, uint64_t* total) {
+    const uint64_t want = c->sites_chunk ? c->sites_chunk : SITES_CHUNK_DEFAULT;
+    TRY(stage_init(c, S.v, want, want + BGZF_MAX_BLOCK, VCF_FRONT + stage_padded(want), "elp_load_known_sites"));
+    VcfHeader h;
+    uint64_t bad_line = 0; const char* why = nullptr;
+    uint64_t at = 0, skip = 0;
+    if (bgzf) {
+        BgzfHead src{c, f, path};
+        const int rc = vcf_header(src, &h, &bad_line, &why);
+        if (rc == E_VCF) return vcf_fail(c, path, file, bad_line, why);
+        TRY(rc);
+        at = src.cz_at;   // the data start in the block that holds byte h.bytes, or in the first block after it (an empty one included)
+        for (const BgzfBlock& b : src.blocks)
+            if (b.out_off + b.isize > h.bytes || (b.isize == 0 && b.out_off >= h.bytes)) { at = b.in_off; skip = h.bytes - b.out_off; break; }
+    } else {
+        PlainHead src{c, f, path};
+        const int rc = vcf_header(src, &h, &bad_line, &why);
+        if (rc == E_VCF) return vcf_fail(c, path, file, bad_line, why);
+        TRY(rc);
+        at = h.bytes;
+    }
+    if (fseeko(f, (off_t)at, SEEK_SET) != 0) return read_fail(c, path);
+    VcfInfoTab info{};
+    TRY(vcf_info_upload(c, X, h, &info));
+    VcfState St;
+    St.line0 = h.lines + 1;
+    return bgzf ? vcf_bgzf(c, S, X, St, info, f, file, path, at, skip, total) : vcf_plain(c, S, X, St, info, f, file, path, total);
+}
+
+// one file: the header on the host, then every line through the device, appended behind *total.  The format comes from the content:
+// the .elsites header, a first byte 0x1f (BGZF VCF, as vcf.Open sniffs it, vcf-files.go:1285-1312), or "##fileformat=VCFv4." (plain VCF)
 int load_file(elp_ctx* c, SitesStage& S, SitesScratch& X, int file, const char* path, uint64_t* total) {
     FILE* f = fopen(path, "rb");
     if (!f) return c->fail(E_INVAL, "elp_load_known_sites: cannot open %s: %s", path, strerror(errno));
@@ -323,7 +623,11 @@ int load_file(elp_ctx* c, SitesStage& S, SitesScratch& X, int file, const char* 
     char hd[SITES_HEADER_LEN];   // bufio.Reader.ReadString('\n') must return exactly ElsitesHeader (intervals.go:204-210)
     const size_t got = fread(hd, 1, SITES_HEADER_LEN, f);
     if (got < SITES_HEADER_LEN && ferror(f)) return c->fail(E_INVAL, "elp_load_known_sites: cannot read %s: %s", path, strerror(errno));
-    if (got < SITES_HEADER_LEN || memcmp(hd, SITES_HEADER, SITES_HEADER_LEN) != 0)
+    const bool elsites = got == SITES_HEADER_LEN && memcmp(hd, SITES_HEADER, SITES_HEADER_LEN) == 0;
+    if (!elsites && got >= 1 && (uint8_t)hd[0] == 0x1f) return fseeko(f, 0, SEEK_SET) ? read_fail(c, path) : load_vcf(c, S, X, file, path, f, true, total);
+    if (!elsites && got >= VCF_PREFIX_LEN && memcmp(hd, VCF_PREFIX, VCF_PREFIX_LEN) == 0)
+        return fseeko(f, 0, SEEK_SET) ? read_fail(c, path) : load_vcf(c, S, X, file, path, f, false, total);
+    if (!elsites)
         return c->fail(E_SITES, "elp_load_known_sites: %s (file %d), line 0 (0-based, header = line 0): not a .elsites file - the first line is not \"# elsites format version 1.0\"", path, file);
     std::vector<uint8_t> carry;
     uint64_t line0 = 1;
@@ -399,7 +703,7 @@ extern "C" int elp_load_known_sites(elp_ctx* c, const char* const* paths, int32_
     if (n_paths) {
         TRY(sites_stage_init(c));
         SitesStage& S = *c->sites;
-        struct Drain { cudaStream_t s; ~Drain() { cudaStreamSynchronize(s); } } drain{S.f.copy};   // no upload outlives the call
+        struct Drain { SitesStage& S; ~Drain() { cudaStreamSynchronize(S.f.copy); if (S.v.copy) cudaStreamSynchronize(S.v.copy); } } drain{S};   // no upload outlives the call
         SitesScratch X;
         CUDA_TRY(c, cudaMemsetAsync(S.d_small.p, 0xff, 8, c->stream));
         CUDA_TRY(c, cudaMemsetAsync(S.d_small.p + 1, 0, 8, c->stream));

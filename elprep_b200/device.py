@@ -83,8 +83,8 @@ class Context:
         self._ck(self.L.elp_set_known_sites(self.h, contig, _vp(se) if se.size else None, se.size // 2, int(already_flat)))
 
     def load_known_sites(self, paths):
-        """--known-sites: .elsites files parsed, sorted and flattened on the device into every contig's list -> lines on chromosomes
-        that are no @SQ SN"""
+        """--known-sites: .elsites and VCF files (plain or BGZF, told apart by content) parsed, sorted and flattened on the device into
+        every contig's list -> lines on chromosomes that are no @SQ SN (VCF: data lines)"""
         arr = _cstrs([os.fspath(p) for p in paths])
         nu = C.c_uint64()
         self._ck(self.L.elp_load_known_sites(self.h, arr, len(paths), C.byref(nu)))

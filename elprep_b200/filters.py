@@ -332,7 +332,7 @@ class BaseRecalibrator:
     """filters.BaseRecalibrator (filters/bqsr.go:417-443): known sites + reference."""
 
     def __init__(self, known_sites, reference):
-        self.known_sites, self.reference = known_sites, reference   # per contig: (k,2) int32 intervals, or .elsites paths; uint8 bases, or a path
+        self.known_sites, self.reference = known_sites, reference   # per contig: (k,2) int32 intervals, or .elsites / VCF paths; uint8 bases, or a path
 
     def _sites_are_files(self):
         ks = self.known_sites
@@ -360,8 +360,8 @@ class BaseRecalibrator:
 
 def NewBaseRecalibrator(knownSites, referenceFasta):
     """filters.NewBaseRecalibrator (filters/bqsr.go:424-443). knownSites: per-contig interval arrays (sorted+flattened
-    inside, as intervals.ParallelSortByStart/ParallelFlatten do), or a list of .elsites paths like the reference's []string
-    (loaded on the device by Context.load_known_sites); referenceFasta: per-contig base arrays (fasta.Seq), or the path of an .elfasta or
+    inside, as intervals.ParallelSortByStart/ParallelFlatten do), or a list of .elsites or VCF (plain or BGZF) paths like the
+    reference's []string (loaded on the device by Context.load_known_sites); referenceFasta: per-contig base arrays (fasta.Seq), or the path of an .elfasta or
     FASTA file (plain or BGZF) like the reference's --reference (loaded on the device by Context.load_reference)."""
     return BaseRecalibrator(knownSites, referenceFasta)
 

@@ -386,8 +386,9 @@ func (d *DeviceSam) SetKnownSites(contig int, startEnd []int32) {
 	check(d.ctx, C.elp_set_known_sites(d.ctx, C.int32_t(contig), p, C.uint64_t(len(startEnd)/2), 0))
 }
 
-// LoadKnownSites: --known-sites as the reference takes it (cmd/filter.go:459,530-538), a list of .elsites files, parsed, sorted and
-// flattened on the device into every contig's list.  Returns the lines whose chromosome is no @SQ SN.
+// LoadKnownSites: --known-sites as the reference takes it (cmd/filter.go:459,530-538), a list of .elsites files or VCF files (plain or
+// BGZF, told apart by content, each read as vcf-to-elsites would convert it), parsed, sorted and flattened on the device into every
+// contig's list.  Returns the lines whose chromosome is no @SQ SN.
 func (d *DeviceSam) LoadKnownSites(paths []string) uint64 {
 	cs := make([]*C.char, len(paths)+1)
 	for i, p := range paths {

@@ -40,6 +40,7 @@ extern "C" {
 #define ELP_ESAM (-20)       /* malformed SAM alignment line; elp_last_error names the line (0-based, within the call) and the field */
 #define ELP_ESITES (-21)     /* malformed .elsites file; elp_last_error names the file (index in paths), the line (0-based, header = line 0) and the reason */
 #define ELP_EFASTA (-22)     /* malformed reference file: elp_last_error names the file, the line (FASTA, 1-based) or byte offset (.elfasta), and the reason */
+#define ELP_EVCF (-23)       /* malformed VCF known-sites file: elp_last_error names the file (index in paths), the line (1-based, header lines counted) and the reason */
 
 /* sam.SortingOrder (sam/sam-types.go:40-58) */
 #define ELP_SO_KEEP 0
@@ -116,7 +117,7 @@ int elp_reset(elp_ctx *ctx);
  * of NewBaseRecalibrator (filters/bqsr.go:424-443). start/end pairs; flattened inside unless already_flat. ---- */
 int elp_set_reference(elp_ctx *ctx, int32_t contig, const uint8_t *bases, uint64_t n);
 int elp_set_known_sites(elp_ctx *ctx, int32_t contig, const int32_t *start_end_pairs, uint64_t n_intervals, int already_flat);
-/* --known-sites a.elsites,b.elsites (cmd/filter.go:459,530-538): NewBaseRecalibrator's loop over the files (filters/bqsr.go:424-443)
+/* --known-sites a.elsites,b.vcf.gz (cmd/filter.go:459,530-538): NewBaseRecalibrator's loop over the files (filters/bqsr.go:424-443)
  * with intervals.FromElsitesFile (intervals/intervals.go:199-254), then ParallelSortByStart + ParallelFlatten per contig, all on the
  * device.  Replaces the known-sites list of EVERY contig (a contig without sites gets an empty list); n_paths == 0 clears them all.
  *  - Header: each file starts with exactly "# elsites format version 1.0\n" (ReadString('\n'), intervals.go:204-210); a "\r\n" header,
@@ -135,7 +136,22 @@ int elp_set_known_sites(elp_ctx *ctx, int32_t contig, const int32_t *start_end_p
  *    serial Flatten (also where ParallelFlatten would panic, see DESIGN.md).
  *  - A missing or unreadable file is ELP_EINVAL (the message names the path); 2^30 or more intervals in total are ELP_ELIMIT.
  *  - Atomic: on any error the previous table is unchanged.  The table survives elp_reset; elp_set_known_sites afterwards replaces one
- *    contig's list, and the two calls mix in either order. */
+ *    contig's list, and the two calls mix in either order.
+ *  - VCF files: the format of each file comes from its content.  The exact .elsites header is an .elsites file; a first byte 0x1f is a
+ *    BGZF VCF (vcf.Open, vcf/vcf-files.go:1285-1312; the BGZF rules of elp_append_bgzf apply, a plain gzip file is ELP_EBGZF); text that
+ *    starts with "##fileformat=VCFv4." is a plain VCF; anything else is ELP_ESITES at line 0.  A list may mix both kinds.  A VCF gives
+ *    the table that `elprep vcf-to-elsites` on it, followed by loading the .elsites it writes in the same position of the list, gives:
+ *    intervals.FromVcfFile (intervals/intervals.go:306-338) with ParseHeader, NewVariantParser and ParseVariant(NSamples = 0)
+ *    (vcf-files.go:73-305,600-782).  The header: the first line starts with "##fileformat=VCFv4."; "##key=value" lines follow (a line
+ *    without '=', a second fileformat, and every panic of ParseFormatInformation / ParseMetaInformation are refused; an INFO Flag with
+ *    Number != 0 and any FORMAT Flag are refused even when unused); then one '#' column line.  Data lines split as .elsites lines do
+ *    (65536 bytes or more is refused).  CHROM, POS, REF, QUAL and FILTER must be followed by a tab unless missing ('.' at the end of
+ *    the line or before a tab, or the line already ended); ID and ALT are lists followed by a tab; POS is strconv.ParseInt(s, 10, 32)
+ *    (-1 when missing); QUAL must pass strconv.ParseFloat(s, 64), overflow to +-Inf included; FILTER "PASS;..." is refused.  INFO keys
+ *    run up to ' ', ':' or a tab; a key equal to a declared ID goes through that ID's parser (Integer and Float always fail there), and
+ *    a key equal to END refuses the line.  Everything after INFO is ignored.  The interval is [POS, POS - 1 + len(REF)] in wrapping
+ *    int32; a missing REF counts as "."; an empty CHROM is refused.  *n_unmatched counts VCF data lines on no @SQ SN.  A refusal is
+ *    ELP_EVCF naming the file, the 1-based line (header lines counted) and the reason; the smallest (file, line) is reported. */
 int elp_load_known_sites(elp_ctx *ctx, const char *const *paths, int32_t n_paths, uint64_t *n_unmatched);
 /* one contig's known sites as the gather uses them: writes up to cap (start, end) pairs and returns the number of pairs (-1 on error);
  * start_end_pairs may be NULL to ask for the count */

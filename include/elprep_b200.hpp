@@ -155,8 +155,8 @@ class DeviceSam {
 
     void SetReference(int contig, const std::string& bases) { check(elp_set_reference(ctx_, contig, reinterpret_cast<const uint8_t*>(bases.data()), bases.size())); }
     void SetKnownSites(int contig, const std::vector<int32_t>& startEnd) { check(elp_set_known_sites(ctx_, contig, startEnd.empty() ? nullptr : startEnd.data(), startEnd.size() / 2, 0)); }
-    // --known-sites a.elsites,b.elsites: every file parsed, sorted and flattened on the device into every contig's list; returns the
-    // lines whose chromosome is no @SQ SN
+    // --known-sites a.elsites,b.vcf.gz: every file (.elsites, or VCF plain or BGZF, told apart by content) parsed, sorted and flattened
+    // on the device into every contig's list; returns the lines whose chromosome is no @SQ SN
     uint64_t LoadKnownSites(const std::vector<std::string>& paths) {
         std::vector<const char*> p;
         for (const auto& s : paths) p.push_back(s.c_str());
