@@ -11,7 +11,7 @@
 // Offsets come from device prefix sums of the lengths.  The raw records stay in a device arena so that the write phase can
 // hand them back (elp_fetch_bam): output order, MAPQ, FLAG and QUAL patched, everything else -- names, CIGAR, tags -- untouched
 // (the counterpart of formatting every *sam.Alignment again, sam/bam-files.go:635-735).  Not handled (error return): the CG:B long-CIGAR convention (:376-392),
-// an RG:Z value that is not an @RG ID of the header.
+// an RG:Z value that is not an @RG ID of the header (unless --replace-read-group puts every read in the one @RG, elp_set_replace_read_group).
 #include <algorithm>
 #include "ctx.h"
 #include "regions.cuh"
@@ -28,6 +28,7 @@ struct BamArgs {
     const uint8_t* raw; const uint64_t* start; uint64_t n_bytes;   // start[i]: offset of record i's block_size field
     int chained;                          // start[] has n + 1 entries and start[i + 1] must be the end of record i (no filter ran)
     int clear_dup;                        // ClearDuplicateFlag: 0x400 cleared in the FLAG column (the stored record keeps its bytes)
+    int rg_replace;                       // --replace-read-group: every read gets read group 0, whatever RG field its record has
     int32_t *refid, *pos, *nref, *pnext, *tlen, *rg; uint16_t* flag; uint8_t* mapq; uint8_t* optf;
     uint32_t *len_qname, *len_cigar, *len_seq, *len_qual;   // [n] lengths, scanned afterwards
     const uint8_t* rg_names; const uint32_t* rg_name_off; int n_rg; int n_contigs;
@@ -118,9 +119,9 @@ __global__ void __launch_bounds__(256) bam_fixed_kernel(BamArgs A) {
     A.nref[k] = nref < 0 ? -1 : nref; A.pnext[k] = pnext + 1; A.tlen[k] = tlen;
     int32_t rg; uint8_t optf;
     const uint32_t bad = check_record(r, rec_len, A.n_contigs, RgNames{A.rg_names, A.rg_name_off, A.n_rg}, &rg, &optf);
-    if (rg == -2) atomicOr(A.err, DERR_BAM_RG);
+    if (A.rg_replace) rg = 0;                  // (the record's RG fields are rewritten at egress; a value that is no @RG ID is not refused)
+    else if (rg == -2) { atomicOr(A.err, DERR_BAM_RG); rg = -1; }
     if (bad) atomicOr(A.err, bad == 2 ? DERR_BAM_CG : DERR_BAM);
-    if (rg == -2) rg = -1;
     A.rg[k] = rg; A.optf[k] = optf;
     A.len_qname[i] = bad ? 0 : l_name - 1; A.len_cigar[i] = bad ? 0 : n_cig;
     A.len_seq[i] = bad ? 0 : (uint32_t)((l_seq + 1) >> 1); A.len_qual[i] = bad ? 0 : (uint32_t)l_seq;
@@ -306,27 +307,25 @@ __device__ __forceinline__ uint64_t tags_start(const uint8_t* r) {
     return BAM_FIXED + (uint64_t)r[12] + 4ull * rd16(r + 16) + ((l_seq + 1) >> 1) + l_seq;
 }
 
-// RemoveOptionalFields / KeepOptionalFields (simple-filters.go:235-288) on BAM records, one warp per output record.
-// measure: the record's length without its dropped fields
+// RemoveOptionalFields / KeepOptionalFields (simple-filters.go:235-288) on BAM records, after SetRG when --replace-read-group is on
+// (tagwalk::out_fields), one warp per output record; drop may be null (no field filter: only the RG field changes).
+// measure: the record's length with the fields it is written with
 __global__ void __launch_bounds__(256) bam_out_fields_measure_kernel(uint64_t n, uint64_t first, const uint32_t* __restrict__ sel, const uint32_t* __restrict__ perm,
                                                                      const uint64_t* __restrict__ all_start, const uint8_t* __restrict__ all, const uint32_t* __restrict__ drop,
-                                                                     uint32_t* __restrict__ len) {
+                                                                     tagwalk::RgSet g, uint32_t* __restrict__ len) {
     const uint64_t kk = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (kk >= n) return;
     const uint8_t* r = all + all_start[perm[out_pos(sel, first, kk)]];
     const uint64_t rec = (uint64_t)rd32(r) + 4;
-    uint64_t t = tags_start(r), x = t;
-    while (t + 3 <= rec) {
-        const uint64_t fe = tagwalk::field_end(r, t, rec);
-        if (!tagwalk::dropped(drop, r[t], r[t + 1])) x += fe - t;
-        t = fe;
-    }
+    const uint64_t t0 = tags_start(r);
+    uint64_t x = t0;
+    tagwalk::out_fields(r, t0, rec, drop, g, [&](uint64_t t, uint64_t fe, bool repl) { x += repl ? tagwalk::rg_field_bytes(g) : fe - t; });
     if ((threadIdx.x & 31) == 0) len[kk] = (uint32_t)x;
 }
-// emit: the fixed part and the variable fields with block_size, MAPQ, FLAG and QUAL patched, then the kept fields in their order
+// emit: the fixed part and the variable fields with block_size, MAPQ, FLAG and QUAL patched, then the fields in their order
 __global__ void __launch_bounds__(256) bam_out_fields_emit_kernel(uint64_t n, uint64_t first, const uint32_t* __restrict__ sel, const uint32_t* __restrict__ perm,
                                                                   const uint64_t* __restrict__ all_start, const uint8_t* __restrict__ all, const uint32_t* __restrict__ drop,
-                                                                  const uint64_t* __restrict__ out_off, uint8_t* __restrict__ out,
+                                                                  tagwalk::RgSet g, const uint64_t* __restrict__ out_off, uint8_t* __restrict__ out,
                                                                   const uint16_t* __restrict__ s_flag, const uint8_t* __restrict__ s_mapq, const uint64_t* __restrict__ s_out_off, const uint8_t* __restrict__ qual_out) {
     const unsigned lane = threadIdx.x & 31;
     const uint64_t kk = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -349,15 +348,12 @@ __global__ void __launch_bounds__(256) bam_out_fields_emit_kernel(uint64_t n, ui
         o[t] = v;
     }
     if (lane == 13) o[13] = mq;                  // (as in bam_out_copy_kernel)
-    uint64_t t = t0, x = t0;
-    while (t + 3 <= rec) {
-        const uint64_t fe = tagwalk::field_end(r, t, rec);
-        if (!tagwalk::dropped(drop, r[t], r[t + 1])) {
-            for (uint64_t j = lane; j < fe - t; j += 32) o[x + j] = r[t + j];
-            x += fe - t;
-        }
-        t = fe;
-    }
+    uint64_t x = t0;
+    tagwalk::out_fields(r, t0, rec, drop, g, [&](uint64_t t, uint64_t fe, bool repl) {
+        if (repl) { tagwalk::rg_field_write(o + x, g); x += tagwalk::rg_field_bytes(g); return; }
+        for (uint64_t j = lane; j < fe - t; j += 32) o[x + j] = r[t + j];
+        x += fe - t;
+    });
 }
 
 }  // namespace
@@ -418,6 +414,18 @@ extern "C" int elp_append_bam(elp_ctx* c, const uint8_t* records, uint64_t n_byt
     return bam_ingest_core(c, n_bytes, nrec);
 }
 
+// @RG ID strings for the RG:Z match at ingest and the RG:Z value of --replace-read-group at egress, uploaded once per context
+int rg_names_upload(elp_ctx* c) {
+    if (c->d_rg_names.p || !c->n_rg) return E_OK;
+    std::vector<uint8_t> names; std::vector<uint32_t> off(1, 0);
+    for (auto& id : c->rg_ids) { names.insert(names.end(), id.begin(), id.end()); off.push_back((uint32_t)names.size()); }
+    CUDA_TRY(c, c->d_rg_names.fit(std::max<size_t>(names.size(), 1)));
+    CUDA_TRY(c, c->d_rg_name_off.fit(off.size()));
+    CUDA_TRY(c, cudaMemcpy(c->d_rg_names.p, names.data(), names.size(), cudaMemcpyHostToDevice));
+    CUDA_TRY(c, cudaMemcpy(c->d_rg_name_off.p, off.data(), off.size() * 4, cudaMemcpyHostToDevice));
+    return E_OK;
+}
+
 // The device-resident part of elp_append_bam, shared with elp_append_sam: nrec records (n_bytes in all) already sit in bam_raw, and
 // bam_off[0..nrec] holds their chained offsets (bam_off[nrec] == n_bytes).  The caller holds append_mu and has checked the phase
 // and the 2^32 read limit.  From here on: ingest filters, fixed fields and RG:Z, segmented copies, QUAL presence, the bam_all arena.
@@ -427,15 +435,7 @@ int bam_ingest_core(elp_ctx* c, uint64_t n_bytes, uint64_t nrec) {
     cudaStream_t s = c->stream;
     TRY(grow(c, c->bam_start, nrec + 2, 0));
     const uint64_t* d_start = c->bam_off.p;                   // without filters: record i is read n0 + i
-    // @RG ID strings for the RG:Z match
-    if (!c->d_rg_names.p && c->n_rg) {
-        std::vector<uint8_t> names; std::vector<uint32_t> off(1, 0);
-        for (auto& id : c->rg_ids) { names.insert(names.end(), id.begin(), id.end()); off.push_back((uint32_t)names.size()); }
-        CUDA_TRY(c, c->d_rg_names.fit(std::max<size_t>(names.size(), 1)));
-        CUDA_TRY(c, c->d_rg_name_off.fit(off.size()));
-        CUDA_TRY(c, cudaMemcpy(c->d_rg_names.p, names.data(), names.size(), cudaMemcpyHostToDevice));
-        CUDA_TRY(c, cudaMemcpy(c->d_rg_name_off.p, off.data(), off.size() * 4, cudaMemcpyHostToDevice));
-    }
+    TRY(rg_names_upload(c));
     if (c->filter_mask || c->filter_min_mapq > 0) {
         TRY(grow(c, c->scan_tmp, nrec + 8, 0)); TRY(grow(c, c->off_stage, nrec + 2, 0));
         c->begin("bam_keep", (double)nrec * 48);
@@ -460,7 +460,7 @@ int bam_ingest_core(elp_ctx* c, uint64_t n_bytes, uint64_t nrec) {
     TRY(grow(c, c->qname_off, n1 + 2, n0 + 1)); TRY(grow(c, c->cigar_off, n1 + 2, n0 + 1)); TRY(grow(c, c->qual_off, n1 + 2, n0 + 1)); TRY(grow(c, c->seq_off, n1 + 2, n0 + 1));
     TRY(grow(c, c->scan_tmp, 4 * (bn + 4) + 8, 0));   // (the keep flags above are dead by now)
     BamArgs A{};
-    A.n = bn; A.n0 = n0; A.raw = c->bam_raw.p; A.start = d_start; A.n_bytes = n_bytes; A.chained = d_start == c->bam_off.p; A.clear_dup = c->clear_dup;
+    A.n = bn; A.n0 = n0; A.raw = c->bam_raw.p; A.start = d_start; A.n_bytes = n_bytes; A.chained = d_start == c->bam_off.p; A.clear_dup = c->clear_dup; A.rg_replace = c->rg_replace;
     A.refid = c->refid.p; A.pos = c->pos.p; A.nref = c->nref.p; A.pnext = c->pnext.p; A.tlen = c->tlen.p; A.rg = c->rg.p; A.flag = c->flag.p; A.mapq = c->mapq.p; A.optf = c->optf.p;
     A.len_qname = c->scan_tmp.p; A.len_cigar = c->scan_tmp.p + (bn + 4); A.len_seq = c->scan_tmp.p + 2 * (bn + 4); A.len_qual = c->scan_tmp.p + 3 * (bn + 4);
     A.rg_names = c->d_rg_names.p; A.rg_name_off = c->d_rg_name_off.p; A.n_rg = c->n_rg; A.n_contigs = c->n_contigs; A.err = c->d_err.p;
@@ -532,7 +532,12 @@ int out_select(elp_ctx* c, const uint32_t** sel, uint64_t* n_out) {
     return E_OK;
 }
 
-// record lengths of the call (without dropped fields when a field filter is set) scanned into off_stage[0..n], *total bytes
+// the RG:Z value the egress writes (elp_set_replace_read_group), or off
+tagwalk::RgSet rg_set(const elp_ctx* c) {
+    return c->rg_replace ? tagwalk::RgSet{c->d_rg_names.p, (uint32_t)c->rg_ids[0].size(), true} : tagwalk::RgSet{nullptr, 0, false};
+}
+
+// record lengths of the call (as the field filter and the read-group replacement write them, when set) scanned into off_stage[0..n], *total bytes
 static int bam_out_prepare(elp_ctx* c, uint64_t first, uint64_t n, uint64_t* total, const uint32_t** sel) {
     if (!c->sorted) return c->fail(E_STATE, "elp_fetch_bam before elp_sort_markdup");
     if (c->bam_reads != c->n) return c->fail(E_STATE, "elp_fetch_bam: not every read of this context came in through elp_append_bam");
@@ -543,9 +548,10 @@ static int bam_out_prepare(elp_ctx* c, uint64_t first, uint64_t n, uint64_t* tot
         return c->fail(E_INVAL, "elp_fetch_bam: range [%llu,%llu) exceeds %llu reads", (unsigned long long)first, (unsigned long long)(first + n), (unsigned long long)n_out);
     }
     TRY(grow(c, c->scan_tmp, n + 8, 0)); TRY(grow(c, c->off_stage, n + 2, 0));
-    if (c->out_fields) {
+    if (c->out_fields || c->rg_replace) {
         c->begin("bam_out_fields_measure", (double)c->n_bam * (double)n / (double)std::max<uint64_t>(c->n, 1) + 4.0 * (double)n);
-        bam_out_fields_measure_kernel<<<nblk(n * 32, 256), 256, 0, c->stream>>>(n, first, *sel, c->perm.p, c->bam_all_off.p, c->bam_all.p, c->d_out_drop.p, c->scan_tmp.p);
+        bam_out_fields_measure_kernel<<<nblk(n * 32, 256), 256, 0, c->stream>>>(n, first, *sel, c->perm.p, c->bam_all_off.p, c->bam_all.p, c->out_fields ? c->d_out_drop.p : nullptr,
+                                                                                 rg_set(c), c->scan_tmp.p);
         c->end();
     } else {
         bam_out_len_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(n, first, *sel, c->perm.p, c->bam_all_off.p, c->bam_all.p, c->scan_tmp.p); c->launches++;
@@ -559,9 +565,10 @@ static int bam_out_prepare(elp_ctx* c, uint64_t first, uint64_t n, uint64_t* tot
 
 // the records of the call (bam_out_prepare ran: off_stage holds their offsets, total their bytes) formatted at dst
 static int bam_out_format(elp_ctx* c, uint64_t first, uint64_t n, const uint32_t* sel, uint64_t total, uint8_t* dst) {
-    if (c->out_fields) {
+    if (c->out_fields || c->rg_replace) {
         c->begin("bam_out_fields_emit", (double)c->n_bam * (double)n / (double)std::max<uint64_t>(c->n, 1) + (double)total);
-        bam_out_fields_emit_kernel<<<nblk(n * 32, 256), 256, 0, c->stream>>>(n, first, sel, c->perm.p, c->bam_all_off.p, c->bam_all.p, c->d_out_drop.p, c->off_stage.p, dst,
+        bam_out_fields_emit_kernel<<<nblk(n * 32, 256), 256, 0, c->stream>>>(n, first, sel, c->perm.p, c->bam_all_off.p, c->bam_all.p, c->out_fields ? c->d_out_drop.p : nullptr,
+                                                                             rg_set(c), c->off_stage.p, dst,
                                                                              c->s_flag.p, c->s_mapq.p, c->s_out_off.p, c->qual_out_valid ? c->qual_out.p : nullptr);
     } else {
         c->begin("bam_format", 2.0 * (double)total);
@@ -653,6 +660,16 @@ extern "C" int elp_set_output_filter(elp_ctx* c, uint32_t mask, const char* cons
         CUDA_TRY(c, cudaStreamSynchronize(c->stream));   // (drop is pageable host memory)
     }
     c->out_mask = mask & ~(uint32_t)ELP_OUT_KEEP_FIELDS; c->out_fields = any; c->out_sel_valid = false;
+    return ELP_OK;
+}
+
+extern "C" int elp_set_replace_read_group(elp_ctx* c, int on) {
+    if (!c) return ELP_EINVAL;
+    cudaSetDevice(c->device);
+    if (c->n || c->sorted || c->bgzf_open) return c->fail(E_STATE, "elp_set_replace_read_group: the context holds reads (call it after elp_create or elp_reset)");
+    if (on && c->n_rg != 1) return c->fail(E_INVAL, "elp_set_replace_read_group: the context must be created with exactly one @RG, the replacement (it has %d)", c->n_rg);
+    if (on) TRY(rg_names_upload(c));
+    c->rg_replace = on != 0;
     return ELP_OK;
 }
 

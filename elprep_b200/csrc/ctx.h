@@ -186,6 +186,8 @@ struct elp_ctx {
     uint32_t out_mask = 0;                    // record bits (ELP_OUT_REMOVE_DUPLICATES, ELP_OUT_REMOVE_OPTIONAL_READS)
     DBuf<uint32_t> d_out_drop; bool out_fields = false;        // 65 536-bit tag table (bit set: the field is dropped); out_fields: some bit is set
     DBuf<uint32_t> out_sel; uint64_t n_out = 0; bool out_sel_valid = false;   // output positions of the records that pass, built on first use
+    bool rg_replace = false;                 // --replace-read-group (elp_set_replace_read_group; survives elp_reset): every read is in @RG 0 and
+                                             // the byte outputs write its RG field as RG:Z:rg_ids[0] (d_rg_names)
     RegionTable regions;                     // --filter-non-overlapping-reads: the ingest filter ELP_FILTER_TARGET_REGIONS (elp_set_target_regions)
     RegionTable bqsr_regions;                // --target-regions: elp_filter_target_regions after marking (elp_set_bqsr_target_regions); both survive elp_reset
     uint64_t n_cleaned = 0;                  // reads whose CIGAR elp_clean_sam rewrote
@@ -368,7 +370,8 @@ int spread_exchange_end(elp_ctx* c);
 int exclusive_scan_u64_from_u32(elp_ctx* c, const uint32_t* in, uint64_t* out, uint64_t n, uint64_t base);   // out[n+1], out[0] = base
 int qual_presence_update(elp_ctx* c, uint64_t first_byte, uint64_t n_bytes);   // api.cu: called by both ingest paths
 int bam_ingest_core(elp_ctx* c, uint64_t n_bytes, uint64_t nrec);   // bam_ingest.cu: records staged in bam_raw / bam_off -> reads (elp_append_bam, elp_append_sam)
-int out_select(elp_ctx* c, const uint32_t** sel, uint64_t* n_out);   // bam_ingest.cu: the record filters' selection (sel null and n_out = n_sorted without record bits)
+int out_select(elp_ctx* c, const uint32_t** sel, uint64_t* n_out);
+int rg_names_upload(elp_ctx* c);   // bam_ingest.cu: @RG IDs -> d_rg_names / d_rg_name_off, once per context   // bam_ingest.cu: the record filters' selection (sel null and n_out = n_sorted without record bits)
 int region_set(elp_ctx* c, RegionTable& t, const char* who, int32_t contig, const int32_t* se, uint64_t n_intervals, int already_flat);   // bam_ingest.cu
 int build_output_columns(elp_ctx* c, const uint32_t* perm, uint64_t n_out, bool refilter);   // coordsort.cu: s_* columns and s_out_off of perm[0, n_out)
 int phase_target_filter(elp_ctx* c, uint64_t* n_removed);   // target_regions.cu

@@ -36,6 +36,7 @@ struct FmtArgs {
     uint64_t n, first;                                                    // lines [first, first + n) of the output order (of sel when sel is set)
     const uint32_t* sel;                                                  // output positions of the records the record filters keep, or null
     const uint32_t* drop;                                                 // 65 536-bit tag table of the field filter, or null
+    tagwalk::RgSet rg;                                                    // --replace-read-group: the RG:Z value every line carries
     const uint32_t* perm; const uint64_t* all_start; const uint8_t* all;
     const uint16_t* flag; const uint8_t* mapq;                            // in output order: FLAG after marking, MAPQ after elp_clean_sam
     const uint64_t* qoff; const uint8_t* qual;                            // qual: recalibrated QUAL in output order, or null (stored QUAL)
@@ -180,10 +181,17 @@ template <int M> __device__ void format_line(const FmtArgs& A, uint64_t kk, cons
     uint64_t t = 36 + l_name + 4ull * ncig + ls + L;
     const uint64_t fb = A.fbase ? A.fbase[kk] : 0;                        // (no float values in the lines: no slots)
     uint64_t fj = 0;                                                      // float values of this line so far
-    while (t + 3 <= rec) {
+    // (out_fields: the fields after SetRG and the field filter; a dropped field has no text and no float slot, nor has the replaced RG field)
+    tagwalk::out_fields(r, t, rec, A.drop, A.rg, [&](uint64_t t, uint64_t fe, bool repl) {
+        if (repl) {                                                       // "\tRG:Z:" id
+            if (W) {
+                for (uint32_t j = lane; j < 6; j += 32) o[x + j] = (uint8_t)"\tRG:Z:"[j];
+                for (uint32_t j = lane; j < A.rg.n; j += 32) o[x + 6 + j] = A.rg.id[j];
+            }
+            x += 6 + A.rg.n;
+            return;
+        }
         const uint8_t t0 = r[t], t1 = r[t + 1], ty = r[t + 2];
-        const uint64_t fe = tagwalk::field_end(r, t, rec);
-        if (A.drop && tagwalk::dropped(A.drop, t0, t1)) { t = fe; continue; }   // no text, no float slot
         t += 3;
         const bool integer = ty == 'c' || ty == 'C' || ty == 's' || ty == 'S' || ty == 'i' || ty == 'I';
         if (W && lane == 0) { o[x] = '\t'; o[x + 1] = t0; o[x + 2] = t1; o[x + 3] = ':'; o[x + 4] = integer ? 'i' : ty; o[x + 5] = ':'; }
@@ -244,9 +252,8 @@ template <int M> __device__ void format_line(const FmtArgs& A, uint64_t kk, cons
                 x += tot;
             }
             if (sub == 'f') fj += cnt;
-            t = fe;
-        } else break;                                                     // (the ingest accepted no other type)
-    }
+        }                                                                 // (the ingest accepted no other type: field_end ended the walk)
+    });
     x += 1;
     if (W && lane == 0) o[x - 1] = '\n';
     if (M == FM_MEASURE && lane == 0) {
@@ -320,7 +327,7 @@ int sam_out_prepare(elp_ctx* c, uint64_t first, uint64_t n, const uint32_t* sel,
     cudaStream_t s = c->stream;
     TRY(grow(c, c->scan_tmp, n + 8, 0)); TRY(grow(c, c->off_stage, n + 2, 0)); TRY(grow(c, S.nf, n + 8, 0));
     FmtArgs A{};
-    A.n = n; A.first = first; A.sel = sel; A.drop = c->out_fields ? c->d_out_drop.p : nullptr; A.perm = c->perm.p; A.all_start = c->bam_all_off.p; A.all = c->bam_all.p;
+    A.n = n; A.first = first; A.sel = sel; A.drop = c->out_fields ? c->d_out_drop.p : nullptr; A.rg = rg_set(c); A.perm = c->perm.p; A.all_start = c->bam_all_off.p; A.all = c->bam_all.p;
     A.flag = c->s_flag.p; A.mapq = c->s_mapq.p; A.qoff = c->s_out_off.p; A.qual = c->qual_out_valid ? c->qual_out.p : nullptr;
     A.names = S.d_names.p; A.name_off = S.d_name_off.p; A.canon = S.d_canon.p; A.n_contigs = c->n_contigs;
     A.len = c->scan_tmp.p; A.nf = S.nf.p; A.small = S.d_small.p;

@@ -1,6 +1,6 @@
 // tagwalk.cuh -- the one statement of the BAM optional-field grammar (sam/bam-files.go:369-397) for the write-phase kernels: where a field
-// ends, and whether the output field filter (elp_set_output_filter) drops it.  format_line (sam_format.cu) and the BAM field-filter
-// kernels (bam_ingest.cu) walk a record's fields with field_end; the ingest validated every record, so no bound is checked here beyond
+// ends, whether the output field filter (elp_set_output_filter) drops it, and where the RG field of --replace-read-group goes.  format_line
+// (sam_format.cu) and the BAM field-filter kernels (bam_ingest.cu) walk a record's fields with out_fields; the ingest validated every record, so no bound is checked here beyond
 // the record's end.  field_end is warp-collective (Z / H search their NUL with a ballot): every lane of the warp must call it with the
 // same arguments.
 #pragma once
@@ -44,4 +44,35 @@ __device__ __forceinline__ bool dropped(const uint32_t* __restrict__ tab, uint8_
     return (__ldg(tab + (i >> 5)) >> (i & 31)) & 1u;
 }
 
+// --replace-read-group (elp_set_replace_read_group): the new RG value, written as the field RG Z id NUL (n id bytes without the NUL).
+// on == false: the records are written as stored.
+struct RgSet { const uint8_t* id; uint32_t n; bool on; };
+
+// The fields a record is written with, in order: aln.SetRG(id) (SmallMap.Set, utils/small-map.go:59-67) followed by the field filter
+// (drop: the 65 536-bit table, or null for none).  With g.on the first field whose tag is RG, of whatever type, is replaced in place by
+// the new RG:Z field and later RG fields stay as they are; a record without an RG field gets the new one behind its last field.  Then
+// every field whose tag the table drops is left out, the new one included (it is tested as RG).  f(t, fe, repl) once per field written:
+// repl false: the stored field r[t, fe); repl true: the new RG:Z field.  Warp-collective like field_end.
+template <class F> __device__ __forceinline__ void out_fields(const uint8_t* r, uint64_t t, uint64_t rec, const uint32_t* drop, RgSet g, F f) {
+    bool seen = !g.on;
+    while (t + 3 <= rec) {
+        const uint64_t fe = field_end(r, t, rec);
+        const bool repl = !seen && r[t] == 'R' && r[t + 1] == 'G';
+        seen |= repl;
+        if (!drop || !dropped(drop, r[t], r[t + 1])) f(t, fe, repl);
+        t = fe;
+    }
+    if (!seen && (!drop || !dropped(drop, 'R', 'G'))) f(rec, rec, true);
+}
+
+// the new RG:Z field's BAM bytes (3 + n + 1) at o, over the warp
+__device__ __forceinline__ uint64_t rg_field_bytes(const RgSet& g) { return 4ull + g.n; }
+__device__ __forceinline__ void rg_field_write(uint8_t* o, const RgSet& g) {
+    const uint32_t m = g.n + 4;
+    for (uint32_t j = threadIdx.x & 31; j < m; j += 32) o[j] = j == 0 ? 'R' : (j == 1 ? 'G' : (j == 2 ? 'Z' : (j < m - 1 ? g.id[j - 3] : 0)));
+}
+
 }  // namespace tagwalk
+
+struct elp_ctx;
+tagwalk::RgSet rg_set(const elp_ctx* c);   // bam_ingest.cu: the context's setting of elp_set_replace_read_group

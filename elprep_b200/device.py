@@ -24,7 +24,7 @@ def _vp(a):
 def _cstrs(items):
     arr = (C.c_char_p * max(1, len(items)))()
     for i, s in enumerate(items):
-        arr[i] = None if s is None else s.encode()
+        arr[i] = None if s is None else s.encode("utf-8", "surrogateescape")
     return arr
 
 
@@ -44,9 +44,11 @@ class Context:
         self.max_cycle = max_cycle
         names = _cstrs(header.contig_names())
         self._clen = header.contig_lengths()
-        ids = _cstrs([r["ID"] for r in header.RG])
+        # an @RG without ID (--replace-read-group "LB:x") goes in as ID "" without PU: readGroupCovariate (filters/bqsr.go:35-51) finds
+        # no @RG whose ID matches the reads' RG:Z:"" and returns "", not PU
+        ids = _cstrs([r.get("ID", "") for r in header.RG])
         lbs = _cstrs([r.get("LB") for r in header.RG])
-        pus = _cstrs([r.get("PU") for r in header.RG])
+        pus = _cstrs([r.get("PU") if "ID" in r else None for r in header.RG])
         sq = np.ascontiguousarray(sqq if sqq is not None else [], dtype=np.uint8)
         cfg = _lib.ElpConfig(device, len(header.SQ), names, _vp(self._clen), len(header.RG), ids, lbs, pus, max_cycle, quantize_levels,
                              _vp(sq) if sq.size else None, int(sq.size), prefix.encode(), optical_pixel_distance, int(profile))
@@ -171,6 +173,12 @@ class Context:
         keep = [t.encode() if isinstance(t, str) else bytes(t) for t in (keep or ())]
         ra, ka = (C.c_char_p * max(1, len(remove)))(*remove), (C.c_char_p * max(1, len(keep)))(*keep)
         self._ck(self.L.elp_set_output_filter(self.h, mask, ra, len(remove), ka, len(keep)))
+
+    def set_replace_read_group(self, on=True):
+        """`--replace-read-group` on the byte paths (elp_set_replace_read_group): the context was created from the header after
+        filters.AddOrReplaceReadGroup (one @RG); every read of append_bam / append_sam / append_bgzf is in it, and fetch_bam / fetch_bgzf /
+        fetch_sam write each record as aln.SetRG(id) leaves it.  Only while the context holds no reads; survives reset()."""
+        self._ck(self.L.elp_set_replace_read_group(self.h, int(bool(on))))
 
     def n_output(self):
         """output records fetch_bam / fetch_sam write (those that pass the record filters of set_output_filter); 0 before sort_markdup"""

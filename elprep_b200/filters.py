@@ -177,6 +177,22 @@ def ClearDuplicateFlag(header):
     return flt
 
 
+def AddOrReplaceReadGroup(readGroup):
+    """filters.AddOrReplaceReadGroup (filters/simple-filters.go:154-162), `--replace-read-group`: readGroup is the flag's string parsed by
+    sam.ParseHeaderLineFromString.  The Filter sets header.RG = [readGroup], so duplicate marking (LB) and BQSR (PU, else ID) read only
+    that @RG; its AlignmentFilter puts every read of the batch in it (rg column 0, aln.SetRG(readGroup["ID"])).  It runs after the phase-1
+    filters that drop reads and before MarkDuplicates, which then refuses an LB without ID with the reference's text.  On the byte paths
+    the device does the same (Context.set_replace_read_group, with the context created from the header after this filter)."""
+    def flt(header):
+        header.RG = [dict(readGroup)]
+
+        def set_rg(batch):
+            batch.rg = np.zeros(batch.n, np.int32)
+            return batch
+        return set_rg
+    return flt
+
+
 def write_phase_filters(removeDuplicates=False, removeOptionalFields="", keepOptionalFields="", header_has_sr=False):
     """the write-phase flags of `elprep filter` as the arguments of Context.set_output_filter / elp_set_output_filter -> (mask, remove, keep),
     as cmd/filter.go:803-902 builds them: RemoveOptionalReads iff the header has @sr (the caller drops @sr from the header it writes);

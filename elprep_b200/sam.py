@@ -258,6 +258,71 @@ class AlignmentBatch:
                               qual=np.frombuffer(bytes(ql), dtype=np.uint8).copy(), **cols)
 
 
+# unicode.IsSpace of Go: the Latin-1 spaces, then the White_Space property above U+00FF
+_GO_SPACE = frozenset([0x09, 0x0A, 0x0B, 0x0C, 0x0D, 0x20, 0x85, 0xA0, 0x1680, 0x2028, 0x2029, 0x202F, 0x205F, 0x3000] + list(range(0x2000, 0x200B)))
+
+
+def _go_rune(b, i):
+    """utf8.DecodeRuneInString(b[i:]) -> (rune, width); an invalid byte is (U+FFFD, 1)"""
+    c = b[i]
+    if c < 0x80:
+        return c, 1
+    if 0xC2 <= c <= 0xDF:
+        n, lo, hi = 1, 0x80, 0xBF
+    elif 0xE0 <= c <= 0xEF:
+        n, lo, hi = 2, (0xA0 if c == 0xE0 else 0x80), (0x9F if c == 0xED else 0xBF)
+    elif 0xF0 <= c <= 0xF4:
+        n, lo, hi = 3, (0x90 if c == 0xF0 else 0x80), (0x8F if c == 0xF4 else 0xBF)
+    else:
+        return 0xFFFD, 1
+    if i + n >= len(b):
+        return 0xFFFD, 1
+    if not lo <= b[i + 1] <= hi or any(not 0x80 <= b[i + k] <= 0xBF for k in range(2, n + 1)):
+        return 0xFFFD, 1
+    r = c & (0x1F if n == 1 else (0x0F if n == 2 else 0x07))
+    for k in range(1, n + 1):
+        r = (r << 6) | (b[i + k] & 0x3F)
+    return r, n + 1
+
+
+def _go_fields(b):
+    """strings.Fields: the runs of bytes between runs of unicode.IsSpace runes"""
+    out, start, i = [], None, 0
+    while i < len(b):
+        r, w = _go_rune(b, i)
+        if r in _GO_SPACE:
+            if start is not None:
+                out.append(b[start:i])
+                start = None
+        elif start is None:
+            start = i
+        i += w
+    if start is not None:
+        out.append(b[start:])
+    return out
+
+
+def ParseHeaderLineFromString(line):
+    """sam.ParseHeaderLineFromString (sam/sam-files.go:153-177), the parser of `--replace-read-group`: TG:value fields separated by white
+    space as strings.Fields splits them (unicode.IsSpace on the decoded runes; a byte that is not valid UTF-8 is no space).  line: str
+    (its UTF-8 bytes, surrogate escapes as the bytes they stand for) or bytes -> dict of the same type.  ValueError where the reference
+    panics: a field whose third byte is not ':' ("incorrectly formatted SAM file field"; also a field shorter than 3 bytes, a Go index
+    panic there) and a repeated tag ("duplicate field tag")."""
+    text = isinstance(line, str)
+    b = line.encode("utf-8", "surrogateescape") if text else bytes(line)
+    dec = (lambda x: x.decode("utf-8", "surrogateescape")) if text else (lambda x: x)
+    txt = lambda x: x.decode("utf-8", "surrogateescape")                 # the message carries the field's bytes, as Go's %v of a string
+    rec = {}
+    for f in _go_fields(b):
+        if len(f) < 3 or f[2] != 0x3A:
+            raise ValueError(f"incorrectly formatted SAM file field {txt(f)}")
+        tag, value = dec(f[:2]), dec(f[3:])
+        if tag in rec:
+            raise ValueError(f"duplicate field tag {txt(f[:2])} in a SAM header line")
+        rec[tag] = value
+    return rec
+
+
 def _is_user_tag(code):
     """IsHeaderUserTag (sam/sam-types.go:49-56): a record type code with a lower-case letter"""
     return any("a" <= ch <= "z" for ch in code)

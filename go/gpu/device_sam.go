@@ -93,7 +93,8 @@ func NewDeviceSam(header *sam.Header, opts Options) *DeviceSam {
 		d.rgIdx[rg["ID"]] = int32(i)
 		lbs[i], noLB[i] = rg["LB"], rg["LB"] == ""
 		_, hasPU := rg["PU"]
-		pus[i], noPU[i] = rg["PU"], !hasPU
+		_, hasID := rg["ID"]
+		pus[i], noPU[i] = rg["PU"], !hasPU || !hasID // an @RG without ID: ID "" and no PU, so that the BQSR covariate is "" (readGroupCovariate, filters/bqsr.go:35-51)
 	}
 	cNames, f1 := cstrings(names, nil)
 	cIDs, f2 := cstrings(ids, nil)
@@ -372,6 +373,19 @@ func (d *DeviceSam) SetOutputFilter(mask uint32, remove []string, keep []string,
 		mask |= C.ELP_OUT_KEEP_FIELDS
 	}
 	check(d.ctx, C.elp_set_output_filter(d.ctx, C.uint32_t(mask), cRemove, C.int32_t(len(remove)), cKeep, C.int32_t(len(keep))))
+}
+
+// SetReplaceReadGroup: --replace-read-group on the byte paths (AppendBgzf, elp_append_bam / elp_append_sam, FetchBgzf and the other byte
+// fetches): every read is in the one @RG of the header, and each record is written as filters.AddOrReplaceReadGroup (simple-filters.go:154-162)
+// leaves it, RG:Z:id in place of its first RG field or behind its last field.  Create the DeviceSam from the header after the filter (its
+// RG is []utils.StringMap{sam.ParseHeaderLineFromString(flag)}) and call this before the first append, or after a reset.  The columnar
+// AddNodes path runs the reference's own filter on the host instead and does not need this call.
+func (d *DeviceSam) SetReplaceReadGroup(on bool) {
+	v := 0
+	if on {
+		v = 1
+	}
+	check(d.ctx, C.elp_set_replace_read_group(d.ctx, C.int(v)))
 }
 
 // SetReference / SetKnownSites: the side inputs of filters.NewBaseRecalibrator (bqsr.go:424-443).

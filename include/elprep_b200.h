@@ -403,6 +403,26 @@ int elp_fetch_sam(elp_ctx *ctx, uint64_t first, uint64_t n, char *out, uint64_t 
 #define ELP_OUT_REMOVE_OPTIONAL_READS 2u  /* RemoveOptionalReads (:146-152): reads with ELP_OPT_SR; the caller sets it iff the header has @sr (and drops @sr from the header it writes) */
 #define ELP_OUT_KEEP_FIELDS           4u  /* KeepOptionalFields(keep_tags) (:261-288); n_keep == 0 drops every optional field */
 int elp_set_output_filter(elp_ctx *ctx, uint32_t mask, const char *const *remove_tags, int32_t n_remove, const char *const *keep_tags, int32_t n_keep);
+/* `--replace-read-group "ID:x LB:y ..."`: filters.AddOrReplaceReadGroup (filters/simple-filters.go:154-162) on the byte paths.  The caller
+ * parses the flag's string (sam.ParseHeaderLineFromString, sam/sam-files.go:153-177) and creates the context from the header after the
+ * filter: exactly one @RG, the replacement, with its ID, LB and PU (an @RG without ID is passed as ID "" without PU, so that the BQSR
+ * covariate is "" as readGroupCovariate returns it, filters/bqsr.go:35-51).  on = 0 turns the setting off.
+ *  - When.  Only while the context holds no reads (after elp_create or elp_reset), else ELP_ESTATE; with on != 0 a context whose
+ *    n_read_groups is not 1 is ELP_EINVAL.  The setting survives elp_reset, like the ingest filter.
+ *  - Ingest (elp_append_bam, elp_append_sam, elp_append_bgzf).  Every read that passes the ingest filters is in read group 0, whatever RG
+ *    field its record has: no RG, an RG:Z value that is no @RG ID (otherwise ELP_EBAM), an RG of another type, several RG fields.  Every
+ *    record is still checked for structure (a malformed RG field is ELP_EBAM with any filter mask, CG:B is still ELP_ELIMIT), and the stored
+ *    records keep the input's bytes.  elp_append_batch is unchanged: the caller's marshaller sets the rg column to 0 (the filter runs on the
+ *    host there, as the other per-record filters do).
+ *  - Egress (elp_fetch_bam, elp_fetch_bam_bytes, elp_fetch_bgzf, elp_fetch_sam, elp_fetch_sam_bytes).  Each record is written as aln.SetRG(id)
+ *    (sam/sam-types.go:357-359, SmallMap.Set utils/small-map.go:59-67) leaves it, followed by the field filter of elp_set_output_filter:
+ *    the first field whose tag is RG, of whatever type, becomes RG Z id NUL in place (SAM: RG:Z:id at the same position), later RG fields
+ *    stay, and a record without an RG field gets the new one behind its last field; block_size is rewritten.  --remove-optional-fields RG
+ *    and --keep-optional-fields lists without RG drop the new field too.  The record filters, FLAG / MAPQ / QUAL and the refusals of the
+ *    fetch calls (after elp_clean_sam rewrote a CIGAR, ...) are as without the setting.  The header bytes (the new @RG line) are the
+ *    caller's, as the prefix of elp_fetch_bgzf.
+ *  - The columnar elp_fetch is unchanged: a columnar caller owns its *Alignments and sets RG itself. */
+int elp_set_replace_read_group(elp_ctx *ctx, int on);
 /* after elp_sort_markdup: the number of records of the output order (elp_n_sorted) that pass the record filters (elp_n_sorted without them);
  * 0 on error or before the sort */
 uint64_t elp_n_output(elp_ctx *ctx);

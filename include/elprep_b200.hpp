@@ -12,6 +12,8 @@
 //   FinalizeBQSRTables + PrintBQSRTables (bqsr.go:677, print-bqsr.go:269)   DeviceSam::FinalizeBQSRTables(recalFile)
 //   ApplyBQSR (bqsr.go:936)                                         DeviceSam::ApplyBQSR()
 //   (*sam.Sam).RunPipeline as PipelineInput (filter-pipeline.go:242-279)   DeviceSam::RunPipeline(sink)
+//   sam.ParseHeaderLineFromString (sam/sam-files.go:153-177)       elprep::ParseHeaderLineFromString
+//   filters.AddOrReplaceReadGroup (filters/simple-filters.go:154-162)   elprep::AddOrReplaceReadGroup, DeviceSam::SetReplaceReadGroup (byte paths)
 //   log.Panic(msg)                                                  throw elprep::Panic(msg)
 #pragma once
 #include <algorithm>
@@ -46,6 +48,71 @@ struct Header {
     struct SQ { std::string SN; int32_t LN; };
     struct ReadGroup { std::string ID, LB, PU; bool hasLB = false, hasPU = false; };
     std::vector<SQ> sq; std::vector<ReadGroup> rg;
+};
+
+// sam.ParseHeaderLineFromString (sam/sam-files.go:153-177), the parser of `--replace-read-group`: TG:value fields separated by white space
+// as strings.Fields splits them (unicode.IsSpace on the runes utf8.DecodeRuneInString decodes; a byte that is not valid UTF-8 is no space).
+// Throws Panic(ELP_EINVAL) where the reference panics: a field whose third byte is not ':' (also one shorter than 3 bytes, a Go index
+// panic there) and a repeated tag.
+inline std::map<std::string, std::string> ParseHeaderLineFromString(const std::string& line) {
+    auto rune = [&](size_t i, size_t* w) -> uint32_t {                 // (U+FFFD, 1) for an invalid byte
+        const uint8_t c = (uint8_t)line[i];
+        *w = 1;
+        if (c < 0x80) return c;
+        int n; uint8_t lo = 0x80, hi = 0xBF;
+        if (c >= 0xC2 && c <= 0xDF) n = 1;
+        else if (c >= 0xE0 && c <= 0xEF) { n = 2; if (c == 0xE0) lo = 0xA0; if (c == 0xED) hi = 0x9F; }
+        else if (c >= 0xF0 && c <= 0xF4) { n = 3; if (c == 0xF0) lo = 0x90; if (c == 0xF4) hi = 0x8F; }
+        else return 0xFFFD;
+        if (i + n >= line.size()) return 0xFFFD;
+        const uint8_t c1 = (uint8_t)line[i + 1];
+        if (c1 < lo || c1 > hi) return 0xFFFD;
+        uint32_t r = c & (n == 1 ? 0x1Fu : (n == 2 ? 0x0Fu : 0x07u));
+        for (int k = 1; k <= n; k++) {
+            const uint8_t ck = (uint8_t)line[i + k];
+            if (ck < 0x80 || ck > 0xBF) return 0xFFFD;
+            r = (r << 6) | (ck & 0x3Fu);
+        }
+        *w = (size_t)n + 1;
+        return r;
+    };
+    auto space = [](uint32_t r) {                                        // unicode.IsSpace
+        return r == '\t' || r == '\n' || r == '\v' || r == '\f' || r == '\r' || r == ' ' || r == 0x85 || r == 0xA0 || r == 0x1680 ||
+               (r >= 0x2000 && r <= 0x200A) || r == 0x2028 || r == 0x2029 || r == 0x202F || r == 0x205F || r == 0x3000;
+    };
+    std::vector<std::string> fields;
+    size_t start = std::string::npos;
+    for (size_t i = 0, w = 1; i < line.size(); i += w) {
+        if (space(rune(i, &w))) { if (start != std::string::npos) { fields.push_back(line.substr(start, i - start)); start = std::string::npos; } }
+        else if (start == std::string::npos) start = i;
+    }
+    if (start != std::string::npos) fields.push_back(line.substr(start));
+    std::map<std::string, std::string> rec;
+    for (const std::string& f : fields) {
+        if (f.size() < 3 || f[2] != ':') throw Panic(ELP_EINVAL, "incorrectly formatted SAM file field " + f);
+        if (!rec.emplace(f.substr(0, 2), f.substr(3)).second) throw Panic(ELP_EINVAL, "duplicate field tag " + f.substr(0, 2) + " in a SAM header line");
+    }
+    return rec;
+}
+
+// filters.AddOrReplaceReadGroup (filters/simple-filters.go:154-162), `--replace-read-group`.  The constructor is the header part:
+// header.rg becomes the one read group (an @RG without ID is ID "" without PU, so that the BQSR covariate is "" as readGroupCovariate
+// returns it, filters/bqsr.go:35-51); build DeviceSam from that header.  operator() is aln.SetRG(id): apply it to every batch before
+// AddNodes marshals it.  On the byte paths (AppendBgzf, FetchBgzf) call DeviceSam::SetReplaceReadGroup(true) instead.
+struct AddOrReplaceReadGroup {
+    std::string id;
+    AddOrReplaceReadGroup(Header& header, const std::map<std::string, std::string>& readGroup) {
+        Header::ReadGroup g;
+        auto it = readGroup.find("ID");
+        const bool hasID = it != readGroup.end();
+        if (hasID) g.ID = it->second;
+        if ((it = readGroup.find("LB")) != readGroup.end()) { g.LB = it->second; g.hasLB = true; }
+        if (hasID && (it = readGroup.find("PU")) != readGroup.end()) { g.PU = it->second; g.hasPU = true; }
+        header.rg.assign(1, g);
+        id = g.ID;
+    }
+    void operator()(Alignment& a) const { a.RG = id; a.hasRG = true; }
+    void operator()(std::vector<Alignment>& batch) const { for (Alignment& a : batch) (*this)(a); }
 };
 
 enum class SortingOrder { Keep = ELP_SO_KEEP, Unknown = ELP_SO_UNKNOWN, Unsorted = ELP_SO_UNSORTED, Queryname = ELP_SO_QUERYNAME, Coordinate = ELP_SO_COORDINATE };
@@ -150,6 +217,9 @@ class DeviceSam {
         out.resize(got);
         return out;
     }
+    // --replace-read-group on the byte paths (elp_set_replace_read_group): every read of AppendBgzf is in the header's one @RG, and FetchBgzf
+    // writes each record as AddOrReplaceReadGroup leaves it; before the first append (or after a reset)
+    void SetReplaceReadGroup(bool on) { check(elp_set_replace_read_group(ctx_, on ? 1 : 0)); }
     // the Finalize of AddNodes: By(CoordinateLess / QNAMELess).ParallelStableSort + filters.MarkDuplicates (+ MarkOpticalDuplicates)
     void Finalize(SortingOrder order) { check(elp_sort_markdup(ctx_, (int)order, opts_.MarkDuplicates ? (opts_.AlsoOpticals ? ELP_MARKDUP_OPTICAL : ELP_MARKDUP) : 0)); }
 
