@@ -6,8 +6,8 @@
 //                       plus a 39-bit (library, QNAME) hash for the mate join and the value ranges that size the keys
 //   fragment groups     key (lib, refid, unclipped pos, strand | is_frag, score desc) -> radix sort of the group bits only ->
 //                       frag_mark_kernel: one thread per group head walks its run (classifyFragment :210-254)
-//   mate join           sort by the (lib,QNAME) hash, verify on bytes, pair up in arrival order
-//                       (DeleteOrStore on pairFragment :336)
+//   mate join           mates next to each other in arrival order pair up in one streaming pass; the rest is sorted by the
+//                       (lib,QNAME) hash, verified on bytes, paired up in arrival order (DeleteOrStore on pairFragment :336)
 //   pair groups         key (lib, refid1, refid2, rev1, rev2, upos1, upos2), 64 bits when it fits, else 128 -> radix sort ->
 //                       pair_mark_kernel (classifyPair :329-396): both mates of every loser get 0x400
 // Results are deterministic; where the reference depends on goroutine scheduling (equal score AND equal QNAME) the
@@ -285,19 +285,82 @@ __global__ void __launch_bounds__(256) frag_mark_kernel(uint64_t m, const uint64
 }
 
 // ---------------------------------------------------------------- mate join
-__global__ void __launch_bounds__(256) join_keys_kernel(uint64_t n, const uint16_t* __restrict__ flag, const uint64_t* __restrict__ qhash,
-                                                         uint64_t* __restrict__ keys, uint32_t* __restrict__ vals, uint32_t* __restrict__ mate) {
-    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const uint16_t f = flag[i];
-    const bool in = (f & (F_UNMAPPED | F_SECONDARY | F_SUPPLEMENTARY)) == 0 && (f & (F_MULTIPLE | F_NEXTUNMAPPED)) == F_MULTIPLE;
-    keys[i] = in ? (qhash[i] & 0x7fffffffull) : (1ull << 31);      // 31 hash bits + the "not a true pair" bit = 32 key bits = 4 passes (equal-hash runs are verified on bytes)
-    vals[i] = (uint32_t)i;
-    mate[i] = NONE;
-}
+// Aligners write the two mates of a pair next to each other, so most true-pair reads find their mate at i + 1 in one streaming
+// pass (join_adjacent).  Only what that pass cannot settle goes through the hash sort: one element per adjacent pair and one per
+// leftover read (join_compact), sorted by 31 hash bits, then matched on bytes inside runs of equal keys (join).
+constexpr uint32_t PAIR_TAG = 0x80000000u;   // reduced-list element: the first read of an adjacent pair (read indices stay below 2^30)
+constexpr int JA_T = 256;
 
+__device__ __forceinline__ bool join_in(uint16_t f) {   // an entering true-pair read (mark-duplicates.go:182-184,436)
+    return (f & (F_UNMAPPED | F_SECONDARY | F_SUPPLEMENTARY)) == 0 && (f & (F_MULTIPLE | F_NEXTUNMAPPED)) == F_MULTIPLE;
+}
 __device__ __forceinline__ int32_t lib_of(const int32_t* rg, const int32_t* rg_lib, int n_rg, uint32_t i) { const int32_t g = rg[i]; return (g >= 0 && g < n_rg) ? rg_lib[g] : -1; }
 
+// four name bytes from arena offset x on (little-endian); the word after x's word is loaded only when a byte of it is needed
+__device__ __forceinline__ uint32_t name_word(const uint8_t* q, uint64_t x, uint32_t nbytes) {
+    const uint32_t* w = reinterpret_cast<const uint32_t*>(q + (x & ~3ull));
+    const uint32_t sh = 8 * (uint32_t)(x & 3);
+    const uint32_t lo = __ldg(w), hi = ((x & 3) + nbytes > 4) ? __ldg(w + 1) : 0u;
+    const uint32_t v = __funnelshift_r(lo, hi, sh);
+    return nbytes >= 4 ? v : v & (0xffffffffu >> (8 * (4 - nbytes)));
+}
+// the names at [a0, a0 + len) and [b0, b0 + len) are equal, compared a word at a time (the QNAME arena is 4-byte aligned)
+__device__ __forceinline__ bool names_equal(const uint8_t* q, uint64_t a0, uint64_t b0, uint64_t len) {
+    for (uint64_t k = 0; k < len; k += 4) {
+        const uint32_t nb = len - k < 4 ? (uint32_t)(len - k) : 4u;
+        if (name_word(q, a0 + k, nb) != name_word(q, b0 + k, nb)) return false;
+    }
+    return true;
+}
+
+// Reads i and i+1 are an adjacent pair when both are in, their 64-bit qhash values are equal, neither i-1 nor i+2 is an in read with
+// that qhash (so adjacent pairs are disjoint), and their libraries and QNAME bytes are equal.  Such a pair gets provisional mates and
+// one element in the reduced list (cnt[i] = 1, cnt[i+1] = 0); every other in read is a leftover with one element of its own.  The hash
+// test needs no name bytes, so thread i owns reads i and i+1 when they pass it and thread i+1 returns: every read is written once.
+__global__ void __launch_bounds__(JA_T) join_adjacent_kernel(uint64_t n, const uint16_t* __restrict__ flag, const uint64_t* __restrict__ qhash,
+                                                              const int32_t* __restrict__ rg, const int32_t* __restrict__ rg_lib, int n_rg,
+                                                              const uint64_t* __restrict__ qname_off, const uint8_t* __restrict__ qname,
+                                                              uint32_t* __restrict__ mate, uint32_t* __restrict__ cnt) {
+    __shared__ uint64_t s_h[JA_T + 4];   // qhash of reads b0-2 .. b0+JA_T+1
+    __shared__ uint8_t s_in[JA_T + 4];
+    const uint64_t b0 = (uint64_t)blockIdx.x * JA_T;
+    for (int k = threadIdx.x; k < JA_T + 4; k += JA_T) {
+        const int64_t r = (int64_t)b0 - 2 + k;
+        const bool ok = r >= 0 && (uint64_t)r < n;
+        const bool in = ok && join_in(flag[r]);
+        s_in[k] = in; s_h[k] = in ? qhash[r] : 0;
+    }
+    __syncthreads();
+    const uint64_t i = b0 + threadIdx.x;
+    if (i >= n) return;
+    const int t = threadIdx.x + 2;   // read i in the window
+    // hash-level pair starting at window slot u (reads u-1 .. u+2 are in the window for u = t-1, t)
+    auto hash_pair = [&](int u) {
+        return s_in[u] && s_in[u + 1] && s_h[u] == s_h[u + 1] && !(s_in[u - 1] && s_h[u - 1] == s_h[u]) && !(s_in[u + 2] && s_h[u + 2] == s_h[u]);
+    };
+    if (hash_pair(t - 1)) return;   // read i belongs to thread i-1
+    if (!hash_pair(t)) { mate[i] = NONE; cnt[i] = s_in[t]; return; }
+    const uint64_t a0 = qname_off[i], a1 = qname_off[i + 1], a2 = qname_off[i + 2];
+    const bool same = lib_of(rg, rg_lib, n_rg, (uint32_t)i) == lib_of(rg, rg_lib, n_rg, (uint32_t)i + 1) && a1 - a0 == a2 - a1 && names_equal(qname, a0, a1, a1 - a0);
+    mate[i] = same ? (uint32_t)i + 1 : NONE; mate[i + 1] = same ? (uint32_t)i : NONE;
+    cnt[i] = 1; cnt[i + 1] = same ? 0u : 1u;
+}
+
+// the reduced list in arrival order: element slot[i] is read i (a leftover) or the adjacent pair (i, i+1), tagged
+__global__ void __launch_bounds__(256) join_compact_kernel(uint64_t n, const uint64_t* __restrict__ slot, const uint32_t* __restrict__ mate,
+                                                            const uint64_t* __restrict__ qhash, uint64_t* __restrict__ keys, uint32_t* __restrict__ vals) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint64_t s = slot[i];
+    if (slot[i + 1] == s) return;
+    keys[s] = qhash[i] & 0x7fffffffull;      // 31 hash bits = 4 passes (equal-hash runs are verified on bytes)
+    vals[s] = (uint32_t)i | (mate[i] == (uint32_t)i + 1 ? PAIR_TAG : 0u);
+}
+
+// one thread per run of equal keys in the sorted reduced list (stable: a run is in arrival order).  A run of one element is a whole
+// (library, QNAME) group: an adjacent pair keeps its provisional mates, a leftover stays unpaired.  A longer run (a hash collision, or a
+// group with members elsewhere) drops its provisional mates, expands every adjacent pair into its two reads, which are consecutive in
+// arrival order, and pairs on bytes: the first unmatched same-(lib,QNAME) read stores, the next one deletes and pairs (:336).
 __global__ void __launch_bounds__(256) join_kernel(uint64_t m, const uint64_t* __restrict__ keys, const uint32_t* __restrict__ vals,
                                                     const int32_t* __restrict__ rg, const int32_t* __restrict__ rg_lib, int n_rg,
                                                     const uint64_t* __restrict__ qname_off, const uint8_t* __restrict__ qname, uint32_t* __restrict__ mate) {
@@ -305,9 +368,10 @@ __global__ void __launch_bounds__(256) join_kernel(uint64_t m, const uint64_t* _
     if (j >= m) return;
     const uint64_t k0 = keys[j];
     if (j > 0 && keys[j - 1] == k0) return;
-    uint64_t e = j + 1;
+    if (j + 1 == m || keys[j + 1] != k0) return;
+    uint64_t e = j + 2;
     while (e < m && keys[e] == k0) e++;
-    if (e - j == 2) {   // the common case: both reads still unpaired (join_keys_kernel), all loads issued before any compare
+    if (e - j == 2 && ((vals[j] | vals[j + 1]) & PAIR_TAG) == 0) {   // two leftover reads: all loads issued before any compare
         const uint32_t va = vals[j], vb = vals[j + 1];
         const int32_t ga = rg[va], gb = rg[vb];
         const uint64_t a0 = qname_off[va], a1 = qname_off[va + 1], b0 = qname_off[vb], b1 = qname_off[vb + 1];
@@ -315,18 +379,31 @@ __global__ void __launch_bounds__(256) join_kernel(uint64_t m, const uint64_t* _
         if (la == lb && qname_compare(qname, a0, a1, b0, b1) == 0) { mate[va] = vb; mate[vb] = va; }
         return;
     }
-    // arrival order inside the run (stable sort): first unmatched same-(lib,QNAME) read stores, the next one deletes and pairs (:336)
     for (uint64_t a = j; a < e; a++) {
-        const uint32_t va = vals[a];
-        if (a > j && mate[va] != NONE) continue;   // the run's first read is still unpaired
-        const int32_t la = lib_of(rg, rg_lib, n_rg, va);
-        for (uint64_t b = a + 1; b < e; b++) {
-            const uint32_t vb = vals[b];
-            if (mate[vb] != NONE) continue;
-            if (la != lib_of(rg, rg_lib, n_rg, vb)) continue;
-            if (qname_compare(qname, qname_off[va], qname_off[va + 1], qname_off[vb], qname_off[vb + 1]) != 0) continue;
-            mate[va] = vb; mate[vb] = va;
-            break;
+        const uint32_t x = vals[a];
+        if (x & PAIR_TAG) { const uint32_t r = x & ~PAIR_TAG; mate[r] = NONE; mate[r + 1] = NONE; }
+    }
+    for (uint64_t a = j; a < e; a++) {
+        const uint32_t xa = vals[a], ra = xa & ~PAIR_TAG, na = (xa & PAIR_TAG) ? 2u : 1u;
+        for (uint32_t s = 0; s < na; s++) {
+            const uint32_t va = ra + s;
+            if (mate[va] != NONE) continue;
+            const int32_t la = lib_of(rg, rg_lib, n_rg, va);
+            const uint64_t a0 = qname_off[va], a1 = qname_off[va + 1];
+            // the later reads of the run: the rest of element a, then elements a+1 .. e-1
+            bool done = false;
+            for (uint64_t b = a; b < e && !done; b++) {
+                const uint32_t xb = vals[b], rb = xb & ~PAIR_TAG, nb = (xb & PAIR_TAG) ? 2u : 1u;
+                for (uint32_t t = (b == a ? s + 1 : 0); t < nb; t++) {
+                    const uint32_t vb = rb + t;
+                    if (mate[vb] != NONE) continue;
+                    if (la != lib_of(rg, rg_lib, n_rg, vb)) continue;
+                    if (qname_compare(qname, a0, a1, qname_off[vb], qname_off[vb + 1]) != 0) continue;
+                    mate[va] = vb; mate[vb] = va;
+                    done = true;
+                    break;
+                }
+            }
         }
     }
 }
@@ -473,19 +550,31 @@ static int mark_pairs(elp_ctx* c, bool optical, uint64_t nt, uint64_t n_true_pai
     int rc;
     if (n_true_pairs < 2) return optical ? phase_optical(c, 0, nullptr, nullptr, 0) : E_OK;
     CUDA_TRY(c, c->mate.reserve(nt + 4, c->stream));
-    c->begin("join_keys", (double)nt * (2 + 8 + 8 + 4 + 4));
-    join_keys_kernel<<<nblk(nt, 256), 256, 0, c->stream>>>(nt, c->flag.p, c->qhash.p, c->keys_a.p, c->vals_a.p, c->mate.p);
-    c->end(); LAUNCH_CHECK(c);
-    bool in_b = false;
-    rc = radix_sort_u64(c, c->keys_a.p, c->keys_b.p, c->vals_a.p, c->vals_b.p, nt, 32, &in_b, "u64");   // 31 hash bits + 1: runs of equal hash are verified on bytes anyway
-    if (rc) return rc;
-    const uint64_t m = n_true_pairs;
-    c->begin("join", (double)m * 12);
-    join_kernel<<<nblk(m, 256), 256, 0, c->stream>>>(m, in_b ? c->keys_b.p : c->keys_a.p, in_b ? c->vals_b.p : c->vals_a.p, c->rg.p, c->d_rg_lib.p, c->n_rg, c->qname_off.p, c->qname.p, c->mate.p);
-    c->end(); LAUNCH_CHECK(c);
-    // deterministic pair list, ordered by the arrival of the later mate
     CUDA_TRY(c, c->scan_tmp.reserve(nt + 4, c->stream));
     uint64_t* slot = c->keys_b.p;   // nt+1 u64, free at this point
+    // adjacent mates, then the reduced list of what they leave (about half the true-pair reads when mates arrive next to each other)
+    c->begin("join_adjacent", (double)nt * (2 + 8 + 4 + 4) + (double)n_true_pairs * (4 + 8) + (double)c->n_qname);
+    join_adjacent_kernel<<<nblk(nt, JA_T), JA_T, 0, c->stream>>>(nt, c->flag.p, c->qhash.p, c->rg.p, c->d_rg_lib.p, c->n_rg, c->qname_off.p, c->qname.p,
+                                                                c->mate.p, c->scan_tmp.p);
+    c->end(); LAUNCH_CHECK(c);
+    rc = exclusive_scan_u32_to_u64(c, c->scan_tmp.p, slot, nt);
+    if (rc) return rc;
+    uint64_t m = 0;
+    CUDA_TRY(c, cudaMemcpyAsync(&m, slot + nt, 8, cudaMemcpyDeviceToHost, c->stream));
+    CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+    if (m) {   // (n_true_pairs >= 2 in reads: never empty)
+        c->begin("join_compact", (double)nt * (8 + 4) + (double)m * (8 + 8 + 4));
+        join_compact_kernel<<<nblk(nt, 256), 256, 0, c->stream>>>(nt, slot, c->mate.p, c->qhash.p, c->keys_a.p, c->vals_a.p);
+        c->end(); LAUNCH_CHECK(c);
+        bool in_b = false;
+        rc = radix_sort_u64(c, c->keys_a.p, c->keys_b.p, c->vals_a.p, c->vals_b.p, m, 31, &in_b, "u64");
+        if (rc) return rc;
+        c->begin("join", (double)m * 12);
+        join_kernel<<<nblk(m, 256), 256, 0, c->stream>>>(m, in_b ? c->keys_b.p : c->keys_a.p, in_b ? c->vals_b.p : c->vals_a.p, c->rg.p, c->d_rg_lib.p, c->n_rg,
+                                                          c->qname_off.p, c->qname.p, c->mate.p);
+        c->end(); LAUNCH_CHECK(c);
+    }
+    // deterministic pair list, ordered by the arrival of the later mate
     c->begin("pair_flag", (double)nt * 8);
     pair_flag_kernel<<<nblk(nt, 256), 256, 0, c->stream>>>(nt, c->mate.p, c->scan_tmp.p);
     c->end(); LAUNCH_CHECK(c);
@@ -508,6 +597,7 @@ static int mark_pairs(elp_ctx* c, bool optical, uint64_t nt, uint64_t n_true_pai
         pair_keys_kernel<<<nblk(nt, 256), 256, 0, c->stream>>>(nt, c->mate.p, slot, c->flag.p, c->refid.p, c->rg.p, c->d_rg_lib.p, c->n_rg, c->upos.p, c->score.p, L,
                                                               c->keys_a.p, c->vals_a.p, c->pair_a.p, c->pair_b.p, c->pair_score.p);
         c->end(); LAUNCH_CHECK(c);
+        bool in_b = false;
         rc = words == 1 ? radix_sort_u64(c, c->keys_a.p, kb2, c->vals_a.p, c->vals_b.p, npairs, L.key_bits, &in_b, "u64")
                         : radix_sort_u128(c, c->keys_a.p, kb2, c->vals_a.p, c->vals_b.p, npairs, L.key_bits, &in_b, "u128");
         if (rc) return rc;
