@@ -31,7 +31,9 @@ struct BamArgs {
     int rg_replace;                       // --replace-read-group: every read gets read group 0, whatever RG field its record has
     int32_t *refid, *pos, *nref, *pnext, *tlen, *rg; uint16_t* flag; uint8_t* mapq; uint8_t* optf;
     uint32_t *len_qname, *len_cigar, *len_seq, *len_qual;   // [n] lengths, scanned afterwards
-    const uint8_t* rg_names; const uint32_t* rg_name_off; int n_rg; int n_contigs;
+    const uint8_t* rg_names; const uint32_t* rg_name_off; int n_rg;
+    int n_ref;                            // refID / next_refID bound of the records (ingest_ref_bound)
+    const int32_t* remap;                 // elp_set_input_dictionary: refID -> output contig of the columns, or null (off)
     uint32_t* err;
 };
 
@@ -115,10 +117,13 @@ __global__ void __launch_bounds__(256) bam_fixed_kernel(BamArgs A) {
     const uint32_t l_name = r[12], mapq = r[13], n_cig = rd16(r + 16), flag = rd16(r + 18);
     const int32_t l_seq = (int32_t)rd32(r + 20), nref = (int32_t)rd32(r + 24), pnext = (int32_t)rd32(r + 28), tlen = (int32_t)rd32(r + 32);
     const uint64_t k = A.n0 + i;
-    A.refid[k] = refid < 0 ? -1 : refid; A.pos[k] = pos + 1; A.flag[k] = (uint16_t)(A.clear_dup ? flag & ~(uint32_t)F_DUPLICATE : flag); A.mapq[k] = (uint8_t)mapq;
-    A.nref[k] = nref < 0 ? -1 : nref; A.pnext[k] = pnext + 1; A.tlen[k] = tlen;
+    // (remap is read only inside the bound: check_record below fails a record outside it)
+    const int32_t ro = refid < 0 ? -1 : (!A.remap ? refid : (refid < A.n_ref ? A.remap[refid] : -1));
+    const int32_t no = nref < 0 ? -1 : (!A.remap ? nref : (nref < A.n_ref ? A.remap[nref] : -1));
+    A.refid[k] = ro; A.pos[k] = pos + 1; A.flag[k] = (uint16_t)(A.clear_dup ? flag & ~(uint32_t)F_DUPLICATE : flag); A.mapq[k] = (uint8_t)mapq;
+    A.nref[k] = no; A.pnext[k] = pnext + 1; A.tlen[k] = tlen;
     int32_t rg; uint8_t optf;
-    const uint32_t bad = check_record(r, rec_len, A.n_contigs, RgNames{A.rg_names, A.rg_name_off, A.n_rg}, &rg, &optf);
+    const uint32_t bad = check_record(r, rec_len, A.n_ref, RgNames{A.rg_names, A.rg_name_off, A.n_rg}, &rg, &optf);
     if (A.rg_replace) rg = 0;                  // (the record's RG fields are rewritten at egress; a value that is no @RG ID is not refused)
     else if (rg == -2) { atomicOr(A.err, DERR_BAM_RG); rg = -1; }
     if (bad) atomicOr(A.err, bad == 2 ? DERR_BAM_CG : DERR_BAM);
@@ -145,7 +150,7 @@ __device__ __forceinline__ bool tag_int(const uint8_t* r, uint64_t x, uint8_t ty
 
 __global__ void __launch_bounds__(256) bam_keep_kernel(uint64_t n, const uint8_t* __restrict__ raw, const uint64_t* __restrict__ rec_off, uint64_t n_bytes,
                                                         uint32_t mask, int32_t min_mapq, const int32_t* const* __restrict__ regions, const uint64_t* __restrict__ n_regions, int n_contigs,
-                                                        RgNames G, uint32_t* __restrict__ keep, uint32_t* __restrict__ err) {
+                                                        int n_ref, const int32_t* __restrict__ remap, bool drop_unmapped_ref, RgNames G, uint32_t* __restrict__ keep, uint32_t* __restrict__ err) {
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const uint64_t st = rec_off[i], len = rec_off[i + 1] - st;
@@ -154,12 +159,15 @@ __global__ void __launch_bounds__(256) bam_keep_kernel(uint64_t n, const uint8_t
     {   // the reference parses a record before any filter sees it: a malformed record fails the call even when a filter would drop it.
         // (CG:B and an unknown RG:Z are left to bam_fixed_kernel, which sees the records that are kept.)
         int32_t rg; uint8_t optf;
-        if (check_record(r, len, n_contigs, G, &rg, &optf) == 1) { atomicOr(err, DERR_BAM); keep[i] = 0; return; }
+        if (check_record(r, len, n_ref, G, &rg, &optf) == 1) { atomicOr(err, DERR_BAM); keep[i] = 0; return; }
     }
     // from here on the record is well-formed: every length fits in len
     const int32_t refid = (int32_t)rd32(r + 4), pos = (int32_t)(rd32(r + 8) + 1u);                                 // int32 + 1 wraps as in Go
     const uint32_t l_name = r[12], mapq = r[13], n_cig = rd16(r + 16), flag = rd16(r + 18);
-    bool k = true;
+    // remap (elp_set_input_dictionary): the output contig of refid; with REPLACE (drop set) a read whose RNAME is not in the new dictionary
+    // is dropped (ReplaceReferenceSequenceDictionary :49-57)
+    const int32_t ro = (remap && refid >= 0) ? remap[refid] : refid;
+    bool k = !(drop_unmapped_ref && refid >= 0 && ro < 0);
     if ((mask & ELP_FILTER_UNMAPPED) && (flag & F_UNMAPPED)) k = false;                                           // RemoveUnmappedReads :73-75
     if ((mask & ELP_FILTER_UNMAPPED_STRICT) && ((flag & F_UNMAPPED) || pos == 0 || refid < 0)) k = false;          // RemoveUnmappedReadsStrict :79-83
     if ((int32_t)mapq < min_mapq) k = false;                                                                      // RemoveMappingQualityLessThan :332-347 (min_mapq as elp_set_ingest_filter stores it)
@@ -180,7 +188,7 @@ __global__ void __launch_bounds__(256) bam_keep_kernel(uint64_t n, const uint8_t
                     if (o == 0 || o == 1 || o == 4 || o == 7 || o == 8) rl += ln; if (o == 0 || o == 2 || o == 3 || o == 7 || o == 8) fl += ln; }
                 if ((int32_t)rl > 0) a_end = (int32_t)((uint32_t)pos + fl - 1u);                                  // aln.End(), sam/sam-types.go:769-775
             }
-            if (refid < 0 || refid >= n_contigs || !regions || !overlap_any(regions[refid], n_regions[refid], pos, a_end)) k = false;   // no regions for RNAME: Overlap(nil) is false
+            if (ro < 0 || ro >= n_contigs || !regions || !overlap_any(regions[ro], n_regions[ro], pos, a_end)) k = false;   // no regions for RNAME: Overlap(nil) is false
         }
         if (k && (mask & ELP_FILTER_NON_EXACT_STRICT)) {                                                          // RemoveNonExactMappingReadsStrict :115-136: X0=1, X1=0, XM=0, XO=0, XG=0
             int64_t want[5] = {1, 0, 0, 0, 0}; uint32_t seen = 0; bool good = true;
@@ -258,11 +266,22 @@ __global__ void __launch_bounds__(256) bam_out_len_kernel(uint64_t n, uint64_t f
     const uint64_t kk = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (kk < n) len[kk] = rd32(all + all_start[perm[out_pos(sel, first, kk)]]) + 4;
 }
+// elp_set_input_dictionary: lanes 4..7 and 24..27 rewrite the bytes of refID and next_refID as the output contig (-1 where there is none),
+// after they copied the stored bytes there in their first step of the per-byte loop
+__device__ __forceinline__ void patch_refids(const uint8_t* r, uint8_t* o, const int32_t* __restrict__ remap) {
+    const unsigned lane = threadIdx.x & 31;
+    if ((lane >= 4 && lane < 8) || (lane >= 24 && lane < 28)) {
+        const int32_t id = (int32_t)rd32(r + (lane & ~3u));
+        const uint32_t v = (uint32_t)(id < 0 ? -1 : remap[id]);
+        o[lane] = (uint8_t)(v >> (8 * (lane & 3u)));
+    }
+}
 // one warp per output record: copy the stored record, patch MAPQ (byte 13 of the record with its block_size; elp_clean_sam sets it to 0
 // for unmapped reads, otherwise it equals the stored byte), FLAG (bytes 18..19) and QUAL
 __global__ void __launch_bounds__(256) bam_out_copy_kernel(uint64_t n, uint64_t first, const uint32_t* __restrict__ sel, const uint32_t* __restrict__ perm, const uint64_t* __restrict__ all_start,
                                                             const uint8_t* __restrict__ all, const uint64_t* __restrict__ out_off, uint8_t* __restrict__ out,
-                                                            const uint16_t* __restrict__ s_flag, const uint8_t* __restrict__ s_mapq, const uint64_t* __restrict__ s_out_off, const uint8_t* __restrict__ qual_out) {
+                                                            const uint16_t* __restrict__ s_flag, const uint8_t* __restrict__ s_mapq, const uint64_t* __restrict__ s_out_off, const uint8_t* __restrict__ qual_out,
+                                                            const int32_t* __restrict__ remap) {
     const unsigned lane = threadIdx.x & 31;
     const uint64_t kk = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (kk >= n) return;
@@ -284,6 +303,7 @@ __global__ void __launch_bounds__(256) bam_out_copy_kernel(uint64_t n, uint64_t 
         o[t] = v;
     }
     if (lane == 13) o[13] = mq;                  // (this lane copied byte 13 in its first step: outside the per-byte loop, no extra compare there)
+    if (remap) patch_refids(r, o, remap);
 }
 
 // ---- write-phase filters (elp_set_output_filter; cmd/filter.go:803-902) ----
@@ -322,11 +342,13 @@ __global__ void __launch_bounds__(256) bam_out_fields_measure_kernel(uint64_t n,
     tagwalk::out_fields(r, t0, rec, drop, g, [&](uint64_t t, uint64_t fe, bool repl) { x += repl ? tagwalk::rg_field_bytes(g) : fe - t; });
     if ((threadIdx.x & 31) == 0) len[kk] = (uint32_t)x;
 }
-// emit: the fixed part and the variable fields with block_size, MAPQ, FLAG and QUAL patched, then the fields in their order
+// emit: the fixed part and the variable fields with block_size, MAPQ, FLAG, QUAL (and, with remap, refID / next_refID) patched, then the
+// fields in their order
 __global__ void __launch_bounds__(256) bam_out_fields_emit_kernel(uint64_t n, uint64_t first, const uint32_t* __restrict__ sel, const uint32_t* __restrict__ perm,
                                                                   const uint64_t* __restrict__ all_start, const uint8_t* __restrict__ all, const uint32_t* __restrict__ drop,
                                                                   tagwalk::RgSet g, const uint64_t* __restrict__ out_off, uint8_t* __restrict__ out,
-                                                                  const uint16_t* __restrict__ s_flag, const uint8_t* __restrict__ s_mapq, const uint64_t* __restrict__ s_out_off, const uint8_t* __restrict__ qual_out) {
+                                                                  const uint16_t* __restrict__ s_flag, const uint8_t* __restrict__ s_mapq, const uint64_t* __restrict__ s_out_off, const uint8_t* __restrict__ qual_out,
+                                                                  const int32_t* __restrict__ remap) {
     const unsigned lane = threadIdx.x & 31;
     const uint64_t kk = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (kk >= n) return;
@@ -348,6 +370,7 @@ __global__ void __launch_bounds__(256) bam_out_fields_emit_kernel(uint64_t n, ui
         o[t] = v;
     }
     if (lane == 13) o[13] = mq;                  // (as in bam_out_copy_kernel)
+    if (remap) patch_refids(r, o, remap);
     uint64_t x = t0;
     tagwalk::out_fields(r, t0, rec, drop, g, [&](uint64_t t, uint64_t fe, bool repl) {
         if (repl) { tagwalk::rg_field_write(o + x, g); x += tagwalk::rg_field_bytes(g); return; }
@@ -429,19 +452,20 @@ int rg_names_upload(elp_ctx* c) {
 // The device-resident part of elp_append_bam, shared with elp_append_sam: nrec records (n_bytes in all) already sit in bam_raw, and
 // bam_off[0..nrec] holds their chained offsets (bam_off[nrec] == n_bytes).  The caller holds append_mu and has checked the phase
 // and the 2^32 read limit.  From here on: ingest filters, fixed fields and RG:Z, segmented copies, QUAL presence, the bam_all arena.
-int bam_ingest_core(elp_ctx* c, uint64_t n_bytes, uint64_t nrec) {
+int bam_ingest_core(elp_ctx* c, uint64_t n_bytes, uint64_t nrec, bool sam_records) {
     uint64_t bn = nrec;                                       // becomes the number of records that pass the filters
     const uint64_t n0 = c->n;
     cudaStream_t s = c->stream;
     TRY(grow(c, c->bam_start, nrec + 2, 0));
     const uint64_t* d_start = c->bam_off.p;                   // without filters: record i is read n0 + i
     TRY(rg_names_upload(c));
-    if (c->filter_mask || c->filter_min_mapq > 0) {
+    const int n_ref = ingest_ref_bound(c, sam_records);
+    if (ingest_keep_on(c)) {
         TRY(grow(c, c->scan_tmp, nrec + 8, 0)); TRY(grow(c, c->off_stage, nrec + 2, 0));
         c->begin("bam_keep", (double)nrec * 48);
         if (c->filter_mask & ELP_FILTER_TARGET_REGIONS) TRY(table_upload(c, c->regions));
         bam_keep_kernel<<<nblk(nrec, 256), 256, 0, s>>>(nrec, c->bam_raw.p, c->bam_off.p, n_bytes, c->filter_mask, c->filter_min_mapq, c->regions.d_ptrs.p, c->regions.d_n.p, c->n_contigs,
-                                                        RgNames{c->d_rg_names.p, c->d_rg_name_off.p, c->n_rg}, c->scan_tmp.p, c->d_err.p);
+                                                        n_ref, ingest_remap(c), (c->dict_mode & ELP_DICT_REPLACE) != 0, RgNames{c->d_rg_names.p, c->d_rg_name_off.p, c->n_rg}, c->scan_tmp.p, c->d_err.p);
         c->end(); LAUNCH_CHECK(c);
         TRY(exclusive_scan_u32_to_u64(c, c->scan_tmp.p, c->off_stage.p, nrec));
         bam_compact_kernel<<<nblk(nrec, 256), 256, 0, s>>>(nrec, c->scan_tmp.p, c->off_stage.p, c->bam_off.p, c->bam_start.p); c->launches++;
@@ -463,7 +487,7 @@ int bam_ingest_core(elp_ctx* c, uint64_t n_bytes, uint64_t nrec) {
     A.n = bn; A.n0 = n0; A.raw = c->bam_raw.p; A.start = d_start; A.n_bytes = n_bytes; A.chained = d_start == c->bam_off.p; A.clear_dup = c->clear_dup; A.rg_replace = c->rg_replace;
     A.refid = c->refid.p; A.pos = c->pos.p; A.nref = c->nref.p; A.pnext = c->pnext.p; A.tlen = c->tlen.p; A.rg = c->rg.p; A.flag = c->flag.p; A.mapq = c->mapq.p; A.optf = c->optf.p;
     A.len_qname = c->scan_tmp.p; A.len_cigar = c->scan_tmp.p + (bn + 4); A.len_seq = c->scan_tmp.p + 2 * (bn + 4); A.len_qual = c->scan_tmp.p + 3 * (bn + 4);
-    A.rg_names = c->d_rg_names.p; A.rg_name_off = c->d_rg_name_off.p; A.n_rg = c->n_rg; A.n_contigs = c->n_contigs; A.err = c->d_err.p;
+    A.rg_names = c->d_rg_names.p; A.rg_name_off = c->d_rg_name_off.p; A.n_rg = c->n_rg; A.n_ref = n_ref; A.remap = ingest_remap(c); A.err = c->d_err.p;
     c->begin("bam_fixed", (double)bn * 36 + (double)n_bytes * 0.2);
     bam_fixed_kernel<<<nblk(bn, 256), 256, 0, s>>>(A);
     c->end(); LAUNCH_CHECK(c);
@@ -569,11 +593,11 @@ static int bam_out_format(elp_ctx* c, uint64_t first, uint64_t n, const uint32_t
         c->begin("bam_out_fields_emit", (double)c->n_bam * (double)n / (double)std::max<uint64_t>(c->n, 1) + (double)total);
         bam_out_fields_emit_kernel<<<nblk(n * 32, 256), 256, 0, c->stream>>>(n, first, sel, c->perm.p, c->bam_all_off.p, c->bam_all.p, c->out_fields ? c->d_out_drop.p : nullptr,
                                                                              rg_set(c), c->off_stage.p, dst,
-                                                                             c->s_flag.p, c->s_mapq.p, c->s_out_off.p, c->qual_out_valid ? c->qual_out.p : nullptr);
+                                                                             c->s_flag.p, c->s_mapq.p, c->s_out_off.p, c->qual_out_valid ? c->qual_out.p : nullptr, ingest_remap(c));
     } else {
         c->begin("bam_format", 2.0 * (double)total);
         bam_out_copy_kernel<<<nblk(n * 32, 256), 256, 0, c->stream>>>(n, first, sel, c->perm.p, c->bam_all_off.p, c->bam_all.p, c->off_stage.p, dst, c->s_flag.p, c->s_mapq.p, c->s_out_off.p,
-                                                                      c->qual_out_valid ? c->qual_out.p : nullptr);
+                                                                      c->qual_out_valid ? c->qual_out.p : nullptr, ingest_remap(c));
     }
     c->end(); LAUNCH_CHECK(c);
     return E_OK;
@@ -670,6 +694,71 @@ extern "C" int elp_set_replace_read_group(elp_ctx* c, int on) {
     if (on && c->n_rg != 1) return c->fail(E_INVAL, "elp_set_replace_read_group: the context must be created with exactly one @RG, the replacement (it has %d)", c->n_rg);
     if (on) TRY(rg_names_upload(c));
     c->rg_replace = on != 0;
+    return ELP_OK;
+}
+
+// the names elp_fetch_sam prints for a stored refID: the input name table, with "chr" prefixed under RENAME (RenameChromosomes runs on
+// RNAME / RNEXT before the output is formatted); elp_config's names while the setting is off
+std::vector<std::string> sam_print_names(const elp_ctx* c) {
+    if (!c->dict_mode) return c->contig_names;
+    std::vector<std::string> v;
+    for (const std::string& s : c->in_tab) v.push_back((c->dict_mode & ELP_DICT_RENAME_CHROMOSOMES) ? "chr" + s : s);
+    return v;
+}
+
+extern "C" int elp_set_input_dictionary(elp_ctx* c, uint32_t mode, const char* const* names, const int32_t* lengths, int32_t n) {
+    if (!c) return ELP_EINVAL;
+    cudaSetDevice(c->device);
+    if (mode & ~(uint32_t)(ELP_DICT_RENAME_CHROMOSOMES | ELP_DICT_REPLACE)) return c->fail(E_INVAL, "elp_set_input_dictionary: unknown mode bits 0x%x", mode);
+    if (n < 0 || (n && (!names || !lengths))) return c->fail(E_INVAL, "elp_set_input_dictionary: bad input dictionary (n = %d)", n);
+    if (c->n || c->sorted || c->bgzf_open) return c->fail(E_STATE, "elp_set_input_dictionary: the context holds reads (call it after elp_create or elp_reset)");
+    if (mode && !c->has_contig_names) return c->fail(E_INVAL, "elp_set_input_dictionary: the context was created without elp_config.contig_names");
+    const bool rename = (mode & ELP_DICT_RENAME_CHROMOSOMES) != 0, replace = (mode & ELP_DICT_REPLACE) != 0;
+    std::vector<std::string> in;
+    for (int32_t i = 0; i < n; i++) {
+        if (!names[i]) return c->fail(E_INVAL, "elp_set_input_dictionary: input name %d is null", i);
+        in.push_back(names[i]);
+    }
+    if (rename && !replace) {
+        if (n != c->n_contigs) return c->fail(E_INVAL, "elp_set_input_dictionary: RENAME_CHROMOSOMES alone: the input has %d @SQ, elp_config %d contigs", n, c->n_contigs);
+        for (int32_t i = 0; i < n; i++)
+            if (c->contig_names[i] != "chr" + in[i])
+                return c->fail(E_INVAL, "elp_set_input_dictionary: RENAME_CHROMOSOMES alone: contig %d of elp_config is '%s', not 'chr%s'", i, c->contig_names[i].c_str(), in[i].c_str());
+    }
+    c->sam_out.reset();                      // (elp_fetch_sam's name table follows the setting)
+    c->in_dict = NameDictBufs();
+    c->in_tab.clear(); c->in_len.clear(); c->n_in = 0; c->dict_mode = 0;
+    if (!mode) return ELP_OK;
+    auto renamed = [&](const std::string& s) { return rename ? "chr" + s : s; };
+    std::map<std::string, int32_t> last_out, last_in_len;   // AddREFID: the last of equal names wins; CleanSam's table likewise
+    for (int j = 0; j < c->n_contigs; j++) last_out[c->contig_names[j]] = j;
+    for (int32_t i = 0; i < n; i++) last_in_len[renamed(in[i])] = lengths[i];
+    std::vector<int32_t> remap;
+    for (int32_t i = 0; i < n; i++) {
+        if (!replace) { remap.push_back(i); continue; }
+        auto it = last_out.find(renamed(in[i]));
+        remap.push_back(it == last_out.end() ? -1 : it->second);
+    }
+    std::vector<std::string> tab = in;
+    if (replace) {   // the SAM extension: replacement names no input name reaches, as the RNAME text that renames to them
+        std::map<std::string, int> known;
+        for (const std::string& s : in) known.emplace(s, 0);
+        for (int j = 0; j < c->n_contigs; j++) {
+            const std::string& N = c->contig_names[j];
+            if (rename && N.compare(0, 3, "chr") != 0) continue;   // unreachable: every renamed RNAME starts with "chr"
+            const std::string text = rename ? N.substr(3) : N;
+            if (text == "*" || !known.emplace(text, 0).second) continue;
+            tab.push_back(text); remap.push_back(last_out[N]);
+        }
+    }
+    remap.push_back(-1);                     // elp_append_sam under REPLACE: an RNAME that reaches nothing
+    std::vector<int32_t> clean_len(std::max(1, c->n_contigs), 0);
+    for (int j = 0; j < c->n_contigs; j++) { auto it = last_in_len.find(c->contig_names[j]); if (it != last_in_len.end()) clean_len[j] = it->second; }
+    CUDA_TRY(c, c->d_remap.fit(remap.size()));
+    CUDA_TRY(c, c->d_clean_len.fit(clean_len.size()));
+    CUDA_TRY(c, cudaMemcpy(c->d_remap.p, remap.data(), remap.size() * 4, cudaMemcpyHostToDevice));
+    CUDA_TRY(c, cudaMemcpy(c->d_clean_len.p, clean_len.data(), clean_len.size() * 4, cudaMemcpyHostToDevice));
+    c->in_tab = tab; c->in_len.assign(lengths, lengths + n); c->n_in = n; c->dict_mode = mode;
     return ELP_OK;
 }
 

@@ -221,12 +221,28 @@ int bgzf_inflate_run(elp_ctx* c, const char* who, const uint8_t* in, uint64_t n_
     return inflate_blocks(c, who, {{in, n_in}}, blocks, total, out);
 }
 
-// the reference list of a complete header at bam_raw[0, hdr) against elp_config: n_ref, every l_ref and (when given) every name
+// the reference list of a complete header at bam_raw[0, hdr) against elp_config, or against the input dictionary of elp_set_input_dictionary
+// while it is set: n_ref, every l_ref and (when given) every name
 static int check_header(elp_ctx* c, uint64_t ref_at, uint64_t hdr) {
     std::vector<uint8_t> h(hdr - ref_at);
     CUDA_TRY(c, cudaMemcpyAsync(h.data(), c->bam_raw.p + ref_at, h.size(), cudaMemcpyDeviceToHost, c->stream));
     CUDA_TRY(c, cudaStreamSynchronize(c->stream));
     const int32_t n_ref = (int32_t)rd32(h.data());
+    if (c->dict_mode) {
+        if (n_ref != c->n_in) return c->fail(E_INVAL, "elp_append_bgzf: the BAM header has %d reference sequences, the input dictionary (elp_set_input_dictionary) has %d", n_ref, c->n_in);
+        uint64_t x = 4;
+        for (int32_t k = 0; k < n_ref; k++) {
+            const uint32_t l_name = rd32(h.data() + x);
+            const char* name = reinterpret_cast<const char*>(h.data() + x + 4);
+            const int32_t l_ref = (int32_t)rd32(h.data() + x + 4 + l_name);
+            const std::string nm(name, l_name ? strnlen(name, l_name) : 0);
+            if (l_ref != c->in_len[k] || nm != c->in_tab[k])
+                return c->fail(E_INVAL, "elp_append_bgzf: reference %d of the BAM header is '%s' of length %d, the input dictionary (elp_set_input_dictionary) says '%s' of length %d",
+                               k, nm.c_str(), l_ref, c->in_tab[k].c_str(), c->in_len[k]);
+            x += 8ull + l_name;
+        }
+        return E_OK;
+    }
     if (n_ref != c->n_contigs) return c->fail(E_INVAL, "elp_append_bgzf: the BAM header has %d reference sequences, elp_config has %d contigs", n_ref, c->n_contigs);
     uint64_t x = 4;
     for (int32_t k = 0; k < n_ref; k++) {
@@ -250,7 +266,7 @@ static int frame_records(elp_ctx* c, uint64_t n, uint64_t* nrec, uint64_t* used)
     cudaStream_t s = c->stream;
     const uint64_t nseg = (n + SEG - 1) / SEG;
     TRY(grow(c, S.seg, 4 * nseg + 4, 0)); TRY(grow(c, S.seg_cnt, nseg + 8, 0)); TRY(grow(c, c->off_stage, nseg + 2, 0));
-    const Frame F{c->bam_raw.p, n, nseg, c->n_contigs};
+    const Frame F{c->bam_raw.p, n, nseg, ingest_ref_bound(c, false)};
     uint64_t *g0 = S.seg.p, *x0 = g0 + nseg, *g1 = x0 + nseg, *x1 = g1 + nseg;   // generation 0 and 1: guesses, then exits
     uint32_t* changed = reinterpret_cast<uint32_t*>(S.d_small.p);
     c->begin("bam_frame", (double)n);

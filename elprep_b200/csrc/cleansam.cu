@@ -79,11 +79,14 @@ extern "C" int elp_clean_sam(elp_ctx* c, uint64_t* n_rewritten) {
     const uint64_t n = c->n;
     if (!n) return ELP_OK;
     cudaStream_t s = c->stream;
+    // the LN CleanSam reads: elp_config's, or while elp_set_input_dictionary is set the input LN of the read's name (CleanSam runs before
+    // the replacement, cmd/filter.go:748-752), which the refid column reaches through d_clean_len
+    const int32_t* clen = c->dict_mode ? c->d_clean_len.p : c->d_contig_len.p;
     CUDA_TRY(c, c->scan_tmp.reserve(n + 8, s));
     uint32_t* d_changed = c->scan_tmp.p + n + 4;
     CUDA_TRY(c, cudaMemsetAsync(d_changed, 0, 4, s));
     c->begin("clean_sam_count", (double)n * 19 + (double)c->n_cigar * 4);
-    clean_count_kernel<<<nblk(n, 256), 256, 0, s>>>(n, c->flag.p, c->mapq.p, c->refid.p, c->pos.p, c->cigar_off.p, c->cigar.p, c->d_contig_len.p, c->n_contigs, c->scan_tmp.p, d_changed, c->d_err.p);
+    clean_count_kernel<<<nblk(n, 256), 256, 0, s>>>(n, c->flag.p, c->mapq.p, c->refid.p, c->pos.p, c->cigar_off.p, c->cigar.p, clen, c->n_contigs, c->scan_tmp.p, d_changed, c->d_err.p);
     c->end(); LAUNCH_CHECK(c);
     uint32_t changed = 0;
     CUDA_TRY(c, cudaMemcpyAsync(&changed, d_changed, 4, cudaMemcpyDeviceToHost, s));
@@ -101,7 +104,7 @@ extern "C" int elp_clean_sam(elp_ctx* c, uint64_t* n_rewritten) {
     CUDA_TRY(c, cudaStreamSynchronize(s));
     CUDA_TRY(c, new_cigar.reserve(std::max<uint64_t>(total + 16, c->cigar.cap), s));
     c->begin("clean_sam_write", (double)n * 26 + (double)c->n_cigar * 8);
-    clean_write_kernel<<<nblk(n, 256), 256, 0, s>>>(n, c->flag.p, c->refid.p, c->pos.p, c->cigar_off.p, c->cigar.p, c->d_contig_len.p, c->n_contigs, new_off.p, new_cigar.p, c->d_err.p);
+    clean_write_kernel<<<nblk(n, 256), 256, 0, s>>>(n, c->flag.p, c->refid.p, c->pos.p, c->cigar_off.p, c->cigar.p, clen, c->n_contigs, new_off.p, new_cigar.p, c->d_err.p);
     c->end(); LAUNCH_CHECK(c);
     CUDA_TRY(c, cudaStreamSynchronize(s));
     std::swap(c->cigar, new_cigar); std::swap(c->cigar_off, new_off);

@@ -188,6 +188,17 @@ struct elp_ctx {
     DBuf<uint32_t> out_sel; uint64_t n_out = 0; bool out_sel_valid = false;   // output positions of the records that pass, built on first use
     bool rg_replace = false;                 // --replace-read-group (elp_set_replace_read_group; survives elp_reset): every read is in @RG 0 and
                                              // the byte outputs write its RG field as RG:Z:rg_ids[0] (d_rg_names)
+    // --rename-chromosomes / --replace-reference-sequences (elp_set_input_dictionary; survives elp_reset).  elp_config holds the output
+    // dictionary; the input's @SQ (in_len, unrenamed) bounds the stored records' refID / next_refID.  The input name table is the input's
+    // names followed by the SAM extension (REPLACE only: the RNAME texts that reach a replacement entry without being an input name);
+    // d_remap[table index] is the output contig (-1: none), with one more entry, -1, for a SAM RNAME that reaches nothing under REPLACE.
+    uint32_t dict_mode = 0;                  // ELP_DICT_* bits; 0: off
+    std::vector<std::string> in_tab;         // the input name table as the file spells it (the extension included)
+    std::vector<int32_t> in_len;             // [n_in] LN of the input's @SQ
+    int n_in = 0;                            // input @SQ entries
+    DBuf<int32_t> d_remap;                   // [in_tab.size() + 1]
+    DBuf<int32_t> d_clean_len;               // [n_contigs] CleanSam's LN per output contig: the input LN of its name (last entry), else 0
+    NameDictBufs in_dict;                    // elp_append_sam's RNAME / RNEXT lookup over in_tab while dict_mode is set (built on first use)
     RegionTable regions;                     // --filter-non-overlapping-reads: the ingest filter ELP_FILTER_TARGET_REGIONS (elp_set_target_regions)
     RegionTable bqsr_regions;                // --target-regions: elp_filter_target_regions after marking (elp_set_bqsr_target_regions); both survive elp_reset
     uint64_t n_cleaned = 0;                  // reads whose CIGAR elp_clean_sam rewrote
@@ -369,9 +380,15 @@ int spread_exchange_begin(elp_ctx* c);
 int spread_exchange_end(elp_ctx* c);
 int exclusive_scan_u64_from_u32(elp_ctx* c, const uint32_t* in, uint64_t* out, uint64_t n, uint64_t base);   // out[n+1], out[0] = base
 int qual_presence_update(elp_ctx* c, uint64_t first_byte, uint64_t n_bytes);   // api.cu: called by both ingest paths
-int bam_ingest_core(elp_ctx* c, uint64_t n_bytes, uint64_t nrec);   // bam_ingest.cu: records staged in bam_raw / bam_off -> reads (elp_append_bam, elp_append_sam)
+int bam_ingest_core(elp_ctx* c, uint64_t n_bytes, uint64_t nrec, bool sam_records = false);   // bam_ingest.cu: records staged in bam_raw / bam_off -> reads (elp_append_bam, elp_append_sam)
+// elp_set_input_dictionary: the refID bound of the stored records (BAM: the input's @SQ; elp_append_sam's records: its name table and the
+// unreached-name entry), the remap table (null while off), and whether bam_keep_kernel runs (a record predicate or the REPLACE drop)
+inline int ingest_ref_bound(const elp_ctx* c, bool sam_records) { return c->dict_mode ? (sam_records ? (int)c->in_tab.size() + 1 : c->n_in) : c->n_contigs; }
+inline const int32_t* ingest_remap(const elp_ctx* c) { return c->dict_mode ? c->d_remap.p : nullptr; }
+inline bool ingest_keep_on(const elp_ctx* c) { return c->filter_mask || c->filter_min_mapq > 0 || (c->dict_mode & 2u /* ELP_DICT_REPLACE */); }
 int out_select(elp_ctx* c, const uint32_t** sel, uint64_t* n_out);
 int rg_names_upload(elp_ctx* c);   // bam_ingest.cu: @RG IDs -> d_rg_names / d_rg_name_off, once per context   // bam_ingest.cu: the record filters' selection (sel null and n_out = n_sorted without record bits)
+std::vector<std::string> sam_print_names(const elp_ctx* c);   // bam_ingest.cu: the names elp_fetch_sam prints for the stored refIDs
 int region_set(elp_ctx* c, RegionTable& t, const char* who, int32_t contig, const int32_t* se, uint64_t n_intervals, int already_flat);   // bam_ingest.cu
 int build_output_columns(elp_ctx* c, const uint32_t* perm, uint64_t n_out, bool refilter);   // coordsort.cu: s_* columns and s_out_off of perm[0, n_out)
 int phase_target_filter(elp_ctx* c, uint64_t* n_removed);   // target_regions.cu

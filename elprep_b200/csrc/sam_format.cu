@@ -23,6 +23,7 @@ struct SamOutState {
     DBuf<uint8_t> d_names; DBuf<uint32_t> d_name_off; DBuf<int32_t> d_canon;   // @SQ names, and per contig the first index with its name
     DBuf<uint32_t> nf, fbits; DBuf<uint64_t> fbase, foff; DBuf<uint8_t> ftext;  // float values: count per line, slots, texts
     DBuf<unsigned long long> d_small;                                           // [0] error bits, [1] float values
+    int n_names = 0;                                                            // entries of d_name_off - 1
 };
 
 void free_state(SamOutState* S) { delete S; }
@@ -280,24 +281,28 @@ __global__ void __launch_bounds__(256) sam_out_flen_kernel(uint64_t n, const uin
     if (i < n) len[i] += (uint32_t)(foff[fbase[i] + nf[i]] - foff[fbase[i]]);
 }
 
-// @SQ names and their canon (first index with the same name), uploaded once per context
+// the names of the stored refIDs (sam_print_names: the @SQ names, or the input name table of elp_set_input_dictionary) and their canon
+// (first index with the same name), uploaded once per context and setting
 int sam_out_tables(elp_ctx* c) {
     if (c->sam_out) return E_OK;
     c->sam_out.reset(new SamOutState());
     SamOutState* S = c->sam_out.get();
-    std::vector<uint8_t> names; std::vector<uint32_t> off(1, 0); std::vector<int32_t> canon(c->n_contigs + 1, -1);
+    const std::vector<std::string> tab = sam_print_names(c);
+    const int nt = (int)tab.size();
+    std::vector<uint8_t> names; std::vector<uint32_t> off(1, 0); std::vector<int32_t> canon(nt + 1, -1);
     std::map<std::string, int32_t> first;
-    for (int i = 0; i < c->n_contigs; i++) {
-        const std::string& s = c->contig_names[i];
+    for (int i = 0; i < nt; i++) {
+        const std::string& s = tab[i];
         names.insert(names.end(), s.begin(), s.end()); off.push_back((uint32_t)names.size());
         canon[i] = first.emplace(s, i).first->second;
     }
     auto star = first.find("*");
-    if (star != first.end()) canon[c->n_contigs] = star->second;
+    if (star != first.end()) canon[nt] = star->second;
     CUDA_TRY(c, S->d_names.fit(std::max<size_t>(names.size(), 1)));
     CUDA_TRY(c, S->d_name_off.fit(off.size()));
     CUDA_TRY(c, S->d_canon.fit(canon.size()));
     CUDA_TRY(c, S->d_small.fit(2));
+    S->n_names = nt;
     CUDA_TRY(c, cudaMemcpy(S->d_names.p, names.data(), names.size(), cudaMemcpyHostToDevice));
     CUDA_TRY(c, cudaMemcpy(S->d_name_off.p, off.data(), off.size() * 4, cudaMemcpyHostToDevice));
     CUDA_TRY(c, cudaMemcpy(S->d_canon.p, canon.data(), canon.size() * 4, cudaMemcpyHostToDevice));
@@ -329,7 +334,7 @@ int sam_out_prepare(elp_ctx* c, uint64_t first, uint64_t n, const uint32_t* sel,
     FmtArgs A{};
     A.n = n; A.first = first; A.sel = sel; A.drop = c->out_fields ? c->d_out_drop.p : nullptr; A.rg = rg_set(c); A.perm = c->perm.p; A.all_start = c->bam_all_off.p; A.all = c->bam_all.p;
     A.flag = c->s_flag.p; A.mapq = c->s_mapq.p; A.qoff = c->s_out_off.p; A.qual = c->qual_out_valid ? c->qual_out.p : nullptr;
-    A.names = S.d_names.p; A.name_off = S.d_name_off.p; A.canon = S.d_canon.p; A.n_contigs = c->n_contigs;
+    A.names = S.d_names.p; A.name_off = S.d_name_off.p; A.canon = S.d_canon.p; A.n_contigs = S.n_names;
     A.len = c->scan_tmp.p; A.nf = S.nf.p; A.small = S.d_small.p;
     CUDA_TRY(c, cudaMemsetAsync(S.d_small.p, 0, 16, s));
     c->begin("sam_out_measure", (double)c->n_bam * (double)n / (double)std::max<uint64_t>(c->n, 1));

@@ -67,7 +67,8 @@ const char* sam_err_text(uint32_t e) {
 // ---- the line parser ----
 struct SamArgs {
     const uint8_t* text; const uint64_t* ls; uint64_t n_lines;
-    NameDict dict;             // "*" and @SQ SN, sorted, with their refid
+    NameDict dict;             // "*" and @SQ SN, sorted, with their refid (the input name table while elp_set_input_dictionary is set)
+    int32_t unreached_ref;     // refID of an RNAME that is neither "*" nor in dict: -1, or under REPLACE the entry whose remap drops the read
     uint32_t* len;             // measure: BAM record length per line
     uint8_t* lost;             // measure: 1 if the record loses the line's RNAME / RNEXT text
     const uint64_t* rec_off;   // emit: record offsets in out
@@ -322,7 +323,8 @@ template <bool W> __device__ int parse_line(const SamArgs& A, uint64_t k, const 
     else if (beg >> 20 == end >> 20) bin = 73u + (uint32_t)(beg >> 20);
     else if (beg >> 23 == end >> 23) bin = 9u + (uint32_t)(beg >> 23);
     else if (beg >> 26 == end >> 26) bin = 1u + (uint32_t)(beg >> 26);
-    put<W>(o, (uint32_t)(rec - 4), 4); put<W>(o + 4, (uint32_t)refid, 4); put<W>(o + 8, (uint32_t)beg, 4);
+    const int32_t rid = (refid < 0 && !rname_star) ? A.unreached_ref : refid;
+    put<W>(o, (uint32_t)(rec - 4), 4); put<W>(o + 4, (uint32_t)rid, 4); put<W>(o + 8, (uint32_t)beg, 4);
     put<W>(o + 12, (uint32_t)(lq + 1) | ((uint32_t)mapq << 8) | ((bin & 0xffff) << 16), 4);
     put<W>(o + 16, ncig | ((uint32_t)flag << 16), 4); put<W>(o + 20, (uint32_t)L, 4); put<W>(o + 24, (uint32_t)nref, 4);
     put<W>(o + 28, (uint32_t)pnext - 1u, 4); put<W>(o + 32, (uint32_t)tlen, 4);
@@ -368,11 +370,12 @@ __global__ void __launch_bounds__(256) sam_fpatch_kernel(uint64_t n, const uint6
     if (i < n) for (int b = 0; b < 4; b++) out[off[i] + b] = (uint8_t)(bits[i] >> (8 * b));
 }
 
-// the RNAME / RNEXT dictionary and the error words, uploaded once per context
+// the RNAME / RNEXT dictionary (elp_config's names, or the input name table of elp_set_input_dictionary) and the error words, uploaded
+// once per context and setting
 int sam_tables(elp_ctx* c) {
     if (!c->sam) c->sam.reset(new SamState());
     CUDA_TRY(c, c->sam->d_small.fit(3));
-    return name_dict_upload(c);
+    return c->dict_mode ? name_dict_build(c, c->in_dict, c->in_tab) : name_dict_upload(c);
 }
 
 // strconv.ParseFloat(s, 32) for a decimal the device already checked: strtof rounds correctly; only overflow is an error in Go
@@ -424,7 +427,8 @@ extern "C" int elp_append_sam(elp_ctx* c, const char* text, uint64_t n_bytes) {
     // measure: validate every line and size its record
     SamArgs A{};
     A.text = S.text.p; A.ls = S.ls.p; A.n_lines = nl;
-    A.dict = c->names.view();
+    A.dict = c->dict_mode ? c->in_dict.view() : c->names.view();
+    A.unreached_ref = (c->dict_mode & ELP_DICT_REPLACE) ? (int32_t)c->in_tab.size() : -1;
     A.len = S.len.p; A.lost = S.lost.p; A.rec_off = c->bam_off.p; A.small = S.d_small.p;
     CUDA_TRY(c, cudaMemsetAsync(S.d_small.p, 0xff, 8, s)); CUDA_TRY(c, cudaMemsetAsync(S.d_small.p + 1, 0, 16, s));
     c->begin("sam_measure", (double)n_bytes);
@@ -467,9 +471,9 @@ extern "C" int elp_append_sam(elp_ctx* c, const char* text, uint64_t n_bytes) {
         CUDA_TRY(c, cudaStreamSynchronize(s));   // (po / pb are pageable host memory)
     }
     const uint64_t n0 = c->n;
-    TRY(bam_ingest_core(c, total, nl));
+    TRY(bam_ingest_core(c, total, nl, true));
     uint64_t lost = small[2];
-    if (lost && (c->filter_mask || c->filter_min_mapq > 0)) {   // count only the lines the filters kept (bam_start: their record starts)
+    if (lost && ingest_keep_on(c)) {   // count only the lines the filters kept (bam_start: their record starts)
         const uint64_t nk = c->n - n0;
         CUDA_TRY(c, cudaMemsetAsync(S.d_small.p + 2, 0, 8, s));
         if (nk) { sam_lost_kept_kernel<<<nblk(nk, 256), 256, 0, s>>>(nk, c->bam_start.p, c->bam_off.p, nl, S.lost.p, S.d_small.p + 2); c->launches++; LAUNCH_CHECK(c); }

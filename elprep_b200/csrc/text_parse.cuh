@@ -82,13 +82,12 @@ __device__ __forceinline__ int32_t refid_of(const NameDict& D, const uint8_t* s,
     return e < 0 ? -1 : D.id[e];
 }
 
-// the dictionary of the context's elp_config.contig_names (c->names), uploaded with blocking copies on first use
-int name_dict_upload(elp_ctx* c) {
-    NameDictBufs& D = c->names;
+// the dictionary of the names src (index = refid) into D, uploaded with blocking copies on first use
+int name_dict_build(elp_ctx* c, NameDictBufs& D, const std::vector<std::string>& src) {
     if (D.n) return E_OK;
     std::map<std::string, std::vector<int32_t>> dict;
     dict["*"];
-    for (int i = 0; i < c->n_contigs; i++) dict[c->contig_names[i]].push_back(i);
+    for (int i = 0; i < (int)src.size(); i++) dict[src[i]].push_back(i);
     std::vector<uint8_t> names; std::vector<uint32_t> off(1, 0), all_off(1, 0); std::vector<int32_t> id, all;
     for (auto& kv : dict) {
         names.insert(names.end(), kv.first.begin(), kv.first.end()); off.push_back((uint32_t)names.size());
@@ -109,5 +108,7 @@ int name_dict_upload(elp_ctx* c) {
     D.n = (int)id.size();
     return E_OK;
 }
+// the dictionary of the context's elp_config.contig_names (c->names)
+int name_dict_upload(elp_ctx* c) { return name_dict_build(c, c->names, c->contig_names); }
 
 }  // namespace

@@ -180,6 +180,15 @@ class Context:
         fetch_sam write each record as aln.SetRG(id) leaves it.  Only while the context holds no reads; survives reset()."""
         self._ck(self.L.elp_set_replace_read_group(self.h, int(bool(on))))
 
+    def set_input_dictionary(self, mode, names=(), lengths=()):
+        """`--rename-chromosomes` (_lib.DICT_RENAME_CHROMOSOMES) and `--replace-reference-sequences` (_lib.DICT_REPLACE) on the byte paths
+        (elp_set_input_dictionary): the context was created from the header after filters.RenameChromosomes and / or
+        ReplaceReferenceSequenceDictionary; names / lengths are the input file's @SQ as it stands in the file.  Ingest remaps refid / nref
+        to the context's contigs and, with REPLACE, drops the reads whose RNAME has no new entry; fetch_bam / fetch_bgzf write the new ids,
+        fetch_sam the (renamed) names.  mode 0 turns it off.  Only while the context holds no reads; survives reset()."""
+        lens = np.ascontiguousarray(lengths, dtype=np.int32).reshape(-1)
+        self._ck(self.L.elp_set_input_dictionary(self.h, int(mode), _cstrs(list(names)), _vp(lens) if lens.size else None, len(names)))
+
     def n_output(self):
         """output records fetch_bam / fetch_sam write (those that pass the record filters of set_output_filter); 0 before sort_markdup"""
         return int(self.L.elp_n_output(self.h))

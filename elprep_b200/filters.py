@@ -193,6 +193,75 @@ def AddOrReplaceReadGroup(readGroup):
     return flt
 
 
+def RenameChromosomes(header):
+    """filters.RenameChromosomes (filters/simple-filters.go:189-204), `--rename-chromosomes`: every @SQ with an SN gets "chr" + SN.  The
+    refid / nref columns index the dictionary, so the AlignmentFilter has nothing to change on the columnar path (the RNAME / RNEXT texts
+    it prefixes exist only in the byte outputs).  On the byte paths the device does it (Context.set_input_dictionary with
+    _lib.DICT_RENAME_CHROMOSOMES, the context created from the header after this filter)."""
+    for e in header.SQ:
+        if "SN" in e:
+            e["SN"] = "chr" + e["SN"]
+    return None
+
+
+def _find_sn(sq, sn):
+    """utils.Find (utils/utils.go:26-33) over a dictionary by SN: the first match, or -1"""
+    for i, e in enumerate(sq):
+        if e.get("SN", "") == sn:
+            return i
+    return -1
+
+
+def dictionary_remap(old_names, new_names):
+    """old @SQ index -> new @SQ index, as AddREFID reaches it after ReplaceReferenceSequenceDictionary: the last new entry with the old
+    entry's name, or -1 (the read is dropped when it is its RNAME, and its RNEXT becomes -1).  The table elp_set_input_dictionary builds
+    from the (renamed) input names and the replacement."""
+    last = {}
+    for j, n in enumerate(new_names):
+        last[n] = j
+    return np.array([last.get(n, -1) for n in old_names], dtype=np.int32).reshape(-1)
+
+
+def ReplaceReferenceSequenceDictionary(dict_):
+    """filters.ReplaceReferenceSequenceDictionary (filters/simple-filters.go:34-60), `--replace-reference-sequences`: dict_ is the new @SQ
+    list.  With SO:coordinate the SO becomes unknown when the new entries found in the old dictionary (utils.Find: the first match) do
+    not appear in increasing old position.  header.SQ becomes dict_; a read is kept iff its RNAME is "*" or an SN of dict_.  On the
+    columnar path the AlignmentFilter remaps the refid / nref columns as AddREFID does after it (dictionary_remap) and drops the reads
+    whose refid has no new entry.  On the byte paths the device does it (Context.set_input_dictionary with _lib.DICT_REPLACE)."""
+    new = [dict(e) for e in dict_]
+
+    def flt(header):
+        if header.HD.get("SO") == sam.Coordinate:
+            prev = -1
+            for e in new:
+                p = _find_sn(header.SQ, e.get("SN", ""))
+                if p >= 0:
+                    if p > prev:
+                        prev = p
+                    else:
+                        header.SetHDSO(sam.Unknown)
+                        break
+        remap = dictionary_remap([e.get("SN", "") for e in header.SQ], [e.get("SN", "") for e in new])
+        header.SQ = [dict(e) for e in new]
+
+        tab = np.append(remap, -1).astype(np.int32)     # (refid -1 indexes the appended -1)
+
+        def replace(batch):
+            r = batch.refid.astype(np.int64)
+            batch.refid, batch.nref = tab[r], tab[batch.nref.astype(np.int64)]
+            return _keep(batch, (r < 0) | (batch.refid >= 0))
+        return replace
+    return flt
+
+
+def ReplaceReferenceSequenceDictionaryFromSamFile(path):
+    """filters.ReplaceReferenceSequenceDictionaryFromSamFile (filters/simple-filters.go:65-69): the @SQ lines of a SAM file or a .dict
+    (a SAM header), parsed by sam.parse_sam_header, as the new dictionary"""
+    with open(path, "rb") as f:
+        header, _ = sam.parse_sam_header(f.read())
+    return ReplaceReferenceSequenceDictionary(header.SQ)
+
+
 def write_phase_filters(removeDuplicates=False, removeOptionalFields="", keepOptionalFields="", header_has_sr=False):
     """the write-phase flags of `elprep filter` as the arguments of Context.set_output_filter / elp_set_output_filter -> (mask, remove, keep),
     as cmd/filter.go:803-902 builds them: RemoveOptionalReads iff the header has @sr (the caller drops @sr from the header it writes);

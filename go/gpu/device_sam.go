@@ -388,6 +388,29 @@ func (d *DeviceSam) SetReplaceReadGroup(on bool) {
 	check(d.ctx, C.elp_set_replace_read_group(d.ctx, C.int(v)))
 }
 
+// The modes of SetInputDictionary (ELP_DICT_RENAME_CHROMOSOMES, ELP_DICT_REPLACE).
+const (
+	DictRenameChromosomes uint32 = 1
+	DictReplace           uint32 = 2
+)
+
+// SetInputDictionary: --rename-chromosomes (DictRenameChromosomes) and --replace-reference-sequences (DictReplace) on the
+// byte paths.  Create the DeviceSam from the header after filters.RenameChromosomes / ReplaceReferenceSequenceDictionary and pass the input
+// file's @SQ as it stands in the file: the appends remap RNAME / RNEXT to the new dictionary as AddREFID would and, with REPLACE, drop the
+// reads whose RNAME it lacks; FetchBgzf and the other byte fetches write the new refIDs, or the (renamed) names in SAM text.  Call it
+// before the first append, or after a reset; mode 0 turns it off.  The columnar AddNodes path runs the reference's own filters instead.
+func (d *DeviceSam) SetInputDictionary(mode uint32, input []utils.StringMap) {
+	names := make([]string, len(input))
+	lens := make([]C.int32_t, len(input)+1)
+	for i, sq := range input {
+		names[i] = sq["SN"]
+		lens[i] = C.int32_t(sam.SQLN(sq))
+	}
+	cNames, free := cstrings(names, nil)
+	defer free()
+	check(d.ctx, C.elp_set_input_dictionary(d.ctx, C.uint32_t(mode), cNames, &lens[0], C.int32_t(len(input))))
+}
+
 // SetReference / SetKnownSites: the side inputs of filters.NewBaseRecalibrator (bqsr.go:424-443).
 func (d *DeviceSam) SetReference(contig int, bases []byte) {
 	check(d.ctx, C.elp_set_reference(d.ctx, C.int32_t(contig), (*C.uint8_t)(unsafe.Pointer(&bases[0])), C.uint64_t(len(bases))))

@@ -423,6 +423,33 @@ int elp_set_output_filter(elp_ctx *ctx, uint32_t mask, const char *const *remove
  *    caller's, as the prefix of elp_fetch_bgzf.
  *  - The columnar elp_fetch is unchanged: a columnar caller owns its *Alignments and sets RG itself. */
 int elp_set_replace_read_group(elp_ctx *ctx, int on);
+/* `--rename-chromosomes` and `--replace-reference-sequences dict`: filters.RenameChromosomes (filters/simple-filters.go:189-204) and
+ * ReplaceReferenceSequenceDictionary (:34-60), followed by AddREFID (:208-231), on the byte paths.  The context is created from the header
+ * after the filters: elp_config's contig_names / contig_lengths are the output @SQ (RENAME alone: the input's with "chr" prefixed; REPLACE:
+ * the replacement dictionary as read).  Everything keyed by contig -- the reference, the known sites, both target-region tables, the sort,
+ * duplicate marking, BQSR, elp_comm_set_partition -- works on the output contigs.  names / lengths: the input file's @SQ as it stands in the
+ * file, unrenamed (BAM / BGZF: its binary reference list).  mode = 0 turns the setting off.
+ *  - Refusals.  ELP_EINVAL for unknown mode bits, n < 0, a context without contig_names, and, with RENAME alone, n != n_contigs or a
+ *    contig_names[i] other than "chr" + names[i].  ELP_ESTATE while the context holds reads or a BGZF file is open.  The setting survives
+ *    elp_reset.
+ *  - The remap.  Input entry i goes to the last output entry whose name equals its (renamed) name, or nowhere; without REPLACE to i.
+ *  - Ingest (elp_append_bam, elp_append_sam, elp_append_bgzf).  refID / next_refID are bounded by the input's entry count, and
+ *    elp_append_bgzf checks the BAM header's reference list against names / lengths.  With REPLACE a read whose refID >= 0 has no output
+ *    entry is dropped (counted in elp_n_filtered), after the other ingest filters; ELP_FILTER_TARGET_REGIONS looks up the output contig of
+ *    a read's refID (elp_set_target_regions stays indexed by output contig; resolve BED names through the input names).  The refid / nref
+ *    columns hold the output contigs (-1 for none); the stored records keep the input's bytes.  elp_append_sam resolves RNAME / RNEXT
+ *    against the input names; with REPLACE also against the replacement names no input name reaches (under RENAME spelled without "chr"),
+ *    and an RNAME that reaches nothing drops the read, as the reference drops it.
+ *  - elp_clean_sam uses per read the input LN of its name (the last input entry with that name, 0 for a name outside the input), as
+ *    CleanSam runs before the replacement.  This holds on every ingest path; elp_append_batch is otherwise unchanged (the caller's
+ *    marshaller remaps refid / nref and drops reads on the host).
+ *  - Egress.  elp_fetch_bam, elp_fetch_bam_bytes and elp_fetch_bgzf write refID and next_refID (bytes 4-7 and 24-27) as the output contig,
+ *    -1 where there is none; bin, PNEXT and everything else are as without the setting.  elp_fetch_sam prints RNAME / RNEXT by the input
+ *    name table ("chr" prefixed under RENAME), so an RNEXT outside the new dictionary keeps its (renamed) name, as in the reference.  The
+ *    header bytes (the new @SQ lines and SO) are the caller's, as the prefix of elp_fetch_bgzf. */
+#define ELP_DICT_RENAME_CHROMOSOMES 1u   /* --rename-chromosomes */
+#define ELP_DICT_REPLACE            2u   /* --replace-reference-sequences */
+int elp_set_input_dictionary(elp_ctx *ctx, uint32_t mode, const char *const *names, const int32_t *lengths, int32_t n);
 /* after elp_sort_markdup: the number of records of the output order (elp_n_sorted) that pass the record filters (elp_n_sorted without them);
  * 0 on error or before the sort */
 uint64_t elp_n_output(elp_ctx *ctx);

@@ -14,6 +14,8 @@
 //   (*sam.Sam).RunPipeline as PipelineInput (filter-pipeline.go:242-279)   DeviceSam::RunPipeline(sink)
 //   sam.ParseHeaderLineFromString (sam/sam-files.go:153-177)       elprep::ParseHeaderLineFromString
 //   filters.AddOrReplaceReadGroup (filters/simple-filters.go:154-162)   elprep::AddOrReplaceReadGroup, DeviceSam::SetReplaceReadGroup (byte paths)
+//   filters.RenameChromosomes (filters/simple-filters.go:189-204)   elprep::RenameChromosomes, DeviceSam::SetInputDictionary (byte paths)
+//   filters.ReplaceReferenceSequenceDictionary (:34-60)             elprep::ReplaceReferenceSequenceDictionary, DeviceSam::SetInputDictionary (byte paths)
 //   log.Panic(msg)                                                  throw elprep::Panic(msg)
 #pragma once
 #include <algorithm>
@@ -48,6 +50,7 @@ struct Header {
     struct SQ { std::string SN; int32_t LN; };
     struct ReadGroup { std::string ID, LB, PU; bool hasLB = false, hasPU = false; };
     std::vector<SQ> sq; std::vector<ReadGroup> rg;
+    std::string SO;                    // @HD SO ("" without one); ReplaceReferenceSequenceDictionary may set it to "unknown"
 };
 
 // sam.ParseHeaderLineFromString (sam/sam-files.go:153-177), the parser of `--replace-read-group`: TG:value fields separated by white space
@@ -113,6 +116,42 @@ struct AddOrReplaceReadGroup {
     }
     void operator()(Alignment& a) const { a.RG = id; a.hasRG = true; }
     void operator()(std::vector<Alignment>& batch) const { for (Alignment& a : batch) (*this)(a); }
+};
+
+// filters.RenameChromosomes (filters/simple-filters.go:189-204), `--rename-chromosomes`.  The constructor is the header part: every @SQ SN
+// becomes "chr" + SN; build DeviceSam from that header.  operator() is the AlignmentFilter: RNAME and RNEXT get the prefix unless they are
+// "=" or "*"; apply it to every batch before AddNodes marshals it.  On the byte paths call DeviceSam::SetInputDictionary instead.
+struct RenameChromosomes {
+    explicit RenameChromosomes(Header& header) { for (Header::SQ& e : header.sq) e.SN = "chr" + e.SN; }
+    bool operator()(Alignment& a) const {
+        if (a.RNAME != "=" && a.RNAME != "*") a.RNAME = "chr" + a.RNAME;
+        if (a.RNEXT != "=" && a.RNEXT != "*") a.RNEXT = "chr" + a.RNEXT;
+        return true;
+    }
+};
+
+// filters.ReplaceReferenceSequenceDictionary (filters/simple-filters.go:34-60), `--replace-reference-sequences`.  The constructor is the
+// header part: with SO coordinate the SO becomes "unknown" when the new entries found in the old dictionary (utils.Find: the first match)
+// do not appear in increasing old position; header.sq becomes dict.  operator() is the AlignmentFilter: a read is kept iff its RNAME is
+// "*" or an SN of dict.  On the byte paths call DeviceSam::SetInputDictionary instead.
+struct ReplaceReferenceSequenceDictionary {
+    std::map<std::string, bool> names;
+    ReplaceReferenceSequenceDictionary(Header& header, const std::vector<Header::SQ>& dict) {
+        if (header.SO == "coordinate") {
+            int previous = -1;
+            for (const Header::SQ& e : dict) {
+                int pos = -1;
+                for (size_t i = 0; i < header.sq.size() && pos < 0; i++) if (header.sq[i].SN == e.SN) pos = (int)i;
+                if (pos < 0) continue;
+                if (pos > previous) previous = pos;
+                else { header.SO = "unknown"; break; }
+            }
+        }
+        names["*"] = true;
+        for (const Header::SQ& e : dict) names[e.SN] = true;
+        header.sq = dict;
+    }
+    bool operator()(const Alignment& a) const { return names.count(a.RNAME) != 0; }
 };
 
 enum class SortingOrder { Keep = ELP_SO_KEEP, Unknown = ELP_SO_UNKNOWN, Unsorted = ELP_SO_UNSORTED, Queryname = ELP_SO_QUERYNAME, Coordinate = ELP_SO_COORDINATE };
@@ -220,6 +259,14 @@ class DeviceSam {
     // --replace-read-group on the byte paths (elp_set_replace_read_group): every read of AppendBgzf is in the header's one @RG, and FetchBgzf
     // writes each record as AddOrReplaceReadGroup leaves it; before the first append (or after a reset)
     void SetReplaceReadGroup(bool on) { check(elp_set_replace_read_group(ctx_, on ? 1 : 0)); }
+    // --rename-chromosomes / --replace-reference-sequences on the byte paths (elp_set_input_dictionary, mode of ELP_DICT_*): the DeviceSam
+    // was built from the header after RenameChromosomes / ReplaceReferenceSequenceDictionary, input is the file's @SQ before them; AppendBgzf
+    // remaps and drops as the filters do and FetchBgzf writes the new refIDs.  Before the first append (or after a reset); mode 0 turns it off
+    void SetInputDictionary(uint32_t mode, const std::vector<Header::SQ>& input) {
+        std::vector<const char*> names; std::vector<int32_t> lens;
+        for (const Header::SQ& e : input) { names.push_back(e.SN.c_str()); lens.push_back(e.LN); }
+        check(elp_set_input_dictionary(ctx_, mode, names.data(), lens.data(), (int32_t)input.size()));
+    }
     // the Finalize of AddNodes: By(CoordinateLess / QNAMELess).ParallelStableSort + filters.MarkDuplicates (+ MarkOpticalDuplicates)
     void Finalize(SortingOrder order) { check(elp_sort_markdup(ctx_, (int)order, opts_.MarkDuplicates ? (opts_.AlsoOpticals ? ELP_MARKDUP_OPTICAL : ELP_MARKDUP) : 0)); }
 
