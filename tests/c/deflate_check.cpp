@@ -1,11 +1,14 @@
-// CPU check of the device DEFLATE encoder: elprep_b200/csrc/deflate.cuh, compiled here as host C++ (a team of one lane).  Every stream it
-// writes must inflate back to its input with zlib (inflateInit2(-15) + inflate(Z_FINISH): Z_STREAM_END with exactly the input's length) and
-// with the project's own decoder (inflate.cuh), every Huffman code it emits must be complete, and every stream must fit the stored bound.
+// CPU check of the device DEFLATE encoder: elprep_b200/csrc/deflate.cuh, compiled here as host C++ (a team of one lane), over the corpus of
+// deflate_corpus.hpp.  Every stream it writes must inflate back to its input with zlib (inflateInit2(-15) + inflate(Z_FINISH): Z_STREAM_END
+// with exactly the input's length) and with the project's own decoder (inflate.cuh), every Huffman code it emits must be complete, and every
+// stream must fit the stored bound.
 // Built with -fsanitize=address,undefined: input and output are heap buffers of exactly the sizes the encoder may touch.
 //
 //   deflate_check                      the corpus; prints OK
 //   deflate_check deflate IN OUT EOF   IN as BGZF (0xff00-byte blocks, the framing of elp_fetch_bgzf; EOF 1: with the EOF marker) into OUT
 //   deflate_check size IN              the bytes of the raw DEFLATE streams of IN's 0xff00-byte blocks
+//   deflate_check dump DIR             every input of the corpus (deflate_corpus.hpp) as DIR/NNNN.bin, and DIR/names.txt: "NNNN.bin<TAB>name"
+//                                      per line; the device test sends them through the device encoder
 #include <zlib.h>
 #include <algorithm>
 #include <cstdio>
@@ -15,6 +18,7 @@
 #include <string>
 #include <vector>
 #include "deflate.cuh"
+#include "deflate_corpus.hpp"
 
 static int n_streams = 0, n_stored = 0, failures = 0;
 static std::mt19937_64 rng(20261017);
@@ -76,59 +80,6 @@ static void check(const std::string& what, const std::vector<uint8_t>& d) {
     std::free(ib); std::free(ob);
 }
 
-// ---- data ----
-static std::vector<uint8_t> random_bytes(size_t n) { std::vector<uint8_t> v(n); for (auto& b : v) b = (uint8_t)rng(); return v; }
-static std::vector<uint8_t> periodic(size_t n, int k) { auto p = random_bytes(k); std::vector<uint8_t> v(n); for (size_t i = 0; i < n; i++) v[i] = p[i % k]; return v; }
-static std::vector<uint8_t> bam_like(size_t n) {
-    std::vector<uint8_t> v;
-    int i = 0;
-    while (v.size() < n) {
-        char name[64]; const int ln = std::snprintf(name, sizeof name, "HWI-ST1234:8:1101:%d:%d", 1000 + (int)(rng() % 20000), i++);
-        const int lseq = 100 + (int)(rng() % 51);
-        const int bs = 32 + ln + 1 + 4 + (lseq + 1) / 2 + lseq + 7;
-        auto put32 = [&](uint32_t x) { for (int k = 0; k < 4; k++) v.push_back((uint8_t)(x >> (8 * k))); };
-        put32(bs); put32(rng() % 3); put32((uint32_t)(rng() % 1000000)); v.push_back((uint8_t)(ln + 1)); v.push_back(60); v.push_back(0); v.push_back(0);
-        v.push_back(1); v.push_back(0); v.push_back(99); v.push_back(0); put32(lseq); put32(0); put32((uint32_t)(rng() % 1000000)); put32(300);
-        v.insert(v.end(), name, name + ln); v.push_back(0);
-        put32((uint32_t)lseq << 4);
-        for (int k = 0; k < (lseq + 1) / 2; k++) v.push_back((uint8_t)(0x11 << (rng() % 4)));
-        for (int k = 0; k < lseq; k++) v.push_back((uint8_t)(30 + rng() % 12));
-        v.push_back('R'); v.push_back('G'); v.push_back('Z'); v.push_back('r'); v.push_back('g'); v.push_back('1'); v.push_back(0);
-    }
-    v.resize(n);
-    return v;
-}
-// literals only: no 3-byte string occurs twice (a de Bruijn-like walk over distinct triples)
-static std::vector<uint8_t> no_repeats(size_t n) {
-    std::vector<uint8_t> v;
-    std::vector<uint8_t> seen(1 << 24, 0);
-    v.push_back(0); v.push_back(0);
-    while (v.size() < n) {
-        const size_t m = v.size();
-        int b = -1;
-        for (int t = 0; t < 256 && b < 0; t++) {
-            const int c = (int)((rng() + t) & 255);
-            const uint32_t k = (uint32_t)v[m - 2] | (uint32_t)v[m - 1] << 8 | (uint32_t)c << 16;
-            if (!seen[k]) { seen[k] = 1; b = c; }
-        }
-        if (b < 0) break;
-        v.push_back((uint8_t)b);
-    }
-    v.resize(std::min(v.size(), n));
-    return v;
-}
-// Fibonacci symbol frequencies: an unlimited Huffman code would need far more than 15 bits
-static std::vector<uint8_t> fibonacci(size_t n, int nsym) {
-    std::vector<uint64_t> f(nsym); f[0] = 1; f[1] = 1;
-    for (int s = 2; s < nsym; s++) f[s] = f[s - 1] + f[s - 2];
-    std::vector<uint8_t> v;
-    for (int s = nsym - 1; s >= 0 && v.size() < n; s--) for (uint64_t k = 0; k < f[s] && v.size() < n; k++) v.push_back((uint8_t)(s * 7 + 1));
-    for (int s = 0; s < nsym; s++) v.push_back((uint8_t)(s * 7 + 1));   // every symbol at least once
-    v.resize(std::min(v.size(), n));
-    std::shuffle(v.begin(), v.end(), rng);                              // (scattered: literals, not one long match)
-    return v;
-}
-
 // ---- BGZF framing, as bgzf_deflate.cu frames its blocks ----
 static const uint8_t BGZF_HDR[18] = {0x1f, 0x8b, 0x08, 0x04, 0, 0, 0, 0, 0x00, 0xff, 0x06, 0x00, 0x42, 0x43, 0x02, 0x00, 0, 0};
 static const uint8_t BGZF_EOF[28] = {0x1f, 0x8b, 0x08, 0x04, 0, 0, 0, 0, 0x00, 0xff, 0x06, 0x00, 0x42, 0x43, 0x02, 0x00, 0x1b, 0x00, 0x03, 0x00, 0, 0, 0, 0, 0, 0, 0, 0};
@@ -142,6 +93,11 @@ static std::vector<uint8_t> read_file(const char* path) {
     while ((k = std::fread(buf, 1, sizeof buf, f)) > 0) v.insert(v.end(), buf, buf + k);
     std::fclose(f);
     return v;
+}
+
+static void write_file(const char* path, const std::vector<uint8_t>& v) {
+    FILE* f = std::fopen(path, "wb");
+    if (!f || (!v.empty() && std::fwrite(v.data(), 1, v.size(), f) != v.size()) || std::fclose(f) != 0) { std::perror(path); std::exit(2); }
 }
 
 int main(int argc, char** argv) {
@@ -160,9 +116,7 @@ int main(int argc, char** argv) {
             put32(out, (uint32_t)blk.size());
         }
         if (std::atoi(argv[4])) out.insert(out.end(), BGZF_EOF, BGZF_EOF + 28);
-        FILE* f = std::fopen(argv[3], "wb");
-        if (!f || std::fwrite(out.data(), 1, out.size(), f) != out.size()) { std::perror(argv[3]); return 2; }
-        std::fclose(f);
+        write_file(argv[3], out);
         return 0;
     }
     if (argc == 3 && !std::strcmp(argv[1], "size")) {
@@ -177,46 +131,22 @@ int main(int argc, char** argv) {
         std::printf("%llu\n", (unsigned long long)total);
         return failures ? 1 : 0;
     }
-    std::vector<std::pair<std::string, std::vector<uint8_t>>> data;
-    data.push_back({"empty", {}});
-    data.push_back({"one byte", {0x42}});
-    data.push_back({"two bytes", {0x42, 0x42}});
-    data.push_back({"three equal bytes", {7, 7, 7}});
-    data.push_back({"bam 0xff00", bam_like(0xff00)});
-    data.push_back({"bam 65535", bam_like(65535)});
-    for (size_t n : {1, 5, 100, 1000, 4097, 30000}) data.push_back({"bam " + std::to_string(n), bam_like(n)});
-    data.push_back({"random 0xff00", random_bytes(0xff00)});
-    data.push_back({"random 65535", random_bytes(65535)});
-    for (size_t n : {1, 2, 3, 10, 300}) data.push_back({"random " + std::to_string(n), random_bytes(n)});
-    data.push_back({"run 0xff00", std::vector<uint8_t>(0xff00, 'A')});
-    data.push_back({"run 259", std::vector<uint8_t>(259, 0)});
-    data.push_back({"run 65535", std::vector<uint8_t>(65535, 0xff)});
-    for (int k = 1; k <= 40; k++) data.push_back({"period " + std::to_string(k), periodic(4000 + 37 * k, k)});
-    for (int k : {255, 256, 257, 258, 259, 1000, 4095, 4096, 4097, 32767, 32768}) data.push_back({"period " + std::to_string(k), periodic(0xff00, k)});
-    {   // matches at distance exactly 32768, and one byte too far
-        auto a = random_bytes(32768); auto b = a; b.insert(b.end(), a.begin(), a.begin() + 0xff00 - 32768); data.push_back({"distance 32768", b});
-        auto c = random_bytes(32769); auto e = c; e.insert(e.end(), c.begin(), c.begin() + 0xff00 - 32769); data.push_back({"distance 32769", e});
+    if (argc == 3 && !std::strcmp(argv[1], "dump")) {
+        std::string names;
+        int k = 0;
+        corpus::for_each_input(rng, [&](corpus::DefKind, const std::string& name, const std::vector<uint8_t>& d) {
+            char file[32]; std::snprintf(file, sizeof file, "%04d.bin", k++);
+            write_file((std::string(argv[2]) + "/" + file).c_str(), d);
+            names += std::string(file) + "\t" + name + "\n";
+        });
+        write_file((std::string(argv[2]) + "/names.txt").c_str(), std::vector<uint8_t>(names.begin(), names.end()));
+        std::printf("%d inputs dumped\n", k);
+        return 0;
     }
-    data.push_back({"literals only", no_repeats(0xff00)});
-    {   // a single literal value, scattered among random bytes and alone
-        auto v = random_bytes(20000); for (size_t i = 0; i < v.size(); i += 2) v[i] = 'Q'; data.push_back({"one literal value in random", v});
-        std::vector<uint8_t> w(2, 'Z'); data.push_back({"one literal value, 2 bytes", w});
-    }
-    for (int nsym : {20, 24, 27}) data.push_back({"fibonacci " + std::to_string(nsym), fibonacci(0xff00, nsym)});
-    data.push_back({"fibonacci short", fibonacci(4000, 18)});
-    for (int t = 0; t < 60; t++) {                                    // mixtures: BAM-like records with random and repeated stretches
-        auto v = bam_like(rng() % 0xff01);
-        for (int k = 0; k < 4 && !v.empty(); k++) {
-            const size_t a = rng() % v.size(), l = std::min<size_t>(v.size() - a, rng() % 3000);
-            const int kind = (int)(rng() % 3);
-            for (size_t i = 0; i < l; i++) v[a + i] = kind == 0 ? (uint8_t)rng() : kind == 1 ? (uint8_t)'N' : v[a + (i % 7)];
-        }
-        data.push_back({"mixture " + std::to_string(t), v});
-    }
-    for (auto& [name, d] : data) check(name, d);
+    corpus::for_each_input(rng, [](corpus::DefKind, const std::string& name, const std::vector<uint8_t>& d) { check(name, d); });
     {   // the random blocks must take the stored path
         for (size_t n : {(size_t)0xff00, (size_t)65535}) {
-            const auto z = encode(random_bytes(n));
+            const auto z = encode(corpus::random_bytes(rng, n));
             if ((z[0] & 7) != 1 || z.size() != n + 5) { std::printf("FAIL random %zu: not stored\n", n); failures++; }
         }
     }

@@ -1,7 +1,13 @@
 // CPU check of the device DEFLATE decoder: elprep_b200/csrc/inflate.cuh, compiled here as host C++ (a team of one lane), against zlib
-// stream by stream.  For every stream: the same accept / reject decision as inflateInit2(-15) + inflate(Z_FINISH) into exactly ISIZE
-// bytes (what elp_bgzf_inflate accepts), and the same bytes on accept.  Built with -fsanitize=address,undefined: input and output are
-// heap buffers of exactly n_in and ISIZE bytes, so any read or write out of bounds stops the run.
+// stream by stream, over the corpus of inflate_corpus.hpp.  For every stream: the same accept / reject decision as inflateInit2(-15) +
+// inflate(Z_FINISH) into exactly ISIZE bytes (what elp_bgzf_inflate accepts), and the same bytes on accept.  Built with
+// -fsanitize=address,undefined: input and output are heap buffers of exactly n_in and ISIZE bytes, so any read or write out of bounds stops
+// the run.
+//
+//   inflate_check             the corpus and the per-lane CRC-32 fold; prints the counts and OK
+//   inflate_check dump FILE   the same checks, and writes to FILE every ZLIB, CRAFTED and EDGE stream and every 4th MUTATED one as records
+//                             of: u8 kind, u16 name length, name, u32 isize, u32 status of the team of one, u8 1 if zlib accepts, u32 stream
+//                             length, stream bytes (little-endian); the device test sends them through the device decoder
 #include <zlib.h>
 #include <cstdio>
 #include <cstdlib>
@@ -10,6 +16,7 @@
 #include <string>
 #include <vector>
 #include "inflate.cuh"
+#include "inflate_corpus.hpp"
 
 static int n_streams = 0, n_accept = 0, n_reject = 0, failures = 0;
 static std::mt19937_64 rng(12345);
@@ -27,7 +34,8 @@ static bool zlib_inflate(const std::vector<uint8_t>& in, uint32_t isize, std::ve
     return ok;
 }
 
-static void check(const char* what, const std::vector<uint8_t>& in, uint32_t isize) {
+// the decoder's status on one stream; *zok: zlib's verdict
+static uint32_t check(const std::string& what, const std::vector<uint8_t>& in, uint32_t isize, bool* zok_out) {
     n_streams++;
     std::vector<uint8_t> zout;
     const bool zok = zlib_inflate(in, isize, zout);
@@ -38,216 +46,44 @@ static void check(const char* what, const std::vector<uint8_t>& in, uint32_t isi
     const uint32_t st = dfl::inflate_stream(dfl::Serial{}, T, ib, (uint32_t)in.size(), ob, isize);
     const bool ok = st == dfl::OK;
     if (ok != zok || (ok && isize && std::memcmp(ob, zout.data(), isize) != 0)) {
-        if (failures < 20) std::printf("MISMATCH %s: n_in %zu isize %u zlib %s decoder %s (%s)\n", what, in.size(), isize, zok ? "accepts" : "rejects",
+        if (failures < 20) std::printf("MISMATCH %s: n_in %zu isize %u zlib %s decoder %s (%s)\n", what.c_str(), in.size(), isize, zok ? "accepts" : "rejects",
                                        ok ? "accepts" : "rejects", dfl::status_text(st));
         failures++;
     }
     (ok ? n_accept : n_reject)++;
     std::free(ib); std::free(ob);
+    *zok_out = zok;
+    return st;
 }
 
-static std::vector<uint8_t> zdeflate(const std::vector<uint8_t>& d, int level, int strategy, int flush_every = 0, int flush_kind = Z_SYNC_FLUSH) {
-    z_stream zs; std::memset(&zs, 0, sizeof zs);
-    deflateInit2(&zs, level, Z_DEFLATED, -15, 8, strategy);
-    std::vector<uint8_t> out(deflateBound(&zs, d.size()) + 64 + (flush_every ? 16 * (d.size() / flush_every + 2) : 0));
-    uint8_t dummy = 0;
-    zs.next_out = out.data(); zs.avail_out = (uInt)out.size();
-    size_t x = 0;
-    do {
-        const size_t step = flush_every ? std::min<size_t>(flush_every, d.size() - x) : d.size() - x;
-        zs.next_in = const_cast<Bytef*>(d.empty() ? &dummy : d.data() + x); zs.avail_in = (uInt)step;
-        x += step;
-        deflate(&zs, x == d.size() ? Z_FINISH : flush_kind);
-    } while (x < d.size());
-    out.resize(zs.total_out);
-    deflateEnd(&zs);
-    return out;
-}
+static void put(FILE* f, uint64_t v, int bytes) { for (int k = 0; k < bytes; k++) std::fputc((int)(v >> (8 * k)) & 255, f); }
 
-// ---- data ----
-static std::vector<uint8_t> random_bytes(size_t n) { std::vector<uint8_t> v(n); for (auto& b : v) b = (uint8_t)rng(); return v; }
-static std::vector<uint8_t> run_of(size_t n, uint8_t c) { return std::vector<uint8_t>(n, c); }
-static std::vector<uint8_t> periodic(size_t n, int k) { auto p = random_bytes(k); std::vector<uint8_t> v(n); for (size_t i = 0; i < n; i++) v[i] = p[i % k]; return v; }
-// BAM-like records: fixed fields, a QNAME, CIGAR, SEQ nibbles, QUAL, a few tags
-static std::vector<uint8_t> bam_like(size_t n) {
-    std::vector<uint8_t> v;
-    int i = 0;
-    while (v.size() < n) {
-        char name[64]; const int ln = std::snprintf(name, sizeof name, "HWI-ST1234:8:1101:%d:%d", 1000 + (int)(rng() % 20000), i++);
-        const int lseq = 100 + (int)(rng() % 51);
-        const int bs = 32 + ln + 1 + 4 + (lseq + 1) / 2 + lseq + 7;
-        auto put32 = [&](uint32_t x) { for (int k = 0; k < 4; k++) v.push_back((uint8_t)(x >> (8 * k))); };
-        put32(bs); put32(rng() % 3); put32((uint32_t)(rng() % 1000000)); v.push_back((uint8_t)(ln + 1)); v.push_back(60); v.push_back(0); v.push_back(0);
-        v.push_back(1); v.push_back(0); v.push_back(99); v.push_back(0); put32(lseq); put32(0); put32((uint32_t)(rng() % 1000000)); put32(300);
-        v.insert(v.end(), name, name + ln); v.push_back(0);
-        put32((uint32_t)lseq << 4);
-        for (int k = 0; k < (lseq + 1) / 2; k++) v.push_back((uint8_t)(0x11 << (rng() % 4)));
-        for (int k = 0; k < lseq; k++) v.push_back((uint8_t)(30 + rng() % 12));
-        v.push_back('R'); v.push_back('G'); v.push_back('Z'); v.push_back('r'); v.push_back('g'); v.push_back('1'); v.push_back(0);
+int main(int argc, char** argv) {
+    FILE* dump = nullptr;
+    if (argc == 3 && !std::strcmp(argv[1], "dump")) {
+        dump = std::fopen(argv[2], "wb");
+        if (!dump) { std::perror(argv[2]); return 2; }
+    } else if (argc != 1) {
+        std::fprintf(stderr, "usage: inflate_check [dump FILE]\n");
+        return 2;
     }
-    v.resize(n);
-    return v;
-}
-
-// ---- hand-built streams ----
-struct BitWriter {
-    std::vector<uint8_t> v; uint64_t acc = 0; int n = 0;
-    void put(uint32_t x, int k) { acc |= (uint64_t)x << n; n += k; while (n >= 8) { v.push_back((uint8_t)acc); acc >>= 8; n -= 8; } }
-    void put_rev(uint32_t code, int len) { uint32_t r = 0; for (int i = 0; i < len; i++) r |= ((code >> i) & 1u) << (len - 1 - i); put(r, len); }   // Huffman codes go MSB first
-    std::vector<uint8_t> done() { if (n) { v.push_back((uint8_t)acc); acc = 0; n = 0; } return v; }
-};
-// fixed-code symbol (RFC 1951 3.2.6)
-static void fixed_sym(BitWriter& w, int s) {
-    if (s < 144) w.put_rev(0x30 + s, 8); else if (s < 256) w.put_rev(0x190 + s - 144, 9); else if (s < 280) w.put_rev(s - 256, 7); else w.put_rev(0xc0 + s - 280, 8);
-}
-// a dynamic block header: HLIT, HDIST, HCLEN, the code-length code lengths in transmission order, then raw (bits, count) pairs
-static std::vector<uint8_t> dynamic_header(int hlit, int hdist, int hclen, const std::vector<int>& clens_in_order, const std::vector<std::pair<int, int>>& syms) {
-    BitWriter w;
-    w.put(1, 1); w.put(2, 2); w.put(hlit - 257, 5); w.put(hdist - 1, 5); w.put(hclen - 4, 4);
-    for (int i = 0; i < hclen; i++) w.put(clens_in_order[i], 3);
-    for (auto& s : syms) w.put(s.first, s.second);
-    for (int i = 0; i < 64; i++) w.put(0, 8);
-    return w.done();
-}
-
-static void crafted() {
-    const int order[19] = {16, 17, 18, 0, 8, 7, 9, 6, 10, 5, 11, 4, 12, 3, 13, 2, 14, 1, 15};
-    {   // block type 3
-        BitWriter w; w.put(1, 1); w.put(3, 2); w.put(0, 16); check("btype 3", w.done(), 0); check("btype 3 isize 1", BitWriter{}.done(), 1);
-    }
-    {   // HLIT > 286, HDIST > 30
-        std::vector<int> cl(19, 4);
-        check("hlit 287", dynamic_header(287, 1, 19, cl, {}), 10);
-        check("hlit 288", dynamic_header(288, 1, 19, cl, {}), 10);
-        check("hdist 31", dynamic_header(257, 31, 19, cl, {}), 10);
-        check("hdist 32", dynamic_header(257, 32, 19, cl, {}), 10);
-    }
-    {   // code-length code: over-subscribed, incomplete, empty
-        std::vector<int> over(19, 1); check("clen over-subscribed", dynamic_header(257, 1, 19, over, {}), 10);
-        std::vector<int> inc(19, 0); inc[0] = 2; check("clen incomplete", dynamic_header(257, 1, 19, inc, {}), 10);
-        std::vector<int> one(19, 0); one[3] = 1; check("clen single code", dynamic_header(257, 1, 19, one, {}), 10);
-        std::vector<int> none(19, 0); check("clen empty", dynamic_header(257, 1, 4, none, {}), 10);
-    }
-    {   // code-length code with lengths: symbols 0..15 -> 5 bits (16 codes), 16, 17, 18 -> 5 bits: 19 codes of length 5 = incomplete; use
-        // 18 of length 5 ... easier: all 19 symbols with lengths making a complete code: 13 of length 4 ... take 16 symbols of length 4
-        // (0..15) -- complete -- plus none for 16..18; then "repeat first" needs symbol 16, so: 0..14 length 4 (15 codes) + 16 length 5 + 17 length 5
-        std::vector<int> L(19, 0);
-        for (int s = 0; s < 15; s++) L[s] = 4;
-        L[16] = 5; L[17] = 5;
-        std::vector<int> inorder(19); for (int i = 0; i < 19; i++) inorder[i] = L[order[i]];
-        // canonical codes: length 4: symbols 0..14 -> codes 0..14; length 5: first = (15) << 1 = 30: 16 -> 30, 17 -> 31
-        auto sym = [&](int s) -> std::pair<int, int> { uint32_t code = s < 15 ? (uint32_t)s : (s == 16 ? 30u : 31u); int len = s < 15 ? 4 : 5;
-                                                        uint32_t r = 0; for (int i = 0; i < len; i++) r |= ((code >> i) & 1u) << (len - 1 - i); return {(int)r, len}; };
-        check("repeat 16 first", dynamic_header(257, 1, 19, inorder, {sym(16), {0, 2}}), 10);
-        std::vector<std::pair<int, int>> lots;                 // 17 with 7 repeats (3 bits = 7 -> 10 zeros) x 40 = 400 > 258: repeat past the end
-        for (int i = 0; i < 40; i++) { lots.push_back(sym(17)); lots.push_back({7, 3}); }
-        check("repeat past end", dynamic_header(257, 1, 19, inorder, lots), 10);
-        // all 258 lengths zero: no end-of-block code
-        std::vector<std::pair<int, int>> zeros;
-        for (int i = 0; i < 25; i++) { zeros.push_back(sym(17)); zeros.push_back({7, 3}); }   // 250 zeros
-        for (int i = 0; i < 8; i++) zeros.push_back(sym(0));
-        check("no end-of-block", dynamic_header(257, 1, 19, inorder, zeros), 10);
-        // literal/length set over-subscribed: 258 lengths of 1
-        std::vector<std::pair<int, int>> ones;
-        for (int i = 0; i < 258; i++) ones.push_back(sym(1));
-        check("lit over-subscribed", dynamic_header(257, 1, 19, inorder, ones), 10);
-        // literal/length set incomplete: only 256 with length 2, 'A' with length 2
-        std::vector<std::pair<int, int>> inc;
-        for (int i = 0; i < 258; i++) inc.push_back(sym(i == 65 || i == 256 ? 2 : 0));
-        check("lit incomplete", dynamic_header(257, 1, 19, inorder, inc), 1);
-        // a lone code of length 1 (EOB only), distances empty: complete enough for zlib; an empty block
-        std::vector<std::pair<int, int>> lone;
-        for (int i = 0; i < 258; i++) lone.push_back(sym(i == 256 ? 1 : 0));
-        {
-            BitWriter w; w.put(1, 1); w.put(2, 2); w.put(0, 5); w.put(0, 5); w.put(15, 4);
-            for (int i = 0; i < 19; i++) w.put(inorder[i], 3);
-            for (auto& s : lone) w.put(s.first, s.second);
-            w.put(0, 1);                                       // EOB = code 0 of length 1
-            check("lone code EOB", w.done(), 0);
-            BitWriter w2 = BitWriter{}; w2.put(1, 1); w2.put(2, 2); w2.put(0, 5); w2.put(0, 5); w2.put(15, 4);
-            for (int i = 0; i < 19; i++) w2.put(inorder[i], 3);
-            for (auto& s : lone) w2.put(s.first, s.second);
-            w2.put(1, 1);                                      // the unused code of a lone-code set
-            check("lone code unused half", w2.done(), 0);
-        }
-    }
-    {   // fixed code: literal/length symbols 286 and 287, distance codes 30 and 31, distance past the block start
-        for (int s : {286, 287}) { BitWriter w; w.put(1, 1); w.put(1, 2); fixed_sym(w, 'a'); fixed_sym(w, 'a'); fixed_sym(w, 'a'); fixed_sym(w, s); w.put(0, 5); fixed_sym(w, 256); check("fixed lit 286/287", w.done(), 6); }
-        for (int d : {30, 31}) { BitWriter w; w.put(1, 1); w.put(1, 2); fixed_sym(w, 'a'); fixed_sym(w, 257); w.put_rev(d, 5); fixed_sym(w, 256); check("fixed dist 30/31", w.done(), 4); }
-        for (int d : {0, 1, 2, 3}) {                           // distance d + 1 after 2 literals: 1 and 2 are fine, 3 and 4 are too far
-            BitWriter w; w.put(1, 1); w.put(1, 2); fixed_sym(w, 'a'); fixed_sym(w, 'b'); fixed_sym(w, 257); w.put_rev(d, 5); fixed_sym(w, 256);
-            check("fixed distance vs start", w.done(), 5);
-        }
-        {   // a non-final empty fixed block, then a final stored block
-            BitWriter w; w.put(0, 1); w.put(1, 2); fixed_sym(w, 256); w.put(1, 1); w.put(0, 2); auto v = w.done();
-            v.push_back(3); v.push_back(0); v.push_back(0xfc); v.push_back(0xff); v.push_back('x'); v.push_back('y'); v.push_back('z');
-            check("fixed then stored", v, 3);
-            auto bad = v; bad[bad.size() - 4] ^= 1; check("stored nlen", bad, 3);
-            auto tr = v; tr.pop_back(); check("stored truncated", tr, 3);
-            auto extra = v; extra.push_back(0x55); extra.push_back(0xaa); check("trailing bytes after final block", extra, 3);
-        }
-    }
-}
-
-int main() {
-    // ---- streams from zlib ----
-    const int strategies[] = {Z_DEFAULT_STRATEGY, Z_FILTERED, Z_HUFFMAN_ONLY, Z_RLE, Z_FIXED};
-    std::vector<std::pair<std::string, std::vector<uint8_t>>> data;
-    data.push_back({"bam", bam_like(0xff00)});
-    data.push_back({"bam 65536", bam_like(65536)});
-    data.push_back({"random", random_bytes(0xff00)});
-    data.push_back({"run", run_of(65536, 'A')});
-    data.push_back({"empty", {}});
-    data.push_back({"one", {0x42}});
-    for (int k = 1; k <= 40; k++) data.push_back({"period " + std::to_string(k), periodic(4000 + 37 * k, k)});
-    {   // distances up to 32768: a random 32 KiB prefix repeated
-        auto a = random_bytes(32768); auto b = a; b.insert(b.end(), a.begin(), a.begin() + 32768); data.push_back({"far", b});
-        auto c = random_bytes(30000); std::vector<uint8_t> d(65536); for (size_t i = 0; i < d.size(); i++) d[i] = c[i % c.size()]; data.push_back({"period 30000", d});
-    }
-    for (auto& [name, d] : data) {
-        for (int level = 0; level <= 9; level++)
-            for (int st : strategies) {
-                if ((level == 0 || level == 6 || level == 1 || level == 9) || st == Z_DEFAULT_STRATEGY || d.size() < 8000) {
-                    auto z = zdeflate(d, level, st);
-                    check((name + " level " + std::to_string(level)).c_str(), z, (uint32_t)d.size());
-                }
-            }
-        // many small blocks per member: sync and full flushes (empty stored blocks between them)
-        auto zs = zdeflate(d, 6, Z_DEFAULT_STRATEGY, 997, Z_SYNC_FLUSH); check((name + " sync flush").c_str(), zs, (uint32_t)d.size());
-        auto zf = zdeflate(d, 1, Z_DEFAULT_STRATEGY, 4096, Z_FULL_FLUSH); check((name + " full flush").c_str(), zf, (uint32_t)d.size());
-        auto z0 = zdeflate(d, 0, Z_DEFAULT_STRATEGY, 100, Z_SYNC_FLUSH); check((name + " stored sync flush").c_str(), z0, (uint32_t)d.size());
-        // output longer / shorter than ISIZE
-        if (!d.empty()) { auto z = zdeflate(d, 6, Z_DEFAULT_STRATEGY); check("isize - 1", z, (uint32_t)d.size() - 1); check("isize + 1", z, (uint32_t)d.size() + 1); }
-    }
-    check("isize 0xff00", zdeflate(bam_like(0xff00), 6, Z_DEFAULT_STRATEGY), 0xff00);
-    // ---- mutated streams: bit flips and truncations ----
-    for (auto& [name, d] : data) {
-        if (d.size() < 16) continue;
-        for (int level : {1, 6, 9}) {
-            for (int st : {Z_DEFAULT_STRATEGY, Z_FIXED, Z_HUFFMAN_ONLY}) {
-                const auto z = zdeflate(d, level, st);
-                for (int t = 0; t < (name.rfind("period", 0) == 0 ? 3 : 40); t++) {
-                    auto m = z;
-                    const int flips = 1 + (int)(rng() % 3);
-                    for (int f = 0; f < flips; f++) { const size_t bit = rng() % (m.size() * 8); m[bit / 8] ^= (uint8_t)(1u << (bit % 8)); }
-                    check((name + " flipped").c_str(), m, (uint32_t)d.size());
-                    auto head = z; head.resize(rng() % z.size());
-                    check((name + " truncated").c_str(), head, (uint32_t)d.size());
-                    auto early = z; early[rng() % std::min<size_t>(early.size(), 64)] ^= (uint8_t)(1u << (rng() % 8));   // the header region
-                    check((name + " header flip").c_str(), early, (uint32_t)d.size());
-                }
-            }
-        }
-    }
-    crafted();
+    int n_mutated = 0, n_dumped = 0;
+    corpus::for_each_stream(rng, [&](corpus::InfKind kind, const std::string& name, const std::vector<uint8_t>& in, uint32_t isize) {
+        bool zok = false;
+        const uint32_t st = check(name, in, isize, &zok);
+        if (!dump || (kind == corpus::MUTATED && n_mutated++ % 4)) return;
+        put(dump, kind, 1); put(dump, name.size(), 2); std::fwrite(name.data(), 1, name.size(), dump);
+        put(dump, isize, 4); put(dump, st, 4); put(dump, zok, 1); put(dump, in.size(), 4);
+        if (!in.empty()) std::fwrite(in.data(), 1, in.size(), dump);
+        n_dumped++;
+    });
     // ---- CRC-32: per-lane chunks folded with the shift table, as bgzf_crc does, against zlib ----
     {
         uint32_t tab[256], x2n[32];
         for (uint32_t i = 0; i < 256; i++) tab[i] = dfl::crc_table_entry(i);
         dfl::x2n_table(x2n);
-        for (int t = 0; t < 200; t++) {
-            const size_t n = t < 4 ? (size_t)t : (size_t)(rng() % 65537);
-            auto d = random_bytes(n);
+        auto fold = [&](const std::vector<uint8_t>& d) {
+            const size_t n = d.size();
             const uint32_t want = (uint32_t)crc32(0, d.data(), (uInt)n);
             const size_t chunk = (n + 31) / 32;
             uint32_t got = 0;
@@ -256,9 +92,14 @@ int main() {
                 got ^= dfl::crc_shift(x2n, dfl::crc_bytes(tab, 0, d.data() + a, (uint32_t)(b - a)), n - b);
             }
             if (got != want) { if (failures < 20) std::printf("MISMATCH crc n %zu: %08x vs %08x\n", n, got, want); failures++; }
-        }
+        };
+        for (int t = 0; t < 200; t++) fold(corpus::random_bytes(rng, t < 4 ? (size_t)t : (size_t)(rng() % 65537)));
+        for (size_t n = 4; n <= 64; n++) fold(corpus::random_bytes(rng, n));      // lanes left empty by chunk = (n + 31) / 32
+        for (size_t n : {1023, 1024, 1025}) fold(corpus::random_bytes(rng, n));
     }
+    if (dump && std::fclose(dump) != 0) { std::perror(argv[2]); return 2; }
     std::printf("%d streams (%d accepted, %d rejected), %d mismatches\n", n_streams, n_accept, n_reject, failures);
+    if (dump) std::printf("%d streams dumped\n", n_dumped);
     if (failures) return 1;
     std::printf("OK\n");
     return 0;

@@ -12,7 +12,7 @@ import pytest
 
 from elprep_b200 import _lib, bgzf, device, synth
 from test_sam_text import HEADER, line
-from util import encode_bam, set_side_inputs
+from util import encode_bam, host_encoder, set_side_inputs  # noqa: F401 (host_encoder: a fixture)
 
 pytestmark = pytest.mark.gpu
 
@@ -45,21 +45,6 @@ def inflate_all(data):
 def header_bytes(w, text=b"@HD\tVN:1.6\tSO:coordinate\n"):
     return b"BAM\1" + struct.pack("<i", len(text)) + text + struct.pack("<i", len(w.header.SQ)) + b"".join(
         struct.pack("<i", len(sq["SN"]) + 1) + sq["SN"].encode() + b"\0" + struct.pack("<i", int(sq["LN"])) for sq in w.header.SQ)
-
-
-@pytest.fixture(scope="module")
-def host_encoder(tmp_path_factory):
-    exe = str(tmp_path_factory.mktemp("deflate") / "deflate_check")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-I", os.path.join(ROOT, "elprep_b200", "csrc"), "-o", exe,
-                           os.path.join(ROOT, "tests", "c", "deflate_check.cpp"), "-lz"])
-
-    def run(data, eof, tmp):
-        src, dst = os.path.join(tmp, "in.bin"), os.path.join(tmp, "out.bgzf")
-        with open(src, "wb") as f:
-            f.write(data)
-        subprocess.check_call([exe, "deflate", src, dst, "1" if eof else "0"])
-        return open(dst, "rb").read()
-    return run
 
 
 @pytest.fixture(scope="module")

@@ -1,9 +1,36 @@
 """Shared helpers for the parity tests: run the same workload through the oracle (CPU restatement of the
 reference) and through the CUDA library (C ABI via ctypes), and return comparable results."""
 import os
+import subprocess
 import tempfile
 
 import numpy as np
+import pytest
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+
+def build_check(name, directory):
+    """tests/c/<name>.cpp built with -O2 against the library's headers and zlib -> the executable's path"""
+    exe = os.path.join(str(directory), name)
+    subprocess.check_call(["g++", "-O2", "-std=c++17", "-I", os.path.join(ROOT, "elprep_b200", "csrc"), "-o", exe,
+                           os.path.join(ROOT, "tests", "c", name + ".cpp"), "-lz"])
+    return exe
+
+
+@pytest.fixture(scope="module")
+def host_encoder(tmp_path_factory):
+    """run(data, eof, tmp) -> the BGZF bytes of the host build of deflate.cuh (deflate_check deflate); run.exe is the binary"""
+    exe = build_check("deflate_check", tmp_path_factory.mktemp("deflate"))
+
+    def run(data, eof, tmp):
+        src, dst = os.path.join(tmp, "in.bin"), os.path.join(tmp, "out.bgzf")
+        with open(src, "wb") as f:
+            f.write(data)
+        subprocess.check_call([exe, "deflate", src, dst, "1" if eof else "0"])
+        return open(dst, "rb").read()
+    run.exe = exe
+    return run
 
 
 def oracle_pipeline(w, bqsr=True, threads=4, max_cycle=500, quantize_levels=0, sqq=None, sort=True, markdup=True):
