@@ -229,6 +229,17 @@ __global__ void __launch_bounds__(AD_T, 1) adapt_kernel(AdaptArgs A) {
 // ---------------------------------------------------------------- fragment groups
 struct FragLayout { int bS, bU, bR, bL; int32_t upos_min, score_max; int key_bits; };
 
+// the group bits of an entering read's fragment key (the key shifted right by bS + 1)
+__device__ __forceinline__ uint64_t frag_group(const FragLayout& L, uint16_t f, int32_t refid, int32_t g, const int32_t* rg_lib, int n_rg, int32_t upos) {
+    const uint64_t lib = (uint64_t)(((g >= 0 && g < n_rg) ? rg_lib[g] : -1) + 1);
+    uint64_t grp = (f & F_REVERSED) ? 1 : 0;
+    int sh = 1;
+    grp |= (uint64_t)(uint32_t)(upos - L.upos_min) << sh; sh += L.bU;
+    grp |= (uint64_t)(uint32_t)(refid + 1) << sh; sh += L.bR;
+    return grp | lib << sh;
+}
+__device__ __forceinline__ bool true_fragment(uint16_t f) { return (f & (F_MULTIPLE | F_NEXTUNMAPPED)) != F_MULTIPLE; }   // isTrueFragment :177-179
+
 __global__ void __launch_bounds__(256) frag_keys_kernel(uint64_t n, const uint16_t* __restrict__ flag, const int32_t* __restrict__ refid, const int32_t* __restrict__ rg,
                                                          const int32_t* __restrict__ rg_lib, int n_rg, const int32_t* __restrict__ upos, const int32_t* __restrict__ score,
                                                          FragLayout L, uint64_t* __restrict__ keys, uint32_t* __restrict__ vals) {
@@ -237,16 +248,8 @@ __global__ void __launch_bounds__(256) frag_keys_kernel(uint64_t n, const uint16
     const uint16_t f = flag[i];
     uint64_t key;
     if ((f & (F_UNMAPPED | F_SECONDARY | F_SUPPLEMENTARY)) == 0) {
-        const int32_t g = rg[i];
-        const uint64_t lib = (uint64_t)(((g >= 0 && g < n_rg) ? rg_lib[g] : -1) + 1);
-        const uint64_t is_frag = ((f & (F_MULTIPLE | F_NEXTUNMAPPED)) != F_MULTIPLE) ? 1 : 0;   // isTrueFragment :177-179
-        key = (uint64_t)(uint32_t)(L.score_max - score[i]);
-        int sh = L.bS;
-        key |= is_frag << sh; sh += 1;
-        key |= (uint64_t)((f & F_REVERSED) ? 1 : 0) << sh; sh += 1;
-        key |= (uint64_t)(uint32_t)(upos[i] - L.upos_min) << sh; sh += L.bU;
-        key |= (uint64_t)(uint32_t)(refid[i] + 1) << sh; sh += L.bR;
-        key |= lib << sh;
+        key = (uint64_t)(uint32_t)(L.score_max - score[i]) | (uint64_t)(true_fragment(f) ? 1 : 0) << L.bS;
+        key |= frag_group(L, f, refid[i], rg[i], rg_lib, n_rg, upos[i]) << (L.bS + 1);
     } else {
         key = L.key_bits >= 64 ? ~0ull : ((1ull << L.key_bits) - 1);   // sorts after every real key (library field holds an unused value)
     }
@@ -282,6 +285,114 @@ __global__ void __launch_bounds__(256) frag_mark_kernel(uint64_t m, const uint64
     for (uint64_t t = j; t < e; t++) {
         if (has_pair ? ((keys[t] >> bS) & 1) != 0 : t != win) atomic_or_u16(flag, vals[t], F_DUPLICATE);
     }
+}
+
+// ---- fragment groups when true fragments are few
+// A true-pair read never gets 0x400 from classifyFragment; it only tells whether its group has a pair read.  So when true fragments
+// are a small share of the entering reads, their group bits go into an open-addressing set of exact group values, every entering
+// true-pair read probes the set and sets the has-pair bit of its group's slot, and only the true fragments are sorted and walked.
+constexpr uint64_t FSET_EMPTY = ~0ull, FSET_HAS_PAIR = 1ull << 63;   // group values use at most 62 bits on this path
+
+__device__ __forceinline__ uint64_t fset_home(uint64_t grp, uint64_t mask) { return mix64(grp) & mask; }
+
+// every true fragment: insert its group into the set and append (key, read index) to the list.  A block takes FS_ITEMS x 256 reads
+// and one list range (one atomic per block: a counter shared by all warps serialises when fragments are many).  The list is in no
+// particular order across blocks; frag_sparse_mark_kernel breaks full ties on the read index instead of on the position in the list.
+constexpr int FS_T = 256, FS_ITEMS = 4;
+
+__global__ void __launch_bounds__(FS_T) frag_set_insert_kernel(uint64_t n, const uint16_t* __restrict__ flag, const int32_t* __restrict__ refid, const int32_t* __restrict__ rg,
+                                                                const int32_t* __restrict__ rg_lib, int n_rg, const int32_t* __restrict__ upos, const int32_t* __restrict__ score,
+                                                                FragLayout L, uint64_t* __restrict__ set, uint64_t mask, uint64_t* __restrict__ keys, uint32_t* __restrict__ vals,
+                                                                uint32_t* __restrict__ count) {
+    __shared__ uint32_t s_warp[FS_T / 32], s_base;
+    const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const uint64_t i0 = (uint64_t)blockIdx.x * FS_T * FS_ITEMS + threadIdx.x;
+    uint16_t f[FS_ITEMS];
+    unsigned ballot[FS_ITEMS];
+    uint32_t in_warp = 0;
+#pragma unroll
+    for (int k = 0; k < FS_ITEMS; k++) {
+        const uint64_t i = i0 + (uint64_t)k * FS_T;
+        f[k] = i < n ? flag[i] : (uint16_t)F_UNMAPPED;
+        ballot[k] = __ballot_sync(FULL_MASK, (f[k] & (F_UNMAPPED | F_SECONDARY | F_SUPPLEMENTARY)) == 0 && true_fragment(f[k]));
+        in_warp += __popc(ballot[k]);
+    }
+    if (lane == 0) s_warp[warp] = in_warp;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        uint32_t t = 0;
+        for (int w = 0; w < FS_T / 32; w++) { const uint32_t c = s_warp[w]; s_warp[w] = t; t += c; }
+        s_base = t ? atomicAdd(count, t) : 0u;
+    }
+    __syncthreads();
+    uint64_t pos = (uint64_t)s_base + s_warp[warp];
+#pragma unroll
+    for (int k = 0; k < FS_ITEMS; k++) {
+        const uint64_t i = i0 + (uint64_t)k * FS_T;
+        if ((ballot[k] >> lane) & 1) {
+            const uint64_t grp = frag_group(L, f[k], refid[i], rg[i], rg_lib, n_rg, upos[i]);
+            const uint64_t p = pos + __popc(ballot[k] & lanemask_lt());
+            keys[p] = (uint64_t)(uint32_t)(L.score_max - score[i]) | (1ull << L.bS) | grp << (L.bS + 1);
+            vals[p] = (uint32_t)i;
+            for (uint64_t s = fset_home(grp, mask);; s = (s + 1) & mask) {
+                const uint64_t old = atomicCAS(reinterpret_cast<unsigned long long*>(set + s), (unsigned long long)FSET_EMPTY, (unsigned long long)grp);
+                if (old == FSET_EMPTY || old == grp) break;
+            }
+        }
+        pos += __popc(ballot[k]);
+    }
+}
+
+// every entering true-pair read of the local reads: a hit sets the has-pair bit of its group
+__global__ void __launch_bounds__(256) frag_set_probe_kernel(uint64_t n, const uint16_t* __restrict__ flag, const int32_t* __restrict__ refid, const int32_t* __restrict__ rg,
+                                                              const int32_t* __restrict__ rg_lib, int n_rg, const int32_t* __restrict__ upos, FragLayout L,
+                                                              uint64_t* __restrict__ set, uint64_t mask) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint16_t f = flag[i];
+    if ((f & (F_UNMAPPED | F_SECONDARY | F_SUPPLEMENTARY)) != 0 || true_fragment(f)) return;
+    const uint64_t grp = frag_group(L, f, refid[i], rg[i], rg_lib, n_rg, upos[i]);
+    for (uint64_t s = fset_home(grp, mask);; s = (s + 1) & mask) {
+        const uint64_t v = set[s];
+        if (v == FSET_EMPTY) return;
+        if ((v & ~FSET_HAS_PAIR) == grp) {
+            if (!(v & FSET_HAS_PAIR)) atomicOr(reinterpret_cast<unsigned long long*>(set + s), (unsigned long long)FSET_HAS_PAIR);
+            return;
+        }
+    }
+}
+
+// the true fragments sorted by their group bits: frag_mark_kernel's walk, with has_pair from the set and full ties (equal score and
+// QNAME) broken on the read index, so that the later arrival survives as it does in arrival order
+__global__ void __launch_bounds__(256) frag_sparse_mark_kernel(uint64_t m, const uint64_t* __restrict__ keys, const uint32_t* __restrict__ vals, int bS,
+                                                                const uint64_t* __restrict__ set, uint64_t mask,
+                                                                const uint64_t* __restrict__ qname_off, const uint8_t* __restrict__ qname, uint16_t* __restrict__ flag) {
+    const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= m) return;
+    const uint64_t g = keys[j] >> (bS + 1);
+    if (j > 0 && (keys[j - 1] >> (bS + 1)) == g) return;   // not a group head
+    uint64_t s = fset_home(g, mask);
+    while ((set[s] & ~FSET_HAS_PAIR) != g) s = (s + 1) & mask;   // every listed group is in the set
+    if (set[s] & FSET_HAS_PAIR) {   // a true-pair read in the group: every true fragment is a duplicate (:225-227)
+        for (uint64_t t = j; t < m && (keys[t] >> (bS + 1)) == g; t++) atomic_or_u16(flag, vals[t], F_DUPLICATE);
+        return;
+    }
+    if (j + 1 == m || (keys[j + 1] >> (bS + 1)) != g) return;   // a read alone in its group is never a duplicate
+    const uint64_t smask = (1ull << bS) - 1;
+    uint64_t e = j + 1, win = j, best = keys[j] & smask;
+    for (; e < m; e++) {
+        const uint64_t k = keys[e];
+        if ((k >> (bS + 1)) != g) break;
+        const uint64_t sc = k & smask;
+        if (sc < best) { best = sc; win = e; }
+        else if (sc == best) {
+            const uint32_t a = vals[e], b = vals[win];
+            const int d = qname_compare(qname, qname_off[a], qname_off[a + 1], qname_off[b], qname_off[b + 1]);
+            if (d < 0 || (d == 0 && a > b)) win = e;
+        }
+    }
+    for (uint64_t t = j; t < e; t++)
+        if (t != win) atomic_or_u16(flag, vals[t], F_DUPLICATE);
 }
 
 // ---------------------------------------------------------------- mate join
@@ -428,7 +539,8 @@ __global__ void __launch_bounds__(256) pair_keys_kernel(uint64_t n, const uint32
                                                          const uint16_t* __restrict__ flag, const int32_t* __restrict__ refid, const int32_t* __restrict__ rg,
                                                          const int32_t* __restrict__ rg_lib, int n_rg, const int32_t* __restrict__ upos, const int32_t* __restrict__ score,
                                                          PairLayout L, uint64_t* __restrict__ keys /*u64, or u128 as lo,hi*/, uint32_t* __restrict__ vals,
-                                                         uint32_t* __restrict__ pair_a, uint32_t* __restrict__ pair_b, int32_t* __restrict__ pair_score) {
+                                                         uint32_t* __restrict__ pair_a, uint32_t* __restrict__ pair_b, int32_t* __restrict__ pair_score,
+                                                         uint32_t* __restrict__ hash, uint32_t hash_mask) {
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const uint32_t m = mate[i];
@@ -453,10 +565,66 @@ __global__ void __launch_bounds__(256) pair_keys_kernel(uint64_t n, const uint32
     else { keys[2 * p] = lo; keys[2 * p + 1] = hi; }
     vals[p] = (uint32_t)p;
     pair_a[p] = a1; pair_b[p] = a2; pair_score[p] = score[a1] + score[a2];
+    if (hash) hash[p] = (uint32_t)(mix64(lo ^ mix64(hi)) >> 32) & hash_mask;
 }
 
 __device__ __forceinline__ bool same_key(const uint64_t* keys, uint64_t a, uint64_t b, int words) {
     return words == 1 ? keys[a] == keys[b] : (keys[2 * a] == keys[2 * b] && keys[2 * a + 1] == keys[2 * b + 1]);
+}
+
+// The pairs sorted by a 32-bit hash of the signature (stable: a run of equal hashes is in pair arrival order).  One thread per run of
+// two or more.  The signatures are read by pair index next to the run; each distinct signature in the run is its own group, led by its
+// first pair in the run, with pair_mark_kernel's winner rule.
+constexpr int PH_SEEN = 8;   // leaders remembered per run; a run with more distinct signatures looks leaders up by scanning back
+
+__device__ __forceinline__ void pair_group_mark(const uint32_t* vals, uint64_t a, uint64_t e, const uint64_t* keys, int words, bool uniform,
+                                                const uint32_t* pair_a, const uint32_t* pair_b, const int32_t* pair_score,
+                                                const uint64_t* qname_off, const uint8_t* qname, uint16_t* flag) {
+    const uint32_t lead = vals[a];
+    uint64_t win = a;
+    int32_t best = pair_score[lead];
+    for (uint64_t t = a + 1; t < e; t++) {
+        const uint32_t p = vals[t];
+        if (!uniform && !same_key(keys, lead, p, words)) continue;
+        const int32_t sc = pair_score[p];
+        if (sc > best) { best = sc; win = t; }
+        else if (sc == best) {
+            const uint32_t x = pair_a[p], y = pair_a[vals[win]];
+            if (qname_compare(qname, qname_off[x], qname_off[x + 1], qname_off[y], qname_off[y + 1]) <= 0) win = t;
+        }
+    }
+    for (uint64_t t = a; t < e; t++) {
+        const uint32_t p = vals[t];
+        if (t == win || (!uniform && !same_key(keys, lead, p, words))) continue;
+        atomic_or_u16(flag, pair_a[p], F_DUPLICATE); atomic_or_u16(flag, pair_b[p], F_DUPLICATE);
+    }
+}
+
+__global__ void __launch_bounds__(256) pair_hash_mark_kernel(uint64_t m, const uint32_t* __restrict__ hkeys, const uint32_t* __restrict__ vals,
+                                                              const uint64_t* __restrict__ keys, int words,
+                                                              const uint32_t* __restrict__ pair_a, const uint32_t* __restrict__ pair_b, const int32_t* __restrict__ pair_score,
+                                                              const uint64_t* __restrict__ qname_off, const uint8_t* __restrict__ qname, uint16_t* __restrict__ flag) {
+    const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= m) return;
+    const uint32_t h = hkeys[j];
+    if (j > 0 && hkeys[j - 1] == h) return;   // not a run head
+    if (j + 1 == m || hkeys[j + 1] != h) return;   // a single pair (most runs): no signature needed
+    uint64_t e = j + 1;
+    bool uniform = true;
+    for (; e < m && hkeys[e] == h; e++) uniform = uniform && same_key(keys, vals[j], vals[e], words);
+    if (uniform) { pair_group_mark(vals, j, e, keys, words, true, pair_a, pair_b, pair_score, qname_off, qname, flag); return; }
+    // a hash collision: lead each signature from its first pair in the run
+    uint32_t seen[PH_SEEN];
+    int n_seen = 0;
+    for (uint64_t a = j; a < e; a++) {
+        const uint32_t p = vals[a];
+        bool known = false;
+        if (n_seen < PH_SEEN) { for (int s = 0; s < n_seen && !known; s++) known = same_key(keys, seen[s], p, words); }
+        else { for (uint64_t b = j; b < a && !known; b++) known = same_key(keys, vals[b], p, words); }
+        if (known) continue;
+        if (n_seen < PH_SEEN) seen[n_seen++] = p;
+        pair_group_mark(vals, a, e, keys, words, false, pair_a, pair_b, pair_score, qname_off, qname, flag);
+    }
 }
 
 // keys sorted by the signature only, so a group is in pair arrival order
@@ -544,6 +712,26 @@ int phase_adapt(elp_ctx* c) {
     return E_OK;
 }
 
+// Which sorts group fragments and pairs.  By default the hashed paths run where they pay off (the size floors and the fragment share
+// in phase_markdup and mark_pairs).  ELPREP_B200_MARKDUP=exact sorts every entering read and every exact pair signature;
+// ELPREP_B200_MARKDUP=hashed drops the size floors, so that small inputs take the hashed paths too.  ELPREP_B200_MARKDUP_HASH_BITS=k
+// keeps k bits of the pair-signature hash (1..32), so that tests can make many signatures collide.  All are read on every call.
+enum class MarkdupSorts { AUTO, EXACT, HASHED };
+static MarkdupSorts markdup_sorts() {
+    const char* e = getenv("ELPREP_B200_MARKDUP");
+    if (e && std::string(e) == "exact") return MarkdupSorts::EXACT;
+    if (e && std::string(e) == "hashed") return MarkdupSorts::HASHED;
+    return MarkdupSorts::AUTO;
+}
+static int pair_hash_bits() {
+    const char* e = getenv("ELPREP_B200_MARKDUP_HASH_BITS");
+    const int k = e ? atoi(e) : 32;
+    return k >= 1 && k <= 32 ? k : 32;
+}
+// Below these sizes both paths take a few microseconds per sort pass, and the exact sorts keep the pass counts that
+// tests/markdup_check.py restates for the oracle comparisons.
+constexpr uint64_t FRAG_SET_MIN_READS = 1ull << 20, PAIR_HASH_MIN_PAIRS = 1ull << 20;
+
 // pairs (classifyPair) over the local reads plus the ghost reads spread_exchange_begin appended (comm.cu); ghosts are true pairs by construction
 static int mark_pairs(elp_ctx* c, bool optical, uint64_t nt, uint64_t n_true_pairs, int bU, int bR, int bL) {
     const DeviceRanges& R = c->h_ranges;
@@ -593,11 +781,29 @@ static int mark_pairs(elp_ctx* c, bool optical, uint64_t nt, uint64_t n_true_pai
         // keys live in keys_a (u128 as (lo,hi) pairs); slot[] occupies keys_b, so sort into a separate buffer
         CUDA_TRY(c, c->bytes_tmp.reserve((size_t)npairs * 8 * words + 64, c->stream));
         uint64_t* kb2 = reinterpret_cast<uint64_t*>(c->bytes_tmp.p);
-        c->begin("pair_keys", (double)nt * 12 + (double)npairs * (2 * 18 + 8 * words + 16));
+        // Pair marking only needs equal signatures next to each other, in arrival order: a stable sort of a 32-bit hash of the
+        // signature (4 passes of 4-byte keys instead of 8 or more of 8- or 16-byte keys), verified on the signatures inside runs.
+        // Optical marking walks the runs as groups, so it keeps the exact sort.
+        const MarkdupSorts mode = markdup_sorts();
+        const bool hashed = !optical && mode != MarkdupSorts::EXACT && (mode == MarkdupSorts::HASHED || npairs >= PAIR_HASH_MIN_PAIRS);
+        const int hbits = pair_hash_bits();
+        uint32_t* ha = reinterpret_cast<uint32_t*>(c->bytes_tmp.p);            // two u32 arrays in the 8-bytes-per-pair buffer
+        uint32_t* hb = ha + ((npairs + 3) & ~3ull);
+        c->begin("pair_keys", (double)nt * 12 + (double)npairs * (2 * 18 + 8 * words + 16 + (hashed ? 4 : 0)));
         pair_keys_kernel<<<nblk(nt, 256), 256, 0, c->stream>>>(nt, c->mate.p, slot, c->flag.p, c->refid.p, c->rg.p, c->d_rg_lib.p, c->n_rg, c->upos.p, c->score.p, L,
-                                                              c->keys_a.p, c->vals_a.p, c->pair_a.p, c->pair_b.p, c->pair_score.p);
+                                                              c->keys_a.p, c->vals_a.p, c->pair_a.p, c->pair_b.p, c->pair_score.p,
+                                                              hashed ? ha : nullptr, hbits == 32 ? ~0u : (1u << hbits) - 1);
         c->end(); LAUNCH_CHECK(c);
         bool in_b = false;
+        if (hashed) {
+            rc = radix_sort_u32(c, ha, hb, c->vals_a.p, c->vals_b.p, npairs, hbits, &in_b, "u32");
+            if (rc) return rc;
+            c->begin("pair_hash_mark", (double)npairs * (4 + 4 + 8 * words + 4));
+            pair_hash_mark_kernel<<<nblk(npairs, 256), 256, 0, c->stream>>>(npairs, in_b ? hb : ha, in_b ? c->vals_b.p : c->vals_a.p, c->keys_a.p, words,
+                                                                            c->pair_a.p, c->pair_b.p, c->pair_score.p, c->qname_off.p, c->qname.p, c->flag.p);
+            c->end(); LAUNCH_CHECK(c);
+            return E_OK;
+        }
         rc = words == 1 ? radix_sort_u64(c, c->keys_a.p, kb2, c->vals_a.p, c->vals_b.p, npairs, L.key_bits, &in_b, "u64")
                         : radix_sort_u128(c, c->keys_a.p, kb2, c->vals_a.p, c->vals_b.p, npairs, L.key_bits, &in_b, "u128");
         if (rc) return rc;
@@ -643,17 +849,47 @@ int phase_markdup(elp_ctx* c, bool optical) {
                 FragLayout L{}; L.bS = bits_for((uint64_t)R.score_max); L.bU = bU; L.bR = bR; L.bL = bL; L.upos_min = R.upos_min; L.score_max = R.score_max;
                 L.key_bits = L.bS + 2 + L.bU + L.bR + L.bL;
                 if (L.key_bits > 64) return c->fail(E_LIMIT, "fragment signature needs %d bits (>64): too many contigs/libraries for the packed key", L.key_bits);
-                c->begin("frag_keys", (double)n * (2 + 4 + 4 + 4 + 4 + 8 + 4));
-                frag_keys_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(n, c->flag.p, c->refid.p, c->rg.p, c->d_rg_lib.p, c->n_rg, c->upos.p, c->score.p, L, c->keys_a.p, c->vals_a.p);
-                c->end(); LAUNCH_CHECK(c);
-                // only the group (bits from bS + 1 up) needs to be contiguous: frag_mark_kernel finds the winner from the low bits
-                bool in_b = false;
-                int r2 = radix_sort_u64(c, c->keys_a.p, c->keys_b.p, c->vals_a.p, c->vals_b.p, n, L.key_bits - (L.bS + 1), &in_b, "u64", L.bS + 1);
-                if (r2) return r2;
-                const uint64_t m = R.n_entering;
-                c->begin("frag_mark", (double)m * 12);
-                frag_mark_kernel<<<nblk(m, 256), 256, 0, c->stream>>>(m, in_b ? c->keys_b.p : c->keys_a.p, in_b ? c->vals_b.p : c->vals_a.p, L.bS, c->qname_off.p, c->qname.p, c->flag.p);
-                c->end(); LAUNCH_CHECK(c);
+                // Few true fragments (mate-unmapped pairs; never single-end input, which is all fragments): sort only them.  At a quarter
+                // of the entering reads the set pass, the probe pass and the smaller sort still move about half the bytes of the full sort.
+                const uint64_t n_frag = (uint64_t)R.n_entering - R.n_true_pairs;
+                const MarkdupSorts mode = markdup_sorts();
+                const bool sparse = mode != MarkdupSorts::EXACT && (mode == MarkdupSorts::HASHED || R.n_entering >= FRAG_SET_MIN_READS) &&
+                                    4 * n_frag <= R.n_entering && L.key_bits - (L.bS + 1) <= 62;
+                if (sparse && n_frag) {
+                    uint64_t cap = 1024;   // load factor at most 1/2
+                    while (cap < 2 * n_frag) cap <<= 1;
+                    CUDA_TRY(c, c->bytes_tmp.reserve(cap * 8 + 64, c->stream));
+                    uint64_t* set = reinterpret_cast<uint64_t*>(c->bytes_tmp.p);
+                    uint32_t* count = reinterpret_cast<uint32_t*>(set + cap);
+                    CUDA_TRY(c, cudaMemsetAsync(set, 0xff, cap * 8, c->stream));
+                    CUDA_TRY(c, cudaMemsetAsync(count, 0, 4, c->stream));
+                    c->begin("frag_set_insert", (double)n * 2 + (double)n_frag * (4 + 4 + 4 + 4 + 8 + 8 + 4));
+                    frag_set_insert_kernel<<<nblk(n, FS_T * FS_ITEMS), FS_T, 0, c->stream>>>(n, c->flag.p, c->refid.p, c->rg.p, c->d_rg_lib.p, c->n_rg, c->upos.p, c->score.p, L,
+                                                                                             set, cap - 1, c->keys_a.p, c->vals_a.p, count);
+                    c->end(); LAUNCH_CHECK(c);
+                    c->begin("frag_set_probe", (double)n * 2 + (double)R.n_true_pairs * (4 + 4 + 4 + 8));
+                    frag_set_probe_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(n, c->flag.p, c->refid.p, c->rg.p, c->d_rg_lib.p, c->n_rg, c->upos.p, L, set, cap - 1);
+                    c->end(); LAUNCH_CHECK(c);
+                    bool in_b = false;
+                    int r2 = radix_sort_u64(c, c->keys_a.p, c->keys_b.p, c->vals_a.p, c->vals_b.p, n_frag, L.key_bits - (L.bS + 1), &in_b, "u64", L.bS + 1);
+                    if (r2) return r2;
+                    c->begin("frag_sparse_mark", (double)n_frag * 20);
+                    frag_sparse_mark_kernel<<<nblk(n_frag, 256), 256, 0, c->stream>>>(n_frag, in_b ? c->keys_b.p : c->keys_a.p, in_b ? c->vals_b.p : c->vals_a.p, L.bS,
+                                                                                      set, cap - 1, c->qname_off.p, c->qname.p, c->flag.p);
+                    c->end(); LAUNCH_CHECK(c);
+                } else if (!sparse) {
+                    c->begin("frag_keys", (double)n * (2 + 4 + 4 + 4 + 4 + 8 + 4));
+                    frag_keys_kernel<<<nblk(n, 256), 256, 0, c->stream>>>(n, c->flag.p, c->refid.p, c->rg.p, c->d_rg_lib.p, c->n_rg, c->upos.p, c->score.p, L, c->keys_a.p, c->vals_a.p);
+                    c->end(); LAUNCH_CHECK(c);
+                    // only the group (bits from bS + 1 up) needs to be contiguous: frag_mark_kernel finds the winner from the low bits
+                    bool in_b = false;
+                    int r2 = radix_sort_u64(c, c->keys_a.p, c->keys_b.p, c->vals_a.p, c->vals_b.p, n, L.key_bits - (L.bS + 1), &in_b, "u64", L.bS + 1);
+                    if (r2) return r2;
+                    const uint64_t m = R.n_entering;
+                    c->begin("frag_mark", (double)m * 12);
+                    frag_mark_kernel<<<nblk(m, 256), 256, 0, c->stream>>>(m, in_b ? c->keys_b.p : c->keys_a.p, in_b ? c->vals_b.p : c->vals_a.p, L.bS, c->qname_off.p, c->qname.p, c->flag.p);
+                    c->end(); LAUNCH_CHECK(c);
+                }
             }
             return mark_pairs(c, optical, nt, (uint64_t)R.n_true_pairs + c->n_ghost, bU, bR, bL);
         }();
