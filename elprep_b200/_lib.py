@@ -45,7 +45,7 @@ class ElpKernelStat(C.Structure):
 EXPORTS = ["elp_create", "elp_destroy", "elp_last_error", "elp_reserve", "elp_reset", "elp_set_reference", "elp_set_known_sites",
            "elp_fetch_opt_flags", "elp_set_target_regions", "elp_set_bqsr_target_regions", "elp_filter_target_regions", "elp_n_sorted", "elp_clean_sam", "elp_debug_cigar", "elp_comm_unique_id", "elp_comm_init", "elp_comm_set_partition", "elp_comm_destroy", "elp_bqsr_tables_allreduce", "elp_optical_allreduce", "elp_bqsr_tables_clear", "elp_bqsr_tables_write_elrecal", "elp_bqsr_tables_add_elrecal", "elp_optical_write_gob", "elp_optical_add_gob", "elp_append_batch", "elp_append_batch_async", "elp_append_wait", "elp_fetch_async", "elp_fetch_wait", "elp_append_bam", "elp_append_sam", "elp_set_ingest_filter", "elp_n_filtered", "elp_n_reads", "elp_sort_markdup", "elp_bqsr_gather", "elp_bqsr_tables_len", "elp_bqsr_n_cov",
            "elp_bqsr_cov_name", "elp_bqsr_tables_get", "elp_bqsr_tables_put", "elp_bqsr_tables_device", "elp_bqsr_finalize",
-           "elp_bqsr_empirical_get", "elp_bqsr_apply", "elp_fetch", "elp_fetch_qual_bytes", "elp_fetch_bam", "elp_fetch_bam_bytes", "elp_fetch_sam", "elp_fetch_sam_bytes", "elp_set_output_filter", "elp_set_replace_read_group", "elp_set_input_dictionary", "elp_n_output", "elp_debug_adapt", "elp_launch_count",
+           "elp_bqsr_empirical_get", "elp_bqsr_apply", "elp_fetch", "elp_fetch_qual_bytes", "elp_fetch_bam", "elp_fetch_bam_bytes", "elp_fetch_sam", "elp_fetch_sam_bytes", "elp_set_output_filter", "elp_set_replace_read_group", "elp_set_input_dictionary", "elp_add_input", "elp_select_input", "elp_set_tag_rename", "elp_n_output", "elp_debug_adapt", "elp_launch_count",
            "elp_kernel_stats", "elp_synchronize", "elp_reset_stats", "elp_timer_start", "elp_timer_stop", "elp_debug_sort_u64", "elp_debug_sort_u128",
            "elp_debug_sort_u64_range", "elp_debug_sort_u128_range", "elp_debug_sort_u32_range", "elp_debug_scan_u32", "elp_debug_join_hash", "elp_debug_coord_chunk_keys",
            "elp_optical_n_libraries", "elp_optical_library_name", "elp_optical_metrics", "elp_optical_histogram", "elp_optical_merge",
@@ -130,6 +130,9 @@ def load():
     L.elp_set_output_filter.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_char_p), C.c_int32, C.POINTER(C.c_char_p), C.c_int32]
     L.elp_set_replace_read_group.argtypes = [C.c_void_p, C.c_int]
     L.elp_set_input_dictionary.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_char_p), C.c_void_p, C.c_int32]
+    L.elp_add_input.argtypes = [C.c_void_p, C.POINTER(C.c_char_p), C.c_void_p, C.c_int32]
+    L.elp_select_input.argtypes = [C.c_void_p, C.c_int32]
+    L.elp_set_tag_rename.argtypes = [C.c_void_p, C.c_char_p, C.POINTER(C.c_char_p), C.POINTER(C.c_char_p), C.c_int32]
     L.elp_n_output.restype = C.c_uint64
     L.elp_n_output.argtypes = [C.c_void_p]
     L.elp_n_filtered.restype = C.c_uint64

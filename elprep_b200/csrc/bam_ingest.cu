@@ -412,6 +412,7 @@ extern "C" int elp_append_bam(elp_ctx* c, const uint8_t* records, uint64_t n_byt
     std::lock_guard<std::mutex> lk(c->append_mu);
     if (c->sorted) return c->fail(E_STATE, "elp_append_bam after elp_sort_markdup (call elp_reset first)");
     if (c->bgzf_open) return c->fail(E_STATE, "elp_append_bam while a BGZF file is open (elp_append_bgzf_end first)");
+    TRY(relabel_check_selected(c, "elp_append_bam"));
     // record offsets: given, or found by walking the block_size chain
     std::vector<uint64_t> walked;
     if (!record_off) {
@@ -456,6 +457,9 @@ int bam_ingest_core(elp_ctx* c, uint64_t n_bytes, uint64_t nrec, bool sam_record
     uint64_t bn = nrec;                                       // becomes the number of records that pass the filters
     const uint64_t n0 = c->n;
     cudaStream_t s = c->stream;
+    // several inputs (merge_inputs.cu): the records as the merged header writes them, in the rewrite's buffer; bam_off follows them
+    const uint8_t* raw = c->bam_raw.p;
+    if (relabel_on(c)) TRY(relabel_records(c, &raw, c->bam_off.p, &n_bytes, nrec, sam_records));
     TRY(grow(c, c->bam_start, nrec + 2, 0));
     const uint64_t* d_start = c->bam_off.p;                   // without filters: record i is read n0 + i
     TRY(rg_names_upload(c));
@@ -464,7 +468,7 @@ int bam_ingest_core(elp_ctx* c, uint64_t n_bytes, uint64_t nrec, bool sam_record
         TRY(grow(c, c->scan_tmp, nrec + 8, 0)); TRY(grow(c, c->off_stage, nrec + 2, 0));
         c->begin("bam_keep", (double)nrec * 48);
         if (c->filter_mask & ELP_FILTER_TARGET_REGIONS) TRY(table_upload(c, c->regions));
-        bam_keep_kernel<<<nblk(nrec, 256), 256, 0, s>>>(nrec, c->bam_raw.p, c->bam_off.p, n_bytes, c->filter_mask, c->filter_min_mapq, c->regions.d_ptrs.p, c->regions.d_n.p, c->n_contigs,
+        bam_keep_kernel<<<nblk(nrec, 256), 256, 0, s>>>(nrec, raw, c->bam_off.p, n_bytes, c->filter_mask, c->filter_min_mapq, c->regions.d_ptrs.p, c->regions.d_n.p, c->n_contigs,
                                                         n_ref, ingest_remap(c), (c->dict_mode & ELP_DICT_REPLACE) != 0, RgNames{c->d_rg_names.p, c->d_rg_name_off.p, c->n_rg}, c->scan_tmp.p, c->d_err.p);
         c->end(); LAUNCH_CHECK(c);
         TRY(exclusive_scan_u32_to_u64(c, c->scan_tmp.p, c->off_stage.p, nrec));
@@ -484,7 +488,7 @@ int bam_ingest_core(elp_ctx* c, uint64_t n_bytes, uint64_t nrec, bool sam_record
     TRY(grow(c, c->qname_off, n1 + 2, n0 + 1)); TRY(grow(c, c->cigar_off, n1 + 2, n0 + 1)); TRY(grow(c, c->qual_off, n1 + 2, n0 + 1)); TRY(grow(c, c->seq_off, n1 + 2, n0 + 1));
     TRY(grow(c, c->scan_tmp, 4 * (bn + 4) + 8, 0));   // (the keep flags above are dead by now)
     BamArgs A{};
-    A.n = bn; A.n0 = n0; A.raw = c->bam_raw.p; A.start = d_start; A.n_bytes = n_bytes; A.chained = d_start == c->bam_off.p; A.clear_dup = c->clear_dup; A.rg_replace = c->rg_replace;
+    A.n = bn; A.n0 = n0; A.raw = raw; A.start = d_start; A.n_bytes = n_bytes; A.chained = d_start == c->bam_off.p; A.clear_dup = c->clear_dup; A.rg_replace = c->rg_replace;
     A.refid = c->refid.p; A.pos = c->pos.p; A.nref = c->nref.p; A.pnext = c->pnext.p; A.tlen = c->tlen.p; A.rg = c->rg.p; A.flag = c->flag.p; A.mapq = c->mapq.p; A.optf = c->optf.p;
     A.len_qname = c->scan_tmp.p; A.len_cigar = c->scan_tmp.p + (bn + 4); A.len_seq = c->scan_tmp.p + 2 * (bn + 4); A.len_qual = c->scan_tmp.p + 3 * (bn + 4);
     A.rg_names = c->d_rg_names.p; A.rg_name_off = c->d_rg_name_off.p; A.n_rg = c->n_rg; A.n_ref = n_ref; A.remap = ingest_remap(c); A.err = c->d_err.p;
@@ -507,7 +511,7 @@ int bam_ingest_core(elp_ctx* c, uint64_t n_bytes, uint64_t nrec, bool sam_record
     TRY(grow(c, c->qname, ends[0] + 64, c->n_qname)); TRY(grow(c, c->cigar, ends[1] + 16, c->n_cigar));
     TRY(grow(c, c->seq, ends[2] + 64, c->n_seq)); TRY(grow(c, c->qual, ends[3] + 64, c->n_qual));
     CopyArgs B{};
-    B.n = bn; B.n0 = n0; B.raw = c->bam_raw.p; B.start = d_start;
+    B.n = bn; B.n0 = n0; B.raw = raw; B.start = d_start;
     B.qname_off = c->qname_off.p; B.cigar_off = c->cigar_off.p; B.seq_off = c->seq_off.p; B.qual_off = c->qual_off.p;
     B.qname = c->qname.p; B.cigar = c->cigar.p; B.seq = c->seq.p; B.qual = c->qual.p;
     c->begin("bam_copy", 2.0 * (double)n_bytes);
@@ -518,7 +522,7 @@ int bam_ingest_core(elp_ctx* c, uint64_t n_bytes, uint64_t nrec, bool sam_record
     // keep the raw records for elp_fetch_bam (only meaningful while every read of the context came in as BAM)
     if (c->bam_reads == n0) {
         TRY(grow(c, c->bam_all, c->n_bam + n_bytes + 64, c->n_bam)); TRY(grow(c, c->bam_all_off, n1 + 2, n0));
-        CUDA_TRY(c, cudaMemcpyAsync(c->bam_all.p + c->n_bam, c->bam_raw.p, n_bytes, cudaMemcpyDeviceToDevice, s));
+        CUDA_TRY(c, cudaMemcpyAsync(c->bam_all.p + c->n_bam, raw, n_bytes, cudaMemcpyDeviceToDevice, s));
         CUDA_TRY(c, cudaMemcpyAsync(c->bam_all_off.p + n0, d_start, bn * 8, cudaMemcpyDeviceToDevice, s));      // start of every kept record
         if (c->n_bam) { add_base_u64_kernel<<<nblk(bn, 256), 256, 0, s>>>(bn, c->bam_all_off.p + n0, c->n_bam); c->launches++; }
         CUDA_TRY(c, cudaStreamSynchronize(s));
@@ -711,6 +715,7 @@ extern "C" int elp_set_input_dictionary(elp_ctx* c, uint32_t mode, const char* c
     cudaSetDevice(c->device);
     if (mode & ~(uint32_t)(ELP_DICT_RENAME_CHROMOSOMES | ELP_DICT_REPLACE)) return c->fail(E_INVAL, "elp_set_input_dictionary: unknown mode bits 0x%x", mode);
     if (n < 0 || (n && (!names || !lengths))) return c->fail(E_INVAL, "elp_set_input_dictionary: bad input dictionary (n = %d)", n);
+    if (mode && relabel_on(c)) return c->fail(E_INVAL, "elp_set_input_dictionary: the context has inputs or tag renames (elp_add_input, elp_set_tag_rename); the two do not combine");
     if (c->n || c->sorted || c->bgzf_open) return c->fail(E_STATE, "elp_set_input_dictionary: the context holds reads (call it after elp_create or elp_reset)");
     if (mode && !c->has_contig_names) return c->fail(E_INVAL, "elp_set_input_dictionary: the context was created without elp_config.contig_names");
     const bool rename = (mode & ELP_DICT_RENAME_CHROMOSOMES) != 0, replace = (mode & ELP_DICT_REPLACE) != 0;

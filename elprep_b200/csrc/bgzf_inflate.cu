@@ -228,6 +228,22 @@ static int check_header(elp_ctx* c, uint64_t ref_at, uint64_t hdr) {
     CUDA_TRY(c, cudaMemcpyAsync(h.data(), c->bam_raw.p + ref_at, h.size(), cudaMemcpyDeviceToHost, c->stream));
     CUDA_TRY(c, cudaStreamSynchronize(c->stream));
     const int32_t n_ref = (int32_t)rd32(h.data());
+    if (!c->inputs.empty()) {   // elp_add_input: the selected input's @SQ
+        const elp_ctx::InputDict& d = c->inputs[c->cur_input];
+        if (n_ref != (int32_t)d.len.size()) return c->fail(E_INVAL, "elp_append_bgzf: the BAM header has %d reference sequences, the selected input (elp_select_input %d) has %zu", n_ref, c->cur_input, d.len.size());
+        uint64_t x = 4;
+        for (int32_t k = 0; k < n_ref; k++) {
+            const uint32_t l_name = rd32(h.data() + x);
+            const char* name = reinterpret_cast<const char*>(h.data() + x + 4);
+            const int32_t l_ref = (int32_t)rd32(h.data() + x + 4 + l_name);
+            const std::string nm(name, l_name ? strnlen(name, l_name) : 0);
+            if (l_ref != d.len[k] || nm != d.names[k])
+                return c->fail(E_INVAL, "elp_append_bgzf: reference %d of the BAM header is '%s' of length %d, the selected input (elp_select_input %d) says '%s' of length %d",
+                               k, nm.c_str(), l_ref, c->cur_input, d.names[k].c_str(), d.len[k]);
+            x += 8ull + l_name;
+        }
+        return E_OK;
+    }
     if (c->dict_mode) {
         if (n_ref != c->n_in) return c->fail(E_INVAL, "elp_append_bgzf: the BAM header has %d reference sequences, the input dictionary (elp_set_input_dictionary) has %d", n_ref, c->n_in);
         uint64_t x = 4;
@@ -266,7 +282,7 @@ static int frame_records(elp_ctx* c, uint64_t n, uint64_t* nrec, uint64_t* used)
     cudaStream_t s = c->stream;
     const uint64_t nseg = (n + SEG - 1) / SEG;
     TRY(grow(c, S.seg, 4 * nseg + 4, 0)); TRY(grow(c, S.seg_cnt, nseg + 8, 0)); TRY(grow(c, c->off_stage, nseg + 2, 0));
-    const Frame F{c->bam_raw.p, n, nseg, ingest_ref_bound(c, false)};
+    const Frame F{c->bam_raw.p, n, nseg, c->inputs.empty() ? ingest_ref_bound(c, false) : relabel_ref_bound(c)};
     uint64_t *g0 = S.seg.p, *x0 = g0 + nseg, *g1 = x0 + nseg, *x1 = g1 + nseg;   // generation 0 and 1: guesses, then exits
     uint32_t* changed = reinterpret_cast<uint32_t*>(S.d_small.p);
     c->begin("bam_frame", (double)n);
@@ -372,6 +388,7 @@ extern "C" int elp_append_bgzf(elp_ctx* c, const uint8_t* data, uint64_t n_bytes
     std::lock_guard<std::mutex> lk(c->append_mu);
     if (c->sorted) return c->fail(E_STATE, "elp_append_bgzf after elp_sort_markdup (call elp_reset first)");
     TRY(bgzf_state(c));
+    if (!c->bgzf_open) TRY(relabel_check_selected(c, "elp_append_bgzf"));
     if (c->bgzf->poisoned) return c->fail(E_STATE, "elp_append_bgzf: an earlier call of this file failed (call elp_reset first)");
     c->bgzf_open = true;
     const int rc = append_bgzf(c, data, n_bytes);

@@ -45,6 +45,8 @@
 #define DERR_BAM_CG 0x1000u      // CG:B long-CIGAR convention
 #define DERR_CLEANSAM 0x4000u    // "Unexpected non-0 relative clipping position in CleanSam." (filters/utils.go:96)
 #define DERR_SPREAD_NAME 0x2000u // QNAME longer than a spread record holds (comm.cu)
+#define DERR_BAM_TAGTYPE 0x8000u // first RG / PG field not of type Z while elp_set_tag_rename renames the tag (merge_inputs.cu)
+#define DERR_BAM_INPUT_REF 0x10000u // refID / next_refID beyond the selected input's @SQ (elp_add_input, merge_inputs.cu)
 
 // FLAG bits (sam/sam-types.go:485-520)
 #define F_MULTIPLE 0x1

@@ -116,8 +116,9 @@ struct SortWorkspace {
 };
 
 // State of a module that the context owns through a StatePtr; each module defines free_state for its type, where the type is complete.
-struct SamState; struct SamOutState; struct BgzfStream; struct DeflateState; struct SitesStage;
+struct SamState; struct SamOutState; struct BgzfStream; struct DeflateState; struct SitesStage; struct RelabelState;
 void free_state(SamState* p); void free_state(SamOutState* p); void free_state(BgzfStream* p); void free_state(DeflateState* p); void free_state(SitesStage* p);
+void free_state(RelabelState* p);
 struct FreeState { template <class T> void operator()(T* p) const { free_state(p); } };
 template <class T> using StatePtr = std::unique_ptr<T, FreeState>;
 
@@ -199,6 +200,14 @@ struct elp_ctx {
     DBuf<int32_t> d_remap;                   // [in_tab.size() + 1]
     DBuf<int32_t> d_clean_len;               // [n_contigs] CleanSam's LN per output contig: the input LN of its name (last entry), else 0
     NameDictBufs in_dict;                    // elp_append_sam's RNAME / RNEXT lookup over in_tab while dict_mode is set (built on first use)
+    // several input files (elp_add_input / elp_select_input / elp_set_tag_rename; survive elp_reset).  elp_config holds the merged header;
+    // each input's @SQ maps to the merged dictionary, and the composed RG / PG maps of the merge rename the first RG / PG value of every
+    // record.  While any of them is set, every appended record is rewritten at ingest (merge_inputs.cu: relabel_records).
+    struct InputDict { std::vector<std::string> names; std::vector<int32_t> len, remap; };   // @SQ SN / LN, merged index of each SN
+    std::vector<InputDict> inputs;
+    int cur_input = -1;                      // elp_select_input
+    std::vector<std::pair<std::string, std::string>> tag_ren[2];   // old -> new value: [0] RG, [1] PG
+    StatePtr<RelabelState> relabel;          // device tables and staging of the rewrite (merge_inputs.cu)
     RegionTable regions;                     // --filter-non-overlapping-reads: the ingest filter ELP_FILTER_TARGET_REGIONS (elp_set_target_regions)
     RegionTable bqsr_regions;                // --target-regions: elp_filter_target_regions after marking (elp_set_bqsr_target_regions); both survive elp_reset
     uint64_t n_cleaned = 0;                  // reads whose CIGAR elp_clean_sam rewrote
@@ -388,7 +397,13 @@ inline const int32_t* ingest_remap(const elp_ctx* c) { return c->dict_mode ? c->
 inline bool ingest_keep_on(const elp_ctx* c) { return c->filter_mask || c->filter_min_mapq > 0 || (c->dict_mode & 2u /* ELP_DICT_REPLACE */); }
 int out_select(elp_ctx* c, const uint32_t** sel, uint64_t* n_out);
 int rg_names_upload(elp_ctx* c);   // bam_ingest.cu: @RG IDs -> d_rg_names / d_rg_name_off, once per context   // bam_ingest.cu: the record filters' selection (sel null and n_out = n_sorted without record bits)
-std::vector<std::string> sam_print_names(const elp_ctx* c);   // bam_ingest.cu: the names elp_fetch_sam prints for the stored refIDs
+std::vector<std::string> sam_print_names(const elp_ctx* c);
+// merge_inputs.cu: whether appended records are rewritten; the refID bound of the selected input's records; ELP_ESTATE when inputs exist
+// and none is selected; the rewrite itself (raw / off / n_bytes in and out)
+bool relabel_on(const elp_ctx* c);
+int relabel_ref_bound(const elp_ctx* c);
+int relabel_check_selected(elp_ctx* c, const char* who);
+int relabel_records(elp_ctx* c, const uint8_t** raw, uint64_t* off, uint64_t* n_bytes, uint64_t nrec, bool sam_records);   // bam_ingest.cu: the names elp_fetch_sam prints for the stored refIDs
 int region_set(elp_ctx* c, RegionTable& t, const char* who, int32_t contig, const int32_t* se, uint64_t n_intervals, int already_flat);   // bam_ingest.cu
 int build_output_columns(elp_ctx* c, const uint32_t* perm, uint64_t n_out, bool refilter);   // coordsort.cu: s_* columns and s_out_off of perm[0, n_out)
 int phase_target_filter(elp_ctx* c, uint64_t* n_removed);   // target_regions.cu

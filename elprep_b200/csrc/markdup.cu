@@ -669,6 +669,8 @@ int check_device_errors(elp_ctx* c) {
     if (e & DERR_TILE_RANGE) return c->fail(E_LIMIT, "optical duplicates: tile/x/y value outside int32");
     if (e & DERR_BAM_CG) return c->fail(E_LIMIT, "BAM record uses the CG:B long-CIGAR convention, which the device parser does not handle");
     if (e & DERR_BAM_RG) return c->fail(E_BAM, "BAM record with an RG:Z value that is not an @RG ID of the header");
+    if (e & DERR_BAM_TAGTYPE) return c->fail(E_BAM, "interface conversion: the first RG or PG field of a record is not a string (elp_set_tag_rename renames the tag)");
+    if (e & DERR_BAM_INPUT_REF) return c->fail(E_BAM, "BAM record with a refID or next_refID beyond the @SQ lines of its input (elp_add_input)");
     if (e & DERR_BAM) return c->fail(E_BAM, "malformed BAM alignment record (field lengths and block_size do not add up)");
     if (e & DERR_READLEN_LIMIT) return c->fail(E_LIMIT, "BQSR: read longer than the device kernel supports");
     if (e & DERR_CLEANSAM) return c->fail(E_LIMIT, "Unexpected non-0 relative clipping position in CleanSam.");

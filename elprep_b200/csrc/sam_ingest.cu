@@ -395,6 +395,7 @@ extern "C" int elp_append_sam(elp_ctx* c, const char* text, uint64_t n_bytes) {
     cudaSetDevice(c->device);
     std::lock_guard<std::mutex> lk(c->append_mu);
     if (c->sorted) return c->fail(E_STATE, "elp_append_sam after elp_sort_markdup (call elp_reset first)");
+    TRY(relabel_check_selected(c, "elp_append_sam"));
     if (c->bgzf_open) return c->fail(E_STATE, "elp_append_sam while a BGZF file is open (elp_append_bgzf_end first)");
     if (c->n_contigs > 0 && !c->has_contig_names) return c->fail(E_INVAL, "elp_append_sam: the context was created without elp_config.contig_names, so RNAME / RNEXT cannot be resolved");
     if (n_bytes == 0) return ELP_OK;

@@ -189,6 +189,26 @@ class Context:
         lens = np.ascontiguousarray(lengths, dtype=np.int32).reshape(-1)
         self._ck(self.L.elp_set_input_dictionary(self.h, int(mode), _cstrs(list(names)), _vp(lens) if lens.size else None, len(names)))
 
+    def add_input(self, names=(), lengths=()):
+        """one input file of several (elp_add_input): its @SQ names / lengths as they stand in the file.  The context was created from
+        the header sam.MergeInputs merged; returns the input's id for select_input.  Only while the context holds no reads; survives
+        reset()."""
+        lens = np.ascontiguousarray(lengths, dtype=np.int32).reshape(-1)
+        rc = self.L.elp_add_input(self.h, _cstrs(list(names)), _vp(lens) if lens.size else None, len(names))
+        self._ck(min(rc, 0))
+        return rc
+
+    def select_input(self, input_id):
+        """the input whose records the next appends carry (elp_select_input); not while a BGZF file is open"""
+        self._ck(self.L.elp_select_input(self.h, int(input_id)))
+
+    def set_tag_rename(self, tag, mapping):
+        """the composed RG or PG value map of sam.MergeInputs (elp_set_tag_rename): tag "RG" or "PG", mapping old value -> new value,
+        applied to the first field of the tag of every appended record.  An empty mapping clears it.  Only while the context holds no
+        reads; survives reset()."""
+        old, new = list(mapping.keys()), [mapping[k] for k in mapping]
+        self._ck(self.L.elp_set_tag_rename(self.h, tag.encode(), _cstrs(old), _cstrs(new), len(old)))
+
     def n_output(self):
         """output records fetch_bam / fetch_sam write (those that pass the record filters of set_output_filter); 0 before sort_markdup"""
         return int(self.L.elp_n_output(self.h))

@@ -38,6 +38,8 @@ class Header:
         self.SQ = [dict(x) for x in (sq or [])]   # [{"SN": name, "LN": int}]
         self.RG = [dict(x) for x in (rg or [])]   # [{"ID":..., "LB":..., "PU":...}]
         self.HD = {"VN": "1.6", "SO": so}
+        self.PG = []                              # [{"ID":..., "PP":..., ...}] (MergeInputs)
+        self.CO = []                              # comment lines (MergeInputs)
         self.UserRecords = {}
 
     def HDSO(self):
@@ -382,3 +384,101 @@ def parse_sam_header(buf):
             raise ValueError(f"unknown SAM record type code {raw[:3]}")
         pos, first = nxt, False
     return h, pos
+
+
+# ---- several input files: sam.MergeInputs (sam/merge-inputs.go:16-219) ----
+
+MERGE_DICT_PANIC = "Cannot merge sequence dictionaries."
+
+
+def _member(d, sn):
+    """memberOfSequenceDictionary (merge-inputs.go:85-92): the first index whose SN is sn, or -1"""
+    for i, sq in enumerate(d):
+        if sq["SN"] == sn:
+            return i
+    return -1
+
+
+def merge_sequence_dictionaries(to_dict, from_dict):
+    """mergeSequenceDictionaries (merge-inputs.go:100-124) as written: order-preserving and recursive.  j is set from an index in
+    from_dict after a recursive merge and from an index in the new dictionary after a shared entry, so a later from_dict[j:iFrom] can
+    start behind its end; Go panics on that slice, and so does this.  ValueError where the reference panics."""
+    new, j = [], 0
+    for i_to, sq in enumerate(to_dict):
+        sn = sq["SN"]
+        i_from = _member(from_dict, sn)
+        if i_from >= 0:
+            i_new = _member(new, sn)
+            if i_new >= 0:
+                if i_new != i_to:
+                    raise ValueError(MERGE_DICT_PANIC)
+                j = i_new + 1
+            else:
+                if j > i_from:
+                    raise ValueError(f"runtime error: slice bounds out of range [{j}:{i_from}]")
+                new = merge_sequence_dictionaries(new, from_dict[j:i_from])
+                new.append(sq)
+                j = i_from + 1
+        else:
+            new.append(sq)
+    new.extend(from_dict[j:])
+    return new
+
+
+def MergeInputs(headers, suffix):
+    """sam.MergeInputs / mergeHeaders (sam/merge-inputs.go:16-219) over the parsed headers of the input files, in file order.  suffix
+    stands for strconv.FormatInt(time.Now().Unix(), 10), the text a colliding @RG or @PG ID gets appended.  The inputs are not changed.
+
+    Returns (merged, sq_maps, rg_map, pg_map):
+      merged  the merged Header: the first header, then each later one merged into it (HD fields and user records overwritten, @SQ
+              merged in order, @RG / @PG appended with colliding IDs renamed, comments appended, SO unknown after any merge);
+      sq_maps per input, its @SQ index -> the index of that SN in the merged dictionary (first match, memberOfSequenceDictionary);
+      rg_map / pg_map  the update filters replaceReadGroupIfExists / replaceProgramIDIfExists, which every record of every file runs in
+              list order, composed into one map of old value -> final value (values it leaves alone are not in it).
+    ValueError with the reference's text where it panics."""
+    import copy
+    merged, filters = None, []
+    for h in headers:
+        if merged is None:
+            merged = copy.deepcopy(h)
+            for a in ("PG", "CO"):
+                setattr(merged, a, [copy.deepcopy(x) for x in getattr(h, a, [])])
+            continue
+        h = copy.deepcopy(h)
+        merged.HD.update(h.HD)                                                     # mergeMetaData
+        merged.SQ = merge_sequence_dictionaries(merged.SQ, h.SQ)
+        ids = {r["ID"] for r in merged.RG}                                         # mergeReadGroups: the IDs before this file
+        for r in h.RG:
+            if r["ID"] in ids:
+                old = r["ID"]
+                r["ID"] = old + suffix
+                filters.append(("RG", old, r["ID"]))
+            merged.RG.append(r)
+        pg_ids, replaced = {r["ID"] for r in merged.PG}, {}                        # mergeProgramLines
+        for r in getattr(h, "PG", []):
+            if r["ID"] in pg_ids:
+                old = r["ID"]
+                r["ID"] = old + suffix
+                filters.append(("PG", old, r["ID"]))
+                replaced[old] = r["ID"]
+            merged.PG.append(r)
+        for i in range(1, len(h.RG)):                                              # (the PP fix-up walks the RG lines, as written)
+            rec = merged.RG[i]
+            if "PP" in rec and rec["PP"] in replaced:
+                rec["PP"] = replaced[rec["PP"]]
+        merged.CO.extend(getattr(h, "CO", []))                                     # mergeCommentLines
+        merged.UserRecords.update(getattr(h, "UserRecords", {}))                  # mergeUserRecords
+        merged.SetHDSO(Unknown)
+    if merged is None:
+        raise ValueError("MergeInputs: no input headers")
+    sq_maps = [[_member(merged.SQ, s["SN"]) for s in h.SQ] for h in headers]
+    maps = {"RG": {}, "PG": {}}
+    for tag in maps:
+        for start in dict.fromkeys(old for t, old, _ in filters if t == tag):
+            v = start
+            for t, old, new in filters:
+                if t == tag and v == old:
+                    v = new
+            if v != start:
+                maps[tag][start] = v
+    return merged, sq_maps, maps["RG"], maps["PG"]

@@ -450,6 +450,35 @@ int elp_set_replace_read_group(elp_ctx *ctx, int on);
 #define ELP_DICT_RENAME_CHROMOSOMES 1u   /* --rename-chromosomes */
 #define ELP_DICT_REPLACE            2u   /* --replace-reference-sequences */
 int elp_set_input_dictionary(elp_ctx *ctx, uint32_t mode, const char *const *names, const int32_t *lengths, int32_t n);
+/* Several input files in one context: a directory of inputs, one BAM per lane, as `elprep filter` and `elprep sfm` take it
+ * (sam.MergeInputs, sam/merge-inputs.go:16-219, and its update filters, sam/split-merge.go:230-311).  The caller merges the files' headers
+ * on the host (elprep_b200.sam.MergeInputs, elprep::MergeInputs) and creates the context from the merged header: elp_config holds the
+ * merged @SQ and the merged @RG lines, colliding IDs renamed.
+ *  - elp_add_input: one input's @SQ as it stands in the file (BAM / BGZF: its binary reference list).  Returns the input's id (0, 1, ...),
+ *    or a negative error code.  Each name maps to the first entry of elp_config.contig_names with that name (memberOfSequenceDictionary);
+ *    a name that is not there is ELP_EINVAL, as is a context without contig_names.  At most ELP_MAX_INPUTS inputs (else ELP_ELIMIT).
+ *  - elp_select_input: the input whose records the next appends carry.  Once an input is added, every append needs one selected
+ *    (ELP_ESTATE without).  ELP_ESTATE while a BGZF file is open: a new file starts after elp_append_bgzf_end, elp_select_input, then
+ *    elp_append_bgzf.
+ *  - elp_set_tag_rename: tag "RG" or "PG"; old_ids[i] -> new_ids[i] is the composed map of the merge's replaceReadGroupIfExists /
+ *    replaceProgramIDIfExists filters (each value through every filter in order).  It applies to the records of every input.  n = 0
+ *    clears the tag's map; an old value given twice is ELP_EINVAL.
+ *  - elp_add_input and elp_set_tag_rename are ELP_ESTATE while the context holds reads or a BGZF file is open.  All three settings survive
+ *    elp_reset; with none of them made, every path is byte for byte as before.  They do not combine with elp_set_input_dictionary
+ *    (ELP_EINVAL either way).
+ *  - Ingest (elp_append_bam, elp_append_sam, elp_append_bgzf).  Every record is rewritten on the device, before the ingest filters, into
+ *    the record the reference writes with the merged header: BAM refID / next_refID through the selected input's map (a value at or past
+ *    the input's entry count is ELP_EBAM); the value of the first RG and the first PG field through the maps (aln.SetRG / SetPG: in place,
+ *    block_size rewritten; a first field of such a tag that is not of type Z is ELP_EBAM, as the filter's string conversion panics).
+ *    elp_append_sam resolves RNAME / RNEXT by name against the merged dictionary, as the reference looks the names up in the merged
+ *    header.  elp_append_bgzf checks the file's reference list against the selected input's names and lengths.
+ *  - Everything after ingest sees records of the merged header: the RG column is the renamed value's @RG, elp_clean_sam reads the merged
+ *    LN, elp_fetch_bam / _bgzf / _sam write the rewritten records, and --replace-read-group and the output field filter apply to them as
+ *    to any record (the replacement wins for RG; the PG rename stays). */
+#define ELP_MAX_INPUTS 255
+int elp_add_input(elp_ctx *ctx, const char *const *names, const int32_t *lengths, int32_t n_sq);
+int elp_select_input(elp_ctx *ctx, int32_t input);
+int elp_set_tag_rename(elp_ctx *ctx, const char *tag, const char *const *old_ids, const char *const *new_ids, int32_t n);
 /* after elp_sort_markdup: the number of records of the output order (elp_n_sorted) that pass the record filters (elp_n_sorted without them);
  * 0 on error or before the sort */
 uint64_t elp_n_output(elp_ctx *ctx);

@@ -16,6 +16,7 @@
 //   filters.AddOrReplaceReadGroup (filters/simple-filters.go:154-162)   elprep::AddOrReplaceReadGroup, DeviceSam::SetReplaceReadGroup (byte paths)
 //   filters.RenameChromosomes (filters/simple-filters.go:189-204)   elprep::RenameChromosomes, DeviceSam::SetInputDictionary (byte paths)
 //   filters.ReplaceReferenceSequenceDictionary (:34-60)             elprep::ReplaceReferenceSequenceDictionary, DeviceSam::SetInputDictionary (byte paths)
+//   sam.MergeInputs (sam/merge-inputs.go:16-219)                   elprep::MergeInputs, DeviceSam::AddInput / SelectInput / SetTagRename (byte paths)
 //   log.Panic(msg)                                                  throw elprep::Panic(msg)
 #pragma once
 #include <algorithm>
@@ -154,6 +155,105 @@ struct ReplaceReferenceSequenceDictionary {
     bool operator()(const Alignment& a) const { return names.count(a.RNAME) != 0; }
 };
 
+// sam.Header with every line as sam.MergeInputs reads it: each record a tag -> value map
+struct HeaderLines {
+    using Record = std::map<std::string, std::string>;
+    Record HD; std::vector<Record> SQ, RG, PG; std::vector<std::string> CO;
+    std::map<std::string, std::vector<Record>> UserRecords;
+};
+
+// mergeSequenceDictionaries (sam/merge-inputs.go:100-124) as written: order-preserving and recursive.  j is set from an index in fromDict
+// after a recursive merge and from an index in the new dictionary after a shared entry, so a later fromDict[j:iFrom] can start behind its
+// end; Go panics on that slice, and so does this.
+inline std::vector<HeaderLines::Record> MergeSequenceDictionaries(const std::vector<HeaderLines::Record>& toDict, const std::vector<HeaderLines::Record>& fromDict) {
+    auto member = [](const std::vector<HeaderLines::Record>& d, const std::string& sn) -> long {   // memberOfSequenceDictionary
+        for (size_t i = 0; i < d.size(); i++) { auto it = d[i].find("SN"); if (it != d[i].end() && it->second == sn) return (long)i; }
+        return -1;
+    };
+    std::vector<HeaderLines::Record> out;
+    long j = 0;
+    for (size_t iTo = 0; iTo < toDict.size(); iTo++) {
+        auto it = toDict[iTo].find("SN");
+        const std::string sn = it == toDict[iTo].end() ? std::string() : it->second;
+        const long iFrom = member(fromDict, sn);
+        if (iFrom < 0) { out.push_back(toDict[iTo]); continue; }
+        const long iNew = member(out, sn);
+        if (iNew >= 0) {
+            if (iNew != (long)iTo) throw Panic(ELP_EINVAL, "Cannot merge sequence dictionaries.");
+            j = iNew + 1;
+        } else {
+            if (j > iFrom) throw Panic(ELP_EINVAL, "runtime error: slice bounds out of range [" + std::to_string(j) + ":" + std::to_string(iFrom) + "]");
+            out = MergeSequenceDictionaries(out, std::vector<HeaderLines::Record>(fromDict.begin() + j, fromDict.begin() + iFrom));
+            out.push_back(toDict[iTo]);
+            j = iFrom + 1;
+        }
+    }
+    for (size_t i = (size_t)j; i < fromDict.size(); i++) out.push_back(fromDict[i]);
+    return out;
+}
+
+// sam.MergeInputs / mergeHeaders (sam/merge-inputs.go:16-219) over the parsed headers of the input files, in file order.  suffix stands for
+// strconv.FormatInt(time.Now().Unix(), 10), the text a colliding @RG or @PG ID gets appended.  header: the merged header; sqMaps[k][i]: the
+// merged index of input k's @SQ i (first match); rgMap / pgMap: the update filters replaceReadGroupIfExists / replaceProgramIDIfExists,
+// which every record of every file runs in list order, composed into old value -> final value.  Build DeviceSam from header, then
+// AddInput(input's @SQ) per file, SetTagRename("RG", rgMap) and SetTagRename("PG", pgMap).  Throws Panic where the reference panics.
+struct MergedInputs {
+    HeaderLines header; std::vector<std::vector<int32_t>> sqMaps; std::map<std::string, std::string> rgMap, pgMap;
+};
+inline MergedInputs MergeInputs(const std::vector<HeaderLines>& headers, const std::string& suffix) {
+    if (headers.empty()) throw Panic(ELP_EINVAL, "MergeInputs: no input headers");
+    MergedInputs m;
+    HeaderLines& to = m.header;
+    to = headers[0];
+    struct Filter { int tag; std::string oldID, newID; };
+    std::vector<Filter> filters;
+    for (size_t f = 1; f < headers.size(); f++) {
+        HeaderLines from = headers[f];
+        for (auto& kv : from.HD) to.HD[kv.first] = kv.second;                           // mergeMetaData
+        to.SQ = MergeSequenceDictionaries(to.SQ, from.SQ);
+        std::map<std::string, bool> ids;                                                 // mergeReadGroups: the IDs before this file
+        for (auto& r : to.RG) ids[r["ID"]] = true;
+        for (auto& r : from.RG) {
+            if (ids.count(r["ID"])) { const std::string old = r["ID"]; r["ID"] = old + suffix; filters.push_back({0, old, r["ID"]}); }
+            to.RG.push_back(r);
+        }
+        std::map<std::string, bool> pgIDs; std::map<std::string, std::string> replaced;   // mergeProgramLines
+        for (auto& r : to.PG) pgIDs[r["ID"]] = true;
+        for (auto& r : from.PG) {
+            if (pgIDs.count(r["ID"])) { const std::string old = r["ID"]; r["ID"] = old + suffix; filters.push_back({1, old, r["ID"]}); replaced[old] = r["ID"]; }
+            to.PG.push_back(r);
+        }
+        for (size_t i = 1; i < from.RG.size(); i++) {                                   // (the PP fix-up walks the RG lines, as written)
+            auto pp = to.RG[i].find("PP");
+            if (pp == to.RG[i].end()) continue;
+            auto nw = replaced.find(pp->second);
+            if (nw != replaced.end()) pp->second = nw->second;
+        }
+        to.CO.insert(to.CO.end(), from.CO.begin(), from.CO.end());                       // mergeCommentLines
+        for (auto& kv : from.UserRecords) to.UserRecords[kv.first] = kv.second;         // mergeUserRecords
+        to.HD["SO"] = "unknown";
+    }
+    for (const HeaderLines& h : headers) {
+        std::vector<int32_t> v;
+        for (auto& s : h.SQ) {
+            int32_t k = -1;
+            for (size_t i = 0; i < to.SQ.size() && k < 0; i++) if (to.SQ[i].at("SN") == s.at("SN")) k = (int32_t)i;
+            v.push_back(k);
+        }
+        m.sqMaps.push_back(v);
+    }
+    for (int tag = 0; tag < 2; tag++) {
+        std::map<std::string, std::string>& out = tag ? m.pgMap : m.rgMap;
+        for (const Filter& s : filters) {
+            if (s.tag != tag || out.count(s.oldID)) continue;
+            std::string v = s.oldID;
+            for (const Filter& g : filters) if (g.tag == tag && v == g.oldID) v = g.newID;
+            if (v != s.oldID) out[s.oldID] = v;
+        }
+    }
+    return m;
+}
+
 enum class SortingOrder { Keep = ELP_SO_KEEP, Unknown = ELP_SO_UNKNOWN, Unsorted = ELP_SO_UNSORTED, Queryname = ELP_SO_QUERYNAME, Coordinate = ELP_SO_COORDINATE };
 
 struct Options {                       // the `elprep filter` flags of the path (cmd/filter.go:435-481)
@@ -266,6 +366,22 @@ class DeviceSam {
         std::vector<const char*> names; std::vector<int32_t> lens;
         for (const Header::SQ& e : input) { names.push_back(e.SN.c_str()); lens.push_back(e.LN); }
         check(elp_set_input_dictionary(ctx_, mode, names.data(), lens.data(), (int32_t)input.size()));
+    }
+    // several input files on the byte paths (elp_add_input, elp_select_input, elp_set_tag_rename): the DeviceSam was built from
+    // MergeInputs(...).header; AddInput once per file with its @SQ (returns its id), SelectInput before the file's AppendBgzf, and the
+    // merge's rgMap / pgMap through SetTagRename.  Before the first append (or after a reset), except SelectInput
+    int AddInput(const std::vector<Header::SQ>& input) {
+        std::vector<const char*> names; std::vector<int32_t> lens;
+        for (const Header::SQ& e : input) { names.push_back(e.SN.c_str()); lens.push_back(e.LN); }
+        const int rc = elp_add_input(ctx_, names.data(), lens.data(), (int32_t)input.size());
+        if (rc < 0) check(rc);
+        return rc;
+    }
+    void SelectInput(int input) { check(elp_select_input(ctx_, input)); }
+    void SetTagRename(const std::string& tag, const std::map<std::string, std::string>& map) {
+        std::vector<const char*> o, n;
+        for (auto& kv : map) { o.push_back(kv.first.c_str()); n.push_back(kv.second.c_str()); }
+        check(elp_set_tag_rename(ctx_, tag.c_str(), o.data(), n.data(), (int32_t)o.size()));
     }
     // the Finalize of AddNodes: By(CoordinateLess / QNAMELess).ParallelStableSort + filters.MarkDuplicates (+ MarkOpticalDuplicates)
     void Finalize(SortingOrder order) { check(elp_sort_markdup(ctx_, (int)order, opts_.MarkDuplicates ? (opts_.AlsoOpticals ? ELP_MARKDUP_OPTICAL : ELP_MARKDUP) : 0)); }
