@@ -922,16 +922,22 @@ FastPlan plan_fast(const elp_ctx* c, const uint32_t present[4]) {
 
 template <int S> int launch_count(elp_ctx* c, CountArgs K, bool indel, unsigned grid) {
     // CTA-private mismatch tables when they are small (<= 24 KB); otherwise the global table takes the (sparse) mismatches directly
-    const size_t mm = ((size_t)K.n_cls * S * 32 * K.lpr + (size_t)(K.n_cls / 2) * S * 16);
+    const size_t n_cyc = (size_t)K.n_cls * S * 32 * K.lpr, mm = n_cyc + (size_t)(K.n_cls / 2) * S * 16;
     K.mm_cells = mm * 4 <= 24 * 1024 ? (uint32_t)mm : 0u;
-    const size_t smem0 = (size_t)CNT_WARPS * (CNT_STAGES * 7 * 512 + CNT_RECRING * K.rec_bytes) + (size_t)K.mm_cells * 4, smem1 = (size_t)CNT_WARPS * (CNT_STAGES * 9 * 512 + CNT_RECRING * K.rec_bytes) + (size_t)K.mm_cells * 4;
-    if (!indel) {
-        CUDA_TRY(c, cudaFuncSetAttribute(bqsr_count_kernel<S, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem0));
-        bqsr_count_kernel<S, false><<<grid, CNT_WARPS * 32, smem0, c->stream>>>(K);
-    } else {
-        CUDA_TRY(c, cudaFuncSetAttribute(bqsr_count_kernel<S, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1));
-        bqsr_count_kernel<S, true><<<grid, CNT_WARPS * 32, smem1, c->stream>>>(K);
+    const size_t stage = (size_t)CNT_WARPS * (CNT_STAGES * (indel ? 9 : 7) * 512 + CNT_RECRING * K.rec_bytes);
+    const auto kern = indel ? bqsr_count_kernel<S, true> : bqsr_count_kernel<S, false>;
+    // the cycle table of the counted bases joins them when CNT_MINB CTAs per SM still fit (the grid is CNT_MINB CTAs per SM)
+    K.cyc_cells = 0;
+    if (K.mm_cells) {
+        const size_t with = stage + (mm + n_cyc) * 4;
+        int fit = 0;
+        CUDA_TRY(c, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)with));
+        CUDA_TRY(c, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&fit, kern, CNT_WARPS * 32, with));
+        if (fit >= CNT_MINB) K.cyc_cells = (uint32_t)n_cyc;
     }
+    const size_t smem = stage + ((size_t)K.mm_cells + K.cyc_cells) * 4;
+    CUDA_TRY(c, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kern<<<grid, CNT_WARPS * 32, smem, c->stream>>>(K);
     return E_OK;
 }
 
